@@ -1,7 +1,7 @@
-"""In-tree build of libacnn.so (sm_100a only) with plain nvcc -- no JIT cache, no torch extension.
+"""In-tree build of libacnn.so (sm_90a only) with plain nvcc -- no JIT cache, no torch extension.
 
 `python -m assembled_cnn_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a
-GPU; the resulting .so sits next to this file so it travels to the GPU box with the repo snapshot.
+GPU; the resulting .so sits next to this file, so the package imports from the source tree.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ OBJ_DIR = os.path.join(HERE, "build")
 LIB_PATH = os.path.join(HERE, "libacnn.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr", "--extended-lambda",
@@ -87,7 +87,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(compile_one, jobs))
     if jobs or not os.path.exists(LIB_PATH):
-        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

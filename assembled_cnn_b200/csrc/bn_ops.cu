@@ -1,7 +1,7 @@
 // Batch-norm, SK and SE elementwise / reduction kernels (HBM-bound; 16-byte vector accesses along
 // the NHWC channel dimension, per-channel reductions through shared memory + one atomic per
 // channel per CTA).  Reference: nets/model_helper.py:26-37, nets/blocks.py:110-184 and the
-// backward formulas of SURVEY App. C.
+// explicit backward formulas of batch normalisation.
 #include "common.h"
 #include "stream_pipe.cuh"
 #include "vec.cuh"
@@ -26,8 +26,7 @@ __global__ void bn_finalize_kernel(const float* __restrict__ stats, int nparts, 
   pdl_entry();
   // 8 channels per CTA x 32 lanes over the partial rows: lane l adds rows l, l+32, ... (<= 5 loads,
   // all in flight at once), then the 32 lane sums are added in lane order -- a fixed tree:
-  // deterministic.  (A single thread walking all rows is a chain of L2 latencies: measured +0.8 ms
-  // per training step over the 190 finalize launches.)
+  // deterministic.  (A single thread walking all rows would be a chain of L2 latencies.)
   __shared__ double red[2][32][9];
   const int cc = threadIdx.x & 7, pl = threadIdx.x >> 3;
   const int c = blockIdx.x * 8 + cc;
@@ -949,7 +948,7 @@ static void launch_sk_image_reduce(const void* y, const void* dv, const float* s
 // Row slabs per image for the image-aligned SK kernels: ~`ctas_per_sm` CTAs per SM overall, at
 // least one trip of the unrolled row loop (4 * rpb rows) per CTA.
 static int row_slabs(int B, int HW, int rpb, int ctas_per_sm = 8) {
-  int s = (148 * ctas_per_sm + B - 1) / B;
+  int s = (kMaxSms * ctas_per_sm + B - 1) / B;
   const int max_s = (HW + 4 * rpb - 1) / (4 * rpb);
   if (s > max_s) s = max_s;
   return s < 1 ? 1 : s;
@@ -962,7 +961,7 @@ static bool cg_ok(int C) {
 
 static int bn_bwd_reduce_grid(int64_t M, int C) {
   const int rpb = kT / (C >> 3);
-  return grid_for(ceil_div64(M, 4 * rpb), 1, 148 * 2);
+  return grid_for(ceil_div64(M, 4 * rpb), 1, kMaxSms * 2);
 }
 
 template <class T>
@@ -1154,7 +1153,8 @@ int acnn_se_bwd_gate(const void* g, const void* y, const float* scale, const flo
 int acnn_gap_fwd(const void* x, void* pooled, int B, int HW, int C, int dtype, void* stream) {
   ACNN_REQUIRE(x && pooled && cg_ok(C) && ACNN_DTYPE_OK(dtype), "gap_fwd: bad arguments C=%d", C);
   // C = 2048 would give every thread its own channel group and all HW rows (one 16-byte load in flight
-  // per thread: 1.8 TB/s under ncu); 512 channels per CTA let four threads share the rows of a group
+  // per thread: too few bytes in flight to fill HBM); 512 channels per CTA let four threads share the
+  // rows of a group
   const int csplit = (C >= 1024 && C % 512 == 0) ? C / 512 : 1;
   ACNN_BY_DTYPE(dtype, (launch_k(image_reduce_kernel<T, 4>, dim3(B, csplit), dim3(kT), 0,
                                  (cudaStream_t)stream, (const T*)x, (const T*)nullptr,

@@ -17,14 +17,13 @@ void set_error(const char* fmt, ...) {
 }
 
 static int pdl_default() {
-  // measured on the full training step: 25.3-25.5 ms with the attribute vs 24.9 ms without (an early
-  // resident dependent takes registers / SM slots from the still-running HBM-bound predecessor), so
-  // it is opt-in
+  // opt-in: an early resident dependent takes registers / SM slots from a still-running HBM-bound
+  // predecessor
   const char* e = getenv("ACNN_PDL");
   return (e && (e[0] == '1' || e[0] == '2')) ? e[0] - '0' : 0;
 }
 int g_use_pdl = pdl_default();
-int g_stream_grid_cap = 148 * 16;   // vec.cuh grid_for(); acnn_set_stream_grid_cap
+int g_stream_grid_cap = kMaxSms * 16;   // vec.cuh grid_for(); acnn_set_stream_grid_cap
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
@@ -50,9 +49,31 @@ int acnn_set_pdl(int on) {
 }
 int acnn_set_stream_grid_cap(int blocks) {
   const int prev = acnn::g_stream_grid_cap;
-  acnn::g_stream_grid_cap = blocks >= 148 ? blocks : 148 * 16;
+  acnn::g_stream_grid_cap = blocks >= acnn::kMaxSms ? blocks : acnn::kMaxSms * 16;
   return prev;
 }
 int64_t acnn_launch_count(void) { return acnn::g_launches.load(std::memory_order_relaxed); }
 
 }  // extern "C"
+
+namespace acnn {
+
+int scratch_alloc(void** p, size_t bytes, cudaStream_t stream, const char* what) {
+  cudaError_t e = cudaMallocAsync(p, bytes, stream);
+  if (e != cudaSuccess) {
+    set_error("%s: scratch of %zu bytes: %s", what, bytes, cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  return ACNN_OK;
+}
+
+int scratch_free(void* p, cudaStream_t stream, const char* what) {
+  cudaError_t e = cudaFreeAsync(p, stream);
+  if (e != cudaSuccess) {
+    set_error("%s: releasing scratch: %s", what, cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  return ACNN_OK;
+}
+
+}  // namespace acnn

@@ -14,6 +14,16 @@ void count_launch(int n = 1);
 
 // Returns ACNN_OK or records the CUDA error (launch-configuration errors surface here).
 int check_launch(const char* what);
+// The H100 SXM's SM count: grid-size heuristics and the capacities of the per-CTA partial-sum
+// buffers (model_plan.h, plan.py) are sized for one wave of it, and the conv launchers use at most
+// this many SMs, so those capacities hold on any device.
+constexpr int kMaxSms = 132;
+
+// Stream-ordered scratch of one launch (split-K partials): cudaMallocAsync on `stream`, released by
+// scratch_free on the same stream after the kernels that use it.  Concurrent streams get distinct
+// buffers; under stream capture both become graph memory nodes.
+int scratch_alloc(void** p, size_t bytes, cudaStream_t stream, const char* what);
+int scratch_free(void* p, cudaStream_t stream, const char* what);
 
 #define ACNN_REQUIRE(cond, ...)        \
   do {                                 \
@@ -28,8 +38,9 @@ int check_launch(const char* what);
 // kernel launched with the programmatic-stream-serialization attribute may be scheduled (CTAs
 // resident, prologue done) while its predecessor drains, and only proceeds past the wait once the
 // predecessor grid has completed and flushed.  Meant to hide the per-kernel launch / drain latency
-// of the ~865 dependent launches of a step; measured NOT to pay here (kept as an opt-in knob).
-extern int g_use_pdl;   // 0 by default (mode 1 measured slower, see common.cu); ACNN_PDL=1|2 / acnn_set_pdl
+// of the dependent launches of a step; opt-in (an early dependent takes SM resources from its
+// still-running predecessor).
+extern int g_use_pdl;   // 0 by default; ACNN_PDL=1|2 / acnn_set_pdl
 
 template <class... KArgs, class... Args>
 inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,

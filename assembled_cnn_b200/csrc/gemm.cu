@@ -1,15 +1,15 @@
-// tcgen05 implicit-GEMM convolutions for sm_100a.
+// wgmma implicit-GEMM convolutions for sm_90a.
 //
 //   conv_gemm_kernel : y[M, Cout] = im2col(x)[M, K] * w[Cout, K]^T          (fprop, dgrad, dense)
 //                      A tiles arrive by TMA (tiled 2-D for 1x1/s1, im2col 4-D otherwise) in the
-//                      128B/64B/32B-swizzled K-major layout tcgen05.mma reads directly; the fp32
-//                      accumulator lives in TMEM; a 4-warp epilogue drains it with tcgen05.ld and
-//                      fuses bias / gradient-accumulate / ReLU-mask / batch-norm column sums.
+//                      128B/64B/32B-swizzled K-major layout wgmma reads directly; the fp32
+//                      accumulator lives in the registers of two consumer warpgroups, which then
+//                      fuse bias / gradient-accumulate / ReLU-mask / batch-norm column sums.
 //   wgrad_gemm_kernel: dw[Cout, K] += dy[P, Cout]^T * im2col(x)[P, K]       (split-K over pixels)
 //                      both operands are MN-major (the pixel index is the GEMM K dimension).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2..5 = epilogue (TMEM lane quarter = warp_idx % 4).
+// Warp roles (384 threads): warp 0 = TMA producer (warps 1..3 idle), warpgroups 1 and 2 = wgmma
+// consumers + epilogue, 64 accumulator rows each.
 //
 // Reference semantics: nets/model_helper.py:67-78 (conv2d_fixed_padding), tf.gradients backward.
 #include <stdlib.h>
@@ -144,319 +144,128 @@ struct ConvGemmParams {
   const float* bias;
   int has_add, has_mask;
   int out_f32;
-  int out_bufs;     // 1 or 2 output staging half tiles (2: a half's TMA store drains under the next)
-  int split_epi;    // two independent 4-warp epilogue groups alternate tiles (implies out_bufs = 2
-                    // and two sets of add / mask staging tiles)
 };
 
-constexpr int kBM = 128;        // output pixels per CTA tile == UMMA M == TMEM lanes
+constexpr int kBM = 128;        // output pixels per CTA tile (two consumer warpgroups x 64 rows)
 constexpr int kStageK = 64;     // K elements per pipeline stage
-constexpr int kThreads = 192;          // wgrad kernel: TMA warp + MMA warp + 4 epilogue warps
-constexpr int kConvThreads = 320;      // conv kernel: TMA warp + MMA warp + 8 epilogue warps
-constexpr int kEpiThreads = 256;
+// 3 warpgroups: warpgroup 0 = TMA producer (warp 0 issues), warpgroups 1 and 2 = wgmma consumers,
+// rows 0..63 and 64..127 of every tile, which then run the epilogue from their accumulator registers
+constexpr int kThreads = 384;
+constexpr int kConsumerThreads = 256;
+constexpr int kConsumerWarps = 8;
 constexpr int kMaxStages = 8;
-constexpr int kSmemBudget = 224 * 1024;   // dynamic smem (227 KiB max per CTA, ~0.2 KiB static)
+constexpr int kSmemBudget = 224 * 1024;   // dynamic smem (227 KiB max per CTA on sm_90)
 
-// MT = 128-row M tiles per CTA tile (1 or 2).  With MT = 2 a CTA computes two output tiles that
-// share every weight stage: twice the tensor work per pipeline round-trip (the single-warp issue
-// loops, not bandwidth, bound the N <= 128 layers) and half the weight traffic per FLOP.
 // (a-plane, b-plane) of the t-th cross product of two 3-plane operands, smallest magnitude first:
 // (2,0) (1,1) (0,2) [2^-16]  (1,0) (0,1) [2^-8]  (0,0)
 __host__ __device__ constexpr int plane_term_a(int t) { return t == 0 ? 2 : ((t == 1 || t == 3) ? 1 : 0); }
 __host__ __device__ constexpr int plane_term_b(int t) { return t == 2 ? 2 : ((t == 1 || t == 4) ? 1 : 0); }
 
 // NP = operand planes: 1 = bf16 operands; 3 = fp32 operands split into three bf16 planes
-// (x = hi + mid + lo, 24 mantissa bits) whose six significant cross products are accumulated in the
-// same fp32 TMEM accumulator -- the fp32 parity mode (acnn.h ACNN_F32) on the same TMA / im2col /
-// descriptor / epilogue code as the bf16 path.
-static inline int fprop_stage_bytes(int bn, int mt, int np, bool pair = false) {
-  return np * (mt * kBM * kStageK * 2 + (pair ? bn / 2 : bn) * kStageK * 2);
-}
-static inline int fprop_stages(int bn, int mt, int np, bool has_add, bool has_mask, bool out_f32,
-                               bool pair = false, int out_bufs = 1, int aux_sets = 1) {
+// (x = hi + mid + lo, 24 mantissa bits) whose six significant cross products are accumulated in
+// fp32 -- the fp32 parity mode (acnn.h ACNN_F32) on the same TMA / im2col / descriptor / epilogue
+// code as the bf16 path.
+static inline int fprop_stage_bytes(int bn, int np) { return np * (kBM * kStageK * 2 + bn * kStageK * 2); }
+static inline int fprop_stages(int bn, int np, bool has_add, bool has_mask, bool out_f32) {
   const int half_n = bn > 128 ? 128 : bn;
   const int tile = kBM * half_n * 2;
-  const int fixed = 1024 + (out_f32 ? 0 : out_bufs * tile) + (has_add ? aux_sets * tile : 0) +
-                    (has_mask ? aux_sets * tile : 0);
-  int st = (kSmemBudget - fixed) / fprop_stage_bytes(bn, mt, np, pair);
+  const int fixed = 1024 + (out_f32 ? 0 : tile) + (has_add ? tile : 0) + (has_mask ? tile : 0);
+  int st = (kSmemBudget - fixed) / fprop_stage_bytes(bn, np);
   if (st > kMaxStages) st = kMaxStages;
   if (st < 2) st = 2;
   return st;
 }
 
-// CG2: a CTA PAIR (tcgen05 cta_group::2) computes one 256 x BN tile: each CTA stages its own 128 rows
-// of A and only HALF of the weight tile, the leader issues one M = 256 MMA that reads both halves.
-// Shared-memory ingest per SM per k-block drops from A + B to A + B/2 -- what bounds the N = 256
-// tiles (DESIGN section 4).
-template <int BN, int MT, int NP = 1, bool CG2 = false>
+template <int BN, int NP = 1>
 struct FpropCfg {
-  static constexpr int kAHalfBytes = kBM * kStageK * 2;   // 16 KiB per M tile
-  static constexpr int kABytes = MT * kAHalfBytes;        // one plane
-  static constexpr int kBRows = CG2 ? BN / 2 : BN;        // weight rows staged by this CTA
-  static constexpr int kBBytes = kBRows * kStageK * 2;    // one plane
+  static constexpr int kABytes = kBM * kStageK * 2;       // one plane, 16 KiB
+  static constexpr int kBBytes = BN * kStageK * 2;        // one plane
   static constexpr int kStageBytes = NP * (kABytes + kBBytes);
   static_assert(2 * kStageBytes + 1024 <= kSmemBudget, "two pipeline stages must fit");
-  // the epilogue handles the accumulator in column halves of <= 128 (one staging buffer each for
-  // the output, add and mask tiles), so a 128 x 256 tile needs no more staging than 128 x 128
+  // the epilogue stages the tile in column halves of <= 128 (one staging buffer each for the
+  // output, add and mask tiles), so a 128 x 256 tile needs no more staging than 128 x 128
   static constexpr int kHalfN = BN > 128 ? 128 : BN;
   static constexpr int kNHalf = BN / kHalfN;
   static constexpr int kSubW = kHalfN < 64 ? kHalfN : 64;  // staging sub-tile width (TMA box)
   static constexpr int kTileBytes = kBM * kHalfN * 2;      // one staged half tile (bf16)
-  // accumulator columns of one stage: MT tiles of BN columns; NP == 3 keeps TWO accumulators per
-  // tile -- the hi*hi products and the five small cross terms separately (added in the epilogue) --
-  // because the tensor core truncates an addend below the accumulator's ulp: small terms summed
-  // into the big accumulator lose ~6 bits each (measured 2e-5 relative at K = 4608)
-  static constexpr int kAccCols = (NP == 3 ? 2 : MT) * BN;
-  static constexpr int kTmemCols = 2 * kAccCols < 32 ? 32 : 2 * kAccCols;   // two accumulator stages
-  static_assert(2 * kAccCols <= 512 && (NP == 1 || MT == 1), "TMEM holds 512 columns");
-  static_assert(!CG2 || (MT == 1 && NP == 1), "CTA pairs: one M tile per CTA, bf16 operands");
+  // NP == 3 keeps TWO accumulators -- the hi*hi products and the five small cross terms
+  // separately (added in the epilogue) -- because the tensor core truncates an addend below the
+  // accumulator's ulp: small terms summed into the big accumulator lose ~6 bits each
+  static_assert(NP == 1 || BN <= 128, "fp32 mode: N tile <= 128 (registers)");
+  // (NP == 3 at BN = 128: acc + acc2 are 128 fp32 registers per thread under the 168-register cap of
+  // a 384-thread CTA, so the epilogue spills a few hundred bytes; the fp32 parity mode is a
+  // correctness mode, the bf16 path does not spill)
   // smem: [stages x (A|B)] [out staging] [add staging] [mask staging]
-  static int stages_for(bool has_add, bool has_mask, bool out_f32, int out_bufs = 1,
-                        int aux_sets = 1) {
-    return fprop_stages(BN, MT, NP, has_add, has_mask, out_f32, CG2, out_bufs, aux_sets);
+  static int stages_for(bool has_add, bool has_mask, bool out_f32) {
+    return fprop_stages(BN, NP, has_add, has_mask, out_f32);
   }
-  static int smem_bytes(int stages, bool has_add, bool has_mask, bool out_f32, int out_bufs = 1,
-                        int aux_sets = 1) {
-    return 1024 + stages * kStageBytes + (out_f32 ? 0 : out_bufs * kTileBytes) +
-           (has_add ? aux_sets * kTileBytes : 0) + (has_mask ? aux_sets * kTileBytes : 0);
+  static int smem_bytes(int stages, bool has_add, bool has_mask, bool out_f32) {
+    return 1024 + stages * kStageBytes + (out_f32 ? 0 : kTileBytes) + (has_add ? kTileBytes : 0) +
+           (has_mask ? kTileBytes : 0);
   }
 };
 
-// Split epilogue of conv_gemm_kernel (one M tile per CTA tile, bf16 output, no bias): the 8 epilogue
-// warps form two independent groups of four (one warp per TMEM lane quarter); group g drains
-// accumulator stage g of the tiles g, g + 2, ... with its own output / add / mask staging tiles, named
-// barrier (1 + g, 128 threads), aux mbarrier and TMA store queue, so the chain of one tile (barrier ->
-// TMEM load -> convert -> stage -> barrier -> store -> statistics, per column half) overlaps the next
-// tile's.  That chain -- not the tensor pipe, not HBM -- paces tiles with one or two k-blocks (the
-// small-K 1x1 convolutions).  Same arithmetic per element as the joint epilogue; the statistics are
-// summed in a different (fixed) order.
-// MT == 2 (two M tiles per CTA tile): the two groups drain the two M tiles of EVERY tile concurrently
-// (group g = M tile g, both waiting on the same accumulator barrier; the "accumulator empty" barrier
-// then counts two arrivals) instead of alternating tiles.
-template <int BN, int MT>
-__device__ __forceinline__ void conv_epilogue_split(
-    const ConvGemmParams& p, const CUtensorMap* tmC, const CUtensorMap* tmAdd,
-    const CUtensorMap* tmMask, uint32_t tmem_base, uint8_t* s_out0, uint8_t* s_add, uint8_t* s_mask,
-    uint64_t* tfull_bar, uint64_t* tempty_bar, uint64_t* aux_bars, int n0, int m_first, int m_step,
-    int my_tiles) {
-  using Cfg = FpropCfg<BN, MT, 1, false>;
-  constexpr bool kPerMt = MT == 2;                     // groups = M tiles of one CTA tile
-  constexpr int kTileM = MT * kBM;
-  constexpr int kHalfN = Cfg::kHalfN;
-  constexpr int kNHalf = Cfg::kNHalf;
-  constexpr int kSubW = Cfg::kSubW;
+// byte offset of the bf16 pair (row r, column c, c even) of a staged half tile: sub-tiles of kSubW
+// columns, rows of kSubW * 2 bytes in the TMA swizzle layout (16-byte piece j of row r at j ^ swz)
+template <int kSubW>
+__device__ __forceinline__ int staged_offset(int r, int c) {
   constexpr int kRowBytes = kSubW * 2;
-  constexpr int kSubBytes = kBM * kRowBytes;
-  constexpr int kNSub = kHalfN / kSubW;
-  constexpr int kNChunk = kHalfN / 8;                  // 16-byte column chunks of a half tile
-  constexpr int kNRg = 128 / kNChunk;                  // row groups inside one epilogue group
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int quarter = warp & 3;
-  const int grp = (warp - 2) >> 2;
-  const int r = quarter * 32 + lane;                   // row inside the tile == TMEM lane
-  const int gt = static_cast<int>(threadIdx.x) - 64 - grp * 128;   // thread index inside the group
-  const bool gleader = gt == 0;
-  const bool stats = p.ch_part != nullptr;
-  const bool has_aux = p.has_add || p.has_mask;
+  const int sub = c / kSubW, cb = (c % kSubW) * 2;
   const int swz = (kRowBytes == 128) ? (r & 7) : ((r >> 1) & 3);
-  uint8_t* so_ = s_out0 + grp * Cfg::kTileBytes;
-  uint8_t* sa_ = s_add + grp * Cfg::kTileBytes;
-  uint8_t* sm_ = s_mask + grp * Cfg::kTileBytes;
-  uint64_t* abar = &aux_bars[grp];
-  const int st_chunk = gt % kNChunk, st_rg = gt / kNChunk;
-  float acc_s[kNHalf][8], acc_q[kNHalf][8];
-#pragma unroll
-  for (int hf = 0; hf < kNHalf; ++hf)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) acc_s[hf][e] = acc_q[hf][e] = 0.f;
-  uint32_t aux_n = 0;
-  auto group_sync = [&]() {
-    if (grp == 0) asm volatile("bar.sync 1, 128;\n" ::: "memory");
-    else asm volatile("bar.sync 2, 128;\n" ::: "memory");
-  };
-  auto issue_aux = [&](int am0, int anh) {
-    mbar_expect_tx(abar, (p.has_add ? Cfg::kTileBytes : 0) + (p.has_mask ? Cfg::kTileBytes : 0));
-#pragma unroll
-    for (int sub = 0; sub < kNSub; ++sub) {
-      if (p.has_add) tma_load_2d(sa_ + sub * kSubBytes, tmAdd, abar, anh + sub * kSubW, am0);
-      if (p.has_mask) tma_load_2d(sm_ + sub * kSubBytes, tmMask, abar, anh + sub * kSubW, am0);
-    }
-  };
-  const int it0 = kPerMt ? 0 : grp, it_step = kPerMt ? 1 : 2;
-  const int m_off = kPerMt ? grp * kBM : 0;            // this group's M tile inside the CTA tile
-  if (gleader && has_aux && it0 < my_tiles) issue_aux((m_first + it0 * m_step) * kTileM + m_off, n0);
-
-  for (int it = it0; it < my_tiles; it += it_step) {
-    const int m0 = (m_first + it * m_step) * kTileM + m_off;
-    const int acc = kPerMt ? (it & 1) : grp;           // TMEM accumulator stage of this tile
-#pragma unroll
-    for (int hf = 0; hf < kNHalf; ++hf) {
-      const int nh = n0 + hf * kHalfN;
-      if (gleader) tma_store_wait_read();              // this group's previous store has read so_
-      group_sync();
-      if (hf == 0) {
-        mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-        tc_fence_after();
-      }
-      if (has_aux) {
-        mbar_wait(abar, aux_n & 1);
-        ++aux_n;
-      }
-#pragma unroll
-      for (int c = 0; c < kHalfN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * Cfg::kAccCols +
-                          (kPerMt ? grp * BN : 0) + hf * kHalfN + c * 32, v);
-        tmem_ld_wait();
-        float f[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-        const int sub = (c * 32) / kSubW;
-        const int j0 = ((c * 32) % kSubW) / 8;
-        const int soff = sub * kSubBytes + r * kRowBytes;
-        if (p.has_add) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint4 u = *reinterpret_cast<const uint4*>(sa_ + soff + (((j0 + q) ^ swz) << 4));
-            const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              bf16x2_add(f[q * 8 + e * 2 + 0], f[q * 8 + e * 2 + 1], w4[e]);
-          }
-        }
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) pk[i] = pack_bf16x2(f[2 * i], f[2 * i + 1]);
-        if (p.has_mask) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint4 u = *reinterpret_cast<const uint4*>(sm_ + soff + (((j0 + q) ^ swz) << 4));
-            pk[q * 4 + 0] &= bf16x2_gt0_mask(u.x);
-            pk[q * 4 + 1] &= bf16x2_gt0_mask(u.y);
-            pk[q * 4 + 2] &= bf16x2_gt0_mask(u.z);
-            pk[q * 4 + 3] &= bf16x2_gt0_mask(u.w);
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-          *reinterpret_cast<uint4*>(so_ + soff + (((j0 + q) ^ swz) << 4)) =
-              make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
-      }
-      if (hf == kNHalf - 1) tc_fence_before();
-      fence_proxy_async();
-      group_sync();
-      if (gleader) {
-        if (hf == kNHalf - 1) mbar_arrive(&tempty_bar[acc]);
-#pragma unroll
-        for (int sub = 0; sub < kNSub; ++sub)
-          tma_store_2d(tmC, so_ + sub * kSubBytes, nh + sub * kSubW, m0);
-        tma_store_commit();
-        if (has_aux) {
-          if (hf + 1 < kNHalf) issue_aux(m0, nh + kHalfN);
-          else if (it + it_step < my_tiles)
-            issue_aux((m_first + (it + it_step) * m_step) * kTileM + m_off, n0);
-        }
-      }
-      if (stats) {
-        // column sums of the half tile as stored (bf16-rounded); rows past M were computed from
-        // zero-filled operands and contribute zero
-        const int sub = st_chunk / (kSubW / 8), jj = st_chunk % (kSubW / 8);
-#pragma unroll 4
-        for (int rr = st_rg; rr < kBM; rr += kNRg) {
-          const int sw = (kRowBytes == 128) ? (rr & 7) : ((rr >> 1) & 3);
-          const uint4 u = *reinterpret_cast<const uint4*>(so_ + sub * kSubBytes + rr * kRowBytes +
-                                                          ((jj ^ sw) << 4));
-          const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            bf16x2_sum_sq(acc_s[hf][2 * e], acc_q[hf][2 * e], acc_s[hf][2 * e + 1],
-                          acc_q[hf][2 * e + 1], w4[e]);
-        }
-      }
-    }
-  }
-  if (gleader) tma_store_wait_all();
-  if (stats && my_tiles > 0) {
-    // cross-group / cross-row-group reduction in the (now idle) staging tiles
-    float* red_sum = reinterpret_cast<float*>(s_out0);
-    float* red_sq = red_sum + 2 * kNRg * BN;
-    static_assert(2 * 2 * kNRg * BN * 4 <= 2 * Cfg::kTileBytes, "staging tiles too small for stats");
-    asm volatile("bar.sync 3, 256;\n" ::: "memory");    // both groups' stores have drained
-#pragma unroll
-    for (int hf = 0; hf < kNHalf; ++hf)
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        red_sum[(grp * kNRg + st_rg) * BN + hf * kHalfN + st_chunk * 8 + e] = acc_s[hf][e];
-        red_sq[(grp * kNRg + st_rg) * BN + hf * kHalfN + st_chunk * 8 + e] = acc_q[hf][e];
-      }
-    asm volatile("bar.sync 3, 256;\n" ::: "memory");
-    for (int col = static_cast<int>(threadIdx.x) - 64; col < BN; col += kEpiThreads) {
-      float ss = 0.f, qq = 0.f;
-      for (int g2 = 0; g2 < 2 * kNRg; ++g2) {
-        ss += red_sum[g2 * BN + col];
-        qq += red_sq[g2 * BN + col];
-      }
-      float* row = p.ch_part + static_cast<size_t>(m_first) * 2 * p.Cout;
-      row[n0 + col] = ss;
-      row[p.Cout + n0 + col] = qq;
-    }
-  }
+  return sub * (kBM * kRowBytes) + r * kRowBytes + ((((cb >> 4) ^ swz)) << 4) + (cb & 15);
 }
 
-// One CTA per SM walks output tiles (fixed N tile, M tiles strided by the grid).  The TMA producer
-// runs ahead across tiles through the smem ring; the MMA issuer alternates between two TMEM
-// accumulators; the 8 epilogue warps (two per TMEM lane quarter, alternating 32-column chunks)
-// drain accumulator i while the tensor core fills i^1.
-template <int BN, int CW, bool IM2COL, int MT, int NP, bool CG2>
-__global__ void __launch_bounds__(kConvThreads, 1)
+// One CTA per SM walks output tiles (fixed N tile, M tiles strided by the grid).  CG2: a cluster of
+// two CTAs walks 256-row tiles (rank r computes rows r*128 ..) of one N tile; each CTA loads half of
+// every weight stage and multicasts it to both, halving the weight traffic per tile.  The TMA producer
+// runs ahead across tiles through the smem ring (it keeps loading the next tile's stages while the
+// consumers run the epilogue); each consumer warpgroup accumulates 64 rows x BN in registers with
+// wgmma, keeping one k-block of MMAs in flight, and releases a stage as soon as the MMAs that read
+// it have completed.
+template <int BN, int CW, bool IM2COL, int NP, bool CG2>
+__global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAdd,
                  const __grid_constant__ CUtensorMap tmMask, const __grid_constant__ CUtensorMap tmA1,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB1,
                  const __grid_constant__ CUtensorMap tmB2, const ConvGemmParams p) {
-  using Cfg = FpropCfg<BN, MT, NP, CG2>;
-  constexpr int kTileM = (CG2 ? 2 : MT) * kBM;  // output pixels per CTA tile (per CTA pair with CG2)
+  using Cfg = FpropCfg<BN, NP>;
   constexpr int kChunks = kStageK / CW;        // A chunks (one filter tap each when Cin < 64)
   constexpr int kChunkBytes = kBM * CW * 2;
-  constexpr int kKSteps = CW / 16;             // UMMA K = 16 bf16
-  constexpr uint32_t kIdesc = make_idesc_bf16_m(CG2 ? 256 : 128, BN, false, false);
+  constexpr int kKSteps = CW / 16;             // wgmma K = 16 bf16
   constexpr int kHalfN = Cfg::kHalfN;
   constexpr int kNHalf = Cfg::kNHalf;
   constexpr int kSubW = Cfg::kSubW;
-  constexpr int kRowBytes = kSubW * 2;
-  constexpr int kSubBytes = kBM * kRowBytes;
+  constexpr int kSubBytes = kBM * kSubW * 2;
   constexpr int kNSub = kHalfN / kSubW;
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[kMaxStages];
   __shared__ uint64_t empty_bar[kMaxStages];
-  __shared__ uint64_t tfull_bar[2];
-  __shared__ uint64_t tempty_bar[2];
-  __shared__ uint64_t aux_bars[2];
-  __shared__ uint32_t tmem_base_smem;
-  uint64_t& aux_bar = aux_bars[0];
+  __shared__ uint64_t aux_bar;
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   const int kStages = p.stages;
-  uint8_t* s_out0 = smem + kStages * Cfg::kStageBytes;
-  uint8_t* s_add = s_out0 + (p.out_f32 ? 0 : p.out_bufs * Cfg::kTileBytes);
-  uint8_t* s_mask = s_add + (p.has_add ? (p.split_epi ? 2 : 1) * Cfg::kTileBytes : 0);
+  uint8_t* s_out = smem + kStages * Cfg::kStageBytes;
+  uint8_t* s_add = s_out + (p.out_f32 ? 0 : Cfg::kTileBytes);
+  uint8_t* s_mask = s_add + (p.has_add ? Cfg::kTileBytes : 0);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_kb = (p.Ktot + kStageK - 1) / kStageK;
   // static tile schedule: this CTA (CG2: this CTA pair) owns N tile n_tile and M tiles m_first,
-  // m_first + m_step, ...; with CG2 the CTA of rank r in its pair computes rows r*128.. of the tile
+  // m_first + m_step, ...; with CG2 the CTA of rank r computes rows r*128 .. of each 256-row tile
+  constexpr int kTileM = (CG2 ? 2 : 1) * kBM;
   const uint32_t cta_rank = CG2 ? cluster_ctarank() : 0u;
-  const int unit = CG2 ? (blockIdx.x >> 1) : blockIdx.x;
-  const int units = CG2 ? (gridDim.x >> 1) : gridDim.x;
+  const int unit = CG2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
+  const int units = CG2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
   const int n_tile = unit % p.n_tiles;
   const int m_first = unit / p.n_tiles;
   const int m_step = units / p.n_tiles;
   const int n0 = n_tile * BN;
   const int my_tiles = m_first < p.m_tiles ? (p.m_tiles - m_first + m_step - 1) / m_step : 0;
-  const int m_rank_off = CG2 ? static_cast<int>(cta_rank) * kBM : 0;
+  const int m_rank_off = static_cast<int>(cta_rank) * kBM;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -472,81 +281,59 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (p.has_mask) tma_prefetch_desc(&tmMask);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      // one arrival per consumer warp (CG2: of both CTAs -- the stage receives the peer's multicast)
+      mbar_init(&empty_bar[s], kConsumerWarps * (CG2 ? 2 : 1));
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      // CG2: the epilogues of both CTAs release it; split epilogue with two M tiles: both groups
-      mbar_init(&tempty_bar[s], (CG2 || (MT == 2 && p.split_epi)) ? 2 : 1);
-    }
-    mbar_init(&aux_bars[0], 1);
-    mbar_init(&aux_bars[1], 1);
+    mbar_init(&aux_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (CG2) tmem_alloc_pair<Cfg::kTmemCols>(&tmem_base_smem);
-    else tmem_alloc<Cfg::kTmemCols>(&tmem_base_smem);
-  }
-  tc_fence_before();
-  if (CG2) cluster_sync();      // the peer's barriers are initialised before any remote arrive
+  if (CG2) cluster_sync();      // the peer's barriers are initialised before any multicast / arrive
   else __syncthreads();
-  tc_fence_after();
-  // everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the tail of
-  // the preceding kernel; its outputs are read only after this point
+  // everything above (barrier init, descriptor prefetch) overlapped the tail of the preceding
+  // kernel; its outputs are read only after this point
   pdl_entry();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  // 32-bit shared-window addresses, computed once: the issue loops below run on one warp each and
-  // are instruction-latency bound (every instruction saved per k-block is ~1% of a small-N layer)
   const uint32_t smem_a0 = smem_u32(smem);
   const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-  const uint32_t stage_wrap = static_cast<uint32_t>(kStages) * Cfg::kStageBytes;
   // chunks of the last k-block (a partial stage exists only when a filter tap is narrower than
   // a stage, i.e. Cin < 64 with an odd tap count)
   const int tail_chunks = kChunks == 1 ? 1 : ((p.Ktot - (num_kb - 1) * kStageK + CW - 1) / CW);
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
-    // The whole warp stays converged (so the uniform-datapath TMA/MMA instructions need no
-    // election loops) and every lane tracks the same loop state; one elected lane issues.
-    uint32_t soff = 0, sbar = 0, phase = 0;             // stage byte offset / barrier offset
-    const uint32_t b_bytes = Cfg::kBRows * (p.b_sw_bytes < 128 ? p.b_sw_bytes : 128);
-    // CG2: both CTAs' loads complete on the LEADER's full barrier (cluster address of rank 0)
-    const uint32_t full_bytes = (CG2 ? 2 : 1) * NP * (MT * kChunks * kChunkBytes + b_bytes);
-    const uint32_t tail_bytes = (CG2 ? 2 : 1) * NP * (MT * tail_chunks * kChunkBytes + b_bytes);
-    const uint32_t full0_lead = CG2 ? mapa_shared(full0, 0) : full0;
-    const int nb0 = n0 + (CG2 ? static_cast<int>(cta_rank) * Cfg::kBRows : 0);
+    // The whole warp stays converged and every lane tracks the same loop state; one elected lane
+    // issues.
+    uint32_t stage = 0, phase = 0;
+    const uint32_t b_bytes = BN * (p.b_sw_bytes < 128 ? p.b_sw_bytes : 128);
+    const uint32_t full_bytes = NP * (kChunks * kChunkBytes + b_bytes);
+    const uint32_t tail_bytes = NP * (tail_chunks * kChunkBytes + b_bytes);
     const int Cin = p.Cin, fkw = p.kw;
     for (int it = 0; it < my_tiles; ++it) {
       const int m0 = (m_first + it * m_step) * kTileM + m_rank_off;
-      int img[MT], h0[MT], w0[MT];
-#pragma unroll
-      for (int h = 0; h < MT; ++h) {
-        img[h] = h0[h] = w0[h] = 0;
-        if (IM2COL) {
-          const int mh = m0 + h * kBM;
-          img[h] = mh / p.HoWo;
-          const int rem = mh - img[h] * p.HoWo;
-          const int po = rem / p.Wo;
-          const int qo = rem - po * p.Wo;
-          h0[h] = po * p.stride - p.pad_h_lo;
-          w0[h] = qo * p.stride - p.pad_w_lo;
-        }
+      int img = 0, h0 = 0, w0 = 0;
+      if (IM2COL) {
+        img = m0 / p.HoWo;
+        const int rem = m0 - img * p.HoWo;
+        const int po = rem / p.Wo;
+        const int qo = rem - po * p.Wo;
+        h0 = po * p.stride - p.pad_h_lo;
+        w0 = qo * p.stride - p.pad_w_lo;
       }
       // filter tap (tr, ts) and channel offset tc of the next chunk, advanced incrementally
       int tr = 0, ts = 0, tc = 0, k0 = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         const bool last = kb == num_kb - 1;
         const int nch = (kChunks > 1 && last) ? tail_chunks : kChunks;
-        mbar_wait_a(empty0 + sbar, phase ^ 1);
+        mbar_wait_a(empty0 + stage * 8, phase ^ 1);
         const bool leader = elect_one();
-        const uint32_t fb = CG2 ? full0_lead + sbar : full0 + sbar;
-        const uint32_t sa = smem_a0 + soff;
+        const uint32_t fb = full0 + stage * 8;
+        const uint32_t sa = smem_a0 + stage * Cfg::kStageBytes;
         if (leader) {
-          if (!CG2 || cta_rank == 0)
-            mbar_expect_tx_a(full0 + sbar, (kChunks > 1 && last) ? tail_bytes : full_bytes);
-          if (CG2) {
-            tma_load_2d_pair(sa + Cfg::kABytes, &tmB, fb, k0, nb0);
+          mbar_expect_tx_a(fb, (kChunks > 1 && last) ? tail_bytes : full_bytes);
+          if (CG2) {      // this CTA's half of the weight rows, into both CTAs of the pair
+            const int half = BN / 2;
+            tma_load_2d_multicast(sa + NP * Cfg::kABytes + cta_rank * half * (b_bytes / BN), &tmB,
+                                  fb, k0, n0 + static_cast<int>(cta_rank) * half, (uint16_t)3);
           } else {
 #pragma unroll
             for (int pl = 0; pl < NP; ++pl)
@@ -561,22 +348,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
               for (int pl = 0; pl < NP; ++pl) {
                 const CUtensorMap* mA = pl == 0 ? &tmA : (pl == 1 ? &tmA1 : &tmA2);
-#pragma unroll
-                for (int h = 0; h < MT; ++h) {
-                  const uint32_t dst =
-                      sa + pl * Cfg::kABytes + h * Cfg::kAHalfBytes + j * kChunkBytes;
-                  if (IM2COL) {
-                    if (CG2)
-                      tma_load_im2col_4d_pair(dst, mA, fb, tc, w0[h], h0[h], img[h], (uint16_t)ts,
-                                              (uint16_t)tr);
-                    else
-                      tma_load_im2col_4d_a(dst, mA, fb, tc, w0[h], h0[h], img[h], (uint16_t)ts,
-                                           (uint16_t)tr);
-                  } else {
-                    if (CG2) tma_load_2d_pair(dst, mA, fb, k0 + j * CW, m0 + h * kBM);
-                    else tma_load_2d_a(dst, mA, fb, k0 + j * CW, m0 + h * kBM);
-                  }
-                }
+                const uint32_t dst = sa + pl * Cfg::kABytes + j * kChunkBytes;
+                if (IM2COL)
+                  tma_load_im2col_4d_a(dst, mA, fb, tc, w0, h0, img, (uint16_t)ts, (uint16_t)tr);
+                else
+                  tma_load_2d_a(dst, mA, fb, k0 + j * CW, m0);
               }
             }
             tc += CW;
@@ -588,119 +364,43 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         __syncwarp();
         k0 += kStageK;
-        soff += Cfg::kStageBytes;
-        sbar += 8;
-        if (soff == stage_wrap) { soff = 0; sbar = 0; phase ^= 1; }
+        if (++stage == static_cast<uint32_t>(kStages)) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    uint32_t soff16 = 0, sbar = 0, phase = 0;            // stage offset in descriptor units (16 B)
-    const uint32_t stage_wrap16 = stage_wrap >> 4;
-    const uint32_t tfull0 = smem_u32(tfull_bar), tempty0 = smem_u32(tempty_bar);
-    // descriptors of stage 0 / chunk 0; everything else is an add on the 14-bit address field
-    const uint64_t a_desc0 = make_smem_desc(smem_a0, 16, 8 * CW * 2, swizzle_layout_type(CW * 2));
-    const uint64_t b_desc0 = make_smem_desc(smem_a0 + NP * Cfg::kABytes, 16, 8 * p.b_sw_bytes,
-                                            swizzle_layout_type(p.b_sw_bytes));
-    // CG2: only the leader CTA of the pair issues MMAs (they span both CTAs' operands and TMEM)
-    for (int it = 0; it < ((!CG2 || cta_rank == 0) ? my_tiles : 0); ++it) {
-      const uint32_t acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait_a(tempty0 + acc * 8, acc_phase ^ 1);   // epilogue(s) have drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * Cfg::kAccCols;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const bool last = kb == num_kb - 1;
-        const int nch = (kChunks > 1 && last) ? tail_chunks : kChunks;
-        mbar_wait_a(full0 + sbar, phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t da0 = a_desc0 + soff16;
-          const uint64_t db0 = b_desc0 + soff16;
-#pragma unroll
-          for (int j = 0; j < kChunks; ++j) {
-            if (j < nch) {
-#pragma unroll
-              for (int h = 0; h < MT; ++h) {
-#pragma unroll
-                for (int ks = 0; ks < kKSteps; ++ks) {
-                  // NP == 3: the six cross products of the (hi, mid, lo) planes that are
-                  // significant at fp32 precision, smallest first
-#pragma unroll
-                  for (int t = 0; t < (NP == 3 ? 6 : 1); ++t) {
-                    const int pa = NP == 3 ? plane_term_a(t) : 0;
-                    const int pb = NP == 3 ? plane_term_b(t) : 0;
-                    // NP == 3: t = 5 is hi*hi -> accumulator 0; t < 5 -> the small-term
-                    // accumulator at column offset BN (its first MMA of a tile is t = 0)
-                    const bool small = NP == 3 && t < 5;
-                    const uint32_t d_col = tmem_d + h * BN + (small ? BN : 0);
-                    const uint64_t da =
-                        da0 + ((pa * Cfg::kABytes + h * Cfg::kAHalfBytes + j * kChunkBytes + ks * 32) >> 4);
-                    const uint64_t db = db0 + ((pb * Cfg::kBBytes + (j * kKSteps + ks) * 32) >> 4);
-                    const uint32_t accum =
-                        (j | ks | (small ? t : 0)) ? 1u : static_cast<uint32_t>(kb != 0);
-                    if (CG2) umma_bf16_pair(d_col, da, db, kIdesc, accum);
-                    else umma_bf16(d_col, da, db, kIdesc, accum);
-                  }
-                }
-              }
-            }
-          }
-          if (CG2) {      // frees the stage / publishes the accumulator in BOTH CTAs
-            umma_commit_pair(empty0 + sbar);
-            if (last) umma_commit_pair(tfull0 + acc * 8);
-          } else {
-            umma_commit_a(empty0 + sbar);
-            if (last) umma_commit_a(tfull0 + acc * 8);
-          }
-        }
-        __syncwarp();
-        soff16 += Cfg::kStageBytes >> 4;
-        sbar += 8;
-        if (soff16 == stage_wrap16) { soff16 = 0; sbar = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (8 warps)
-    if constexpr (NP == 1 && !CG2) {
-      if (p.split_epi) {
-        conv_epilogue_split<BN, MT>(p, &tmC, &tmAdd, &tmMask, tmem_base, s_out0, s_add, s_mask,
-                                    tfull_bar, tempty_bar, aux_bars, n0, m_first, m_step, my_tiles);
-        goto epilogue_done;
-      }
-    }
-    {
-    const int quarter = warp & 3;                      // TMEM lane quarter this warp may read
-    const int egrp = (warp - 2) >> 2;                  // 0 / 1: even / odd 32-column chunks
-    const int r = quarter * 32 + lane;                 // row inside the tile == TMEM lane
-    const bool leader = (warp == 2 && lane == 0);
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------------ wgmma consumers
+    const int cg = (warp >> 2) - 1;                    // consumer warpgroup: rows cg*64 ..
+    const int ct = static_cast<int>(threadIdx.x) - 128;   // 0 .. 255
+    const bool leader = ct == 0;
     const bool stats = p.ch_part != nullptr;
     const bool has_aux = p.has_add || p.has_mask;
-    const int swz = (kRowBytes == 128) ? (r & 7) : ((r >> 1) & 3);
+    const int r0 = cg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0, r0 + 8
+    const int cq = (lane & 3) * 2;                              // fragment column offset
+    // descriptors of stage 0 / chunk 0 (K-major, 8-row groups SBO apart); this group's 64 rows
+    // start 64 rows into every A chunk
+    const uint64_t a_desc0 = make_smem_desc(smem_a0 + cg * 64 * CW * 2, 16, 8 * CW * 2,
+                                            swizzle_layout_type(CW * 2));
+    const uint64_t b_desc0 = make_smem_desc(smem_a0 + NP * Cfg::kABytes, 16, 8 * p.b_sw_bytes,
+                                            swizzle_layout_type(p.b_sw_bytes));
+    float acc[BN / 2];
+    float acc2[NP == 3 ? BN / 2 : 1];
     // batch-norm statistics: thread t owns the 8 columns of 16-byte chunk `st_chunk` (of every
-    // column half) over the rows st_rg, st_rg + kNRg, ... of every tile, read back from the
-    // staged bf16 tile
+    // column half) over the rows st_rg, st_rg + kNRg, ... of every tile, read back from the staged
+    // bf16 tile
     constexpr int kNChunk = kHalfN / 8;
-    constexpr int kStatThreads = (BN == 32) ? 128 : kEpiThreads;
+    constexpr int kStatThreads = (BN == 32) ? 128 : kConsumerThreads;
     constexpr int kNRg = kStatThreads / kNChunk;       // row groups; kBM / kNRg rows per thread
-    const int st_t = threadIdx.x - 64;
-    const bool st_on = st_t < kStatThreads;
-    const int st_chunk = st_t % kNChunk, st_rg = st_t / kNChunk;
+    const bool st_on = ct < kStatThreads;
+    const int st_chunk = ct % kNChunk, st_rg = ct / kNChunk;
     float acc_s[kNHalf][8], acc_q[kNHalf][8];
 #pragma unroll
     for (int hf = 0; hf < kNHalf; ++hf)
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc_s[hf][e] = acc_q[hf][e] = 0.f;
     uint32_t aux_n = 0;                                // completed aux-barrier phases
-    // output staging: with two buffers the TMA store of a half tile keeps draining (its shared-
-    // memory reads are paced by the memory system accepting the writes) under the next half's TMEM
-    // reads instead of stalling all 8 warps -- what bounded the store-heavy small-K tiles
-    const bool two_out = p.out_bufs == 2;
-    uint32_t ebuf = 0;
     // add / mask half tiles are fetched ONE HALF AHEAD: the loads of the next half are issued as
-    // soon as every thread has consumed the current one (they then overlap this half's TMA store,
-    // the statistics pass and the next half's TMEM reads instead of stalling all 8 warps for an
-    // L2 / HBM round trip per half -- what bounded the small-K dgrad layers)
+    // soon as every thread has consumed the current one (they overlap this half's TMA store, the
+    // statistics pass and the next tile's k-loop)
     auto issue_aux = [&](int am0, int anh) {
       mbar_expect_tx(&aux_bar, (p.has_add ? Cfg::kTileBytes : 0) +
                                    (p.has_mask ? Cfg::kTileBytes : 0));
@@ -713,128 +413,124 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     };
     if (leader && has_aux && my_tiles > 0) issue_aux(m_first * kTileM + m_rank_off, n0);
+    // a stage is released to this CTA's producer and (CG2) to the peer's, whose multicast fills it too
+    const uint32_t empty_peer = CG2 ? mapa_shared(empty0, cta_rank ^ 1u) : 0u;
+    auto release = [&](int st) {
+      if (CG2) {
+        mbar_arrive_cluster(mapa_shared(empty0, cta_rank) + st * 8);
+        mbar_arrive_cluster(empty_peer + st * 8);
+      } else {
+        mbar_arrive(&empty_bar[st]);
+      }
+    };
 
+    uint32_t stage = 0, phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
+      const int m0 = (m_first + it * m_step) * kTileM + m_rank_off;
+      // ---- k-loop: one k-block of wgmma in flight; the stage before it is released
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const bool last = kb == num_kb - 1;
+        const int nch = (kChunks > 1 && last) ? tail_chunks : kChunks;
+        mbar_wait_a(full0 + stage * 8, phase);
+        wgmma_fence_operand(acc);
+        if (NP == 3) wgmma_fence_operand(acc2);
+        wgmma_fence();
+        const uint64_t da0 = a_desc0 + ((stage * Cfg::kStageBytes) >> 4);
+        const uint64_t db0 = b_desc0 + ((stage * Cfg::kStageBytes) >> 4);
 #pragma unroll
-      for (int mh = 0; mh < MT; ++mh) {
-      const int m0 = (m_first + it * m_step) * kTileM + mh * kBM + m_rank_off;
-      const uint32_t acc_col = acc * Cfg::kAccCols + mh * BN;
-      const int row = m0 + r;
-      const bool row_ok = row < p.M;
+        for (int j = 0; j < kChunks; ++j) {
+          if (j < nch) {
+#pragma unroll
+            for (int ks = 0; ks < kKSteps; ++ks) {
+              // NP == 3: the six cross products of the (hi, mid, lo) planes that are significant
+              // at fp32 precision, smallest first; t = 5 is hi*hi -> acc, t < 5 -> acc2
+#pragma unroll
+              for (int t = 0; t < (NP == 3 ? 6 : 1); ++t) {
+                const int pa = NP == 3 ? plane_term_a(t) : 0;
+                const int pb = NP == 3 ? plane_term_b(t) : 0;
+                const bool small = NP == 3 && t < 5;
+                const uint64_t da = da0 + ((pa * Cfg::kABytes + j * kChunkBytes + ks * 32) >> 4);
+                const uint64_t db = db0 + ((pb * Cfg::kBBytes + (j * kKSteps + ks) * 32) >> 4);
+                const uint32_t accum = (j | ks | (small ? t : 0)) ? 1u : static_cast<uint32_t>(kb != 0);
+                if constexpr (NP == 3) {
+                  if (small) Wgmma<BN>::template mma<0, 0>(acc2, da, db, accum);
+                  else Wgmma<BN>::template mma<0, 0>(acc, da, db, accum);
+                } else {
+                  Wgmma<BN>::template mma<0, 0>(acc, da, db, accum);
+                }
+              }
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_fence_operand(acc);
+        if (NP == 3) wgmma_fence_operand(acc2);
+        wgmma_wait<1>();
+        __syncwarp();
+        if (prev >= 0 && lane == 0) release(prev);
+        prev = static_cast<int>(stage);
+        if (++stage == static_cast<uint32_t>(kStages)) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      if (NP == 3) {
+        wgmma_fence_operand(acc2);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += acc2[i];
+      }
+      __syncwarp();
+      if (lane == 0) release(prev);
+
+      // ---- epilogue, per column half: (+bias) (+add) (x mask) -> bf16 -> swizzled staging ->
+      // TMA store; statistics from the staged (rounded) tile
 #pragma unroll
       for (int hf = 0; hf < kNHalf; ++hf) {
         const int nh = n0 + hf * kHalfN;               // first output column of this half
-        uint8_t* s_out = s_out0 + ebuf * Cfg::kTileBytes;
-        if (leader && !p.out_f32) {
-          // the TMA store that last used this staging buffer must have finished READING it
-          if (two_out) tma_store_wait_read1();
-          else tma_store_wait_read();
-        }
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");   // staging buffers free for everyone
-        if (hf == 0 && mh == 0) {
-          mbar_wait(&tfull_bar[acc], acc_phase);
-          tc_fence_after();
-        }
+        // the TMA store that last used the staging buffer must have finished READING it
+        if (leader && !p.out_f32) tma_store_wait_read();
+        named_bar_sync(1, kConsumerThreads);
         if (has_aux) {
           mbar_wait(&aux_bar, aux_n & 1);
           ++aux_n;
         }
 #pragma unroll
-        for (int c2 = 0; c2 < (kHalfN / 32 + 1) / 2; ++c2) {
-          const int c = c2 * 2 + egrp;                   // this warp group's chunk
-          if (c >= kHalfN / 32) break;                   // warp-uniform
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc_col +
-                            hf * kHalfN + c * 32, v);
-          tmem_ld_wait();
-          float f[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-          if (NP == 3) {   // + the small-term accumulator
-            tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc_col + BN +
-                              hf * kHalfN + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) f[i] += __uint_as_float(v[i]);
-          }
-          const int col0 = nh + c * 32;
-          const int sub = (c * 32) / kSubW;
-          const int j0 = ((c * 32) % kSubW) / 8;
-          const int soff = sub * kSubBytes + r * kRowBytes;
+        for (int jj = 0; jj < kHalfN / 8; ++jj) {
+          const int j = hf * (kHalfN / 8) + jj;
+          const int c = jj * 8 + cq;                   // column inside the half
+          float b0 = 0.f, b1 = 0.f;
           if (p.bias) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) f[i] += __ldg(p.bias + col0 + i);
+            b0 = __ldg(p.bias + nh + c);
+            b1 = __ldg(p.bias + nh + c + 1);
           }
-          if (p.has_add) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint4 u =
-                  *reinterpret_cast<const uint4*>(s_add + soff + (((j0 + q) ^ swz) << 4));
-              const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                bf16x2_add(f[q * 8 + e * 2 + 0], f[q * 8 + e * 2 + 1], w4[e]);
-            }
-          }
-          // ReLU mask of the destination tensor: 0xffff per bf16 half that is > 0, applied to the
-          // packed bf16 output below (zeroing the half == zeroing the fp32 value before rounding)
-          if (p.out_f32) {
-            if (p.has_mask) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint4 u =
-                    *reinterpret_cast<const uint4*>(s_mask + soff + (((j0 + q) ^ swz) << 4));
-                const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const uint32_t k2 = bf16x2_gt0_mask(w4[e]);
-                  if (!(k2 & 0xffffu)) f[q * 8 + e * 2 + 0] = 0.f;
-                  if (!(k2 >> 16)) f[q * 8 + e * 2 + 1] = 0.f;
-                }
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + h * 8;
+            float v0 = acc[j * 4 + h * 2] + b0, v1 = acc[j * 4 + h * 2 + 1] + b1;
+            const int off = staged_offset<kSubW>(r, c);
+            if (p.has_add) bf16x2_add(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
+            // ReLU mask of the destination tensor: 0xffff per bf16 half that is > 0, applied to the
+            // packed bf16 output (zeroing the half == zeroing the fp32 value before rounding)
+            if (p.out_f32) {
+              if (p.has_mask) {
+                const uint32_t k2 = bf16x2_gt0_mask(*reinterpret_cast<const uint32_t*>(s_mask + off));
+                if (!(k2 & 0xffffu)) v0 = 0.f;
+                if (!(k2 >> 16)) v1 = 0.f;
               }
+              if (m0 + r < p.M)
+                *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) +
+                                           static_cast<size_t>(m0 + r) * p.Cout + nh + c) =
+                    make_float2(v0, v1);
+            } else {
+              uint32_t pk = pack_bf16x2(v0, v1);
+              if (p.has_mask) pk &= bf16x2_gt0_mask(*reinterpret_cast<const uint32_t*>(s_mask + off));
+              *reinterpret_cast<uint32_t*>(s_out + off) = pk;
             }
-            if (row_ok) {
-              float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.y) +
-                                                      static_cast<size_t>(row) * p.Cout + col0);
-#pragma unroll
-              for (int q = 0; q < 8; ++q)
-                dst[q] = make_float4(f[q * 4], f[q * 4 + 1], f[q * 4 + 2], f[q * 4 + 3]);
-            }
-          } else {
-            uint32_t pk[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) pk[i] = pack_bf16x2(f[2 * i], f[2 * i + 1]);
-            if (p.has_mask) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint4 u =
-                    *reinterpret_cast<const uint4*>(s_mask + soff + (((j0 + q) ^ swz) << 4));
-                pk[q * 4 + 0] &= bf16x2_gt0_mask(u.x);
-                pk[q * 4 + 1] &= bf16x2_gt0_mask(u.y);
-                pk[q * 4 + 2] &= bf16x2_gt0_mask(u.z);
-                pk[q * 4 + 3] &= bf16x2_gt0_mask(u.w);
-              }
-            }
-            // stage in the TMA swizzle layout: 16-byte piece j of row r at piece j ^ swz
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              *reinterpret_cast<uint4*>(s_out + soff + (((j0 + q) ^ swz) << 4)) =
-                  make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
           }
         }
-        // half drained and staged: (after the last half) hand TMEM back, then store
-        if (hf == kNHalf - 1 && mh == MT - 1) tc_fence_before();
         if (!p.out_f32) fence_proxy_async();             // generic smem writes -> async proxy
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
+        named_bar_sync(1, kConsumerThreads);
         if (leader) {
-          if (hf == kNHalf - 1 && mh == MT - 1) {
-            if (CG2 && cta_rank != 0)     // the leader's MMA warp waits for both CTAs' epilogues
-              mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[acc]), 0));
-            else
-              mbar_arrive(&tempty_bar[acc]);
-          }
           if (!p.out_f32) {
 #pragma unroll
             for (int sub = 0; sub < kNSub; ++sub)
@@ -845,14 +541,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             // the staging tiles were consumed by everyone before the barrier above: fetch the next
             // half's (same rows / next column half, else the next M tile of this CTA)
             if (hf + 1 < kNHalf) issue_aux(m0, nh + kHalfN);
-            else if (mh + 1 < MT) issue_aux(m0 + kBM, n0);
-            else if (it + 1 < my_tiles)
-              issue_aux((m_first + (it + 1) * m_step) * kTileM + m_rank_off, n0);
+            else if (it + 1 < my_tiles) issue_aux((m_first + (it + 1) * m_step) * kTileM + m_rank_off, n0);
           }
         }
         if (stats && st_on) {
           // column sums of the half tile as stored (bf16-rounded); rows past M were computed
           // from zero-filled operands and contribute zero.  Overlaps the TMA store (both read).
+          constexpr int kRowBytes = kSubW * 2;
           const int sub = st_chunk / (kSubW / 8), jj = st_chunk % (kSubW / 8);
 #pragma unroll 4
           for (int i = 0; i < kBM / kNRg; ++i) {
@@ -867,17 +562,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                             acc_q[hf][2 * e + 1], w4[e]);
           }
         }
-        if (two_out) ebuf ^= 1;
       }
-      }   // mh
     }
     if (leader && !p.out_f32) tma_store_wait_all();
     if (stats && my_tiles > 0) {
       // final cross-row-group reduction in the (now idle) output staging buffer
-      float* red_sum = reinterpret_cast<float*>(s_out0);
+      float* red_sum = reinterpret_cast<float*>(s_out);
       float* red_sq = red_sum + kNRg * BN;
       static_assert(2 * kNRg * BN * 4 <= Cfg::kTileBytes, "staging buffer too small for stats");
-      asm volatile("bar.sync 1, 256;\n" ::: "memory");   // the last TMA store has drained
+      named_bar_sync(1, kConsumerThreads);             // the last TMA store has drained
       if (st_on) {
 #pragma unroll
         for (int hf = 0; hf < kNHalf; ++hf)
@@ -887,8 +580,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             red_sq[st_rg * BN + hf * kHalfN + st_chunk * 8 + e] = acc_q[hf][e];
           }
       }
-      asm volatile("bar.sync 1, 256;\n" ::: "memory");
-      for (int col = st_t; col < BN; col += kEpiThreads) {
+      named_bar_sync(1, kConsumerThreads);
+      for (int col = ct; col < BN; col += kConsumerThreads) {
         float ss = 0.f, qq = 0.f;
         for (int g2 = 0; g2 < kNRg; ++g2) {
           ss += red_sum[g2 * BN + col];
@@ -903,37 +596,25 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         row[p.Cout + n0 + col] = qq;
       }
     }
-    }
-  epilogue_done:;
   }
-  __syncwarp();
-  tc_fence_before();
-  if (CG2) cluster_sync();      // neither CTA may leave (or free TMEM) while the pair is in flight
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG2) tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
-    else tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
+  // CG2: neither CTA leaves while the peer may still multicast into it or arrive on its barriers
+  if (CG2) cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------
 // 3x3 / stride 1 / pad 1 convolution WITHOUT im2col copies ("halo" kernel).
 //
-// The im2col kernel above fetches every input pixel nine times (once per filter tap) from L2 into
-// shared memory; for small-N layers (N <= 128: the stem, the 56x56 SK convs and their dgrads) that
-// ingest -- not the tensor pipe, not HBM -- is the bound (147 KB of A per 128 x 64-channel tile).
-// Here a CTA tile is a 16 x 8 PATCH of output pixels of one image, and ONE 18 x 10 pixel halo tile
-// per 64-channel chunk is loaded by a 4-D tiled TMA box at (h0-1, w0-1) (out-of-image pixels are
+// The im2col kernel fetches every input pixel nine times (once per filter tap) from L2 into shared
+// memory.  Here a CTA tile is a 16 x 8 PATCH of output pixels of one image, and ONE 18 x 10 pixel halo
+// tile per channel chunk is loaded by a 4-D tiled TMA box at (h0-1, w0-1) (out-of-image pixels are
 // zero-filled: the padding).  The A operand of filter tap (r, s) is the same shared-memory tile read
-// through a descriptor that starts (r*10 + s) pixel rows further on, with 10 pixel rows between 8-row
-// groups (group g = output row h0+g, 8 pixels): the tensor core's swizzle is a function of the
-// absolute shared-memory address, like TMA's, so any row may start a descriptor and the group stride
-// need not be a multiple of the swizzle atom (probed on the B200: tools/microtests/halo_desc.cu,
-// profiles/r02_microtest_halo_desc.txt).  23 KB of A per tile and chunk instead of 147 KB.
+// through a wgmma descriptor that starts (r*10 + s) pixel rows further on, with 10 pixel rows between
+// 8-row groups (group g = output row h0+g, 8 pixels): the swizzle is a function of the absolute
+// shared-memory address (as for TMA), so any row may start a descriptor and the group stride need
+// not be a multiple of the swizzle atom.  Consumer warpgroup g covers output rows 8g .. 8g+7.
 // Weight tiles [BN x CW] per (tap, chunk) stream through their own ring; when the whole N-tile slab
-// fits the ring it is loaded once and stays (weights-stationary: the stem layers).
-// Epilogue = the im2col kernel's (mask / add one half ahead, bf16 staging, TMA store, statistics),
+// fits the ring it is loaded once and stays (weights-stationary).
+// Epilogue = the im2col kernel's (add / mask one tile ahead, bf16 staging, TMA store, statistics),
 // with 4-D boxes for the patch and the out-of-image rows excluded from the statistics.
 // ------------------------------------------------------------------------------------------
 constexpr int kHaloH = 18, kHaloW = 10, kPatchH = 16, kPatchW = 8;
@@ -945,8 +626,6 @@ struct HaloParams {
   int n_tiles, ph, pw;    // N tiles; patches per image
   int m_tiles;            // B * ph * pw
   int a_stages, b_slots, stationary;
-  int out_bufs;           // 1 or 2 output staging tiles (2: the TMA store of tile i overlaps tile i+1)
-  int split_epi;          // N <= 64: two independent 4-warp epilogue groups alternate tiles
   float* ch_part;
   int has_add, has_mask;
 };
@@ -959,12 +638,10 @@ struct HaloCfg {
   static constexpr int kBTile = BN * kRowB;
   static constexpr int kSubW = BN < 64 ? BN : 64;
   static constexpr int kTileBytes = kBM * BN * 2;
-  static constexpr int kTmemCols = 2 * BN < 32 ? 32 : 2 * BN;
   static_assert(BN <= 128 && kBTile % 512 == 0, "halo kernel: N tile <= 128");
 };
 
-// Patch coordinates of the tiles first, first + step, ... advanced without divisions (three integer
-// divisions per tile sat on the epilogue's critical path).
+// Patch coordinates of the tiles first, first + step, ... advanced without divisions.
 struct PatchIter {
   int img, row, col;          // image, patch row / column inside the image
   int d_img, d_row, d_col;
@@ -990,34 +667,29 @@ struct PatchIter {
 };
 
 template <int BN, int CW>
-__global__ void __launch_bounds__(kConvThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAdd,
                  const __grid_constant__ CUtensorMap tmMask, const HaloParams p) {
   using Cfg = HaloCfg<BN, CW>;
   constexpr int kRowB = Cfg::kRowB;
   constexpr int kKSteps = CW / 16;
-  constexpr uint32_t kIdesc = make_idesc_bf16_m(128, BN, false, false);
   constexpr uint32_t kLayout = swizzle_layout_type(kRowB);
   constexpr int kSubW = Cfg::kSubW;
-  constexpr int kSubRowB = kSubW * 2;
-  constexpr int kSubBytes = kBM * kSubRowB;
+  constexpr int kSubBytes = kBM * kSubW * 2;
   constexpr int kNSub = BN / kSubW;
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t a_full[4], a_empty[4];
   __shared__ uint64_t b_full[kHaloMaxB], b_empty[kHaloMaxB];
-  __shared__ uint64_t tfull_bar[2], tempty_bar[2];
-  __shared__ uint64_t aux_bars[2];
-  __shared__ uint32_t tmem_base_smem;
-  uint64_t& aux_bar = aux_bars[0];
+  __shared__ uint64_t aux_bar;
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   const int AS = p.a_stages, NB = p.b_slots;
-  uint8_t* s_out0 = smem + AS * Cfg::kAStage + NB * Cfg::kBTile;
-  uint8_t* s_add = s_out0 + p.out_bufs * Cfg::kTileBytes;
-  uint8_t* s_mask = s_add + (p.has_add ? (p.split_epi ? 2 : 1) * Cfg::kTileBytes : 0);
+  uint8_t* s_out = smem + AS * Cfg::kAStage + NB * Cfg::kBTile;
+  uint8_t* s_add = s_out + Cfg::kTileBytes;
+  uint8_t* s_mask = s_add + (p.has_add ? Cfg::kTileBytes : 0);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -1037,33 +709,23 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (p.has_mask) tma_prefetch_desc(&tmMask);
     for (int s = 0; s < AS; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], kConsumerWarps);
     }
     for (int s = 0; s < NB; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
+      mbar_init(&b_empty[s], kConsumerWarps);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 1);
-    }
-    mbar_init(&aux_bars[0], 1);
-    mbar_init(&aux_bars[1], 1);
+    mbar_init(&aux_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(&tmem_base_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_entry();
-  const uint32_t tmem_base = tmem_base_smem;
   const uint32_t a_base = smem_u32(smem), b_base = a_base + AS * Cfg::kAStage;
-  const uint32_t afull0 = smem_u32(a_full), aempty0 = smem_u32(a_empty);
-  const uint32_t bfull0 = smem_u32(b_full), bempty0 = smem_u32(b_empty);
+  const uint32_t afull0 = smem_u32(a_full), bfull0 = smem_u32(b_full);
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
-    // ring positions / phases advance incrementally (no runtime division in the issue loops)
+    const uint32_t aempty0 = smem_u32(a_empty), bempty0 = smem_u32(b_empty);
     uint32_t sa = 0, a_ph = 0, sb = 0, b_ph = 0;
     if (p.stationary && my_tiles > 0) {
       // the whole weight slab of this N tile: loaded once, ONE barrier, stays for the CTA's lifetime
@@ -1103,306 +765,175 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t tfull0 = smem_u32(tfull_bar), tempty0 = smem_u32(tempty_bar);
-    uint32_t sa = 0, a_ph = 0, sb = 0, b_ph = 0;
-    // descriptors are built once; every tap / k-step / ring slot is an add on the address field
-    const uint64_t a_desc0 = make_smem_desc(a_base, 16, kHaloW * kRowB, kLayout);
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------------ wgmma consumers
+    const int cg = (warp >> 2) - 1;                    // output rows 8cg .. 8cg+7 of the patch
+    const int ct = static_cast<int>(threadIdx.x) - 128;
+    const bool leader = ct == 0;
+    const bool stats = p.ch_part != nullptr;
+    const bool has_aux = p.has_add || p.has_mask;
+    const int r0 = cg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0, r0 + 8
+    const int cq = (lane & 3) * 2;
+    const uint64_t a_desc0 = make_smem_desc(a_base + cg * 8 * kHaloW * kRowB, 16, kHaloW * kRowB, kLayout);
     const uint64_t b_desc0 = make_smem_desc(b_base, 16, 8 * kRowB, kLayout);
-    if (p.stationary && my_tiles > 0) {
-      mbar_wait_a(bfull0, 0);
-      tc_fence_after();
-    }
+    float acc[BN / 2];
+    constexpr int kNChunk = BN / 8;
+    constexpr int kStatThreads = (BN == 32) ? 128 : kConsumerThreads;
+    constexpr int kNRg = kStatThreads / kNChunk;
+    const bool st_on = ct < kStatThreads;
+    const int st_chunk = ct % kNChunk, st_rg = ct / kNChunk;
+    float acc_s[8], acc_q[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc_s[e] = acc_q[e] = 0.f;
+    uint32_t aux_n = 0;
+    auto issue_aux = [&](int img, int h0, int w0) {
+      mbar_expect_tx(&aux_bar, (p.has_add ? Cfg::kTileBytes : 0) + (p.has_mask ? Cfg::kTileBytes : 0));
+#pragma unroll
+      for (int sub = 0; sub < kNSub; ++sub) {
+        if (p.has_add)
+          tma_load_4d_tile_a(smem_u32(s_add + sub * kSubBytes), &tmAdd, smem_u32(&aux_bar),
+                             n0 + sub * kSubW, w0, h0, img);
+        if (p.has_mask)
+          tma_load_4d_tile_a(smem_u32(s_mask + sub * kSubBytes), &tmMask, smem_u32(&aux_bar),
+                             n0 + sub * kSubW, w0, h0, img);
+      }
+    };
+    // resources read by the most recent committed wgmma group, released once it has completed
+    int pend_a = -1, pend_b = -1;
+    auto release_pending = [&]() {
+      __syncwarp();
+      if (lane == 0) {
+        if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+        if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
+      }
+      pend_a = pend_b = -1;
+    };
+    PatchIter pi(m_first, m_step, p.ph, p.pw);
+    if (leader && has_aux && my_tiles > 0) issue_aux(pi.img, pi.row * kPatchH, pi.col * kPatchW);
+    if (p.stationary && my_tiles > 0) mbar_wait_a(bfull0, 0);
+    uint32_t sa = 0, a_ph = 0, sb = 0, b_ph = 0;
     for (int it = 0; it < my_tiles; ++it) {
-      const uint32_t acc = it & 1;
-      mbar_wait_a(tempty0 + acc * 8, ((it >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * BN;
+      const int img = pi.img, h0 = pi.row * kPatchH, w0 = pi.col * kPatchW;
+      pi.next();
       for (int kc = 0; kc < nchunks; ++kc) {
         mbar_wait_a(afull0 + sa * 8, a_ph);
-        tc_fence_after();
         const uint64_t a_st = a_desc0 + ((sa * Cfg::kAStage) >> 4);
         if (p.stationary) {
-          if (elect_one()) {
-            const uint64_t b_st = b_desc0 + ((static_cast<uint32_t>(kc) * 9 * Cfg::kBTile) >> 4);
+          wgmma_fence_operand(acc);
+          wgmma_fence();
+          const uint64_t b_st = b_desc0 + ((static_cast<uint32_t>(kc) * 9 * Cfg::kBTile) >> 4);
 #pragma unroll
-            for (int t = 0; t < 9; ++t) {
-              // tap (r, s): the halo tile read (r*10 + s) pixel rows further on; 8-row groups (one
-              // output row each) 10 pixel rows apart
+          for (int t = 0; t < 9; ++t)
 #pragma unroll
-              for (int ks = 0; ks < kKSteps; ++ks)
-                umma_bf16(tmem_d, a_st + ((((t / 3) * kHaloW + (t % 3)) * kRowB + ks * 32) >> 4),
-                          b_st + ((t * Cfg::kBTile + ks * 32) >> 4), kIdesc,
-                          (t | ks) ? 1u : static_cast<uint32_t>(kc != 0));
-            }
-            umma_commit_a(aempty0 + sa * 8);
-            if (kc == nchunks - 1) umma_commit_a(tfull0 + acc * 8);
-          }
-          __syncwarp();
+            for (int ks = 0; ks < kKSteps; ++ks)
+              Wgmma<BN>::template mma<0, 0>(
+                  acc, a_st + ((((t / 3) * kHaloW + (t % 3)) * kRowB + ks * 32) >> 4),
+                  b_st + ((t * Cfg::kBTile + ks * 32) >> 4), (t | ks) ? 1u : static_cast<uint32_t>(kc != 0));
+          wgmma_commit();
+          wgmma_fence_operand(acc);
+          wgmma_wait<1>();
+          release_pending();
+          pend_a = static_cast<int>(sa);
         } else {
 #pragma unroll 1
           for (int t = 0; t < 9; ++t) {
             mbar_wait_a(bfull0 + sb * 8, b_ph);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint64_t a_tap = a_st + ((((t / 3) * kHaloW + (t % 3)) * kRowB) >> 4);
-              const uint64_t b_tap = b_desc0 + ((sb * Cfg::kBTile) >> 4);
+            wgmma_fence_operand(acc);
+            wgmma_fence();
+            const uint64_t a_tap = a_st + ((((t / 3) * kHaloW + (t % 3)) * kRowB) >> 4);
+            const uint64_t b_tap = b_desc0 + ((sb * Cfg::kBTile) >> 4);
 #pragma unroll
-              for (int ks = 0; ks < kKSteps; ++ks)
-                umma_bf16(tmem_d, a_tap + ((ks * 32) >> 4), b_tap + ((ks * 32) >> 4), kIdesc,
-                          (kc | t | ks) ? 1u : 0u);
-              umma_commit_a(bempty0 + sb * 8);
-              if (t == 8) {
-                umma_commit_a(aempty0 + sa * 8);
-                if (kc == nchunks - 1) umma_commit_a(tfull0 + acc * 8);
-              }
-            }
-            __syncwarp();
+            for (int ks = 0; ks < kKSteps; ++ks)
+              Wgmma<BN>::template mma<0, 0>(acc, a_tap + ((ks * 32) >> 4), b_tap + ((ks * 32) >> 4),
+                                            (kc | t | ks) ? 1u : 0u);
+            wgmma_commit();
+            wgmma_fence_operand(acc);
+            wgmma_wait<1>();
+            release_pending();
+            pend_b = static_cast<int>(sb);
+            if (t == 8) pend_a = static_cast<int>(sa);
             if (++sb == static_cast<uint32_t>(NB)) { sb = 0; b_ph ^= 1; }
           }
         }
         if (++sa == static_cast<uint32_t>(AS)) { sa = 0; a_ph ^= 1; }
       }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (8 warps)
-    const int quarter = warp & 3;
-    const int egrp = (warp - 2) >> 2;
-    const int r = quarter * 32 + lane;                 // TMEM lane = patch pixel (r/8, r%8)
-    const bool stats = p.ch_part != nullptr;
-    const bool has_aux = p.has_add || p.has_mask;
-    const int swz = (kSubRowB == 128) ? (r & 7) : ((r >> 1) & 3);
-    constexpr int kNChunk = BN / 8;
-    float acc_s[8], acc_q[8];
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      release_pending();
+
+      // ---- epilogue: (+add) (x mask) -> bf16 -> swizzled staging -> 4-D TMA store; statistics
+      if (leader) tma_store_wait_read();
+      named_bar_sync(1, kConsumerThreads);
+      if (has_aux) {
+        mbar_wait(&aux_bar, aux_n & 1);
+        ++aux_n;
+      }
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc_s[e] = acc_q[e] = 0.f;
-    uint32_t aux_n = 0;
-    // one 32-column chunk of the accumulator: TMEM -> (+add) (x mask) -> bf16 -> swizzled staging
-    auto drain_chunk = [&](uint32_t taddr, int c, const uint8_t* sa_, const uint8_t* sm_,
-                           uint8_t* so_) {
-      uint32_t v[32];
-      tmem_ld_32x32(taddr, v);
-      tmem_ld_wait();
-      float f[32];
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = j * 8 + cq;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-      const int sub = (c * 32) / kSubW;
-      const int j0 = ((c * 32) % kSubW) / 8;
-      const int soff = sub * kSubBytes + r * kSubRowB;
-      if (p.has_add) {
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + h * 8;
+          float v0 = acc[j * 4 + h * 2], v1 = acc[j * 4 + h * 2 + 1];
+          const int off = staged_offset<kSubW>(r, c);
+          if (p.has_add) bf16x2_add(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
+          uint32_t pk = pack_bf16x2(v0, v1);
+          if (p.has_mask) pk &= bf16x2_gt0_mask(*reinterpret_cast<const uint32_t*>(s_mask + off));
+          *reinterpret_cast<uint32_t*>(s_out + off) = pk;
+        }
+      }
+      fence_proxy_async();
+      named_bar_sync(1, kConsumerThreads);
+      if (leader) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint4 u = *reinterpret_cast<const uint4*>(sa_ + soff + (((j0 + q) ^ swz) << 4));
+        for (int sub = 0; sub < kNSub; ++sub)
+          tma_store_4d(&tmC, s_out + sub * kSubBytes, n0 + sub * kSubW, w0, h0, img);
+        tma_store_commit();
+        if (has_aux && it + 1 < my_tiles) issue_aux(pi.img, pi.row * kPatchH, pi.col * kPatchW);
+      }
+      if (stats && st_on) {
+        // column sums of the tile as stored (bf16-rounded); patch pixels outside the image excluded
+        // (they were computed from real neighbours and are clipped by the store)
+        constexpr int kRowBytes = kSubW * 2;
+        const int sub = st_chunk / (kSubW / 8), jj = st_chunk % (kSubW / 8);
+#pragma unroll 4
+        for (int rr = st_rg; rr < kBM; rr += kNRg) {
+          if (h0 + (rr >> 3) >= p.H || w0 + (rr & 7) >= p.W) continue;
+          const int sw = (kRowBytes == 128) ? (rr & 7) : ((rr >> 1) & 3);
+          const uint4 u = *reinterpret_cast<const uint4*>(s_out + sub * kSubBytes + rr * kRowBytes +
+                                                          ((jj ^ sw) << 4));
           const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
           for (int e = 0; e < 4; ++e)
-            bf16x2_add(f[q * 8 + e * 2 + 0], f[q * 8 + e * 2 + 1], w4[e]);
-        }
-      }
-      uint32_t pk[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) pk[i] = pack_bf16x2(f[2 * i], f[2 * i + 1]);
-      if (p.has_mask) {        // ReLU mask of the destination tensor, applied to the packed halves
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint4 u = *reinterpret_cast<const uint4*>(sm_ + soff + (((j0 + q) ^ swz) << 4));
-          pk[q * 4 + 0] &= bf16x2_gt0_mask(u.x);
-          pk[q * 4 + 1] &= bf16x2_gt0_mask(u.y);
-          pk[q * 4 + 2] &= bf16x2_gt0_mask(u.z);
-          pk[q * 4 + 3] &= bf16x2_gt0_mask(u.w);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(so_ + soff + (((j0 + q) ^ swz) << 4)) =
-            make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
-    };
-    // column sums of the tile as stored (bf16-rounded): this thread's 16-byte chunk `chunk` over the
-    // rows rg, rg + nrg, ...; patch pixels outside the image excluded (they were computed from real
-    // neighbours and are clipped by the store)
-    auto stat_rows = [&](const uint8_t* so_, int chunk, int rg, int nrg, int h0, int w0) {
-      const int sub = chunk / (kSubW / 8), jj = chunk % (kSubW / 8);
-#pragma unroll 4
-      for (int rr = rg; rr < kBM; rr += nrg) {
-        if (h0 + (rr >> 3) >= p.H || w0 + (rr & 7) >= p.W) continue;
-        const int sw = (kSubRowB == 128) ? (rr & 7) : ((rr >> 1) & 3);
-        const uint4 u = *reinterpret_cast<const uint4*>(so_ + sub * kSubBytes + rr * kSubRowB +
-                                                        ((jj ^ sw) << 4));
-        const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          bf16x2_sum_sq(acc_s[2 * e], acc_q[2 * e], acc_s[2 * e + 1], acc_q[2 * e + 1], w4[e]);
-      }
-    };
-    auto issue_aux = [&](uint64_t* bar, uint8_t* sa_, uint8_t* sm_, int img, int h0, int w0) {
-      mbar_expect_tx(bar, (p.has_add ? Cfg::kTileBytes : 0) + (p.has_mask ? Cfg::kTileBytes : 0));
-#pragma unroll
-      for (int sub = 0; sub < kNSub; ++sub) {
-        if (p.has_add)
-          tma_load_4d_tile_a(smem_u32(sa_ + sub * kSubBytes), &tmAdd, smem_u32(bar),
-                             n0 + sub * kSubW, w0, h0, img);
-        if (p.has_mask)
-          tma_load_4d_tile_a(smem_u32(sm_ + sub * kSubBytes), &tmMask, smem_u32(bar),
-                             n0 + sub * kSubW, w0, h0, img);
-      }
-    };
-
-    if (BN <= 64 && p.split_epi) {
-      // ---- two independent 4-warp groups: group g drains accumulator g of the tiles g, g + 2, ...
-      // with its own staging / aux buffers, named barrier and TMA store queue, so the per-tile chain
-      // (barrier -> TMEM load -> convert -> stage -> barrier -> store -> statistics) of one tile
-      // overlaps the next tile's: the chain, not the tensor pipe, paced the N <= 64 tiles
-      const int gt = threadIdx.x - 64 - egrp * 128;      // thread index inside the group
-      const bool gleader = gt == 0;
-      uint8_t* so_ = s_out0 + egrp * Cfg::kTileBytes;
-      uint8_t* sa_ = s_add + egrp * Cfg::kTileBytes;
-      uint8_t* sm_ = s_mask + egrp * Cfg::kTileBytes;
-      uint64_t* abar = &aux_bars[egrp];
-      constexpr int kNRgS = 128 / kNChunk;               // row groups inside one epilogue group
-      const int st_chunk = gt % kNChunk, st_rg = gt / kNChunk;
-      PatchIter pi(m_first + egrp * m_step, 2 * m_step, p.ph, p.pw);
-      if (gleader && has_aux && egrp < my_tiles)
-        issue_aux(abar, sa_, sm_, pi.img, pi.row * kPatchH, pi.col * kPatchW);
-      for (int it = egrp; it < my_tiles; it += 2) {
-        const int img = pi.img, h0 = pi.row * kPatchH, w0 = pi.col * kPatchW;
-        pi.next();
-        if (gleader) tma_store_wait_read();              // this group's previous store has read so_
-        if (egrp == 0) asm volatile("bar.sync 1, 128;\n" ::: "memory");
-        else asm volatile("bar.sync 2, 128;\n" ::: "memory");
-        mbar_wait(&tfull_bar[egrp], (it >> 1) & 1);
-        tc_fence_after();
-        if (has_aux) {
-          mbar_wait(abar, aux_n & 1);
-          ++aux_n;
-        }
-#pragma unroll
-        for (int c = 0; c < BN / 32; ++c)
-          drain_chunk(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + egrp * BN + c * 32, c,
-                      sa_, sm_, so_);
-        tc_fence_before();
-        fence_proxy_async();
-        if (egrp == 0) asm volatile("bar.sync 1, 128;\n" ::: "memory");
-        else asm volatile("bar.sync 2, 128;\n" ::: "memory");
-        if (gleader) {
-          mbar_arrive(&tempty_bar[egrp]);
-#pragma unroll
-          for (int sub = 0; sub < kNSub; ++sub)
-            tma_store_4d(&tmC, so_ + sub * kSubBytes, n0 + sub * kSubW, w0, h0, img);
-          tma_store_commit();
-          if (has_aux && it + 2 < my_tiles)
-            issue_aux(abar, sa_, sm_, pi.img, pi.row * kPatchH, pi.col * kPatchW);
-        }
-        if (stats) stat_rows(so_, st_chunk, st_rg, kNRgS, h0, w0);
-      }
-      if (gleader) tma_store_wait_all();
-      if (stats && my_tiles > 0) {
-        // cross-group / cross-row-group reduction in the (now idle) staging buffers
-        float* red_sum = reinterpret_cast<float*>(s_out0);
-        float* red_sq = red_sum + 2 * kNRgS * BN;
-        static_assert(BN > 64 || 2 * 2 * kNRgS * BN * 4 <= 2 * Cfg::kTileBytes,
-                      "staging buffers too small for stats");
-        asm volatile("bar.sync 3, 256;\n" ::: "memory");  // both groups' stores have drained
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          red_sum[(egrp * kNRgS + st_rg) * BN + st_chunk * 8 + e] = acc_s[e];
-          red_sq[(egrp * kNRgS + st_rg) * BN + st_chunk * 8 + e] = acc_q[e];
-        }
-        asm volatile("bar.sync 3, 256;\n" ::: "memory");
-        for (int col = threadIdx.x - 64; col < BN; col += kEpiThreads) {
-          float ss = 0.f, qq = 0.f;
-          for (int g2 = 0; g2 < 2 * kNRgS; ++g2) {
-            ss += red_sum[g2 * BN + col];
-            qq += red_sq[g2 * BN + col];
-          }
-          float* row = p.ch_part + static_cast<size_t>(m_first) * 2 * p.Cout;
-          row[n0 + col] = ss;
-          row[p.Cout + n0 + col] = qq;
-        }
-      }
-    } else {
-      // ---- all 8 warps on one tile at a time (two warps per TMEM lane quarter, alternating chunks)
-      const bool leader = (warp == 2 && lane == 0);
-      constexpr int kStatThreads = (BN == 32) ? 128 : kEpiThreads;
-      constexpr int kNRg = kStatThreads / kNChunk;
-      const int st_t = threadIdx.x - 64;
-      const bool st_on = st_t < kStatThreads;
-      const int st_chunk = st_t % kNChunk, st_rg = st_t / kNChunk;
-      PatchIter pi(m_first, m_step, p.ph, p.pw);
-      if (leader && has_aux && my_tiles > 0)
-        issue_aux(&aux_bar, s_add, s_mask, pi.img, pi.row * kPatchH, pi.col * kPatchW);
-      for (int it = 0; it < my_tiles; ++it) {
-        const int acc = it & 1;
-        const int img = pi.img, h0 = pi.row * kPatchH, w0 = pi.col * kPatchW;
-        pi.next();
-        // staging buffer free again: with two buffers only the store issued two tiles ago must
-        // have finished reading (the previous tile's store drains under this tile's TMEM reads)
-        uint8_t* s_out = s_out0 + ((p.out_bufs == 2 && (it & 1)) ? Cfg::kTileBytes : 0);
-        if (leader) {
-          if (p.out_bufs == 2) tma_store_wait_read1();
-          else tma_store_wait_read();
-        }
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
-        mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-        tc_fence_after();
-        if (has_aux) {
-          mbar_wait(&aux_bar, aux_n & 1);
-          ++aux_n;
-        }
-#pragma unroll
-        for (int c2 = 0; c2 < (BN / 32 + 1) / 2; ++c2) {
-          const int c = c2 * 2 + egrp;
-          if (c >= BN / 32) break;                       // warp-uniform
-          drain_chunk(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + c * 32, c,
-                      s_add, s_mask, s_out);
-        }
-        tc_fence_before();
-        fence_proxy_async();
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
-        if (leader) {
-          mbar_arrive(&tempty_bar[acc]);
-#pragma unroll
-          for (int sub = 0; sub < kNSub; ++sub)
-            tma_store_4d(&tmC, s_out + sub * kSubBytes, n0 + sub * kSubW, w0, h0, img);
-          tma_store_commit();
-          if (has_aux && it + 1 < my_tiles)
-            issue_aux(&aux_bar, s_add, s_mask, pi.img, pi.row * kPatchH, pi.col * kPatchW);
-        }
-        if (stats && st_on) stat_rows(s_out, st_chunk, st_rg, kNRg, h0, w0);
-      }
-      if (leader) tma_store_wait_all();
-      if (stats && my_tiles > 0) {
-        float* red_sum = reinterpret_cast<float*>(s_out0);
-        float* red_sq = red_sum + kNRg * BN;
-        static_assert(2 * kNRg * BN * 4 <= Cfg::kTileBytes, "staging buffer too small for stats");
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
-        if (st_on) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            red_sum[st_rg * BN + st_chunk * 8 + e] = acc_s[e];
-            red_sq[st_rg * BN + st_chunk * 8 + e] = acc_q[e];
-          }
-        }
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
-        for (int col = st_t; col < BN; col += kEpiThreads) {
-          float ss = 0.f, qq = 0.f;
-          for (int g2 = 0; g2 < kNRg; ++g2) {
-            ss += red_sum[g2 * BN + col];
-            qq += red_sq[g2 * BN + col];
-          }
-          float* row = p.ch_part + static_cast<size_t>(m_first) * 2 * p.Cout;
-          row[n0 + col] = ss;
-          row[p.Cout + n0 + col] = qq;
+            bf16x2_sum_sq(acc_s[2 * e], acc_q[2 * e], acc_s[2 * e + 1], acc_q[2 * e + 1], w4[e]);
         }
       }
     }
-  }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+    if (leader) tma_store_wait_all();
+    if (stats && my_tiles > 0) {
+      float* red_sum = reinterpret_cast<float*>(s_out);
+      float* red_sq = red_sum + kNRg * BN;
+      static_assert(2 * kNRg * BN * 4 <= Cfg::kTileBytes, "staging buffer too small for stats");
+      named_bar_sync(1, kConsumerThreads);
+      if (st_on) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          red_sum[st_rg * BN + st_chunk * 8 + e] = acc_s[e];
+          red_sq[st_rg * BN + st_chunk * 8 + e] = acc_q[e];
+        }
+      }
+      named_bar_sync(1, kConsumerThreads);
+      for (int col = ct; col < BN; col += kConsumerThreads) {
+        float ss = 0.f, qq = 0.f;
+        for (int g2 = 0; g2 < kNRg; ++g2) {
+          ss += red_sum[g2 * BN + col];
+          qq += red_sq[g2 * BN + col];
+        }
+        float* row = p.ch_part + static_cast<size_t>(m_first) * 2 * p.Cout;
+        row[n0 + col] = ss;
+        row[p.Cout + n0 + col] = qq;
+      }
+    }
   }
 }
 
@@ -1420,62 +951,53 @@ struct WgradParams {
   int pix;               // pixels per stage (64 or 128)
   int stages_total;      // ceil(P / pix)
   int stages_per_split;
+  int splits;            // CTAs along the pixel range (gridDim.z)
   float* dw;
+  float* part;           // splits > 1: [splits][tiles][128 x BN] fp32 partial tiles
+  unsigned* counters;    // splits > 1: arrivals per tile (zeroed before the launch)
 };
 
-constexpr int kWgPix = 64;   // default pixels per pipeline stage (4 UMMA K-steps); PIX = 128: 8 steps
+constexpr int kWgPix = 64;   // default pixels per pipeline stage (4 wgmma K-steps); PIX = 128: 8 steps
 
-// MT = 128-row blocks of (tap,ci) per CTA (1 or 2): with MT = 2 two accumulators share every dy
-// stage, i.e. twice the tensor work per pipeline round-trip and half the dy traffic per FLOP.
-// PIX = pixels (GEMM K) per pipeline stage: 64, or 128 (twice the MMAs per TMA / barrier round trip
-// of the single-warp issue loops, which bound the small-N layers)
-template <int BN, int MT, int NP = 1, int PIX = kWgPix>
+// PIX = pixels (GEMM K) per pipeline stage: 64, or 128 (twice the MMAs per TMA / barrier round trip)
+template <int BN, int NP = 1, int PIX = kWgPix>
 struct WgradCfg {
-  static constexpr int kAHalfBytes = PIX * 128 * 2;   // PIX pixels x 128 (tap,ci) columns
-  static constexpr int kABytes = MT * kAHalfBytes;       // one plane
+  static constexpr int kABytes = PIX * 128 * 2;   // PIX pixels x 128 (tap,ci) columns, one plane
   static constexpr int kBBytes = PIX * BN * 2;    // PIX pixels x BN output channels, one plane
   static constexpr int kStageBytes = NP * (kABytes + kBBytes);
   static constexpr int kStagesFit = (kSmemBudget - 1024) / kStageBytes;
   static constexpr int kStages =
       PIX != kWgPix ? (kStagesFit > 4 ? 4 : kStagesFit)
       : NP == 3 ? (kStagesFit > 3 ? 3 : kStagesFit)
-              : (MT == 1 ? ((BN >= 256) ? 4 : ((BN == 128) ? 3 : 4))
-                         : (kStagesFit > 5 ? 5 : kStagesFit));
+              : ((BN >= 256) ? 4 : ((BN == 128) ? 3 : 4));
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024;
-  // NP == 3: a second accumulator (columns BN..2BN) for the small cross terms, see FpropCfg
-  static constexpr int kAccCols = (NP == 3 ? 2 : MT) * BN;
-  static constexpr int kTmemCols = kAccCols < 32 ? 32 : kAccCols;
-  static_assert(kAccCols <= 512 && (NP == 1 || MT == 1) && kStages >= (NP == 3 ? 2 : 3),
-                "wgrad tile does not fit");
+  static_assert((NP == 1 || BN <= 128) && kStages >= (NP == 3 ? 2 : 3), "wgrad tile does not fit");
 };
 
 // CW: channel width of one im2col chunk of x (16/32/64), CWB: channel width of one dy chunk.
-template <int BN, int CW, int CWB, bool IM2COL, int MT, int NP, int PIX>
+// Both operands are MN-major in shared memory (the pixel index is the GEMM K dimension): one pixel
+// row = width*2 bytes, 8-row groups SBO apart, column blocks (64/32/16 channels) LBO apart.
+template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX>
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmDY,
                   const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
                   const __grid_constant__ CUtensorMap tmDY1,
                   const __grid_constant__ CUtensorMap tmDY2, const WgradParams p) {
-  using Cfg = WgradCfg<BN, MT, NP, PIX>;
+  using Cfg = WgradCfg<BN, NP, PIX>;
   constexpr int kStages = Cfg::kStages;
-  constexpr int kAChunks = MT * 128 / CW;        // chunks of both 128-row blocks, consecutive
-  constexpr int kBChunks = BN / CWB;
+  constexpr int kAChunks = 128 / CW;
   constexpr int kAChunkBytes = PIX * CW * 2;
   constexpr int kBChunkBytes = PIX * CWB * 2;
-  constexpr uint32_t kIdesc = make_idesc_bf16(BN, true, true);
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[kStages];
   __shared__ uint64_t empty_bar[kStages];
-  __shared__ uint64_t tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * (MT * 128);   // first (tap,ci) column of dw handled here
-  const bool second = MT == 2 && m0 + 128 < p.Ktot;   // the second 128-row block exists
+  const int m0 = blockIdx.x * 128;          // first (tap,ci) column of dw handled here
   const int co0 = blockIdx.y * BN;
   const int ks_begin = blockIdx.z * p.stages_per_split;
   int ks_end = ks_begin + p.stages_per_split;
@@ -1485,26 +1007,21 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
   int a_chunks = 0;
 #pragma unroll
   for (int j = 0; j < kAChunks; ++j) a_chunks += (m0 + j * CW < p.Ktot) ? 1 : 0;
-  int b_chunks = (p.Cout - co0 < BN ? p.Cout - co0 : BN) / CWB;
+  const int b_chunks = (p.Cout - co0 < BN ? p.Cout - co0 : BN) / CWB;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kConsumerWarps);
     }
-    mbar_init(&tmem_full_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(&tmem_base_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  // everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the tail of
-  // the preceding kernel; its outputs are read only after this point
+  // everything above (barrier init, descriptor prefetch) overlapped the tail of the preceding
+  // kernel; its outputs are read only after this point
   pdl_entry();
-  const uint32_t tmem_base = tmem_base_smem;
 
   if (warp == 0) {
     // whole warp converged, one elected lane issues (no election loops around TMA instructions)
@@ -1560,90 +1077,112 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       __syncwarp();
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1) {
-    int stage = 0;
+  } else if (warp >= 4) {
+    // consumer warpgroup cg: rows (tap,ci) cg*64 .. of the 128, i.e. A chunks from cg*64/CW on
+    const int cg = (warp >> 2) - 1;
+    const uint32_t sbase = smem_u32(smem);
+    const uint64_t a_desc0 = make_smem_desc(sbase + (cg * 64 / CW) * kAChunkBytes, kAChunkBytes,
+                                            8 * CW * 2, swizzle_layout_type(CW * 2));
+    const uint64_t b_desc0 = make_smem_desc(sbase + NP * Cfg::kABytes, kBChunkBytes, 8 * CWB * 2,
+                                            swizzle_layout_type(CWB * 2));
+    float acc[BN / 2];
+    float acc2[NP == 3 ? BN / 2 : 1];
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
-    // MN-major operands: one pixel row = width*2 bytes, 8-row groups SBO apart, column blocks
-    // (64/32/16 channels) LBO apart.  16 pixel rows per UMMA.
-    const uint64_t a_desc0 = make_smem_desc(smem_u32(smem), kAChunkBytes, 8 * CW * 2,
-                                            swizzle_layout_type(CW * 2));
-    const uint64_t b_desc0 = make_smem_desc(smem_u32(smem) + NP * Cfg::kABytes, kBChunkBytes,
-                                            8 * CWB * 2, swizzle_layout_type(CWB * 2));
     for (int it = 0; it < num_ks; ++it) {
       mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t da0 = a_desc0 + static_cast<uint64_t>(stage * (Cfg::kStageBytes >> 4));
-        const uint64_t db0 = b_desc0 + static_cast<uint64_t>(stage * (Cfg::kStageBytes >> 4));
+      wgmma_fence_operand(acc);
+      if (NP == 3) wgmma_fence_operand(acc2);
+      wgmma_fence();
+      const uint64_t da0 = a_desc0 + static_cast<uint64_t>(stage * (Cfg::kStageBytes >> 4));
+      const uint64_t db0 = b_desc0 + static_cast<uint64_t>(stage * (Cfg::kStageBytes >> 4));
 #pragma unroll
-        for (int h = 0; h < MT; ++h) {
-          if (h == 0 || second) {
+      for (int ks = 0; ks < PIX / 16; ++ks) {
 #pragma unroll
-            for (int ks = 0; ks < PIX / 16; ++ks) {
-#pragma unroll
-              for (int t = 0; t < (NP == 3 ? 6 : 1); ++t) {
-                const int pa = NP == 3 ? plane_term_a(t) : 0;
-                const int pb = NP == 3 ? plane_term_b(t) : 0;
-                const bool small = NP == 3 && t < 5;
-                umma_bf16(tmem_base + h * BN + (small ? BN : 0),
-                          da0 + ((pa * Cfg::kABytes + h * Cfg::kAHalfBytes + ks * 16 * CW * 2) >> 4),
-                          db0 + ((pb * Cfg::kBBytes + ks * 16 * CWB * 2) >> 4), kIdesc,
-                          (it | ks | (small ? t : 0)) ? 1u : 0u);
-              }
-            }
+        for (int t = 0; t < (NP == 3 ? 6 : 1); ++t) {
+          const int pa = NP == 3 ? plane_term_a(t) : 0;
+          const int pb = NP == 3 ? plane_term_b(t) : 0;
+          const bool small = NP == 3 && t < 5;
+          const uint64_t da = da0 + ((pa * Cfg::kABytes + ks * 16 * CW * 2) >> 4);
+          const uint64_t db = db0 + ((pb * Cfg::kBBytes + ks * 16 * CWB * 2) >> 4);
+          const uint32_t accum = (it | ks | (small ? t : 0)) ? 1u : 0u;
+          if constexpr (NP == 3) {
+            if (small) Wgmma<BN>::template mma<1, 1>(acc2, da, db, accum);
+            else Wgmma<BN>::template mma<1, 1>(acc, da, db, accum);
+          } else {
+            Wgmma<BN>::template mma<1, 1>(acc, da, db, accum);
           }
         }
-        umma_commit(&empty_bar[stage]);
-        if (it == num_ks - 1) umma_commit(&tmem_full_bar);
       }
+      wgmma_commit();
+      wgmma_fence_operand(acc);
+      if (NP == 3) wgmma_fence_operand(acc2);
+      wgmma_wait<1>();
       __syncwarp();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-  } else {
-    // TMEM lane = row of D = (tap,ci) column of dw; consecutive lanes -> consecutive addresses.
-    const int quarter = warp & 3;
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int h = 0; h < MT; ++h) {
-      if (h == 1 && !second) break;          // warp-uniform
-      const int n = m0 + h * 128 + quarter * 32 + lane;
-      const bool n_ok = n < p.Ktot;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        if (co0 + c * 32 >= p.Cout) break;   // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + h * BN + c * 32,
-                      v);
-        tmem_ld_wait();
-        if (NP == 3) {   // + the small-term accumulator
-          uint32_t v2[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + BN + c * 32, v2);
-          tmem_ld_wait();
+    wgmma_wait<0>();
+    wgmma_fence_operand(acc);
+    if (NP == 3) {
+      wgmma_fence_operand(acc2);
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(v2[i]));
-        }
-        if (n_ok) {
-          float* dst = p.dw + static_cast<size_t>(co0 + c * 32) * p.Ktot + n;
+      for (int i = 0; i < BN / 2; ++i) acc[i] += acc2[i];
+    }
+    // fragment row = (tap,ci) column n of dw, fragment column = output channel
+    const int rl = cg * 64 + (warp & 3) * 16 + (lane >> 2);   // row inside the 128-row tile
+    const int rb = m0 + rl;
+    const int cq = (lane & 3) * 2;
+    __shared__ int s_last;
+    if (p.splits > 1) {
+      // split-K, ordered: every split stores its partial tile; the LAST split to arrive adds the
+      // partials in split order (the arrival order does not enter the sum)
+      const int tile = blockIdx.y * gridDim.x + blockIdx.x;
+      const size_t tiles = static_cast<size_t>(gridDim.x) * gridDim.y;
+      float* mine = p.part + (static_cast<size_t>(blockIdx.z) * tiles + tile) * (128 * BN);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            // (measured: replacing these atomics by plain stores changes the training step by
-            // 0.13 ms of 25.5 -- profiles/r02_exp_knobs.txt -- the split-K reduction is not what
-            // bounds wgrad)
-            if (co0 + c * 32 + i < p.Cout)
-              atomicAdd(dst + static_cast<size_t>(i) * p.Ktot, __uint_as_float(v[i]));
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(mine + (rl + h * 8) * BN + j * 8 + cq) =
+              make_float2(acc[j * 4 + h * 2], acc[j * 4 + h * 2 + 1]);
+      __threadfence();
+      named_bar_sync(1, kConsumerThreads);
+      if (threadIdx.x == 128) s_last = atomicAdd(p.counters + tile, 1u) == static_cast<unsigned>(p.splits - 1);
+      named_bar_sync(1, kConsumerThreads);
+      if (!s_last) return;
+      __threadfence();
+      const float* first = p.part + static_cast<size_t>(tile) * (128 * BN);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float2 t = make_float2(0.f, 0.f);
+          for (int sp = 0; sp < p.splits; ++sp) {
+            const float2 v = __ldcg(reinterpret_cast<const float2*>(
+                first + sp * tiles * (128 * BN) + (rl + h * 8) * BN + j * 8 + cq));
+            t.x += v.x;
+            t.y += v.y;
           }
+          acc[j * 4 + h * 2] = t.x;
+          acc[j * 4 + h * 2 + 1] = t.y;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int n = rb + h * 8;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int co = co0 + j * 8 + cq + e;
+          // one add per dw element (the whole pixel range of this tile is summed above)
+          if (n < p.Ktot && co < p.Cout)
+            atomicAdd(p.dw + static_cast<size_t>(co) * p.Ktot + n, acc[j * 4 + h * 2 + e]);
         }
       }
     }
-  }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 
@@ -1656,7 +1195,8 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    // at most kMaxSms: the partial statistics rows (one per CTA of an N tile) are sized for it
+    if (g_num_sms <= 0 || g_num_sms > kMaxSms) g_num_sms = kMaxSms;
   }
   return g_num_sms;
 }
@@ -1665,40 +1205,24 @@ struct ConvMaps {
   CUtensorMap a[3], b[3], c, add, mask;
 };
 
-// output staging buffers of the conv GEMM epilogue: 0 = two where the ring stays deep, 1 = always
-// one (default: the interleaved A/B of the c3 step shows no difference beyond noise -- 23.76 / 23.69
-// / 23.86 ms for 1 / 0 / 2, profiles/r02_exp_ab.txt -- so the deeper ring is kept), 2 = two wherever
-// shared memory allows (acnn_set_conv_out_bufs; ACNN_CONV_OUT_BUFS sets the initial value)
-static int conv_out_bufs_default() {
-  const char* e = getenv("ACNN_CONV_OUT_BUFS");
-  return e ? (e[0] - '0') : 1;
-}
-static int g_conv_out_bufs = conv_out_bufs_default();
+// Epilogue / tiling knobs of the C ABI from earlier kernel generations.  The sm_90 kernels have one
+// epilogue organisation (the consumer warpgroups drain their own registers) and one 128-pixel M
+// tile per CTA: these setters keep and return their value and change nothing.
+static int g_conv_out_bufs = 1;
+static int g_conv_split_epi = 1;
+static int g_conv_split_mt2 = 1;
+static int g_conv_mtiles_mode = -1;
+// CTA pairs (clusters of two sharing the weight stages by TMA multicast): 1 = the N = 128 tiles with
+// K >= 512 and enough tiles for every SM; 0 (default) = single CTAs (acnn_set_conv_cta_pairs).  Off
+// by default: c3 step on an H100 SXM at 700 W, 80.3 ms with pairs against 61.3 ms without
+static int g_conv_pairs = 0;
 
-// split epilogue of the conv GEMM kernel: 0 = off, 1 (default) = where the epilogue chain paces the
-// tile (K <= 256), 2 = wherever it fits (acnn_set_conv_split_epilogue; ACNN_CONV_SPLIT_EPI sets the
-// initial value).  Interleaved A/B of the c3 step: 23.36 / 23.14 / 23.19 ms for 0 / 1 / 2
-// (profiles/r02_exp_ab.txt); per layer profiles/r02_exp_split_epilogue_layers.txt
-static int conv_split_epi_default() {
-  const char* e = getenv("ACNN_CONV_SPLIT_EPI");
-  return e ? (e[0] - '0') : 1;
-}
-static int g_conv_split_epi = conv_split_epi_default();
-// the same for two-M-tile CTA tiles (the two groups take the two M tiles of every tile): 0 = off,
-// 1 (default) = K <= 256, 2 = wherever it fits (acnn_set_conv_split_mt2; ACNN_CONV_SPLIT_MT2 sets
-// the initial value).  Interleaved A/B of the c3 step: 23.28 / 23.11 / 23.17 ms for 0 / 1 / 2
-static int conv_split_mt2_default() {
-  const char* e = getenv("ACNN_CONV_SPLIT_MT2");
-  return e ? (e[0] - '0') : 1;
-}
-static int g_conv_split_mt2 = conv_split_mt2_default();
-
-template <int BN, int CW, bool IM2COL, int MT, int NP, bool CG2 = false>
+template <int BN, int CW, bool IM2COL, int NP, bool CG2 = false>
 static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per_n,
                             cudaStream_t stream) {
-  using Cfg = FpropCfg<BN, MT, NP, CG2>;
+  using Cfg = FpropCfg<BN, NP>;
   static bool attr_set = false;
-  auto kern = conv_gemm_kernel<BN, CW, IM2COL, MT, NP, CG2>;
+  auto kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          kSmemBudget + 2048);
@@ -1709,47 +1233,15 @@ static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per
     attr_set = true;
   }
   ConvGemmParams q = p;
-  // a second output staging half tile where the ring stays deep enough without its bytes: all of K
-  // in flight, or >= 4 stages (g_conv_out_bufs: 0 = this rule, 1 / 2 = force where it fits)
-  q.out_bufs = 1;
-  if (!p.out_f32 && g_conv_out_bufs != 1) {
-    const int st2 = Cfg::stages_for(p.has_add, p.has_mask, p.out_f32, 2);
-    const int num_kb = ceil_div(p.Ktot, kStageK);
-    const int need = g_conv_out_bufs == 2 ? (MT == 2 ? 3 : 2)
-                                          : (num_kb + 1 < 4 ? num_kb + 1 : 4);
-    if (st2 >= need && st2 >= (MT == 2 ? 3 : 2) &&
-        Cfg::smem_bytes(st2, p.has_add, p.has_mask, p.out_f32, 2) <= kSmemBudget + 1024)
-      q.out_bufs = 2;
-  }
-  // split epilogue (two 4-warp groups alternate tiles): one M tile per CTA tile, bf16 output, no
-  // bias; needs two output staging tiles and two sets of add / mask tiles.  Mode 1 = where the
-  // epilogue chain, not the k-loop, paces a tile (K <= 256: at most four k-blocks) and the ring still
-  // holds all of K or 3 stages; mode 2 = wherever it fits with >= 2 stages
-  q.split_epi = 0;
-  const int split_mode = MT == 2 ? g_conv_split_mt2 : g_conv_split_epi;
-  if (NP == 1 && !CG2 && !p.out_f32 && !p.bias && split_mode > 0) {
-    const int num_kb = ceil_div(p.Ktot, kStageK);
-    const int st2 = Cfg::stages_for(p.has_add, p.has_mask, false, 2, 2);
-    const int min_st = MT == 2 ? 3 : 2;
-    const bool fits = st2 >= min_st && Cfg::smem_bytes(st2, p.has_add, p.has_mask, false, 2, 2) <=
-                                           kSmemBudget + 1024;
-    const int need = num_kb + 1 < 3 ? num_kb + 1 : 3;
-    if (fits && (split_mode >= 2 || (num_kb <= 4 && st2 >= need))) {
-      q.split_epi = 1;
-      q.out_bufs = 2;
-    }
-  }
-  const int aux_sets = q.split_epi ? 2 : 1;
-  q.stages = Cfg::stages_for(p.has_add, p.has_mask, p.out_f32, q.out_bufs, aux_sets);
-  q.m_tiles = ceil_div(p.M, (CG2 ? 2 : MT) * kBM);
+  q.stages = Cfg::stages_for(p.has_add, p.has_mask, p.out_f32);
+  q.m_tiles = ceil_div(p.M, (CG2 ? 2 : 1) * kBM);
   q.n_tiles = p.Cout / BN;
-  const int smem =
-      Cfg::smem_bytes(q.stages, p.has_add, p.has_mask, p.out_f32, q.out_bufs, aux_sets);
+  const int smem = Cfg::smem_bytes(q.stages, p.has_add, p.has_mask, p.out_f32);
   if (CG2) {
-    // per_n CTA PAIRS per N tile, launched as clusters of two (ranks 2i, 2i+1 share a TPC)
+    // per_n CTA PAIRS per N tile, launched as clusters of two
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(2 * per_n * q.n_tiles);
-    cfg.blockDim = dim3(kConvThreads);
+    cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
     cudaLaunchAttribute at[1];
@@ -1762,62 +1254,38 @@ static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per
     (void)cudaLaunchKernelEx(&cfg, kern, tm.a[0], tm.b[0], tm.c, tm.add, tm.mask, tm.a[1], tm.a[2],
                              tm.b[1], tm.b[2], q);
   } else {
-    launch_k(kern, dim3(per_n * q.n_tiles), dim3(kConvThreads), smem, stream, tm.a[0], tm.b[0], tm.c,
+    launch_k(kern, dim3(per_n * q.n_tiles), dim3(kThreads), smem, stream, tm.a[0], tm.b[0], tm.c,
              tm.add, tm.mask, tm.a[1], tm.a[2], tm.b[1], tm.b[2], q);
   }
   count_launch();
   return check_launch("conv_gemm_kernel");
 }
 
-// -1: choose per problem; 1 / 2: force that many M tiles per CTA tile where the shape allows it
-static int g_conv_mtiles_mode = -1;
-
 // Tile shape and persistent grid of one conv GEMM: a pure function of the problem, shared by the
 // launcher and by acnn_conv_stats_parts() (the number of partial statistics rows = per_n).
 struct ConvTiling {
   int bn;      // N tile
-  int mt;      // M tiles (128 pixels) per CTA tile
   int per_n;   // CTAs (pair = 1: CTA pairs) per N tile
-  int pair;    // 1: CTA pairs (tcgen05 cta_group::2), one 256 x bn tile per pair
+  int pair;    // 1: clusters of two CTAs sharing the weight stages, one 256 x bn tile per pair
   int parts;   // rows of the partial statistics buffer (= CTAs per N tile)
 };
 
-// 1 (default): N = 256 tiles with K >= 512 run on CTA pairs; 0: off (acnn_set_conv_cta_pairs;
-// ACNN_CONV_PAIRS=0|1 sets the initial value)
-static int conv_pairs_default() {
-  const char* e = getenv("ACNN_CONV_PAIRS");
-  return e ? (e[0] == '1') : 1;
-}
-static int g_conv_pairs = conv_pairs_default();
-
 static ConvTiling conv_tiling(int M, int Cout, int Ktot, int cw, bool has_add, bool has_mask,
                               bool out_f32, int np) {
+  (void)has_add;
+  (void)has_mask;
   ConvTiling t;
-  // N tile: 256 halves the A-operand traffic per FLOP (128 B/clk of smem reads at BN=128 is the
-  // SM's whole shared-memory bandwidth); dense / tiny-M problems keep 128 for more CTAs
+  // N tile <= 128: a 64 x 256 fp32 accumulator per consumer warpgroup (128 registers per thread)
+  // does not fit next to the epilogue under the 168-register limit of a 384-thread CTA
   t.bn = (Cout % 128 == 0) ? 128 : ((Cout % 64 == 0) ? 64 : 32);
-  if (np == 1 && Cout % 256 == 0 && !out_f32 && (int64_t)ceil_div(M, kBM) * (Cout / 256) >= 96)
-    t.bn = 256;
-  // Two M tiles per CTA when TMEM has room (N <= 128), the smem ring stays >= 3 stages deep and
-  // there are enough tiles to keep every SM busy for several rounds.
-  // (at N = 128 that rules out only the add + mask epilogue: two 32 KiB aux staging tiles)
-  t.mt = 1;
-  if (np == 1 && t.bn <= 128 && !out_f32) {
-    const bool fits = fprop_stages(t.bn, 2, 1, has_add, has_mask, out_f32) >= 3;
-    const int64_t tiles = (int64_t)ceil_div(M, 2 * kBM) * (Cout / t.bn);
-    if (fits && (g_conv_mtiles_mode == 2 ||
-                 (g_conv_mtiles_mode == -1 && tiles >= 4 * (int64_t)num_sms())))
-      t.mt = 2;
-  }
   // persistent grid: a multiple of n_tiles so that every CTA keeps one N tile (its weights and
   // its per-channel statistics), at most one CTA per SM
   const int n_tiles = Cout / t.bn;
-  // CTA pairs: measured per layer (profiles/r02_exp_cta_pairs.txt) -- K >= 512 gains 15-25 % (the
-  // k-loop is shared-memory-ingest bound), small K loses 10-20 % (epilogue-bound tiles, and a pair
-  // schedules half as many, twice as large units); 64-channel chunks only (instantiation count)
-  t.pair = (g_conv_pairs && t.bn == 256 && np == 1 && t.mt == 1 && cw == 64 && Ktot >= 512 &&
-            ceil_div(M, 2 * kBM) * n_tiles >= num_sms() / 2) ? 1 : 0;
-  const int m_tiles = ceil_div(M, (t.pair ? 2 : t.mt) * kBM);
+  // CTA pairs: full-width (64-channel) chunks, K >= 512 (the k-loop, not the epilogue, paces the
+  // tile) and at least one pair tile per SM pair
+  t.pair = (g_conv_pairs && t.bn == 128 && np == 1 && !out_f32 && cw == 64 && Ktot >= 512 &&
+            (int64_t)ceil_div(M, 2 * kBM) * n_tiles >= num_sms() / 2) ? 1 : 0;
+  const int m_tiles = ceil_div(M, (t.pair ? 2 : 1) * kBM);
   t.per_n = (t.pair ? num_sms() / 2 : num_sms()) / n_tiles;
   if (t.per_n < 1) t.per_n = 1;
   if (t.per_n > m_tiles) t.per_n = m_tiles;
@@ -1825,33 +1293,32 @@ static ConvTiling conv_tiling(int M, int Cout, int Ktot, int cw, bool has_add, b
   return t;
 }
 
-template <int BN, int MT, int NP>
+template <int BN, int NP>
 static int dispatch_conv_cw(int cw, bool im2col, const ConvMaps& tm, const ConvGemmParams& p,
                             int per_n, cudaStream_t s) {
   if (im2col) {
-    if (cw == 64) return launch_conv_gemm<BN, 64, true, MT, NP>(tm, p, per_n, s);
-    if (cw == 32) return launch_conv_gemm<BN, 32, true, MT, NP>(tm, p, per_n, s);
-    return launch_conv_gemm<BN, 16, true, MT, NP>(tm, p, per_n, s);
+    if (cw == 64) return launch_conv_gemm<BN, 64, true, NP>(tm, p, per_n, s);
+    if (cw == 32) return launch_conv_gemm<BN, 32, true, NP>(tm, p, per_n, s);
+    return launch_conv_gemm<BN, 16, true, NP>(tm, p, per_n, s);
   }
-  if (cw == 64) return launch_conv_gemm<BN, 64, false, MT, NP>(tm, p, per_n, s);
-  if (cw == 32) return launch_conv_gemm<BN, 32, false, MT, NP>(tm, p, per_n, s);
-  return launch_conv_gemm<BN, 16, false, MT, NP>(tm, p, per_n, s);
+  if (cw == 64) return launch_conv_gemm<BN, 64, false, NP>(tm, p, per_n, s);
+  if (cw == 32) return launch_conv_gemm<BN, 32, false, NP>(tm, p, per_n, s);
+  return launch_conv_gemm<BN, 16, false, NP>(tm, p, per_n, s);
 }
 
 template <int BN>
 static int dispatch_conv_gemm(const ConvTiling& t, int np, int cw, bool im2col, const ConvMaps& tm,
                               const ConvGemmParams& p, cudaStream_t s) {
-  if constexpr (BN == 256) {
+  if constexpr (BN == 128) {
     if (t.pair) {     // full-width (64-channel) chunks only: bounds the instantiation count
-      if (im2col) return launch_conv_gemm<256, 64, true, 1, 1, true>(tm, p, t.per_n, s);
-      return launch_conv_gemm<256, 64, false, 1, 1, true>(tm, p, t.per_n, s);
+      if (im2col) return launch_conv_gemm<128, 64, true, 1, true>(tm, p, t.per_n, s);
+      return launch_conv_gemm<128, 64, false, 1, true>(tm, p, t.per_n, s);
     }
   }
   if constexpr (BN <= 128) {
-    if (np == 3) return dispatch_conv_cw<BN, 1, 3>(cw, im2col, tm, p, t.per_n, s);
-    if (t.mt == 2) return dispatch_conv_cw<BN, 2, 1>(cw, im2col, tm, p, t.per_n, s);
+    if (np == 3) return dispatch_conv_cw<BN, 3>(cw, im2col, tm, p, t.per_n, s);
   }
-  return dispatch_conv_cw<BN, 1, 1>(cw, im2col, tm, p, t.per_n, s);
+  return dispatch_conv_cw<BN, 1>(cw, im2col, tm, p, t.per_n, s);
 }
 
 static int chunk_width(int cin) { return cin % 64 == 0 ? 64 : (cin % 32 == 0 ? 32 : 16); }
@@ -1870,27 +1337,20 @@ static int64_t input_elems(const acnn_conv_geom& g) {
 }
 
 // ---- halo (im2col-free 3x3) kernel: eligibility, tiling, launch --------------------------------
-// 0: off; 1 (default): where measured to pay (use_halo below); 2: wherever the kernel applies
-// (acnn_set_conv_halo; ACNN_CONV_HALO=0|1|2 sets the initial value)
-static int conv_halo_default() {
-  const char* e = getenv("ACNN_CONV_HALO");
-  return e ? (e[0] - '0') : 1;
-}
-static int g_conv_halo = conv_halo_default();
+// 0: off; 1 (default): where the weight slab stays in shared memory and the images are large (the
+// use_halo rule below; c3 step on an H100 SXM at 700 W: 59.8 ms against 61.3 ms with 0); 2: wherever
+// the kernel applies (acnn_set_conv_halo)
+static int g_conv_halo = 1;
 
 static int halo_bn(int Cout) { return Cout % 128 == 0 ? 128 : (Cout % 64 == 0 ? 64 : 32); }
 
 // Shared-memory plan of the halo kernel for one problem (a pure function of the shape).
 struct HaloPlan {
-  int a_stages, b_slots, stationary, out_bufs, split_epi, smem;
+  int a_stages, b_slots, stationary, smem;
 };
-// 1 (default): N <= 64 tiles use two independent epilogue groups; 0: all 8 warps on one tile
-// (acnn_set_conv_halo_split; ACNN_CONV_HALO_SPLIT sets the initial value)
-static int conv_halo_split_default() {
-  const char* e = getenv("ACNN_CONV_HALO_SPLIT");
-  return e ? (e[0] - '0') : 1;
-}
-static int g_conv_halo_split = conv_halo_split_default();
+// epilogue organisation of an earlier kernel generation: the sm_90 halo kernel has one (the
+// consumer warpgroups drain their registers); acnn_set_conv_halo_split keeps and returns the value
+static int g_conv_halo_split = 1;
 
 static HaloPlan halo_plan(int bn, int cw, int Cin, bool has_add, bool has_mask) {
   HaloPlan h;
@@ -1899,13 +1359,7 @@ static HaloPlan halo_plan(int bn, int cw, int Cin, bool has_add, bool has_mask) 
   const int b_tile = bn * row_b;
   const int tile = kBM * bn * 2;
   const int nchunks = Cin / cw;
-  // two output staging tiles where they are cheap (N <= 64: 8 / 16 KiB); the split epilogue also
-  // doubles the add / mask staging (one set per group)
-  h.out_bufs = bn <= 64 ? 2 : 1;
-  h.split_epi = (bn <= 64 && g_conv_halo_split) ? 1 : 0;
-  const int aux_sets = h.split_epi ? 2 : 1;
-  const int fixed =
-      1024 + tile * (h.out_bufs + (has_add ? aux_sets : 0) + (has_mask ? aux_sets : 0));
+  const int fixed = 1024 + tile * (1 + (has_add ? 1 : 0) + (has_mask ? 1 : 0));
   h.a_stages = 3;
   h.b_slots = (kSmemBudget - fixed - h.a_stages * a_stage) / b_tile;
   if (h.b_slots < nchunks * 9) {         // one A stage fewer if that makes the slab stationary
@@ -1932,9 +1386,8 @@ static bool use_halo(const acnn_conv_geom& g, int np, bool out_f32, bool has_bia
                        g.Cout % 32 == 0;
   if (!applies) return false;
   if (g_conv_halo >= 2) return true;
-  // mode 1 = where measured to pay (profiles/r02_exp_halo_layers.txt): the weight slab of an N tile
-  // stays in shared memory (otherwise the weight stream replaces the im2col re-reads as the ingest
-  // bound: 56x56 128->64 dgrad 0.163 -> 0.243 ms) and the images have >= 56 rows (16 x 8 patches
+  // mode 1: the weight slab of an N tile stays in shared memory (otherwise the weight stream
+  // replaces the im2col re-reads as the ingest bound) and the images have >= 56 rows (16 x 8 patches
   // waste <= 12.5 % of a 56 x 56 image, 27 % of 28 x 28)
   const HaloPlan h = halo_plan(halo_bn(g.Cout), g.Cin % 64 == 0 ? 64 : 32, g.Cin, has_add, has_mask);
   return h.stationary && g.H >= 56;
@@ -1992,10 +1445,7 @@ static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* 
   p.ch_part = ch_part;
   p.has_add = add_src != nullptr;
   p.has_mask = mask_src != nullptr;
-  const int nchunks = g.Cin / CW;
   const HaloPlan hp = halo_plan(BN, CW, g.Cin, p.has_add != 0, p.has_mask != 0);
-  p.out_bufs = hp.out_bufs;
-  p.split_epi = hp.split_epi;
   p.a_stages = hp.a_stages;
   p.b_slots = hp.b_slots;
   p.stationary = hp.stationary;
@@ -2013,7 +1463,7 @@ static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* 
   if (mask_src && (rc = make_map_4d(&tmMask, mask_src, g.Cout, g.W, g.H, g.B, Cfg::kSubW, kPatchW,
                                     kPatchH)))
     return rc;
-  launch_k(kern, dim3(halo_per_n(g) * p.n_tiles), dim3(kConvThreads), smem, stream, tmA, tmB, tmC,
+  launch_k(kern, dim3(halo_per_n(g) * p.n_tiles), dim3(kThreads), smem, stream, tmA, tmB, tmC,
            tmAdd, tmMask, p);
   count_launch();
   return check_launch("conv_halo_kernel");
@@ -2061,7 +1511,6 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   if (use_halo(g, precision ? 3 : 1, out_f32 != 0, bias != nullptr, add_src != nullptr,
                mask_src != nullptr))
     return conv_halo_host(g, x, w, y, ch_part, add_src, mask_src, stream);
-
   const bool plain = is_plain(g);
   const int cw = chunk_width(g.Cin);
   const int np = precision ? 3 : 1;
@@ -2114,7 +1563,6 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   if (!out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw))) return rc;
   if (add_src && (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw))) return rc;
   if (mask_src && (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw))) return rc;
-  if (bn == 256) return dispatch_conv_gemm<256>(t, np, cw, !plain, tm, p, stream);
   if (bn == 128) return dispatch_conv_gemm<128>(t, np, cw, !plain, tm, p, stream);
   if (bn == 64) return dispatch_conv_gemm<64>(t, np, cw, !plain, tm, p, stream);
   return dispatch_conv_gemm<32>(t, np, cw, !plain, tm, p, stream);
@@ -2125,17 +1573,20 @@ struct WgradMaps {
 };
 
 // fixed cost of one wgrad CTA (pipeline fill + atomic epilogue) in units of pipeline stages, for
-// the split-K cost model (default 16: measured, profiles/r02_exp_wgrad_split.txt: -0.5 ms per c3 step
-// against 0 = the round-1 "two waves of CTAs" rule; flat from 4 to 1000); acnn_set_wgrad_overhead_stages
+// the split-K cost model (0 = the "two waves of CTAs" rule); acnn_set_wgrad_overhead_stages
 static int g_wgrad_overhead_stages = 16;
 
-template <int BN, int CW, int CWB, bool IM2COL, int MT, int NP, int PIX = kWgPix>
+// Split-K partial tiles are bounded (the split count is capped to fit): 64 MiB per launch.
+constexpr size_t kWgPartFloats = size_t(16) << 20;
+constexpr int kWgCounters = 1 << 16;
+
+template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX = kWgPix>
 static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int deterministic,
                         cudaStream_t stream) {
-  using Cfg = WgradCfg<BN, MT, NP, PIX>;
+  using Cfg = WgradCfg<BN, NP, PIX>;
   static bool attr_set = false;
-  auto kern = wgrad_gemm_kernel<BN, CW, CWB, IM2COL, MT, NP, PIX>;
-  const int m_tiles = ceil_div(p.Ktot, MT * 128);
+  auto kern = wgrad_gemm_kernel<BN, CW, CWB, IM2COL, NP, PIX>;
+  const int m_tiles = ceil_div(p.Ktot, 128);
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
@@ -2145,20 +1596,23 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int det
     }
     attr_set = true;
   }
-  // split the pixel (K) range over CTAs; deterministic mode: no split -- every dw element receives
-  // exactly one (atomic) add onto the zeroed buffer
-  const int ctas_per_sm = Cfg::kSmemBytes <= 110 * 1024 ? 2 : 1;
+  // split the pixel (K) range over CTAs; the partial tiles are summed in split order, so the result
+  // does not depend on which split finishes first.  deterministic: no split -- one add per dw
+  // element.  One CTA per SM (384 threads with register accumulators).
   const int tiles = m_tiles * n_tiles;
-  const int max_splits = p.stages_total >= 8 ? p.stages_total / 4 : 1;
+  int max_splits = p.stages_total >= 8 ? p.stages_total / 4 : 1;
+  const int64_t tile_floats = (int64_t)tiles * 128 * BN;
+  if ((int64_t)max_splits * tile_floats > (int64_t)kWgPartFloats)
+    max_splits = (int)(kWgPartFloats / tile_floats);
+  if (max_splits < 1 || tiles > kWgCounters) max_splits = 1;
   int splits;
   if (g_wgrad_overhead_stages <= 0) {
-    // (round-1 rule: roughly two waves of CTAs)
-    splits = ceil_div(2 * ctas_per_sm * num_sms(), tiles);
+    // (simple rule: roughly two waves of CTAs)
+    splits = ceil_div(2 * num_sms(), tiles);
   } else {
-    // cost model: an SM runs its CTAs' pipeline stages back to back (co-resident CTAs share the
-    // tensor pipe) and pays a fixed pipeline-fill + epilogue cost, worth g_wgrad_overhead_stages
-    // stages, once per round of resident CTAs; pick the split count with the least modelled time
-    // (avoids e.g. 2.2 waves of CTAs where 0.97 waves do the same work in less time)
+    // cost model: an SM runs its CTAs' pipeline stages back to back and pays a fixed pipeline-fill
+    // + epilogue cost, worth g_wgrad_overhead_stages stages, once per CTA; pick the split count
+    // with the least modelled time
     splits = 1;
     int64_t best = -1;
     for (int s = 1; s <= max_splits; ++s) {
@@ -2166,8 +1620,7 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int det
       const int s_eff = ceil_div(p.stages_total, per);
       if (s_eff != s) continue;
       const int per_sm = ceil_div(tiles * s, num_sms());
-      const int64_t t = (int64_t)per_sm * per +
-                        (int64_t)ceil_div(per_sm, ctas_per_sm) * g_wgrad_overhead_stages;
+      const int64_t t = (int64_t)per_sm * per + (int64_t)per_sm * g_wgrad_overhead_stages;
       if (best < 0 || t < best) { best = t; splits = s; }
     }
   }
@@ -2175,11 +1628,32 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int det
   if (splits < 1 || deterministic) splits = 1;
   p.stages_per_split = ceil_div(p.stages_total, splits);
   splits = ceil_div(p.stages_total, p.stages_per_split);
+  p.splits = splits;
+  p.part = nullptr;
+  p.counters = nullptr;
+  void* scratch = nullptr;
+  if (splits > 1) {
+    // this launch's partial tiles + arrival counters, stream-ordered (per stream, capturable)
+    const size_t part_bytes = (size_t)splits * tiles * 128 * BN * sizeof(float);
+    int rc = scratch_alloc(&scratch, part_bytes + (size_t)tiles * sizeof(unsigned), stream, "wgrad");
+    if (rc) return rc;
+    p.part = static_cast<float*>(scratch);
+    p.counters = reinterpret_cast<unsigned*>(static_cast<char*>(scratch) + part_bytes);
+    if (cudaMemsetAsync(p.counters, 0, (size_t)tiles * sizeof(unsigned), stream) != cudaSuccess) {
+      set_error("wgrad: clearing the split counters: %s", cudaGetErrorString(cudaGetLastError()));
+      return ACNN_ERR_CUDA;
+    }
+  }
   dim3 grid(m_tiles, n_tiles, splits);
   launch_k(kern, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, tm.x[0], tm.dy[0], tm.x[1],
            tm.x[2], tm.dy[1], tm.dy[2], p);
   count_launch();
-  return check_launch("wgrad_gemm_kernel");
+  const int rc = check_launch("wgrad_gemm_kernel");
+  if (scratch) {
+    const int rc2 = scratch_free(scratch, stream, "wgrad");
+    if (rc == ACNN_OK) return rc2;
+  }
+  return rc;
 }
 
 template <int BN, int CW, bool IM2COL>
@@ -2188,32 +1662,23 @@ static int dispatch_wgrad_cwb(int cwb, int np, const WgradMaps& tm, const WgradP
   if constexpr (BN <= 128) {
     if (np == 3) {
       if constexpr (BN >= 64) {
-        if (cwb == 64) return launch_wgrad<BN, CW, 64, IM2COL, 1, 3>(tm, p, nt, det, s);
+        if (cwb == 64) return launch_wgrad<BN, CW, 64, IM2COL, 3>(tm, p, nt, det, s);
       }
-      return launch_wgrad<BN, CW, 32, IM2COL, 1, 3>(tm, p, nt, det, s);
+      return launch_wgrad<BN, CW, 32, IM2COL, 3>(tm, p, nt, det, s);
     }
   }
   if constexpr (BN >= 64) {
     if (cwb == 64) {
-      // two 128-row blocks per CTA (full-width chunks only, to bound the instantiation count)
-      if constexpr (CW == 64) {
-        // measured: pays when the (tap,ci) extent and the pixel count are both large (otherwise
-        // halving the number of CTAs costs more than the shared dy stage saves)
-        const bool big = (p.Ktot >= 1024 && p.P >= 50176) || p.Ktot >= 4096;
-        if (p.pix == 64 && p.Ktot > 128 &&
-            (g_conv_mtiles_mode == 2 || (g_conv_mtiles_mode == -1 && big)))
-          return launch_wgrad<BN, CW, 64, IM2COL, 2, 1>(tm, p, nt, det, s);
-      }
       if constexpr (BN <= 128) {
-        if (p.pix == 128) return launch_wgrad<BN, CW, 64, IM2COL, 1, 1, 128>(tm, p, nt, det, s);
+        if (p.pix == 128) return launch_wgrad<BN, CW, 64, IM2COL, 1, 128>(tm, p, nt, det, s);
       }
-      return launch_wgrad<BN, CW, 64, IM2COL, 1, 1>(tm, p, nt, det, s);
+      return launch_wgrad<BN, CW, 64, IM2COL, 1>(tm, p, nt, det, s);
     }
   }
   if constexpr (BN <= 128) {
-    if (p.pix == 128) return launch_wgrad<BN, CW, 32, IM2COL, 1, 1, 128>(tm, p, nt, det, s);
+    if (p.pix == 128) return launch_wgrad<BN, CW, 32, IM2COL, 1, 128>(tm, p, nt, det, s);
   }
-  return launch_wgrad<BN, CW, 32, IM2COL, 1, 1>(tm, p, nt, det, s);
+  return launch_wgrad<BN, CW, 32, IM2COL, 1>(tm, p, nt, det, s);
 }
 
 template <int BN, bool IM2COL>
@@ -2236,8 +1701,7 @@ static int dispatch_wgrad(int bn, int cw, int cwb, int np, const WgradMaps& tm, 
 // 0: choose per problem; 64 / 128: force the pixels per stage where the shape allows it
 static int g_wgrad_pix = 0;
 static bool wgrad_wants_pix128(const WgradParams&, int) {
-  // measured (profiles/r02_exp_ab.txt, interleaved A/B under the one-round split rule): 128-pixel
-  // stages wherever they fit (N tile <= 128) take 0.24 ms off the c3 step
+  // 128-pixel stages wherever they fit (N tile <= 128): twice the MMAs per barrier round trip
   return true;
 }
 

@@ -467,7 +467,7 @@ class Builder {
   }
 
   // dx = conv_transpose(dy) (+ add_src) (* relu mask).  bf16 mode fuses the accumulate / mask into the
-  // GEMM epilogue; fp32 mode (fp32 output straight from TMEM) runs them as one extra elementwise pass
+  // GEMM epilogue; fp32 mode (fp32 output straight from the accumulators) runs them as one extra elementwise pass
   void emit_dgrad(int dy, int w, int out, const Geom& g, int add, int mask, int64_t alg_macs) {
     const Val alg = alg_macs >= 0 ? vint(alg_macs) : Val();
     if (fp32_ && (add >= 0 || mask >= 0)) {
@@ -806,7 +806,7 @@ void Builder::run() {
     fail(ACNN_ERR_INVALID, "embedding_size must be a power of two between 32 and 2048 (tensor-core N tile, "
          "channel groups of the batch-norm kernels)");
   if (c.loss_type != "softmax")
-    fail(ACNN_ERR_UNSUPPORTED, "only the softmax loss is on the hot path (SURVEY 8a a11)");
+    fail(ACNN_ERR_UNSUPPORTED, "only the softmax loss is on the hot path");
   if (!c.anti_alias_type.empty() && (c.anti_alias_filter_size < 1 || c.anti_alias_filter_size > 7))
     fail(ACNN_ERR_INVALID, "anti_alias_filter_size must be in 1..7");
   if (c.resnet_version == 2 && (c.bl_alpha < 1 || c.bl_beta < 1 || (64 / c.bl_alpha) % 32))

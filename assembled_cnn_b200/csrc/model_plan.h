@@ -11,6 +11,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "common.h"
+
 #include <functional>
 #include <map>
 #include <string>
@@ -24,9 +26,9 @@ namespace model {
 
 constexpr int64_t kAlign = 256;   // every tensor of a flat buffer starts at a multiple of 256 elements
 // capacities (rows) of the per-CTA partial-sum buffers the reductions write
-constexpr int64_t kStatsPartsCap = 148;
-constexpr int64_t kBwdPartsCap = 296;
-constexpr int64_t kSgdScratch = 148 * 8 + 1;
+constexpr int64_t kStatsPartsCap = kMaxSms;
+constexpr int64_t kBwdPartsCap = 2 * kMaxSms;
+constexpr int64_t kSgdScratch = kMaxSms * 8 + 1;
 
 inline int64_t round_up(int64_t n, int64_t a = kAlign) { return (n + a - 1) / a * a; }
 

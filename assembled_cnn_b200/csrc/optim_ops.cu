@@ -253,14 +253,14 @@ int acnn_s2d_wgrad_unpack(const float* dw2, float* dw, int Cout, int k, int pad,
   return check_launch("s2d_wgrad_unpack");
 }
 
-int acnn_sgd_scratch_floats(void) { return 148 * 8 + 1; }
+int acnn_sgd_scratch_floats(void) { return acnn::kMaxSms * 8 + 1; }
 
 int acnn_sgd_momentum(float* w, const float* grad, float* acc, int64_t n,
                       const uint8_t* decay_flag, const float* hp, float* l2_acc, float* scratch,
                       void* stream) {
   ACNN_REQUIRE(w && grad && acc && decay_flag && hp && n % 256 == 0 && (!l2_acc || scratch),
                "sgd_momentum: bad arguments (n must be a multiple of 256; l2_acc needs scratch)");
-  launch_k(sgd_momentum_kernel, dim3(grid_for(n / 4, 256, 148 * 8)), dim3(256), 0,
+  launch_k(sgd_momentum_kernel, dim3(grid_for(n / 4, 256, acnn::kMaxSms * 8)), dim3(256), 0,
            (cudaStream_t)stream, w, grad, acc, n, decay_flag, hp, l2_acc, scratch);
   count_launch();
   return check_launch("sgd_momentum");

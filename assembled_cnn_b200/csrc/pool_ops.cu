@@ -31,14 +31,13 @@ __device__ __forceinline__ int reflect(int i, int n) {
 
 // ---------------------------------------------------------------------------- blur-pool
 // Every thread handles kBlurRows consecutive output rows of one (column, channel-group): the loads
-// of all its windows are independent and issued back to back (one row per thread measured 0.33-0.44
-// of the HBM peak forward and 0.07-0.14 backward: too little in flight per short-lived CTA).
+// of all its windows are independent and issued back to back (with one row per thread a short-lived
+// CTA keeps too little in flight to fill HBM).
 constexpr int kBlurRows = 4;
 
 // FS = filt * 8 + stride as a compile-time constant (0: runtime values): the reference's sconv / 3
 // configuration (filt 3, stride 2) gets shifts and fully unrolled windows instead of runtime
-// divisions and data-dependent loop bounds (the generic backward measured 0.07-0.14 of the HBM peak
-// with 5 % DRAM utilisation: integer-instruction bound)
+// divisions and data-dependent loop bounds (the generic backward is integer-instruction bound)
 template <class T, int FS>
 __global__ void __launch_bounds__(kPT)
 blurpool_fwd_kernel(const T* __restrict__ x, T* __restrict__ out, Binomial bw, int H, int W,
@@ -217,8 +216,8 @@ __device__ __forceinline__ int window_count(int p, int stride, int pad, int k, i
 // STRIDE > 0 makes the stride a compile-time constant (shifts instead of divisions).  Every thread
 // handles kRows consecutive rows of one (column, channel-group): the two full-size streams (add /
 // mask tiles) of all its rows are requested first (2 * kRows 16-byte loads in flight per thread),
-// the small dout gather (L2 hits) overlaps them.  (One vector per thread measured 2.2 TB/s: the
-// CTAs were too short-lived to keep the memory system full.)
+// the small dout gather (L2 hits) overlaps them.  (With one vector per thread the CTAs are too
+// short-lived to keep the memory system full.)
 constexpr int kPoolRows = 4;
 
 template <class T, int STRIDE>

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the conv GEMM kernels use:
-// mbarrier, TMA (tiled + im2col), tcgen05 (alloc / mma / commit / ld), fences.
+// Thin inline-PTX wrappers for the sm_90a features the conv GEMM kernels use:
+// mbarrier, TMA (tiled + im2col), wgmma (mma_async / commit / wait), fences.
 // Everything here is device-only and header-only.
 #pragma once
 #include <cuda.h>
@@ -96,12 +96,6 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
 }
 
 // ---------------------------------------------------------------- fences
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
@@ -197,113 +191,121 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory");
 }
 
-// ---------------------------------------------------------------- TMEM / tcgen05
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_dst)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+// ---------------------------------------------------------------- wgmma (sm_90a)
+// D[64 x N, registers of one warpgroup] (+)= A[smem, 64 x 16] * B[smem, 16 x N]; TA / TB = 1 for an
+// MN-major operand.  Accumulator fragment: register 4j + 2h + e of lane l in warp w of the group
+// holds row 16w + l/4 + 8h, column 8j + 2(l%4) + e.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
 }
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(COLS)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// Arrive on an mbarrier once every tcgen05.mma issued so far by this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-__device__ __forceinline__ void umma_commit_a(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar)
-      : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (lane == TMEM row).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<32> {
+  template <int TA, int TB>
+  __device__ static __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, %19, %20;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<64> {
+  template <int TA, int TB>
+  __device__ static __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, %35, %36;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<128> {
+  template <int TA, int TB>
+  __device__ static __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<256> {
+  template <int TA, int TB>
+  __device__ static __forceinline__ void mma(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, %131, %132;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
 
 // ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (sm_100 "version 1").  Offsets are in bytes here.
-//   layout_type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
+// Shared-memory matrix descriptor of wgmma (sm_90).  Offsets are in bytes here.
+//   layout_type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes,
                                                    uint32_t sbo_bytes, uint32_t layout_type) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(layout_type & 7) << 61;
+  d |= static_cast<uint64_t>(layout_type & 3) << 62;
   return d;
 }
 __host__ __device__ constexpr uint32_t swizzle_layout_type(int bytes) {
-  return bytes == 128 ? 2u : (bytes == 64 ? 4u : 6u);
-}
-// Instruction descriptor for kind::f16, BF16 x BF16 -> FP32, M = 128.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int n, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                        // D format  = F32
-         | (1u << 7)                      // A format  = BF16
-         | (1u << 10)                     // B format  = BF16
-         | ((a_mn_major ? 1u : 0u) << 15) // A major
-         | ((b_mn_major ? 1u : 0u) << 16) // B major
-         | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(128 >> 4) << 24);
+  return bytes == 128 ? 1u : (bytes == 64 ? 2u : 3u);
 }
 
-// Mixed-precision epilogue arithmetic on packed bf16 pairs (sm_100: FHADD.BF16 / FHFMA.BF16 /
-// HSET2.BF16_V2 -- one instruction per element where unpack + FADD / FFMA / FSETP + FSEL took two to
-// three).  Results are bit-identical to unpacking to fp32 first: the bf16 operand converts exactly
-// and the fp32 add / fma rounds once.
+// named barrier over `count` threads (the consumer warpgroups of a kernel)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory");
+}
+
+// Epilogue arithmetic on packed bf16 pairs: each bf16 half converts exactly to fp32 (a shift), the
+// fp32 add / fma rounds once.
+__device__ __forceinline__ float bf16_lo(uint32_t pair) { return __uint_as_float(pair << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t pair) { return __uint_as_float(pair & 0xffff0000u); }
 // c0 += lo(pair), c1 += hi(pair)
 __device__ __forceinline__ void bf16x2_add(float& c0, float& c1, uint32_t pair) {
-  asm("{\n\t.reg .b16 lo, hi;\n\t"
-      "mov.b32 {lo, hi}, %2;\n\t"
-      "add.f32.bf16 %0, lo, %0;\n\t"
-      "add.f32.bf16 %1, hi, %1;\n\t}\n"
-      : "+f"(c0), "+f"(c1)
-      : "r"(pair));
+  c0 += bf16_lo(pair);
+  c1 += bf16_hi(pair);
 }
 // (s0, q0) += (lo, lo^2), (s1, q1) += (hi, hi^2)
 __device__ __forceinline__ void bf16x2_sum_sq(float& s0, float& q0, float& s1, float& q1,
                                               uint32_t pair) {
-  asm("{\n\t.reg .b16 lo, hi;\n\t"
-      "mov.b32 {lo, hi}, %4;\n\t"
-      "add.f32.bf16 %0, lo, %0;\n\t"
-      "fma.rn.f32.bf16 %1, lo, lo, %1;\n\t"
-      "add.f32.bf16 %2, hi, %2;\n\t"
-      "fma.rn.f32.bf16 %3, hi, hi, %3;\n\t}\n"
-      : "+f"(s0), "+f"(q0), "+f"(s1), "+f"(q1)
-      : "r"(pair));
+  const float lo = bf16_lo(pair), hi = bf16_hi(pair);
+  s0 += lo;
+  q0 = __fmaf_rn(lo, lo, q0);
+  s1 += hi;
+  q1 = __fmaf_rn(hi, hi, q1);
 }
 // 0xffff in each half whose bf16 value is > 0 (false for -0, 0, NaN), else 0
 __device__ __forceinline__ uint32_t bf16x2_gt0_mask(uint32_t pair) {
@@ -322,10 +324,9 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 
 }  // namespace acnn
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster (ranks 2i, 2i+1 = one TPC) issue ONE tcgen05.mma of M = 256: each CTA holds
-// its own 128 rows of A and its own half of the B tile in shared memory and its own 128 lanes of
-// the accumulator in TMEM; only the even-rank ("leader") CTA issues the MMA.
+// ---------------------------------------------------------------- CTA pairs (clusters of two)
+// Two CTAs of a cluster share the weight tile of an N tile: each loads half of it and multicasts it
+// into both CTAs' shared memory; a stage is refilled once the consumers of BOTH CTAs released it.
 namespace acnn {
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -347,70 +348,16 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr)
                : "memory");
 }
-
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_dst)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(COLS)
-               : "memory");
-}
-
-// D[tmem, 256 rows over the CTA pair] (+)= A * B; issued by ONE thread of the leader CTA.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                               uint32_t idesc, uint32_t accumulate) {
+// 2-D tiled load written to the same shared-memory offset of every CTA in `mask`; each destination
+// CTA's mbarrier at the offset of `bar` receives the complete_tx of its copy
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t smem_dst, const CUtensorMap* m,
+                                                      uint32_t bar, int32_t c0, int32_t c1,
+                                                      uint16_t mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
-}
-// arrive on the barrier at the same shared-memory offset in BOTH CTAs of the pair once every MMA
-// issued so far has completed
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;\n" ::"r"(bar),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-// TMA loads of a CTA pair: `bar` is a shared::cluster address and may name the LEADER's barrier
-// (the leader's MMA thread waits for both CTAs' bytes on one barrier).
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t smem_dst, const CUtensorMap* m,
-                                                 uint32_t bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];\n" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_im2col_4d_pair(uint32_t smem_dst, const CUtensorMap* m,
-                                                        uint32_t bar, int32_t c, int32_t w,
-                                                        int32_t h, int32_t n, uint16_t off_w,
-                                                        uint16_t off_h) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};\n" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w),
-      "h"(off_h)
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16, BF16 x BF16 -> FP32 with an explicit M (128, or 256 for a
-// CTA pair).
-__host__ __device__ constexpr uint32_t make_idesc_bf16_m(int m, int n, bool a_mn_major,
-                                                         bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-         ((b_mn_major ? 1u : 0u) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 }  // namespace acnn

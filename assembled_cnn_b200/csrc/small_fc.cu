@@ -1,8 +1,8 @@
 // The tiny fully-connected layers of the SK / SE attention paths (<= 0.3 MMAC per image):
 // fp32 CUDA-core GEMMs on [B, <=2048] descriptors.  nets/blocks.py:136-151 (SK), :171-182 (SE).
 //
-// One shared-memory-tiled SGEMM (64x64x16 tile, 4x4 micro-tile per thread, split-K with fp32
-// atomics) serves all of them through generic element strides; the batch-norm-over-batch, gate and
+// One shared-memory-tiled SGEMM (64x64x16 tile, 4x4 micro-tile per thread, split-K with partials
+// summed in split order) serves all of them through generic element strides; the batch-norm-over-batch, gate and
 // activation glue are separate one-warp-per-channel / elementwise kernels.
 #include "common.h"
 #include "vec.cuh"
@@ -18,7 +18,7 @@ static int num_sms_small() {
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) {
       (void)cudaGetLastError();
-      return 148;        // no device (host-only sizing queries)
+      return 132;        // no device (host-only sizing queries): the H100 SXM's SM count
     }
     n = v;
   }
@@ -30,10 +30,11 @@ constexpr int kTM = 64, kTN = 64, kTK = 16;
 
 // C[M][N] (row-major, ldc = N) += sum_k A(m,k) * B(k,n)
 //   A(m,k) = A[m*sAm + k*sAk],  B(k,n) = B[k*sBk + n*sBn]
-// gridDim = (ceil(N/64), ceil(M/64), splits); every CTA atomically adds its partial tile.
+// gridDim = (ceil(N/64), ceil(M/64), splits).  part == nullptr (one split): the CTA adds its tile
+// to C; else split z stores its partial tile at part + z*M*N and sgemm_reduce_kernel adds them.
 __global__ void __launch_bounds__(kFT)
 sgemm_acc_kernel(const float* __restrict__ A, const float* __restrict__ B, float* C, int M, int N,
-                 int K, int sAm, int sAk, int sBk, int sBn, int k_per_split) {
+                 int K, int sAm, int sAk, int sBk, int sBn, int k_per_split, float* part) {
   pdl_entry();
   __shared__ float As[kTK][kTM + 4];
   __shared__ float Bs[kTK][kTN + 4];
@@ -88,13 +89,27 @@ sgemm_acc_kernel(const float* __restrict__ A, const float* __restrict__ B, float
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
-      if (n < N) atomicAdd(C + (size_t)m * N + n, acc[i][j]);
+      if (n >= N) continue;
+      if (part) part[((size_t)blockIdx.z * M + m) * N + n] = acc[i][j];
+      else C[(size_t)m * N + n] += acc[i][j];
     }
   }
 }
 
-// C (+)= A*B with split-K sized so that ~2 CTAs per SM are in flight.
-// det: no split-K -- every element of C receives exactly one add (bit-reproducible).
+// C[i] += sum over splits s (in order) of part[s][i]
+__global__ void __launch_bounds__(kFT)
+sgemm_reduce_kernel(const float* __restrict__ part, float* C, int64_t n, int splits) {
+  pdl_entry();
+  for (int64_t i = blockIdx.x * (int64_t)kFT + threadIdx.x; i < n; i += (int64_t)gridDim.x * kFT) {
+    float t = 0.f;
+    for (int s = 0; s < splits; ++s) t += part[s * n + i];
+    C[i] += t;
+  }
+}
+
+// C (+)= A*B with split-K sized so that ~2 CTAs per SM are in flight; the partials of a split-K
+// product are summed in split order (bit-reproducible).  det: no split-K -- every element of C
+// receives exactly one add.
 static int sgemm(const float* A, const float* B, float* C, int M, int N, int K, int sAm, int sAk,
                  int sBk, int sBn, bool zero_c, int det, cudaStream_t s) {
   if (zero_c) {
@@ -105,16 +120,36 @@ static int sgemm(const float* A, const float* B, float* C, int M, int N, int K, 
     }
   }
   const int tiles = ceil_div(M, kTM) * ceil_div(N, kTN);
-  int splits = ceil_div(296, tiles);
+  int splits = ceil_div(2 * num_sms_small(), tiles);
   const int max_splits = ceil_div(K, 2 * kTK);
   if (splits > max_splits) splits = max_splits;
   if (splits < 1 || det) splits = 1;
   int kps = ceil_div(ceil_div(K, splits), kTK) * kTK;
   splits = ceil_div(K, kps);
   dim3 grid(ceil_div(N, kTN), ceil_div(M, kTM), splits);
-  launch_k(sgemm_acc_kernel, dim3(grid), dim3(kFT), 0, s, A, B, C, M, N, K, sAm, sAk, sBk, sBn, kps);
+  if (splits == 1) {
+    launch_k(sgemm_acc_kernel, dim3(grid), dim3(kFT), 0, s, A, B, C, M, N, K, sAm, sAk, sBk, sBn, kps,
+             (float*)nullptr);
+    count_launch();
+    return check_launch("sgemm_acc");
+  }
+  // split-K partials in a stream-ordered scratch, then one ordered reduction into C
+  void* part = nullptr;
+  const int64_t n = (int64_t)M * N;
+  int rc = scratch_alloc(&part, (size_t)splits * n * sizeof(float), s, "sgemm");
+  if (rc) return rc;
+  launch_k(sgemm_acc_kernel, dim3(grid), dim3(kFT), 0, s, A, B, C, M, N, K, sAm, sAk, sBk, sBn, kps,
+           static_cast<float*>(part));
   count_launch();
-  return check_launch("sgemm_acc");
+  rc = check_launch("sgemm_acc");
+  if (rc == ACNN_OK) {
+    launch_k(sgemm_reduce_kernel, dim3(grid_for(n, kFT, 2 * num_sms_small())), dim3(kFT), 0, s,
+             static_cast<const float*>(part), C, n, splits);
+    count_launch();
+    rc = check_launch("sgemm_reduce");
+  }
+  const int rc2 = scratch_free(part, s, "sgemm");
+  return rc ? rc : rc2;
 }
 
 // One warp per channel j: batch-norm over the batch dimension, then ReLU.
@@ -246,17 +281,16 @@ static int ew(const float* in, const float* act, float* out, int64_t n, int mode
 // Fused SK attention chains: ONE cooperative launch per direction instead of 4 kernels + 2 memsets
 // (forward) / 6 kernels + 2 memsets (backward) per SK block -- 19 blocks per Assemble-ResNet-50
 // step, i.e. 266 of the step's ~1000 graph nodes, every one of them a few microseconds of launch
-// latency around almost no work.  The whole grid (<= 148 CTAs, all resident: cooperative launch)
+// latency around almost no work.  The whole grid (<= kMaxSms CTAs, all resident: cooperative launch)
 // walks the phases of the chain separated by grid barriers:
 //   * a GEMM phase deals (64x64 output tile, K split) units round-robin to the CTAs; every unit
 //     writes its partial tile to scratch (plain stores, one owner per element),
 //   * the consumer phase sums the partials in split order -- deterministic, nothing to zero, no
 //     atomics -- fused with whatever follows (batch-norm over the batch + ReLU, the 2-way softmax
 //     gate, the += into the gradient buffer).
-// (Round 2's first attempt ran the chain on ONE 8-CTA cluster without K splits: 5x slower than the
-// multi-launch path -- profiles/r02_exp_knobs.txt; the phases need the whole GPU, not a cluster.)
+// (One 8-CTA cluster without K splits would be too small: the phases need the whole GPU.)
 // ------------------------------------------------------------------------------------------
-constexpr int kGridMax = 148;      // scratch is sized for this many CTAs (plan.py mirrors it)
+constexpr int kGridMax = kMaxSms;  // scratch is sized for this many CTAs (plan.py mirrors it)
 constexpr int kMaxSplits = 8;
 
 struct GJob {
@@ -547,11 +581,10 @@ static int launch_coop(void (*kern)(const Args), const Args& a, int grid, cudaSt
 
 // -1 (default): the fused cooperative kernels when the caller asks for deterministic results (they
 // are bit-reproducible and need no zeroing; the multi-launch path then runs WITHOUT split-K),
-// otherwise the multi-launch split-K path; 0 / 1 force one of them.  MEASURED (c3 step, interleaved
-// A/B, profiles/r02_exp_ab.txt): fused 24.06 ms vs multi-launch 23.69 ms -- a grid barrier costs
-// about what a kernel boundary inside a CUDA graph costs (~2 us), so fusing the 10 launches of a
-// block into 2 only trades 8 boundaries for 7 barriers; the chain needs fewer PHASES, not fewer
-// launches, to get faster.
+// otherwise the multi-launch split-K path; 0 / 1 force one of them.  A grid barrier costs about
+// what a kernel boundary inside a CUDA graph costs, so fusing the 10 launches of a block into 2 only
+// trades 8 boundaries for 7 barriers; the chain needs fewer PHASES, not fewer launches, to get
+// faster.
 static int g_sk_fc_fused = -1;
 static bool use_fused(int deterministic) {
   return g_sk_fc_fused == 1 || (g_sk_fc_fused == -1 && deterministic);

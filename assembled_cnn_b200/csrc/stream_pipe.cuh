@@ -2,8 +2,8 @@
 //
 // A plain "load a few 16-byte vectors, compute, store" loop keeps only (resident threads x loads in
 // flight x 16 B) bytes in flight per SM, and the per-(image, channel) coefficient registers of the
-// SK kernels cap the residency at 512 threads: ~64 KiB in flight, gone to zero between trips, which
-// measured 30-50 % of the HBM roofline.  Here one thread per CTA streams the operand rows of the
+// SK kernels cap the residency at 512 threads: ~64 KiB in flight, gone to zero between trips, far
+// from what HBM needs.  Here one thread per CTA streams the operand rows of the
 // next trips into a ring of shared-memory stages with bulk asynchronous copies (cp.async.bulk,
 // completion on an mbarrier) while all threads compute on the current stage: the bytes in flight are
 // (stages - 1) x stage size x resident CTAs (~100-150 KiB per SM), independent of register use.

@@ -1,5 +1,5 @@
 """Data-parallel plumbing of the training step (the reference's MirroredStrategy,
-official/utils/misc/distribution_utils.py:24-76, SURVEY 3.4 / 8e), shared by the CUDA Trainer and
+official/utils/misc/distribution_utils.py:24-76), shared by the CUDA Trainer and
 by the CPU (gloo) tests so that both exercise the same code:
 
   * gradients: SUM over replicas of the flat fp32 gradient buffer, bucketed in reverse layer order

@@ -1,6 +1,6 @@
 """Flag names and defaults of the reference's model / training surface, as a plain dict.
 
-Only the flags the hot path consumes (SURVEY 8b); each entry cites where the reference defines it.
+Only the flags the hot path consumes; each entry cites where the reference defines it.
 `params_from_flags(**overrides)` builds the `params` dict that `model_fn_cls` receives from
 `nets/run_loop_classification.py:322-366`.
 """
@@ -42,7 +42,7 @@ DEFAULTS = {
     # official/utils/flags/_base.py:50-105, _performance.py:74-137
     "batch_size": 32,
     "train_epochs": 90,                   # main_classification.py:38
-    "dtype": "bf16",                      # reference enum is fp32|fp16; bf16 added (SURVEY 0.5)
+    "dtype": "bf16",                      # reference enum is fp32|fp16; bf16 added
     "loss_scale": 1,
     "data_format": "channels_last",       # NHWC is the only layout of this implementation
     "num_gpus": 1,

@@ -1,4 +1,4 @@
-"""The reference's operator surface for the hot path, executing on B200 through libacnn.so.
+"""The reference's operator surface for the hot path, executing on H100 through libacnn.so.
 
 Mirrors (same names, argument meaning and error behaviour):
   * functions/model_fns.py:138-198   Model(resnet_size, data_format, num_classes, ...)
@@ -31,8 +31,8 @@ from .native import NativeModel, NativeRuntime
 DEFAULT_VERSION = 1
 # dtype: 'bf16' = production path (bf16 storage, fp32 accumulation -- the analogue of the reference's
 # fp16 mode); 'fp32' = the reference's default (nets/resnet_model.py:30-33,
-# official/utils/flags/_performance.py:29-32): fp32 storage, 3-way bf16-split tcgen05 GEMMs,
-# bit-reproducible reductions -- the mode the 1e-3 parity tests run in.  'fp16' has no B200
+# official/utils/flags/_performance.py:29-32): fp32 storage, 3-way bf16-split wgmma GEMMs,
+# bit-reproducible reductions -- the mode the 1e-3 parity tests run in.  'fp16' has no H100
 # counterpart here (bf16 replaces it) and is rejected.
 ALLOWED_TYPES = ("bf16", "fp32")
 
@@ -387,8 +387,8 @@ class Trainer:
     def _fwd_bwd(self):
         rt = self.rt
         rt.run_forward()
-        # (a second stream for the wgrad GEMMs was measured to give nothing under a CUDA graph:
-        # every kernel already spans the GPU; Runtime.run(..., overlap_wgrad=True) keeps the option)
+        # (a second stream for the wgrad GEMMs: Runtime.run(..., overlap_wgrad=True); off by default,
+        # every kernel already spans the GPU)
         rt.run(rt.plan.backward, overlap_wgrad=os.environ.get("ACNN_OVERLAP_WGRAD", "0") == "1")
 
     def prefetch(self, images, labels):
@@ -484,7 +484,7 @@ class Trainer:
     # ---------------------------------------------------------------- data parallelism
     def sync_moving_statistics(self):
         """MirroredStrategy keeps the BN moving statistics as mirrored variables whose per-replica
-        updates are MEAN-aggregated (official/utils/misc/distribution_utils.py:24-45, SURVEY 3.4)."""
+        updates are MEAN-aggregated (official/utils/misc/distribution_utils.py:24-45)."""
         dp.average_moving_statistics(self.rt.state, self.world)
 
     def _fwd_bwd_allreduce(self):

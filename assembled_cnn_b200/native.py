@@ -265,7 +265,7 @@ def _runtime_base():
 
 
 class NativeRuntime(_runtime_base()):
-    """Executes a NativeModel on one B200 through acnn_bind / acnn_run_ops.  Same surface as
+    """Executes a NativeModel on one H100 through acnn_bind / acnn_run_ops.  Same surface as
     runtime.Runtime (params / state / grads / momentum / hp / t[name] / run(ops) / capture ...), so that
     Model, Trainer, checkpoint and the data-parallel schedule work on either; here every buffer of the
     step is a view into ONE workspace tensor laid out by the library, and run() is a loop inside
@@ -274,7 +274,7 @@ class NativeRuntime(_runtime_base()):
     def __init__(self, model: NativeModel, device="cuda:0", share: "NativeRuntime | None" = None):
         import torch
         if not torch.cuda.is_available():
-            raise _lib.AcnnError("assembled_cnn_b200.NativeRuntime needs a CUDA device (sm_100a); "
+            raise _lib.AcnnError("assembled_cnn_b200.NativeRuntime needs a CUDA device (sm_90a); "
                                  "there is no CPU fallback")
         self.lib = model.lib
         self.plan = self.model = model

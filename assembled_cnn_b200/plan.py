@@ -1,7 +1,7 @@
 """Layer plan of the assembled-ResNet hot path: a static list of kernel launches over named buffers.
 
 The reference builds a TF graph once and then runs `session.run(train_op)` per step
-(SURVEY 3.1); here the "graph" is this plan -- forward, backward and SGD ops in execution order over
+; here the "graph" is this plan -- forward, backward and SGD ops in execution order over
 statically shaped NHWC bf16 buffers -- built once by walking the same topology as
 nets/resnet_model.py:305-599 / functions/model_fns.py:98-198, and executed by runtime.py through
 the C ABI (optionally captured into one CUDA graph).
@@ -12,7 +12,7 @@ gradient through the consumers' fused epilogues (`add_src`), and the LAST contri
 the ReLU mask of the tensor (`mask_src`), so a gradient buffer always holds dL/d(pre-ReLU).
 
 Parameters are enumerated in the reference's variable creation order with TF-style names
-(SURVEY App. E); the flat fp32 master buffer stores conv kernels as OHWI ([Cout][kh][kw][Cin]).
+; the flat fp32 master buffer stores conv kernels as OHWI ([Cout][kh][kw][Cin]).
 """
 from __future__ import annotations
 
@@ -33,7 +33,7 @@ def _sk_job_floats(M, N, K, share):
     return -(-K // kper) * M * N
 
 
-def sk_fc_scratch_floats(B, f, d, G=148):
+def sk_fc_scratch_floats(B, f, d, G=132):
     """Mirror of acnn_sk_fc_scratch_floats (csrc/small_fc.cu; tests/test_abi_cpu.py compares them):
     da [B,2f] + dz [B,d] + the K-split partial tiles of the widest phase of the fused SK chains."""
     fwd = max(_sk_job_floats(B, d, f, G), _sk_job_floats(B, 2 * f, d, G))
@@ -44,9 +44,10 @@ def sk_fc_scratch_floats(B, f, d, G=148):
 
 # capacities (rows) of the per-CTA partial-sum buffers the reductions write (include/acnn.h:
 # acnn_conv_stats_parts / acnn_bn_bwd_reduce_parts / acnn_sk_bn_bwd_reduce_parts give the real counts)
-STATS_PARTS_CAP = 148
-BWD_PARTS_CAP = 296
-SGD_SCRATCH = 148 * 8 + 1
+# (the H100 SXM's 132 SMs: csrc/common.h kMaxSms)
+STATS_PARTS_CAP = 132
+BWD_PARTS_CAP = 2 * 132
+SGD_SCRATCH = 132 * 8 + 1
 
 
 def _round_up(n, a=ALIGN):
@@ -186,7 +187,7 @@ class ModelConfig:
             raise ValueError("embedding_size must be a power of two between 32 and 2048 (tensor-core N tile, "
                              "channel groups of the batch-norm kernels)")
         if self.loss_type != "softmax":
-            raise NotImplementedError("only the softmax loss is on the hot path (SURVEY 8a a11)")
+            raise NotImplementedError("only the softmax loss is on the hot path")
         if self.anti_alias_type and self.anti_alias_filter_size not in range(1, 8):
             raise ValueError("anti_alias_filter_size must be in 1..7")
         if self.resnet_version == 2 and (self.bl_alpha < 1 or self.bl_beta < 1 or (64 // self.bl_alpha) % 32):
@@ -612,7 +613,7 @@ class PlanBuilder:
 
     def emit_dgrad(self, dy, w, out, g, add, mask, alg_macs=None):
         """dx = conv_transpose(dy) (+ add_src) (* relu mask).  bf16 mode fuses the accumulate / mask
-        into the GEMM epilogue; fp32 mode (fp32 output straight from TMEM) runs them as one extra
+        into the GEMM epilogue; fp32 mode (fp32 output straight from the accumulators) runs them as one extra
         elementwise pass."""
         if self.fp32 and (add is not None or mask is not None):
             shape = self.plan.tensors[out].shape

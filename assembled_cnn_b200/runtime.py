@@ -1,4 +1,4 @@
-"""Executes a layer plan on one B200 through the C ABI (libacnn.so).
+"""Executes a layer plan on one H100 through the C ABI (libacnn.so).
 
 PyTorch is used only as the device-memory container (`torch.empty(..., device='cuda')`,
 `data_ptr()`), for streams and for CUDA-graph capture; every kernel on the path is ours.  There is
@@ -20,7 +20,7 @@ class Runtime:
     def __init__(self, plan: Plan, device="cuda:0", eps: float = 1e-5, share: "Runtime | None" = None,
                  deterministic: "bool | None" = None):
         if not torch.cuda.is_available():
-            raise _lib.AcnnError("assembled_cnn_b200.Runtime needs a CUDA device (sm_100a); "
+            raise _lib.AcnnError("assembled_cnn_b200.Runtime needs a CUDA device (sm_90a); "
                                  "there is no CPU fallback")
         self.lib = _lib.load()
         self.plan = plan
@@ -33,8 +33,9 @@ class Runtime:
         self.fp32 = plan.meta.get("dtype", "bf16") == "fp32"
         self.adt = 1 if self.fp32 else 0               # ACNN_F32 / ACNN_BF16
         self.planes = 3 if self.fp32 else 1
-        # deterministic: also the split-K of wgrad and of the small SK / SE GEMMs is disabled, so two
-        # runs are bit-identical (every other reduction of the library is ordered in both modes)
+        # deterministic: also the split-K of wgrad and of the small SK / SE GEMMs is disabled (one add
+        # per output element).  Every reduction is ordered in both modes (split-K partials are summed
+        # in split order), so two runs are bit-identical either way.
         self.det = int(self.fp32 if deterministic is None else bool(deterministic))
         f32 = dict(dtype=torch.float32, device=self.dev)
         if share is not None:

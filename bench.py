@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Benchmark of the assembled-ResNet training step on B200 (BASELINE.json's metric).
+"""Benchmark of the assembled-ResNet training step on one H100 (BASELINE.json's metric).
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...      # the reference's CPU path (oracle port) on host cores
+    python bench.py --dump-outputs DIR ...    # + what the last timed step computed, as DIR/<name>.npy
 
 One JSON line on stdout (rank 0).  A "step" = one full training step of Assemble-ResNet-50
 (resnet_version=2, SK, anti-alias sconv/3) on one synthetic batch: mixup type 1 -> forward -> label-
@@ -68,7 +69,8 @@ def read_peaks():
         with open(path) as fh:
             d = json.load(fh)
         return dict(tflops=d["bf16_tflops_sustained"], hbm=d["hbm_gbs"], source="measured")
-    return dict(tflops=1400.0, hbm=6650.0, source="fallback")   # B200_PROFILING.md fallback
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3; a 700 W card): an upper bound, not a measurement
+    return dict(tflops=989.0, hbm=3350.0, source="H100 SXM data sheet (dense bf16 peak, not a measurement)")
 
 
 class ClockSampler:
@@ -263,7 +265,7 @@ def cpu_baseline_subprocess(cfg_name, timeout_s=240):
 
 def run_reference_arm(args):
     """`--impl reference`: the reference's CPU path (oracle port) on the host cores, EXACTLY
-    --steps K timed steps after --warmup W, on the b200 arm's configuration / metric / unit; each
+    --steps K timed steps after --warmup W, on the GPU arm's configuration / metric / unit; each
     step is a bounded sample of the workload (a small CPU batch, shrunk further if a probe step says
     K + W steps would not end within a few minutes).  Rank 0 only."""
     rank = int(os.environ.get("RANK", "0"))
@@ -376,6 +378,9 @@ def main():
                     help="fp32 = the parity mode (not the metric's dtype; reported as such)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as "
+                         "DIR/<name>.npy (float32; fixed seeded samples of the large buffers)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -393,7 +398,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 path has no CPU fallback "
+        raise SystemExit("bench.py: no CUDA device; the GPU path has no CPU fallback "
                          "(use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     if world > 1:
@@ -456,7 +461,8 @@ def main():
     # launches of OUR kernels per step (counted on an eager step; graph replays re-issue them)
     was_graph = tr.use_graph
     tr.use_graph = False
-    dev_step_fn(x_dev, y_dev)                 # first call: one-time setup launches excluded
+    out_dev = dev_step_fn(x_dev, y_dev)       # first call: one-time setup launches excluded
+                                              # (every step writes its result to this buffer)
     torch.cuda.synchronize()
     c0 = lib.acnn_launch_count()
     dev_step_fn(x_dev, y_dev)
@@ -466,7 +472,8 @@ def main():
 
     # ---- device-resident arm -------------------------------------------------------------
     dev_step = lambda: dev_step_fn(x_dev, y_dev)
-    # a batch-1 forward touches ~100 MB (weights) < the 126 MB L2: flush L2 between iterations there
+    # a batch-1 forward touches ~100 MB (weights), comparable to the 50 MB L2: flush L2 between
+    # iterations there
     flush = None
     if cfg["kind"] == "eval":
         flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -475,12 +482,13 @@ def main():
     sampler.start()
     for _ in range(args.warmup):
         dev_step()
-    if world == 1:
+    if world == 1 and not args.dump_outputs:
         while sampler.proc is not None and not sampler.lines:  # keep the GPU loaded meanwhile
             dev_step()
             sampler.wait_first_sample(0.05)
     else:
-        # every rank must issue the same number of collectives: no data-dependent extra steps
+        # every rank must issue the same number of collectives (and a dump must come from the same
+        # step every run): no data-dependent extra steps
         sampler.wait_first_sample(3.0)
         for _ in range(args.warmup):
             dev_step()
@@ -502,6 +510,8 @@ def main():
         ms_total = sum(a.elapsed_time(b) for a, b in evs)
     clocks = sampler.stop()
     ms_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, cfg, rt, out_dev)
     value = B * world / (ms_step / 1e3)
 
     # ---- end-to-end arm: pinned host -> H2D -> step -> D2H result, every step -----------------
@@ -518,7 +528,7 @@ def main():
     e2e_value = B * world / (ms_e2e / 1e3)
     last = e2e_step()
 
-    # ---- roofline of the tcgen05 conv GEMMs, timed live (CUDA events around every launch) ---
+    # ---- roofline of the wgmma conv GEMMs, timed live (CUDA events around every launch) -----
     peaks = read_peaks()
     roof = None
     if rank == 0:
@@ -538,7 +548,7 @@ def main():
             "config": {"workload": cfg["workload"], "name": args.config,
                        "per_gpu_batch": B, "global_batch": B * world, "parallelism": "dp%d" % world,
                        "l2": ("L2 flushed (256 MiB write) between timed iterations" if flush else
-                              "per-step working set (activations + gradients, several GB) >> 126 MB L2"),
+                              "per-step working set (activations + gradients, several GB) >> 50 MB L2"),
                        "cuda_graph": tr.use_graph,
                        "executor": ("libacnn model-level C ABI (acnn_create / acnn_bind / acnn_run_ops)"
                                     if hasattr(rt.plan, "conv_info") else "python plan + per-op ctypes"),
@@ -552,7 +562,7 @@ def main():
                                    "achieved_tflops": gflop * value / 1e3,
                                    "peak_tflops": peaks["tflops"] * world,
                                    "frac": gflop * value / 1e3 / (peaks["tflops"] * world),
-                                   "peak_source": peaks["source"] + " bf16_tflops_sustained"},
+                                   "peak_source": peaks["source"] + (" bf16_tflops_sustained" if peaks["source"] == "measured" else "")},
             "roofline": roof,
             "cpu_baseline": cpu,
         }
@@ -563,8 +573,45 @@ def main():
         dist.destroy_process_group()
 
 
+DUMP_SAMPLE = 1 << 20      # elements of each sampled buffer (4 MiB of float32)
+
+
+def dump_outputs(path, cfg, rt, out):
+    """What the device-resident arm computed in its last timed step, as float32 .npy files: the
+    step's result (logits of an eval forward; the loss vector of a training-mode step), the logits
+    of a training-mode step, and for a training step fixed seeded samples of the updated parameters,
+    the gradients and the momentum buffer.  The inputs and the number of steps before the dump are
+    fixed by the arguments, so two builds can be compared file by file."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(path, exist_ok=True)
+    arrs = {}
+    if cfg["kind"] == "eval":
+        arrs["logits"] = out[:, :1001]
+    else:
+        arrs["loss"] = out
+        m = rt.plan.meta
+        if "logits" in m:
+            arrs["logits"] = rt.t[m["logits"]][:, :1001]
+    if cfg["kind"] == "train":
+        for name in ("params", "grads", "momentum"):
+            buf = getattr(rt, name, None)
+            if buf is None:
+                continue
+            flat = buf.reshape(-1)
+            g = torch.Generator().manual_seed(0)
+            n = min(DUMP_SAMPLE, flat.numel())
+            idx = torch.randperm(flat.numel(), generator=g)[:n].sort().values
+            arrs[name + "_sample"] = flat[idx.to(flat.device)]
+            arrs[name + "_sample_index"] = idx.double()
+    for name, a in arrs.items():
+        a = a.detach().float().cpu().numpy() if not name.endswith("_index") else a.numpy()
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def conv_roofline(tr, rt, step_fn, peaks, ms_step):
-    """Time every tcgen05 GEMM launch (fprop / dgrad / wgrad) of one eager step with CUDA events
+    """Time every wgmma GEMM launch (fprop / dgrad / wgrad) of one eager step with CUDA events
     on the launching stream; achieved = ALGORITHMIC FLOPs of those launches / their summed time.
     Work the implementation adds on top (the stem's K padded 147 -> 256 by the space-to-depth
     form, the stride-2 dgrads run on zero-inserted gradients) is reported separately as
@@ -636,25 +683,18 @@ def conv_roofline(tr, rt, step_fn, peaks, ms_step):
     alg_bytes = sum(e[3] for e in evs)
     executed = sum(e[4] for e in evs)
     achieved = fl / (t_ms / 1e3) / 1e12
-    # DRAM traffic of the same launches from the committed ncu launch list (profiles/): bytes per
-    # step over all tcgen05 launches, the same basis as `achieved`
+    # DRAM traffic needs a hardware-counter profile of the same launches: not measured here
     traffic, traffic_src = None, None
-    try:
-        tj = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles",
-                                         "conv_dram_traffic.json")))
-        if tj.get("launches") == len(evs):
-            traffic, traffic_src = tj["dram_bytes_per_step"], tj["source"]
-    except (OSError, ValueError, KeyError):
-        pass
     return {"bound": "tensor", "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s",
             "frac": achieved / peaks["tflops"], "traffic": traffic, "traffic_unit": "bytes per step "
-            "(dram__bytes_read+write summed over the same launches, ncu)", "traffic_source": traffic_src,
+            "(DRAM reads + writes of the same launches; needs hardware counters: not measured)", "traffic_source": traffic_src,
             "algorithmic_bytes_per_step": alg_bytes,
-            "kernel": "conv_gemm_kernel + conv_halo_kernel + wgrad_gemm_kernel (all %d tcgen05 launches of a step)" % len(evs),
+            "kernel": "conv_gemm_kernel + conv_halo_kernel + wgrad_gemm_kernel (all %d wgmma launches of a step)" % len(evs),
             "launch_ms_sum": t_ms, "share_of_step": t_ms / ms_step,
             "algorithmic_gflop_per_step": fl / 1e9,
             "executed_gflop_per_step": executed / 1e9,
-            "peak_source": peaks["source"] + " bf16_tflops_sustained (kernel timed inside a long step)"}
+            "peak_source": peaks["source"] + (" bf16_tflops_sustained" if peaks["source"] == "measured" else "") +
+                           " (kernel timed inside a long step)"}
 
 
 if __name__ == "__main__":

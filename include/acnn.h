@@ -1,5 +1,5 @@
 /*
- * acnn.h -- C ABI of libacnn.so: the B200 (sm_100a) kernels behind the assembled-ResNet hot path.
+ * acnn.h -- C ABI of libacnn.so: the H100 (sm_90a) kernels behind the assembled-ResNet hot path.
  *
  * The reference (clovaai/assembled-cnn) has no FFI layer: every op below is a TensorFlow-1.14 graph
  * op emitted by the reference's Python.  Each entry point cites the reference call site it replaces
@@ -42,45 +42,33 @@ int acnn_version(void);
 /* Number of kernels this library has launched since load (bench.py's gpu_launches). */
 int64_t acnn_launch_count(void);
 /* Programmatic dependent launch (no effect on results): 0 (default) = plain stream order, 1 = every
- * kernel (measured slower on the full step), 2 = only light dependents (<= 320 CTAs, <= 48 KiB
+ * kernel, 2 = only light dependents (<= 320 CTAs, <= 48 KiB
  * shared memory).  Returns the previous setting. */
 int acnn_set_pdl(int on);
-/* Tuning knob of the conv GEMM launcher (no effect on results): M tiles (128 output pixels each)
- * per CTA tile.  -1 = choose per problem (default), 1 = always one, 2 = two wherever the shape
- * allows it (N tile <= 128).  Returns the previous mode. */
-int acnn_set_conv_mtiles(int mode);
-/* 1 (default): the N = 256 conv tiles with K >= 512 run on CTA pairs (tcgen05 cta_group::2: a cluster
- * of two CTAs computes one 256 x 256 tile, each staging half of the weight tile); 0: single-CTA tiles.
- * Results are bit-identical; changes acnn_conv_stats_parts().  Returns the previous setting. */
+/* 1: the N = 128 conv tiles with 64-channel chunks, K >= 512 and at least one 256-row tile per SM
+ * pair run on CTA pairs (a cluster of two CTAs computes one 256 x 128 tile; each CTA loads half of
+ * every weight stage and multicasts it to both); 0 (default): single-CTA tiles (measured faster on
+ * the c3 step: 61.3 against 80.3 ms on an H100 SXM at 700 W).  Results are bit-identical; changes
+ * acnn_conv_stats_parts().  Returns the previous setting. */
 int acnn_set_conv_cta_pairs(int on);
 /* 3x3 / stride 1 / pad 1 convolutions (fprop and dgrad) on the im2col-free "halo" kernel: a CTA tile
  * is a 16 x 8 patch of output pixels, one 18 x 10 halo tile per 64-channel chunk is loaded once and
- * the nine filter taps read shifted windows of it through the tensor core's shared-memory
- * descriptors.  0 = off (im2col TMA kernel everywhere); 1 (default) = where it pays (the weight slab
- * of an N tile fits shared memory next to the halo ring, Cin a multiple of 64, >= 56 rows);
- * 2 = wherever it applies.  Same results up to fp32 summation order of the statistics; changes
- * acnn_conv_stats_parts().  Returns the previous setting. */
+ * the nine filter taps read shifted windows of it through the wgmma shared-memory descriptors.
+ * 0 = off (im2col TMA kernel everywhere); 1 (default) = where the weight slab of an N tile fits
+ * shared memory next to the halo ring, Cin a multiple of 64 and >= 56 rows (c3 step on an H100 SXM
+ * at 700 W: 59.8 against 61.3 ms with 0); 2 = wherever it applies.
+ * Same results up to fp32 summation order; changes acnn_conv_stats_parts().  Returns the previous
+ * setting. */
 int acnn_set_conv_halo(int mode);
-/* Halo kernel epilogue at N <= 64 (no effect on results beyond fp32 summation order of the
- * statistics): 1 (default) = two independent 4-warp groups alternate tiles (own accumulator stage,
- * staging buffers, named barrier and TMA store queue), 0 = all 8 warps on one tile at a time.
- * Returns the previous setting. */
+/* Conv tuning knobs of earlier kernel generations, kept for ABI compatibility: M tiles per CTA
+ * tile, the split epilogues (conv GEMM and halo kernel) and the number of output staging buffers.
+ * The sm_90a kernels have one organisation (one 128-pixel M tile per CTA, two wgmma consumer
+ * warpgroups that run the epilogue from their registers, one output staging buffer): each setter
+ * stores its value, returns the previous one and changes nothing else. */
+int acnn_set_conv_mtiles(int mode);
 int acnn_set_conv_halo_split(int on);
-/* Epilogue organisation of the conv GEMM kernel (one-M-tile, single-CTA tiles with bf16 output; no
- * effect on results beyond fp32 summation order of the statistics): 0 = all 8 epilogue warps on one
- * tile at a time; 1 (default) = two independent 4-warp groups alternate tiles where the epilogue
- * chain paces the tile (K <= 256) and shared memory holds the doubled staging; 2 = wherever it fits.
- * Returns the previous setting. */
 int acnn_set_conv_split_epilogue(int mode);
-/* The same for CTA tiles of two M tiles (N <= 128): the two groups drain the two M tiles of every tile
- * concurrently.  0 = off, 1 (default) = where K <= 256, 2 = wherever the doubled staging fits with a
- * ring of >= 3 stages.  Returns the previous setting. */
 int acnn_set_conv_split_mt2(int mode);
-/* Output staging buffers of the conv GEMM epilogue (no effect on results): 1 (default) = one half-
- * tile buffer; 0 = a second one where the shared-memory ring stays deep enough without its bytes
- * (all of K in flight or >= 4 stages), so that a half tile's TMA store drains under the next
- * half's TMEM reads (measured: no difference on the c3 step); 2 = two wherever they fit.  Returns
- * the previous setting. */
 int acnn_set_conv_out_bufs(int mode);
 /* Tuning knob of the wgrad launcher (no effect on results beyond fp32 summation order): pixels
  * (GEMM K) per pipeline stage, 64 or 128 (N tile <= 128 only); 0 = choose per problem (default).
@@ -88,21 +76,21 @@ int acnn_set_conv_out_bufs(int mode);
 int acnn_set_wgrad_pixels(int pix);
 /* Tuning knob of the wgrad launcher's split-K choice (no effect on results beyond fp32 summation
  * order): the fixed cost of one CTA (pipeline fill + atomic epilogue) in pipeline stages used by the
- * cost model that picks the number of pixel splits (default 16); 0 = the round-1 "two waves of CTAs"
+ * cost model that picks the number of pixel splits (default 16); 0 = the "two waves of CTAs"
  * rule.  Returns the previous setting. */
 int acnn_set_wgrad_overhead_stages(int stages);
 /* Tuning knob: the largest grid (CTAs) of the grid-stride elementwise kernels (bn_act, bn_bwd_apply,
- * ...); no effect on results.  Values below 148 restore the default.  Returns the previous setting. */
+ * ...); no effect on results.  Values below 132 restore the default (16 x 132).  Returns the previous setting. */
 int acnn_set_stream_grid_cap(int blocks);
 /* SK attention chains (acnn_sk_fc_fwd / acnn_sk_fc_bwd): 1 = ONE cooperative launch per direction
  * (the whole grid walks GEMM / batch-norm / gate phases separated by grid barriers; K-split partials
  * summed in split order: deterministic, no atomics, nothing to zero); 0 = the multi-launch path (4 + 6
  * kernels and 4 memsets per SK block; split-K with atomics unless deterministic); -1 (default) = fused
- * when the call asks for deterministic results, multi-launch otherwise (measured 0.37 ms per c3 step
- * faster than fused).  Same results up to fp32 summation order.  Returns the previous setting. */
+ * when the call asks for deterministic results, multi-launch otherwise.
+ * Same results up to fp32 summation order.  Returns the previous setting. */
 int acnn_set_sk_fc_fused(int on);
 /* floats of the `scratch` argument of acnn_sk_fc_fwd / acnn_sk_fc_bwd (da [B,2f] + dz [B,d] + the
- * K-split partial tiles of the widest phase, sized for 148 CTAs; callable without a GPU) */
+ * K-split partial tiles of the widest phase, sized for 132 CTAs; callable without a GPU) */
 int64_t acnn_sk_fc_scratch_floats(int B, int f, int d);
 
 /* Convolution geometry (correlation, no bias) -- nets/model_helper.py:67-78 conv2d_fixed_padding
@@ -117,7 +105,7 @@ typedef struct acnn_conv_geom {
   int32_t x_pix_stride, x_row_pitch, x_img_pitch, reserved_;
 } acnn_conv_geom;
 
-/* y[B,Ho,Wo,Cout] = conv(x[B,H,W,Cin], w[Cout,kh,kw,Cin])  as a tcgen05 implicit GEMM
+/* y[B,Ho,Wo,Cout] = conv(x[B,H,W,Cin], w[Cout,kh,kw,Cin])  as a wgmma implicit GEMM
  * (tf.layers.conv2d: nets/model_helper.py:74-78; tf.layers.dense: nets/resnet_model.py:595-597
  * when kh=kw=H=W=1).  Optional fused epilogue, applied in this order:
  *   + bias[Cout] (fp32)            -> dense bias
@@ -132,14 +120,14 @@ typedef struct acnn_conv_geom {
  * precision 0: x, w bf16.  precision 1 (fp32 parity mode): x and w are each three consecutive bf16
  * planes hi / mid / lo of an fp32 tensor (acnn_split3, acnn_prep_weights(planes = 3)); plane p of x
  * starts at x + p * numel(x), plane p of w at w + p * w_plane_stride elements; the six significant
- * cross products accumulate in the fp32 TMEM accumulator; requires out_f32 and no add / mask /
+ * cross products accumulate in fp32 register accumulators; requires out_f32 and no add / mask /
  * statistics epilogue. */
 int acnn_conv_fprop(const acnn_conv_geom* g, const void* x, const void* w, void* y,
                     float* ch_part, const void* add_src, const void* mask_src,
                     const float* bias, int out_f32, int precision, int64_t w_plane_stride,
                     void* stream);
 /* Rows of the partial statistics buffer acnn_conv_fprop(g, ..., ch_part, ...) writes (a pure
- * function of the geometry and the device's SM count; <= 148). */
+ * function of the geometry and the device's SM count; <= 132). */
 int acnn_conv_stats_parts(const acnn_conv_geom* g);
 
 /* dx[B,H,W,Cin] = conv_transpose(dy[B,Ho,Wo,Cout]) for a stride-1 conv of geometry g (the backward
@@ -151,9 +139,11 @@ int acnn_conv_dgrad(const acnn_conv_geom* g, const void* dy, const void* w_dgrad
                     const void* add_src, const void* mask_src, int precision,
                     int64_t w_plane_stride, void* stream);
 
-/* dw[Cout,kh,kw,Cin] (fp32) += sum_pixels x (*) dy  -- weight gradient, split-K over pixels with
- * fp32 atomics; dw must be zeroed (or hold the running sum) by the caller.  deterministic != 0:
- * no split (one add per element: bit-reproducible).  precision 1: x and dy are 3-plane operands. */
+/* dw[Cout,kh,kw,Cin] (fp32) += sum_pixels x (*) dy  -- weight gradient, split-K over pixels: the
+ * splits store partial tiles in a stream-ordered scratch of the launch (cudaMallocAsync on `stream`)
+ * and the last split of a tile adds them to dw in split order (bit-reproducible).  dw must be zeroed
+ * (or hold the running sum) by the caller.  deterministic != 0: no split (one add per element).
+ * precision 1: x and dy are 3-plane operands. */
 int acnn_conv_wgrad(const acnn_conv_geom* g, const void* x, const void* dy, float* dw,
                     int precision, int deterministic, void* stream);
 /* planes bf16 [3][n] = (hi, mid, lo) of x fp32 [n], x = hi + mid + lo to 24 bits (n % 8 == 0). */

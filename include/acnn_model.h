@@ -1,5 +1,5 @@
 /*
- * acnn_model.h -- MODEL-LEVEL C ABI of libacnn.so (SURVEY 8(b)): the whole assembled-ResNet training /
+ * acnn_model.h -- MODEL-LEVEL C ABI of libacnn.so: the whole assembled-ResNet training /
  * inference step behind one handle.  acnn.h is the op level (one entry point per TF graph op the
  * reference emits); this header is the level a host in any language binds when it wants the reference's
  * `Model(...)` + `model(inputs, training)` + `resnet_model_fn` TRAIN branch as a drop-in:
@@ -23,7 +23,9 @@
  *
  * Every call returns 0 or an ACNN_ERR_* code (acnn_last_error() has the text), never throws across
  * the ABI, only ENQUEUES on `stream` (a cudaStream_t passed as void*), performs no hidden
- * synchronisation or allocation after acnn_bind(), and is CUDA-graph capturable (inputs are read from
+ * synchronisation after acnn_bind(), allocates nothing but the stream-ordered split-K scratch of the
+ * wgrad / small GEMM launches (cudaMallocAsync / cudaFreeAsync on `stream`: per stream, and graph
+ * memory nodes under capture), and is CUDA-graph capturable (inputs are read from
  * the static input buffers inside the workspace; hyper-parameters from the device vector `hp`).
  * One host thread per handle; the calling thread's current CUDA device must be the one that owns the
  * bound buffers (one process per GPU sets it once).  acnn_create() needs no GPU (the layer plan is host

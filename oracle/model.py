@@ -16,7 +16,7 @@ functions/model_fns.py:98-198 (topology constants), nets/run_loop_classification
 assembly) and nets/optimizer_setting.py:23-38 (momentum step) on top of oracle/tf_ops.py.
 Gradients come from torch autograd over this forward.
 
-Variables are created in the reference's program order with TF-style names (SURVEY App. E); kernels
+Variables are created in the reference's program order with TF-style names; kernels
 are HWIO, dense kernel [in, out] -- the "TF layout" that the product's set_weights() consumes.
 """
 from __future__ import annotations
@@ -373,7 +373,7 @@ def train_step(model, vs, momentum_buf, images, onehot, *, lr, momentum=0.9, use
                label_smoothing=0.0, weight_decay=0.0, n_replicas=1, teacher_labels=None,
                kd_temp=0.0, keep_prob=1.0, dropblock_u=None):
     """One full training step on one replica (or the average over `n_replicas` shards of the batch,
-    each with its own BN statistics: MirroredStrategy semantics, SURVEY 3.4).  Updates vs.vars and
+    each with its own BN statistics: MirroredStrategy semantics).  Updates vs.vars and
     momentum_buf in place; returns dict(loss, cross_entropy, l2_loss, logits, grads)."""
     names = [n for n in vs.vars if vs.trainable[n]]
     shards = images.shape[0] // n_replicas

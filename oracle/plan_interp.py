@@ -1,7 +1,7 @@
 """CPU interpreter of the product's layer plan (assembled_cnn_b200/plan.py) in plain torch.
 
 TEST INFRASTRUCTURE ONLY (see oracle/tf_ops.py header).  It gives every op kind of the plan an
-independent reference meaning (explicit backward formulas of SURVEY App. C, written with torch ops,
+independent reference meaning (explicit backward formulas, written with torch ops,
 adjoints taken by autograd where that is the definition), so that
 
   * on CPU, the whole plan -- topology, gradient accumulation, parameter order -- is checked

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generates tests/golden/oracle_digests.json: digests of the oracle's outputs under fixed seeds.
 
-The reference ships no golden vectors for this path (SURVEY 4) and TensorFlow 1.14 cannot be run
+The reference ships no golden vectors for this path and TensorFlow 1.14 cannot be run
 here, so these fixtures pin the ORACLE (oracle/model.py) against silent change; they use the
 reference's own digest convention (official/utils/testing/reference_data.py:105-124:
 shape, first, last, sum).  Re-run only when the oracle is intentionally changed:

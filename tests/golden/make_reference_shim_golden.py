@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Golden vectors produced by EXECUTING the reference's own model code (nets/resnet_model.py,
-nets/blocks.py, nets/model_helper.py under /root/reference) through the TF-1.14 API stand-in in
-tests/golden/tf1_shim/ (TensorFlow itself cannot be installed here).  Run in the build container:
+nets/blocks.py, nets/model_helper.py of a checkout of the original project) through the TF-1.14 API
+stand-in in tests/golden/tf1_shim/ (TensorFlow 1.14 has no Python 3.12 build):
 
-    python tests/golden/make_reference_shim_golden.py            # rewrites reference_shim_golden.json
+    python tests/golden/make_reference_shim_golden.py REFERENCE_DIR   # rewrites reference_shim_golden.json
 
 What a golden entry holds, per model configuration: the variable names / shapes / initializer kinds in
 the reference's creation order (a digest + the count), and for seeded inputs and seeded variable
 values the logits in training and in inference mode plus digests of the updated BN moving statistics.
 tests/test_reference_shim_golden_cpu.py replays the oracle on the same seeds against this file; it
-does not need /root/reference.
+does not need the original project.
 
 The stand-in computes in float64 (TF_SHIM_FLOAT64=1, set below) with kernels that are not the oracle's
 (Hugging Face's TF-'SAME' padding port, ATen batch norm: see the stand-in's docstring): the golden
@@ -32,6 +32,8 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT = os.path.join(HERE, "reference_shim_golden.json")
+# checkout of the original project whose code is executed (first argument)
+REF_ROOT = None     # set from the command line (the module is also imported by the tests)
 
 # configuration name -> (constructor flags of functions/model_fns.py:Model, use_resnet_d, batch, size)
 CONFIGS = {
@@ -55,7 +57,7 @@ CONFIGS = {
                                                     bl_alpha=1, bl_beta=2), False, 4, 64),
     # (batch 4 for the 152-layer nets: on a batch of 2 the SK-attention batch norms see two samples and
     # the training-mode logits are chaotic even in float64 -- a 1e-14 input perturbation moves them 8 %)
-    # SURVEY 8(f) rows: GeM pooling + embedding head, flatten pooling (nets/resnet_model.py:552-599)
+    # GeM pooling + embedding head, flatten pooling (nets/resnet_model.py:552-599)
     "assemble_r50_gem_embedding256": (dict(resnet_size=50, resnet_version=2, use_sk_block=True,
                                            anti_alias_type="sconv", anti_alias_filter_size=3,
                                            pool_type="gem", embedding_size=256), False, 4, 64),
@@ -119,7 +121,7 @@ def reference_function(rel_path, name):
     import ast
     sys.path.insert(0, os.path.join(HERE, "tf1_shim"))
     import tensorflow as tf
-    src = open(os.path.join("/root/reference", rel_path)).read()
+    src = open(os.path.join(REF_ROOT, rel_path)).read()
     # (ast.walk: also finds functions nested inside other functions, e.g. exclude_batch_norm)
     node = next(n for n in ast.walk(ast.parse(src)) if isinstance(n, ast.FunctionDef) and n.name == name)
     ns = {"tf": tf}
@@ -155,7 +157,7 @@ def reference_if_blocks(rel_path, func_name, test_src):
     import ast
     sys.path.insert(0, os.path.join(HERE, "tf1_shim"))
     import tensorflow as tf
-    src = open(os.path.join("/root/reference", rel_path)).read()
+    src = open(os.path.join(REF_ROOT, rel_path)).read()
     fn = next(n for n in ast.walk(ast.parse(src)) if isinstance(n, ast.FunctionDef) and n.name == func_name)
     blocks = sorted((n for n in ast.walk(fn) if isinstance(n, ast.If) and ast.unparse(n.test) == test_src),
                     key=lambda n: n.lineno)            # source order (ast.walk is breadth-first)
@@ -165,7 +167,7 @@ def reference_if_blocks(rel_path, func_name, test_src):
 
 def run_reference(flags, use_resnet_d, batch, size):
     sys.path.insert(0, os.path.join(HERE, "tf1_shim"))
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REF_ROOT)
     import tensorflow as tf          # the shim
     from nets import resnet_model   # the REAL reference code
     f = dict(flags)
@@ -266,7 +268,7 @@ def run_reference_c3_composition():
     utils/data_util.mixup(keep_batch_size=False) on images and one-hot labels -> Assemble-ResNet-50 in
     training mode -> losses/cls_losses.get_sup_loss with label smoothing 0.1; gradients by autograd."""
     sys.path.insert(0, os.path.join(HERE, "tf1_shim"))
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REF_ROOT)
     import tensorflow as tf
     from nets import resnet_model
     flags, d, _, _ = CONFIGS["assemble_r50_rv2_sk_sconv"]
@@ -302,7 +304,7 @@ def run_reference_c3_composition():
 
 def run_reference_dropblock(flags, batch, size, keep_prob):
     sys.path.insert(0, os.path.join(HERE, "tf1_shim"))
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REF_ROOT)
     import tensorflow as tf
     from nets import resnet_model
     f = dict(flags)
@@ -417,7 +419,7 @@ def reference_flag_defaults():
     (literal defaults only)."""
     import ast
     out = {}
-    tree = ast.parse(open("/root/reference/nets/hparams_config.py").read())
+    tree = ast.parse(open(os.path.join(REF_ROOT, "nets", "hparams_config.py")).read())
     for node in ast.walk(tree):
         if isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and \
                 node.func.attr.startswith("DEFINE_"):
@@ -517,7 +519,7 @@ def run_train_pieces():
     # nets/run_loop_classification.py:126-130: the `predictions` dict (classes / probabilities /
     # probabilities_sigmoid), the assignment statement executed from the source
     import ast
-    src = open("/root/reference/nets/run_loop_classification.py").read()
+    src = open(os.path.join(REF_ROOT, "nets", "run_loop_classification.py")).read()
     fn = next(n for n in ast.walk(ast.parse(src)) if isinstance(n, ast.FunctionDef) and n.name == "resnet_model_fn")
     node = next(n for n in ast.walk(fn) if isinstance(n, ast.Assign) and getattr(n.targets[0], "id", "") == "predictions")
     logits, _ = loss_inputs()
@@ -553,6 +555,10 @@ def run_train_pieces():
 
 
 if __name__ == "__main__":
+    if len(sys.argv) != 2 or not os.path.isdir(os.path.join(sys.argv[1], "nets")):
+        sys.exit("usage: python tests/golden/make_reference_shim_golden.py REFERENCE_DIR\n"
+                 "  REFERENCE_DIR: a checkout of clovaai/assembled-cnn (the directory holding nets/)")
+    REF_ROOT = os.path.abspath(sys.argv[1])
     gold = {"train_pieces": run_train_pieces()}
     print("train pieces:", sorted(gold["train_pieces"]))
     for name, (flags, d, b, s) in CONFIGS.items():

@@ -1,9 +1,8 @@
 """A minimal eager stand-in for the TensorFlow 1.14 API surface that the reference's model-building
 code touches (nets/resnet_model.py, nets/blocks.py, nets/model_helper.py), backed by torch on CPU.
 
-TEST INFRASTRUCTURE ONLY (used by tests/golden/make_reference_shim_golden.py, here, in the build
-container, where /root/reference is mounted).  TensorFlow 1.14 cannot be installed (no Python 3.12
-wheel, no network), so the reference's own Python — topology, scopes, variable names, padding
+TEST INFRASTRUCTURE ONLY (used by tests/golden/make_reference_shim_golden.py with a checkout of the
+original project).  TensorFlow 1.14 has no Python 3.12 wheel, so the reference's own Python — topology, scopes, variable names, padding
 choices, block order — is EXECUTED through this shim to produce golden vectors that pin the oracle.
 What the shim pins and what it does not:
   * pinned: everything the reference's Python decides (which ops, in which order, with which

@@ -33,8 +33,8 @@ def test_build_and_symbols():
     assert ctypes.sizeof(_lib.ConvGeom) == 64 and ctypes.sizeof(_lib.WeightDesc) == 40
 
 
-def test_sass_uses_tcgen05_and_tma():
-    """The conv kernels really are tcgen05/TMA code (B200_PROFILING.md SASS mnemonics)."""
+def test_sass_uses_wgmma_and_tma():
+    """The conv kernels really are wgmma/TMA code (sm_90a SASS mnemonics)."""
     from assembled_cnn_b200 import _lib
     cuobjdump = "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
@@ -42,10 +42,10 @@ def test_sass_uses_tcgen05_and_tma():
     sass = subprocess.run([cuobjdump, "-sass", os.path.join(ROOT, "assembled_cnn_b200", "build",
                                                              "gemm.o")],
                           capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass          # tcgen05.mma kind::f16
-    assert "LDTM" in sass             # tcgen05.ld
+    assert "HGMMA" in sass            # wgmma.mma_async (bf16 -> fp32)
     assert "UTMALDG" in sass          # TMA tensor loads (tiled + im2col)
-    assert "HGMMA" not in sass and "HMMA.16816" not in sass   # no legacy tensor path
+    assert "UTMASTG" in sass          # TMA tensor stores of the staged epilogue tiles
+    assert "HMMA.16816" not in sass   # no legacy (mma.sync) tensor path
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
@@ -77,7 +77,7 @@ def test_model_argument_errors_match_reference():
 
 def test_flag_defaults_match_reference():
     from assembled_cnn_b200.hparams import DEFAULTS, params_from_flags
-    # nets/hparams_config.py / official/utils/flags defaults (SURVEY 8b)
+    # nets/hparams_config.py / official/utils/flags defaults
     assert DEFAULTS["resnet_version"] == 1 and DEFAULTS["bl_alpha"] == 2 and DEFAULTS["bl_beta"] == 4
     assert DEFAULTS["weight_decay"] == 4e-5 and DEFAULTS["momentum"] == 0.9
     assert DEFAULTS["bn_momentum"] == 0.997 and DEFAULTS["label_smoothing"] == 0.0

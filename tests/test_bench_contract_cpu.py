@@ -1,5 +1,5 @@
-"""CPU-side checks of bench.py's launch contract (the timed arms themselves need a B200 / minutes of
-host time; their JSON lines are kept under profiles/)."""
+"""CPU-side checks of bench.py's launch contract (the timed arms themselves need an H100 / minutes of
+host time; their JSON lines are kept under tests/golden/bench_lines/)."""
 import json
 import os
 import subprocess
@@ -33,11 +33,11 @@ def test_b200_arm_has_no_cpu_fallback():
     assert "no CPU fallback" in (r.stderr + r.stdout)
 
 
-@pytest.mark.parametrize("name", ["r01_bench_final.json", "r01_bench_reference_arm_final.json",
-                                  "r01_bench_dp2_final.json"])
+@pytest.mark.parametrize("name", ["h100_bench_c3.json", "bench_reference_arm_c3.json"])
 def test_committed_bench_lines_follow_the_contract(name):
-    """The lines the last GPU run produced (profiles/) carry every key the driver reads."""
-    path = os.path.join(ROOT, "profiles", name)
+    """Recorded bench.py lines (one H100 run of the GPU arm, one run of the CPU reference arm) carry
+    every key a consumer of the result line reads."""
+    path = os.path.join(ROOT, "tests", "golden", "bench_lines", name)
     line = json.loads(open(path).read().strip().splitlines()[-1])
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step",
               "higher_is_better", "scaling", "vs_baseline", "dtype", "data", "config", "e2e"):

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM convolutions (through the C ABI) against the CPU oracle.
+"""GPU parity of the wgmma implicit-GEMM convolutions (through the C ABI) against the CPU oracle.
 
 Inputs are bf16-representable, so the only differences are fp32 accumulation order and the final
 bf16 rounding of the output: tolerance = 2^-8 relative to the tensor's max magnitude for bf16
@@ -45,10 +45,10 @@ def _relerr(a, b):
 
 @pytest.fixture(autouse=True, params=[0, 2], ids=["epi_joint", "epi_split"])
 def conv_split_epilogue(request, lib):
-    """Every test of this file under both epilogue organisations of conv_gemm_kernel
-    (acnn_set_conv_split_epilogue / acnn_set_conv_split_mt2: 0 = all 8 warps on one tile, 2 = two
-    4-warp groups -- alternating tiles, or one M tile each of a two-M-tile CTA tile -- wherever the
-    doubled staging fits)."""
+    """Every test of this file under both values of acnn_set_conv_split_epilogue /
+    acnn_set_conv_split_mt2.  They select epilogue organisations of earlier kernel generations; the
+    sm_90a kernels accept and ignore them, and these runs check that neither setting changes a
+    result."""
     prev = lib.acnn_set_conv_split_epilogue(request.param)
     prev2 = lib.acnn_set_conv_split_mt2(request.param)
     yield request.param
@@ -58,7 +58,9 @@ def conv_split_epilogue(request, lib):
 
 @contextlib.contextmanager
 def _mtiles(lib, mode):
-    """acnn_set_conv_mtiles: 2 forces two 128-pixel M tiles per CTA tile wherever legal."""
+    """acnn_set_conv_mtiles (M tiles per CTA tile in earlier kernel generations; accepted and ignored
+    by the sm_90a kernels, which run one 128-pixel M tile per CTA: both settings must give the same
+    results)."""
     prev = lib.acnn_set_conv_mtiles(mode)
     try:
         yield
@@ -103,7 +105,7 @@ def test_fprop_matches_oracle(lib, case, mt):
     st = torch.cuda.current_stream().cuda_stream
     with _mtiles(lib, mt):
         parts = lib.acnn_conv_stats_parts(g)
-        assert 1 <= parts <= 148
+        assert 1 <= parts <= 132
         # partial (sum, sumsq) rows: poisoned first -- the kernel must STORE every row it owns
         sp = torch.full((parts, 2, Cout), float("nan"), device="cuda")
         _lib.check(lib.acnn_conv_fprop(g, xd.data_ptr(), wd.data_ptr(), yd.data_ptr(),
@@ -125,9 +127,8 @@ def test_fprop_matches_oracle(lib, case, mt):
 @pytest.mark.parametrize("mt", MT, ids=MT_IDS)
 @pytest.mark.parametrize("cout", [64, 128])
 def test_many_tiles_per_cta(lib, mt, cout):
-    """392 M tiles (196 double tiles): every persistent CTA walks several tiles, the smem ring
-    wraps many times and both TMEM accumulator stages are reused; with add + mask epilogue tiles
-    (which at N = 128 forces the single-M-tile kernel even in mode 2)."""
+    """392 M tiles: every persistent CTA walks several tiles, the smem ring wraps many times and the
+    register accumulators are reused tile after tile; with add + mask epilogue tiles."""
     from assembled_cnn_b200 import _lib
     B, H, W, Cin, Cout = 16, 56, 56, 64, cout
     g = _geom(B, H, W, Cin, Cout, 3, 1)
@@ -263,7 +264,7 @@ def test_large_shapes_linearity(lib):
 
 # ---------------------------------------------------------------------------------------------
 # fp32 parity mode: operands split into three bf16 planes (acnn_split3), six cross products in the
-# fp32 TMEM accumulator.  Inputs are full-precision fp32; tolerance 5e-6 relative to the output's
+# fp32 accumulator.  Inputs are full-precision fp32; tolerance 5e-6 relative to the output's
 # max magnitude against an fp64 oracle (the tensor core's fp32 accumulation truncates: measured
 # 1-3e-6 at K = 2304; fp32 rounding of the result itself is 6e-8).
 # ---------------------------------------------------------------------------------------------
@@ -332,7 +333,7 @@ def test_fp32_mode_fprop_dgrad_wgrad(lib, case):
 
 
 # ---------------------------------------------------------------------------------------------
-# CTA pairs (tcgen05 cta_group::2) for the N = 256 tiles: acnn_set_conv_cta_pairs(1)
+# CTA pairs (clusters of two sharing the weight stages by TMA multicast): acnn_set_conv_cta_pairs(1)
 # ---------------------------------------------------------------------------------------------
 @contextlib.contextmanager
 def _pairs(lib, on):
@@ -344,10 +345,10 @@ def _pairs(lib, on):
 
 
 PAIR_CASES = [
-    # B, H, W, Cin, Cout, k   (M / 256 * Cout / 256 >= 74 pair tiles, 64-channel chunks)
+    # B, H, W, Cin, Cout, k   (64-channel chunks; pairs where K >= 512 and the pair tiles fill the GPU)
     (64, 28, 28, 64, 256, 1),       # 1x1, one k-block, 196 pair tiles
     (16, 28, 28, 256, 512, 1),      # 1x1, K = 256, two N tiles
-    (37, 14, 14, 128, 256, 3),      # 3x3 im2col, ragged M (7252 = 28.3 pair tiles... x1 -> below 74: single-CTA path)
+    (37, 14, 14, 128, 256, 3),      # 3x3 im2col, ragged M (7252 = 28.3 pair tiles x 2 N tiles: single-CTA path)
     (64, 14, 14, 128, 512, 3),      # 3x3 im2col, 49 pair tiles x 2 N tiles
     (50, 20, 20, 64, 256, 3),       # ragged: M = 20000 (78.1 pair tiles), tiles cross image borders
 ]
@@ -416,7 +417,7 @@ HALO_CASES = [
 
 @pytest.fixture(params=[1, 0], ids=["split_epilogue", "joint_epilogue"])
 def halo_split(request, lib):
-    """Both epilogue organisations of the halo kernel at N <= 64 (acnn_set_conv_halo_split)."""
+    """Both settings of acnn_set_conv_halo_split (one epilogue organisation on sm_90a)."""
     prev = lib.acnn_set_conv_halo_split(request.param)
     yield request.param
     lib.acnn_set_conv_halo_split(prev)
@@ -443,7 +444,7 @@ def test_halo_kernel_fprop_dgrad_match_oracle_and_im2col(lib, case, halo_split):
     for mode in (0, 2, 2):
         with _halo(lib, mode):
             parts = lib.acnn_conv_stats_parts(g)
-            assert 1 <= parts <= 148
+            assert 1 <= parts <= 132
             sp = torch.full((parts, 2, Cout), float("nan"), device="cuda")
             y = torch.full((B, H, W, Cout), float("nan"), dtype=torch.bfloat16, device="cuda")
             y2 = torch.full((B, H, W, Cout), float("nan"), dtype=torch.bfloat16, device="cuda")

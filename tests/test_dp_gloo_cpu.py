@@ -3,7 +3,7 @@ its shard (torch interpreter standing in for the kernels) and drives the SAME da
 Trainer.train_step (assembled_cnn_b200/dp.py): the backward cut into segments, each followed by the
 sum-all-reduce of its gradient bucket, the 1/N folded into the SGD step, and the mean aggregation of
 the BN moving statistics.  The result must equal the oracle's MirroredStrategy semantics
-(per-replica BN statistics, averaged gradients, averaged moving statistics; SURVEY 3.4 /
+(per-replica BN statistics, averaged gradients, averaged moving statistics;
 official/utils/misc/distribution_utils.py:24-76)."""
 import os
 import socket
@@ -14,7 +14,7 @@ import torch.multiprocessing as mp
 
 KW = dict(resnet_size=50, resnet_version=2, use_sk_block=True, anti_alias_type="sconv",
           anti_alias_filter_size=3)
-HW, B_LOCAL, WORLD = 64, 4, 2   # >= 4 samples per BN everywhere (SURVEY 8d: B=2 degenerates)
+HW, B_LOCAL, WORLD = 64, 4, 2   # >= 4 samples per BN everywhere (B=2 degenerates)
 
 
 def _free_port():

@@ -3,7 +3,7 @@
 reproduce the oracle's MirroredStrategy semantics -- oracle.model.train_step(n_replicas=2): per-replica
 BN statistics, averaged gradients, averaged moving statistics (official/utils/misc/
 distribution_utils.py:24-76).  fp32 mode, so the comparison is tight.  With >= 2 GPUs
-(`gpurun --gpus 2`) the ranks sit on their own GPUs under NCCL; on a one-GPU box both ranks share
+(two GPUs) the ranks sit on their own GPUs under NCCL; on a one-GPU box both ranks share
 cuda:0 and the collectives go over gloo (CUDA tensors) -- the same Trainer schedule either way."""
 import os
 import socket
@@ -38,7 +38,7 @@ def _worker(rank, port, out_path, use_graph):
     import torch.distributed as dist
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
-    # two GPUs: NCCL, one rank per GPU.  One GPU (the driver's test box): the SAME Trainer code path
+    # two GPUs: NCCL, one rank per GPU.  One GPU: the SAME Trainer code path
     # (bucketed, overlapped all-reduce between the backward segments / CUDA graphs, mean of the moving
     # statistics) with both ranks on cuda:0 over gloo, which accepts CUDA tensors
     two = torch.cuda.device_count() >= 2

@@ -1,4 +1,4 @@
-"""CPU checks of the SURVEY 8(f) rows (no GPU): the layer plan of DropBlock, the KD loss term, GeM /
+"""CPU checks of the extra features (no GPU): the layer plan of DropBlock, the KD loss term, GeM /
 flatten pooling and the embedding head against the autograd oracle (float64, 1e-6); the ECE metric;
 checkpoint naming, the warm-start filter and the best-checkpoint keeper; the data-parallel bucket
 schedule."""

@@ -1,4 +1,4 @@
-"""GPU checks of the SURVEY 8(f) rows through the public surface (Model / Trainer / model_fn_cls):
+"""GPU checks of the extra features through the public surface (Model / Trainer / model_fn_cls):
 DropBlock with the device RNG, the KD loss term, the embedding head, checkpoint round trips and the
 EVAL-mode loss / metrics.  The kernels themselves are pinned op by op in tests/test_plan_gpu.py
 (test_feature_rows_lockstep)."""

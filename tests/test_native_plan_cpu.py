@@ -345,7 +345,7 @@ def test_native_and_python_plans_refuse_the_same_flag_sets(case):
 
 def test_op_conv_info_gives_the_algorithmic_flops_of_the_survey():
     """acnn_op_conv_info (what bench.py's roofline reads): geometry of every GEMM op of the library's C3
-    plan equals the Python plan's, and the ALGORITHMIC multiply-accumulates add up to SURVEY 8(d)'s
+    plan equals the Python plan's, and the ALGORITHMIC multiply-accumulates add up to the
     34.12 GFLOP per image for the Assemble-ResNet-50 training step (11.45 forward), while the executed
     ones are higher (space-to-depth stem, zero-inserted stride-2 dgrads)."""
     B = 8
@@ -369,7 +369,7 @@ def test_op_conv_info_gives_the_algorithmic_flops_of_the_survey():
             executed += ex
             fwd += macs if nop.phase == 0 else 0
             n += 1
-    assert n == 230                                           # tcgen05 launches of a step
+    assert n == 230                                           # conv GEMM launches of a step
     gflop = 2.0 * alg / B / 1e9
     assert abs(gflop - 34.12) < 0.15 and abs(2.0 * fwd / B / 1e9 - 11.45) < 0.1, (gflop, fwd)
     assert executed > alg

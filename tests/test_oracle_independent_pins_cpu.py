@@ -1,4 +1,4 @@
-"""Independent pins of the TF-1.14 KERNEL semantics the oracle restates (SURVEY 8c / App. B).
+"""Independent pins of the TF-1.14 KERNEL semantics the oracle restates.
 
 TensorFlow is not installable here (no wheel for this interpreter, no network), so the oracle cannot be
 run against the reference's own kernels.  Besides the hand-computed vectors of

@@ -1,5 +1,5 @@
 """Known-answer micro-vectors that pin the oracle to the TF-1.14 semantics the reference relies on
-(SURVEY App. B).  The reference ships no tests for this path and TensorFlow 1.14 cannot be installed,
+.  The reference ships no tests for this path and TensorFlow 1.14 cannot be installed,
 so these hand-computed vectors are one of three pins of the TF kernel semantics (see the header of
 oracle/tf_ops.py): the others are third-party implementations rule by rule
 (tests/test_oracle_independent_pins_cpu.py) and the reference's own model code executed on third-party
@@ -170,7 +170,7 @@ def test_learning_rate_schedules():
 
 
 def test_parameter_inventory_matches_survey():
-    """SURVEY App. E totals: trainable tensors / parameters / BN layers per configuration."""
+    """Totals: trainable tensors / parameters / BN layers per configuration."""
     cases = [
         (dict(resnet_size=50, resnet_version=1), False, 161, 25_559_081, 53),
         (dict(resnet_size=50, resnet_version=2, use_sk_block=True, anti_alias_type="sconv",

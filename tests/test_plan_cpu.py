@@ -73,7 +73,7 @@ def _check_train_step(kw, d, mix, hw, B, plan_dtype):
         assert any(o.kind == "bn_stats" for o in plan.forward)
         assert all(t.dtype != "bf16" or n.startswith("planes") for n, t in plan.tensors.items())
     names = [n for n in vs.vars if vs.trainable[n]]
-    # same variables, same creation order, same TF-style names (SURVEY App. E)
+    # same variables, same creation order, same TF-style names
     assert names == list(plan.params)
     assert [n for n in vs.vars if not vs.trainable[n]] == list(plan.state)
     for n, p in plan.params.items():
@@ -122,7 +122,7 @@ def test_bench_model_inventory():
     cfg = ModelConfig(**ASSEMBLE)
     plan = build_plan(cfg, 8, 224, 224, training=True, mixup_type=1, label_smoothing=0.1)
     convs = [o for o in plan.forward if o.kind == "conv"]
-    assert len(convs) == 76 + 1                       # 76 spatial convs + dense (SURVEY App. A.2)
+    assert len(convs) == 76 + 1                       # 76 spatial convs + dense
     assert sum(1 for o in plan.forward if o.kind == "sk_fc") == 19
     assert sum(1 for o in plan.forward if o.kind == "blurpool") == 6
     assert sum(1 for o in plan.forward if o.kind == "avgpool") == 6
@@ -133,12 +133,12 @@ def test_bench_model_inventory():
     macs = sum(o.geom.B * o.geom.Ho * o.geom.Wo * o.geom.Cout * o.geom.kh * o.geom.kw * o.geom.Cin
                for o in convs)
     # stem runs as a 4x4x16 space-to-depth conv (256 instead of 147 MACs per output) -- a little
-    # more than the reference's 5.726 GMAC/img (SURVEY App. D)
+    # more than the reference's 5.726 GMAC/img
     assert 5.7e9 < macs / 8 < 5.9e9
 
 
 def test_assemble_r152_inventory():
-    """BASELINE config 5: Assemble-ResNet-152 (rv=2, bl_alpha=1, bl_beta=2): SURVEY App. A.3."""
+    """BASELINE config 5: Assemble-ResNet-152 (rv=2, bl_alpha=1, bl_beta=2)."""
     cfg = ModelConfig(resnet_size=152, resnet_version=2, use_sk_block=True, anti_alias_type="sconv",
                       anti_alias_filter_size=3, bl_alpha=1, bl_beta=2)
     plan = build_plan(cfg, 2, 224, 224, training=True, mixup_type=1)
@@ -158,7 +158,7 @@ def test_flag_validation_errors_match_reference():
         ModelConfig(resnet_size=77).validate()
     with pytest.raises(NotImplementedError):
         ModelConfig(pool_type="max").validate()
-    ModelConfig(pool_type="gem", embedding_size=256).validate()      # SURVEY 8(f) rows: supported
+    ModelConfig(pool_type="gem", embedding_size=256).validate()      # supported
     with pytest.raises(ValueError):
         ModelConfig(embedding_size=100).validate()
 

@@ -7,7 +7,7 @@ Tolerances (relative to the output's max magnitude): bf16 tensors 2^-7 (one bf16
 of the range: accumulation-order differences can flip a rounding), fp32 vectors 2e-3 where sums
 of bf16 data cancel (BN backward sums), 1e-4 otherwise.
 
-The fp32 parity mode (dtype='fp32': fp32 storage, 3-plane tcgen05 GEMMs) runs the same lock-step
+The fp32 parity mode (dtype='fp32': fp32 storage, 3-plane wgmma GEMMs) runs the same lock-step
 against the exact fp32 interpreter with every tensor at 2e-5 and the reductions at 2e-4.
 """
 import os
@@ -238,7 +238,7 @@ def test_train_step_lockstep_fp32_mode(name):
 
 
 FEATURE_CONFIGS = {
-    # SURVEY 8(f) rows: GeM pooling + embedding head + KD (mixup 2: the teacher-label quirk);
+    # GeM pooling + embedding head + KD (mixup 2: the teacher-label quirk);
     # flatten pooling + KD in the fp32 mode; DropBlock on both block kinds (needs 224 px: the
     # stage-4 feature map must be >= the 7 x 7 block)
     "gem_embedding_kd_mix2": dict(cfg=dict(pool_type="gem", embedding_size=64, resnet_size=50,

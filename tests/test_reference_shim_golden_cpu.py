@@ -1,7 +1,7 @@
 """The oracle against golden vectors produced by RUNNING THE REFERENCE'S OWN MODEL CODE
 (nets/resnet_model.py + nets/blocks.py + nets/model_helper.py) through a TF-1.14 API stand-in
-(tests/golden/tf1_shim, generator tests/golden/make_reference_shim_golden.py; executed in the build
-container where /root/reference is mounted -- this test only reads the committed json).
+(tests/golden/tf1_shim, generator tests/golden/make_reference_shim_golden.py, run against a checkout
+of the original project -- this test only reads the committed json).
 
 Pinned: variable names / shapes / initializer kinds / creation order of 9 model configurations
 (including the Assemble-ResNet-50 of the north star, ResNet-D, SE, proj anti-alias, zero-gamma, R101,
@@ -533,7 +533,7 @@ def test_native_plan_inventory_matches_reference_code(name):
 
 
 # ---------------------------------------------------------------------------------------------
-# SURVEY 8(f) rows against the reference's own code: DropBlock, GeM pooling, KD teacher mixup
+# The feature rows against the reference's own code: DropBlock, GeM pooling, KD teacher mixup
 # (the GeM / embedding / flatten model configurations are part of mg.CONFIGS above)
 # ---------------------------------------------------------------------------------------------
 def test_gem_pooling_matches_reference_code():

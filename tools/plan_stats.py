@@ -2,9 +2,9 @@
 """Static figures of the layer plans the library builds (acnn_create: host logic, no GPU needed) for the
 BASELINE configurations: variables, ops per phase, GEMM ops, algorithmic / executed GFLOP per image
 (acnn_op_conv_info), device memory of one replica (flat buffers + workspace) and the largest per-GPU batch
-that fits 180 GB of HBM3e.
+that fits 76 GB of the H100's 80 GB of HBM3 (the rest left to the CUDA context and allocator).
 
-    python tools/plan_stats.py > profiles/r02_plan_stats.md
+    python tools/plan_stats.py
 """
 import os
 import sys
@@ -38,7 +38,7 @@ def device_bytes(nm):
 
 print("# Layer plans of the BASELINE configurations (built by acnn_create; `tools/plan_stats.py`)\n")
 print("| configuration | variables (trainable elems) | ops fwd / bwd / update | GEMM ops | algorithmic / executed "
-      "GFLOP per image | flat buffers | workspace | largest batch in 180 GB |")
+      "GFLOP per image | flat buffers | workspace | largest batch in 76 GB |")
 print("|---|---:|---:|---:|---:|---:|---:|---:|")
 for label, flags, B, kw in CASES:
     nm = native.NativeModel(ModelConfig(**flags), B, 224, 224, **kw)
@@ -55,7 +55,7 @@ for label, flags, B, kw in CASES:
     flat, ws = device_bytes(nm)
     # the workspace grows linearly with the batch (activations / gradients); the flat buffers do not
     per_img = ws / B
-    fit = int((180e9 - flat) / per_img)
+    fit = int((76e9 - flat) / per_img)
     print("| %s | %d (%.2f M) | %d / %d / %d | %d | %.2f / %.2f | %.2f GB | %.2f GB | %d |" % (
         label, s.n_variables, s.param_elems / 1e6, s.n_forward, 0 if fwd_only else s.n_backward,
         0 if fwd_only else s.n_update, n,

@@ -38,7 +38,7 @@ dx = torch.empty_like(x)
 dw = torch.zeros(a.Cout, a.k, a.k, a.Cin, device=dev)
 s1 = torch.zeros(a.Cout, device=dev)
 s2 = torch.zeros(a.Cout, device=dev)
-sp = torch.zeros(148, 2, a.Cout, device=dev)     # partial BN statistics rows
+sp = torch.zeros(lib.acnn_conv_stats_parts(g), 2, a.Cout, device=dev)     # partial BN statistics rows
 st = torch.cuda.current_stream().cuda_stream
 flops = 2.0 * a.B * Ho * Wo * a.Cout * a.k * a.k * a.Cin
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Launch the HBM-bound pooling kernels of the north star (blur-pool forward / backward, global average
 pool forward / backward, the SK block's pooled descriptor, the BigLittle 3x3/2 average pool) once each
-at their Assemble-ResNet-50 B=256 shapes, for `ncu --set full -k regex:...` (tools/calls/call19.sh), and
+at their Assemble-ResNet-50 B=256 shapes, for a kernel profiler, and
 print their CUDA-event times with the algorithmic GB/s (tensors read + written, bf16)."""
 import os
 import sys
@@ -57,7 +57,7 @@ for HW, f in ((3136, 64), (784, 128), (196, 256)):
                                                                   s.data_ptr(), B, HW, f, 0, st))
 
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-peak = 6585.8
+peak = 3350.0     # GB/s: H100 SXM data sheet (HBM3)
 once = os.environ.get("ACNN_PROFILE_ONCE") == "1"     # under ncu: warm-up + ONE profiled launch per job
 for name, nbytes, fn in jobs:
     _lib.check(fn(), name)                      # warm-up (first-launch attributes)

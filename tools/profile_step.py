@@ -81,7 +81,7 @@ for op, a, b in records:
         byt = 2.0 * (nin + nout)
         if op.kind == "conv_dgrad":
             byt += 2.0 * nin * ((op.add_src is not None) + (op.mask_src is not None))
-        ideal = max(fl / 1423.5e9, byt / 6572.9e6)          # ms: tensor vs HBM roofline
+        ideal = max(fl / 989e9, byt / 3350e6)   # ms: tensor vs HBM roofline (H100 SXM data sheet)
         rows.append((ms, op.kind, "%dx%d %d->%d k%d s%d" % (g.H, g.W, g.Cin, g.Cout, g.kh, g.stride),
                      fl / ms / 1e9, ideal))
 total = sum(v[0] for v in by_kind.values())
