@@ -14,6 +14,8 @@
 // Reference semantics: nets/model_helper.py:67-78 (conv2d_fixed_padding), tf.gradients backward.
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "common.h"
 #include "ptx.cuh"
 
@@ -1193,8 +1195,11 @@ static int g_num_sms = 0;
 static int num_sms() {
   if (g_num_sms == 0) {
     int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+      (void)cudaGetLastError();   // no device (host-only queries): size for the H100's kMaxSms
+      g_num_sms = 0;
+    }
     // at most kMaxSms: the partial statistics rows (one per CTA of an N tile) are sized for it
     if (g_num_sms <= 0 || g_num_sms > kMaxSms) g_num_sms = kMaxSms;
   }
@@ -1580,13 +1585,91 @@ static int g_wgrad_overhead_stages = 16;
 constexpr size_t kWgPartFloats = size_t(16) << 20;
 constexpr int kWgCounters = 1 << 16;
 
+// 0: the cost model picks the split count; n > 0: n splits, within the capacity caps
+// (acnn_set_wgrad_splits)
+static int g_wgrad_splits = 0;
+
+// 0: choose per problem; 64 / 128: force the pixels per stage where the shape allows it
+static int g_wgrad_pix = 0;
+static bool wgrad_wants_pix128(int) {
+  // 128-pixel stages wherever they fit (N tile <= 128): twice the MMAs per barrier round trip
+  return true;
+}
+
+// Tiling and split-K layout of one wgrad launch: a pure host function of the geometry, the
+// precision, `deterministic`, the tuning knobs and the SM count, shared by the launcher and
+// acnn_conv_wgrad_plan.
+struct WgradPlan {
+  int P;                 // pixels (GEMM K)
+  int bn;                // N tile
+  int n_tiles, m_tiles;
+  int pix;               // pixels per pipeline stage
+  int stages_total;
+  int splits;            // CTAs along the pixel range
+  int stages_per_split;  // every split but the last runs this many stages
+};
+
+static int wgrad_plan(const acnn_conv_geom& g, int precision, int deterministic, WgradPlan* w) {
+  ACNN_REQUIRE(g.Cin % 16 == 0 && g.Cout % 32 == 0, "wgrad: Cin %% 16 / Cout %% 32 required");
+  ACNN_REQUIRE(precision == 0 || precision == 1, "wgrad: precision must be 0 (bf16) or 1 (fp32)");
+  int Ho, Wo;
+  ACNN_REQUIRE(out_hw(g, &Ho, &Wo), "wgrad: empty output");
+  const int np = precision ? 3 : 1;
+  w->P = g.B * Ho * Wo;
+  int bn = g.Cout >= 256 ? 256 : (g.Cout >= 128 ? 128 : (g.Cout >= 64 ? 64 : 32));
+  if (np == 3 && bn > 128) bn = 128;   // three operand planes per stage: smem
+  ACNN_REQUIRE(g.Cout % bn == 0, "wgrad: Cout=%d not a multiple of its N tile %d", g.Cout, bn);
+  w->bn = bn;
+  w->n_tiles = g.Cout / bn;
+  w->m_tiles = ceil_div(g.kh * g.kw * g.Cin, 128);
+  // 128-pixel stages: only the bf16 path, N tile <= 128 (smem), enough pixels to split
+  w->pix = kWgPix;
+  if (np == 1 && bn <= 128 && w->P >= 4096 &&
+      (g_wgrad_pix == 128 || (g_wgrad_pix == 0 && wgrad_wants_pix128(bn))))
+    w->pix = 128;
+  w->stages_total = ceil_div(w->P, w->pix);
+  // split the pixel (K) range over CTAs; the partial tiles are summed in split order, so the result
+  // does not depend on which split finishes first.  deterministic: no split -- one add per dw
+  // element.  One CTA per SM (384 threads with register accumulators).
+  const int tiles = w->m_tiles * w->n_tiles;
+  // capacity: the partial tiles of all splits fit kWgPartFloats, one arrival counter per tile
+  const int64_t tile_floats = (int64_t)tiles * 128 * bn;
+  int cap = (int)std::min<int64_t>(w->stages_total, (int64_t)kWgPartFloats / tile_floats);
+  if (cap < 1 || tiles > kWgCounters) cap = 1;
+  const int max_splits = std::min(cap, w->stages_total >= 8 ? w->stages_total / 4 : 1);
+  int splits;
+  if (g_wgrad_splits > 0) {
+    splits = std::min(g_wgrad_splits, cap);
+  } else if (g_wgrad_overhead_stages <= 0) {
+    // (simple rule: roughly two waves of CTAs)
+    splits = std::min(ceil_div(2 * num_sms(), tiles), max_splits);
+  } else {
+    // cost model: an SM runs its CTAs' pipeline stages back to back and pays a fixed pipeline-fill
+    // + epilogue cost, worth g_wgrad_overhead_stages stages, once per CTA; pick the split count
+    // with the least modelled time
+    splits = 1;
+    int64_t best = -1;
+    for (int s = 1; s <= max_splits; ++s) {
+      const int per = ceil_div(w->stages_total, s);
+      const int s_eff = ceil_div(w->stages_total, per);
+      if (s_eff != s) continue;
+      const int per_sm = ceil_div(tiles * s, num_sms());
+      const int64_t t = (int64_t)per_sm * per + (int64_t)per_sm * g_wgrad_overhead_stages;
+      if (best < 0 || t < best) { best = t; splits = s; }
+    }
+  }
+  if (splits < 1 || deterministic) splits = 1;
+  w->stages_per_split = ceil_div(w->stages_total, splits);
+  w->splits = ceil_div(w->stages_total, w->stages_per_split);
+  return ACNN_OK;
+}
+
 template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX = kWgPix>
-static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int deterministic,
+static int launch_wgrad(const WgradMaps& tm, WgradParams p, int m_tiles, int n_tiles,
                         cudaStream_t stream) {
   using Cfg = WgradCfg<BN, NP, PIX>;
   static bool attr_set = false;
   auto kern = wgrad_gemm_kernel<BN, CW, CWB, IM2COL, NP, PIX>;
-  const int m_tiles = ceil_div(p.Ktot, 128);
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
@@ -1596,39 +1679,8 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int det
     }
     attr_set = true;
   }
-  // split the pixel (K) range over CTAs; the partial tiles are summed in split order, so the result
-  // does not depend on which split finishes first.  deterministic: no split -- one add per dw
-  // element.  One CTA per SM (384 threads with register accumulators).
   const int tiles = m_tiles * n_tiles;
-  int max_splits = p.stages_total >= 8 ? p.stages_total / 4 : 1;
-  const int64_t tile_floats = (int64_t)tiles * 128 * BN;
-  if ((int64_t)max_splits * tile_floats > (int64_t)kWgPartFloats)
-    max_splits = (int)(kWgPartFloats / tile_floats);
-  if (max_splits < 1 || tiles > kWgCounters) max_splits = 1;
-  int splits;
-  if (g_wgrad_overhead_stages <= 0) {
-    // (simple rule: roughly two waves of CTAs)
-    splits = ceil_div(2 * num_sms(), tiles);
-  } else {
-    // cost model: an SM runs its CTAs' pipeline stages back to back and pays a fixed pipeline-fill
-    // + epilogue cost, worth g_wgrad_overhead_stages stages, once per CTA; pick the split count
-    // with the least modelled time
-    splits = 1;
-    int64_t best = -1;
-    for (int s = 1; s <= max_splits; ++s) {
-      const int per = ceil_div(p.stages_total, s);
-      const int s_eff = ceil_div(p.stages_total, per);
-      if (s_eff != s) continue;
-      const int per_sm = ceil_div(tiles * s, num_sms());
-      const int64_t t = (int64_t)per_sm * per + (int64_t)per_sm * g_wgrad_overhead_stages;
-      if (best < 0 || t < best) { best = t; splits = s; }
-    }
-  }
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1 || deterministic) splits = 1;
-  p.stages_per_split = ceil_div(p.stages_total, splits);
-  splits = ceil_div(p.stages_total, p.stages_per_split);
-  p.splits = splits;
+  const int splits = p.splits;
   p.part = nullptr;
   p.counters = nullptr;
   void* scratch = nullptr;
@@ -1657,66 +1709,60 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int n_tiles, int det
 }
 
 template <int BN, int CW, bool IM2COL>
-static int dispatch_wgrad_cwb(int cwb, int np, const WgradMaps& tm, const WgradParams& p, int nt,
-                              int det, cudaStream_t s) {
+static int dispatch_wgrad_cwb(int cwb, int np, const WgradMaps& tm, const WgradParams& p, int mt,
+                              int nt, cudaStream_t s) {
   if constexpr (BN <= 128) {
     if (np == 3) {
       if constexpr (BN >= 64) {
-        if (cwb == 64) return launch_wgrad<BN, CW, 64, IM2COL, 3>(tm, p, nt, det, s);
+        if (cwb == 64) return launch_wgrad<BN, CW, 64, IM2COL, 3>(tm, p, mt, nt, s);
       }
-      return launch_wgrad<BN, CW, 32, IM2COL, 3>(tm, p, nt, det, s);
+      return launch_wgrad<BN, CW, 32, IM2COL, 3>(tm, p, mt, nt, s);
     }
   }
   if constexpr (BN >= 64) {
     if (cwb == 64) {
       if constexpr (BN <= 128) {
-        if (p.pix == 128) return launch_wgrad<BN, CW, 64, IM2COL, 1, 128>(tm, p, nt, det, s);
+        if (p.pix == 128) return launch_wgrad<BN, CW, 64, IM2COL, 1, 128>(tm, p, mt, nt, s);
       }
-      return launch_wgrad<BN, CW, 64, IM2COL, 1>(tm, p, nt, det, s);
+      return launch_wgrad<BN, CW, 64, IM2COL, 1>(tm, p, mt, nt, s);
     }
   }
   if constexpr (BN <= 128) {
-    if (p.pix == 128) return launch_wgrad<BN, CW, 32, IM2COL, 1, 128>(tm, p, nt, det, s);
+    if (p.pix == 128) return launch_wgrad<BN, CW, 32, IM2COL, 1, 128>(tm, p, mt, nt, s);
   }
-  return launch_wgrad<BN, CW, 32, IM2COL, 1>(tm, p, nt, det, s);
+  return launch_wgrad<BN, CW, 32, IM2COL, 1>(tm, p, mt, nt, s);
 }
 
 template <int BN, bool IM2COL>
 static int dispatch_wgrad_cw(int cw, int cwb, int np, const WgradMaps& tm, const WgradParams& p,
-                             int nt, int det, cudaStream_t s) {
-  if (cw == 64) return dispatch_wgrad_cwb<BN, 64, IM2COL>(cwb, np, tm, p, nt, det, s);
-  if (cw == 32) return dispatch_wgrad_cwb<BN, 32, IM2COL>(cwb, np, tm, p, nt, det, s);
-  return dispatch_wgrad_cwb<BN, 16, IM2COL>(cwb, np, tm, p, nt, det, s);
+                             int mt, int nt, cudaStream_t s) {
+  if (cw == 64) return dispatch_wgrad_cwb<BN, 64, IM2COL>(cwb, np, tm, p, mt, nt, s);
+  if (cw == 32) return dispatch_wgrad_cwb<BN, 32, IM2COL>(cwb, np, tm, p, mt, nt, s);
+  return dispatch_wgrad_cwb<BN, 16, IM2COL>(cwb, np, tm, p, mt, nt, s);
 }
 
 template <bool IM2COL>
 static int dispatch_wgrad(int bn, int cw, int cwb, int np, const WgradMaps& tm, const WgradParams& p,
-                          int nt, int det, cudaStream_t s) {
-  if (bn == 256) return dispatch_wgrad_cw<256, IM2COL>(cw, cwb, np, tm, p, nt, det, s);
-  if (bn == 128) return dispatch_wgrad_cw<128, IM2COL>(cw, cwb, np, tm, p, nt, det, s);
-  if (bn == 64) return dispatch_wgrad_cw<64, IM2COL>(cw, cwb, np, tm, p, nt, det, s);
-  return dispatch_wgrad_cw<32, IM2COL>(cw, cwb, np, tm, p, nt, det, s);
-}
-
-// 0: choose per problem; 64 / 128: force the pixels per stage where the shape allows it
-static int g_wgrad_pix = 0;
-static bool wgrad_wants_pix128(const WgradParams&, int) {
-  // 128-pixel stages wherever they fit (N tile <= 128): twice the MMAs per barrier round trip
-  return true;
+                          int mt, int nt, cudaStream_t s) {
+  if (bn == 256) return dispatch_wgrad_cw<256, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
+  if (bn == 128) return dispatch_wgrad_cw<128, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
+  if (bn == 64) return dispatch_wgrad_cw<64, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
+  return dispatch_wgrad_cw<32, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
 }
 
 static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* dy, float* dw,
                            int precision, int deterministic, cudaStream_t stream) {
-  ACNN_REQUIRE(g.Cin % 16 == 0 && g.Cout % 32 == 0, "wgrad: Cin %% 16 / Cout %% 32 required");
-  ACNN_REQUIRE(precision == 0 || precision == 1, "wgrad: precision must be 0 (bf16) or 1 (fp32)");
-  int Ho, Wo;
-  ACNN_REQUIRE(out_hw(g, &Ho, &Wo), "wgrad: empty output");
-  int rc = load_driver_fns();
+  WgradPlan w;
+  int rc = wgrad_plan(g, precision, deterministic, &w);
   if (rc) return rc;
+  rc = load_driver_fns();
+  if (rc) return rc;
+  int Ho, Wo;
+  out_hw(g, &Ho, &Wo);
   const bool plain = is_plain(g);
   const int np = precision ? 3 : 1;
   WgradParams p;
-  p.P = g.B * Ho * Wo;
+  p.P = w.P;
   p.Cout = g.Cout;
   p.Cin = g.Cin;
   p.Ktot = g.kh * g.kw * g.Cin;
@@ -1726,19 +1772,13 @@ static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* d
   p.stride = g.stride;
   p.pad_h_lo = g.pad_h_lo;
   p.pad_w_lo = g.pad_w_lo;
-  int bn = g.Cout >= 256 ? 256 : (g.Cout >= 128 ? 128 : (g.Cout >= 64 ? 64 : 32));
-  if (np == 3 && bn > 128) bn = 128;   // three operand planes per stage: smem
-  // 128-pixel stages: only the bf16 path, N tile <= 128 (smem), enough pixels to split
-  p.pix = kWgPix;
-  if (np == 1 && bn <= 128 && p.P >= 4096 &&
-      (g_wgrad_pix == 128 || (g_wgrad_pix == 0 && wgrad_wants_pix128(p, bn))))
-    p.pix = 128;
-  p.stages_total = ceil_div(p.P, p.pix);
-  p.stages_per_split = p.stages_total;
+  p.pix = w.pix;
+  p.stages_total = w.stages_total;
+  p.stages_per_split = w.stages_per_split;
+  p.splits = w.splits;
   p.dw = dw;
   const int cw = chunk_width(g.Cin);
   const int cwb = (g.Cout % 64 == 0) ? 64 : 32;
-  ACNN_REQUIRE(g.Cout % bn == 0, "wgrad: Cout=%d not a multiple of its N tile %d", g.Cout, bn);
   WgradMaps tm;
   const int64_t x_plane = input_elems(g), dy_plane = (int64_t)p.P * g.Cout;
   for (int pl = 0; pl < np; ++pl) {
@@ -1757,9 +1797,8 @@ static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* d
     tm.x[pl] = tm.x[0];
     tm.dy[pl] = tm.dy[0];
   }
-  const int nt = g.Cout / bn;
-  if (plain) return dispatch_wgrad<false>(bn, cw, cwb, np, tm, p, nt, deterministic, stream);
-  return dispatch_wgrad<true>(bn, cw, cwb, np, tm, p, nt, deterministic, stream);
+  if (plain) return dispatch_wgrad<false>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
+  return dispatch_wgrad<true>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
 }
 
 }  // namespace acnn
@@ -1815,6 +1854,27 @@ int acnn_set_wgrad_pixels(int pix) {
   const int prev = acnn::g_wgrad_pix;
   acnn::g_wgrad_pix = (pix == 64 || pix == 128) ? pix : 0;
   return prev;
+}
+
+int acnn_set_wgrad_splits(int n) {
+  const int prev = acnn::g_wgrad_splits;
+  acnn::g_wgrad_splits = n < 0 ? 0 : n;
+  return prev;
+}
+
+int acnn_conv_wgrad_plan(const acnn_conv_geom* g, int precision, int deterministic, int* pix,
+                         int* splits, int* stages_per_split) {
+  if (!g) {
+    acnn::set_error("acnn_conv_wgrad_plan: null geometry");
+    return ACNN_ERR_INVALID;
+  }
+  acnn::WgradPlan w;
+  const int rc = acnn::wgrad_plan(*g, precision, deterministic, &w);
+  if (rc) return rc;
+  if (pix) *pix = w.pix;
+  if (splits) *splits = w.splits;
+  if (stages_per_split) *stages_per_split = w.stages_per_split;
+  return ACNN_OK;
 }
 
 int acnn_conv_stats_parts(const acnn_conv_geom* g) {

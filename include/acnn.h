@@ -79,13 +79,19 @@ int acnn_set_wgrad_pixels(int pix);
  * cost model that picks the number of pixel splits (default 16); 0 = the "two waves of CTAs"
  * rule.  Returns the previous setting. */
 int acnn_set_wgrad_overhead_stages(int stages);
+/* Tuning knob of the wgrad launcher: n > 0 asks for n pixel splits, clamped to the capacity of the
+ * partial-tile scratch (64 MiB, one arrival counter per tile) and to the number of pipeline stages;
+ * 0 (default) = the cost model above.  deterministic != 0 still runs one split.  Returns the previous
+ * setting. */
+int acnn_set_wgrad_splits(int n);
 /* Tuning knob: the largest grid (CTAs) of the grid-stride elementwise kernels (bn_act, bn_bwd_apply,
  * ...); no effect on results.  Values below 132 restore the default (16 x 132).  Returns the previous setting. */
 int acnn_set_stream_grid_cap(int blocks);
 /* SK attention chains (acnn_sk_fc_fwd / acnn_sk_fc_bwd): 1 = ONE cooperative launch per direction
  * (the whole grid walks GEMM / batch-norm / gate phases separated by grid barriers; K-split partials
  * summed in split order: deterministic, no atomics, nothing to zero); 0 = the multi-launch path (4 + 6
- * kernels and 4 memsets per SK block; split-K with atomics unless deterministic); -1 (default) = fused
+ * kernels and 4 memsets per SK block; unless deterministic, split-K GEMMs whose per-split partials
+ * a reduction kernel adds in split order: bit-reproducible, one more launch per GEMM); -1 (default) = fused
  * when the call asks for deterministic results, multi-launch otherwise.
  * Same results up to fp32 summation order.  Returns the previous setting. */
 int acnn_set_sk_fc_fused(int on);
@@ -146,6 +152,14 @@ int acnn_conv_dgrad(const acnn_conv_geom* g, const void* dy, const void* w_dgrad
  * precision 1: x and dy are 3-plane operands. */
 int acnn_conv_wgrad(const acnn_conv_geom* g, const void* x, const void* dy, float* dw,
                     int precision, int deterministic, void* stream);
+/* The split layout acnn_conv_wgrad(g, ..., precision, deterministic, ...) would launch with the
+ * current tuning knobs: *pix pixels per pipeline stage (128 only for bf16 with Cout < 256, i.e. an
+ * N tile <= 128, and P = B*Ho*Wo >= 4096, unless acnn_set_wgrad_pixels(64); else 64), the P pixels
+ * in ceil(P / pix) stages, *splits CTAs along them, every
+ * split but the last running *stages_per_split stages (splits = ceil(stages / stages_per_split)).
+ * Host only, callable without a GPU: without a device the SM count is taken as 132 (the H100's). */
+int acnn_conv_wgrad_plan(const acnn_conv_geom* g, int precision, int deterministic, int* pix,
+                         int* splits, int* stages_per_split);
 /* planes bf16 [3][n] = (hi, mid, lo) of x fp32 [n], x = hi + mid + lo to 24 bits (n % 8 == 0). */
 int acnn_split3(const float* x, void* planes, int64_t n, void* stream);
 

@@ -113,3 +113,59 @@ def test_sk_fc_scratch_formula_matches_library():
         for f in (64, 128, 256, 512, 96):
             d = max(f // 2, 32)
             assert lib.acnn_sk_fc_scratch_floats(B, f, d) == sk_fc_scratch_floats(B, f, d), (B, f)
+
+
+def test_conv_wgrad_plan_properties():
+    """acnn_conv_wgrad_plan (host only: the SM count is the H100's 132 without a device) against
+    the rules include/acnn.h states, over a grid of geometries and both precisions: one split when
+    deterministic, a stage partition whose last split is non-empty, the partial tiles within 64 MiB,
+    the documented pixels per stage, and a forced split count honoured within the capacity caps."""
+    import ctypes as C
+    from assembled_cnn_b200 import _lib
+    lib = _lib.load()
+
+    def plan(g, precision, det):
+        pix, splits, sps = C.c_int(), C.c_int(), C.c_int()
+        _lib.check(lib.acnn_conv_wgrad_plan(g, precision, det, C.byref(pix), C.byref(splits),
+                                            C.byref(sps)), "acnn_conv_wgrad_plan")
+        return pix.value, splits.value, sps.value
+
+    geoms = []
+    for B in (1, 3, 32, 256):
+        for H in (7, 14, 56):
+            for Cin, Cout in ((16, 32), (64, 64), (32, 128), (64, 256), (256, 512), (2048, 1024)):
+                for k, stride in ((1, 1), (3, 1), (3, 2), (1, 2)):
+                    p = (k - 1) // 2
+                    geoms.append(_lib.ConvGeom(B, H, H, Cin, Cout, k, k, stride, p, k - 1 - p, p,
+                                               k - 1 - p))
+    n_split = 0
+    prev_s, prev_p = lib.acnn_set_wgrad_splits(0), lib.acnn_set_wgrad_pixels(0)
+    try:
+        for g in geoms:
+            Ho, Wo = g.out_hw()
+            P = g.B * Ho * Wo
+            # the partial tiles of one split: ceil(Ktot / 128) x 128 rows by Cout columns (fp32)
+            split_bytes = -(-g.kh * g.kw * g.Cin // 128) * 128 * g.Cout * 4
+            for precision in (0, 1):
+                pix, splits, sps = plan(g, precision, 0)
+                assert pix == (128 if precision == 0 and g.Cout < 256 and P >= 4096 else 64)
+                stages = -(-P // pix)
+                assert splits * sps >= stages > (splits - 1) * sps >= 0
+                assert splits == 1 or splits * split_bytes <= 64 << 20
+                n_split += splits > 1
+                assert plan(g, precision, 1) == (pix, 1, stages)
+                lib.acnn_set_wgrad_pixels(64)
+                assert plan(g, precision, 0)[0] == 64
+                lib.acnn_set_wgrad_pixels(0)
+                for n in (1, 2, 3, 7, 1000):
+                    lib.acnn_set_wgrad_splits(n)
+                    want = max(min(n, stages, (64 << 20) // split_bytes), 1)
+                    want = -(-stages // -(-stages // want))      # re-normalised: no empty split
+                    assert plan(g, precision, 0) == (pix, want, -(-stages // want)), (n, P)
+                    assert plan(g, precision, 1) == (pix, 1, stages)
+                lib.acnn_set_wgrad_splits(0)
+    finally:
+        lib.acnn_set_wgrad_splits(prev_s)
+        lib.acnn_set_wgrad_pixels(prev_p)
+    assert n_split > len(geoms) // 4          # the default cost model does split
+    assert lib.acnn_set_wgrad_splits(0) == 0

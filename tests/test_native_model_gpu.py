@@ -4,10 +4,11 @@ The op-by-op parity of the plan against the oracle is proven on the Python execu
 lockstep with oracle/plan_interp.py) and the two plans are the same text (test_native_plan_cpu.py).
 What remains to prove is that the library's launch records call the op level with the same pointers
 and arguments: run the SAME step through both executors on the same weights and inputs in
-deterministic mode and require every buffer of the step -- logits, loss, every gradient, the updated
+deterministic mode -- and, for the bf16 configurations, in the default mode too, where wgrad and the
+small SK / SE GEMMs run split-K with ordered reductions -- and require every buffer of the step -- logits, loss, every gradient, the updated
 weights, momentum and moving statistics -- to be BIT-IDENTICAL.  Plus: the pure C-ABI call sequence
 with host arrays (acnn_set_inputs ... acnn_get_loss) against the oracle, piecewise == acnn_step, and
-CUDA-graph capture of acnn_step."""
+CUDA-graph capture of acnn_step, in both modes."""
 import ctypes as C
 
 import numpy as np
@@ -32,7 +33,11 @@ CASES = {
                          4, 64, dict(training=True, label_smoothing=0.1)),
     "c5_r152_topology": (dict(ASSEMBLE, resnet_size=152, bl_alpha=1, bl_beta=2), 4, 64,
                          dict(training=True, mixup_type=1)),
+    # B = 64 > 32: the weight-gradient GEMMs of the SK and SE layers (K = batch) split
+    "sk_se_b64": (dict(ASSEMBLE, use_se_block=True), 64, 64, dict(training=True, mixup_type=1)),
 }
+# bf16 configurations also run in the default mode (deterministic=None: split-K on)
+DEFAULT_MODE_CASES = ("c3_assemble_mixup1", "se_proj_resnet_d", "c5_r152_topology", "sk_se_b64")
 
 
 def _weights(plan, seed=5):
@@ -69,14 +74,15 @@ def _feeds(plan, seed=9):
     return f
 
 
-def _pair(flags, B, hw, kw):
+def _pair(flags, B, hw, kw, deterministic=True):
     from assembled_cnn_b200 import native
     from assembled_cnn_b200.plan import ModelConfig, build_plan
     from assembled_cnn_b200.runtime import Runtime
     cfg = ModelConfig(**flags)
     plan = build_plan(cfg, B, hw, hw, **kw)
-    rt_py = Runtime(plan, deterministic=True)
-    rt_nat = native.NativeRuntime(native.NativeModel(cfg, B, hw, hw, deterministic=True, **kw))
+    rt_py = Runtime(plan, deterministic=deterministic)
+    rt_nat = native.NativeRuntime(native.NativeModel(cfg, B, hw, hw, deterministic=deterministic, **kw))
+    assert rt_py.det == rt_nat.det
     w = _weights(plan)
     feeds = _feeds(plan)
     hp = dict(lr=0.05, momentum=0.9, weight_decay=1e-4, keep_prob=0.9, step=3)
@@ -99,8 +105,18 @@ def _assert_same(a, b, what):
 
 @pytest.mark.parametrize("case", sorted(CASES))
 def test_native_step_bit_identical_to_python_executor(case):
+    _step_bit_identical(case, deterministic=True)
+
+
+@pytest.mark.parametrize("case", DEFAULT_MODE_CASES)
+def test_native_step_bit_identical_to_python_executor_default_mode(case):
+    """The bf16 configurations with deterministic=None: wgrad and the SK / SE GEMMs run split-K."""
+    _step_bit_identical(case, deterministic=None)
+
+
+def _step_bit_identical(case, deterministic):
     flags, B, hw, kw = CASES[case]
-    plan, rt_py, rt_nat = _pair(flags, B, hw, kw)
+    plan, rt_py, rt_nat = _pair(flags, B, hw, kw, deterministic)
     training = kw.get("training", True)
     for step in range(2):
         for rt in (rt_py, rt_nat):
@@ -184,10 +200,19 @@ def test_c_abi_call_sequence_with_host_arrays_against_oracle():
 def test_piecewise_equals_step_and_graph_replay():
     """acnn_forward + acnn_loss + acnn_backward_range (3 segments) + acnn_sgd_step == acnn_step, eager
     == CUDA-graph replay of acnn_step; all bit-identical (deterministic mode)."""
+    _piecewise_step_graph(deterministic=True)
+
+
+def test_piecewise_equals_step_and_graph_replay_default_mode():
+    """The same in the default mode (deterministic=None: split-K wgrad and SK / SE GEMMs)."""
+    _piecewise_step_graph(deterministic=None)
+
+
+def _piecewise_step_graph(deterministic):
     from assembled_cnn_b200 import _lib, native
     from assembled_cnn_b200.plan import ModelConfig
     cfg = ModelConfig(**ASSEMBLE)
-    kw = dict(training=True, mixup_type=1, label_smoothing=0.1, deterministic=True)
+    kw = dict(training=True, mixup_type=1, label_smoothing=0.1, deterministic=deterministic)
     outs = []
     for mode in ("step", "piecewise", "graph"):
         nm = native.NativeModel(cfg, 4, 64, 64, **kw)

@@ -367,8 +367,20 @@ def test_fp32_mode_two_runs_bit_identical():
 
 
 def test_bf16_mode_forward_and_bn_reductions_bit_identical():
-    """bf16 production mode: everything except the split-K wgrad is ordered too -- two runs give a
-    bit-identical loss, logits and BN statistics; with deterministic=True also the gradients."""
+    """bf16 production mode (deterministic=None): every reduction is ordered -- the batch-norm
+    partial rows, the split-K wgrad and the SK / SE GEMMs, whose partials are added in split order.
+    Two eager steps and a CUDA-graph replay of the step give bit-identical loss, logits, BN
+    statistics, gradients, weights and momentum."""
+    _bf16_step_bit_identical(deterministic=None)
+
+
+def test_bf16_mode_forward_and_bn_reductions_bit_identical_deterministic():
+    """The same with deterministic=True (one split everywhere)."""
+    _bf16_step_bit_identical(deterministic=True)
+
+
+def _bf16_step_bit_identical(deterministic):
+    import ctypes as C
     from assembled_cnn_b200.plan import ModelConfig, build_plan
     from assembled_cnn_b200.runtime import Runtime
     B, hw = 8, 128
@@ -377,8 +389,8 @@ def test_bf16_mode_forward_and_bn_reductions_bit_identical():
     plan = build_plan(ModelConfig(**ASSEMBLE), B, hw, hw, training=True, mixup_type=1,
                       label_smoothing=0.1)
     outs = []
-    for run in range(2):
-        rt = Runtime(plan, deterministic=True)
+    for run in ("eager", "eager", "graph"):
+        rt = Runtime(plan, deterministic=deterministic)
         torch.manual_seed(0)
         rt.params.copy_(torch.randn(rt.params.shape, generator=torch.Generator().manual_seed(1)) * 0.05)
         for p in plan.params.values():
@@ -389,9 +401,25 @@ def test_bf16_mode_forward_and_bn_reductions_bit_identical():
         rt.t[m["labels"]].copy_(lab)
         rt.t[m["lam1"]].copy_(lam)
         rt.set_hparams(lr=0.05, momentum=0.9, weight_decay=1e-4, grad_scale=1.0)
-        rt.run_step()
+        if run == "graph":
+            rt.capture(train=True)
+            rt.graph.replay()
+        else:
+            rt.run_step()
         torch.cuda.synchronize()
         outs.append((rt.slot_view(m["loss"]).cpu().clone(), rt.t[m["logits"]].cpu().clone(),
-                     rt.state.cpu().clone(), rt.grads.cpu().clone()))
-    for a, b in zip(outs[0], outs[1]):
-        assert torch.equal(a, b)
+                     rt.state.cpu().clone(), rt.grads.cpu().clone(), rt.params.cpu().clone(),
+                     rt.momentum.cpu().clone()))
+    for other in outs[1:]:
+        for a, b, what in zip(outs[0], other, ("loss", "logits", "moving statistics", "gradients",
+                                                "weights", "momentum")):
+            assert torch.equal(a, b), what
+    # the default mode really ran split-K wgrads (acnn_conv_wgrad_plan: the layout the launcher uses)
+    n_split = 0
+    for op in plan.backward:
+        if op.kind == "conv_wgrad":
+            splits = C.c_int()
+            assert rt.lib.acnn_conv_wgrad_plan(rt.geom(op.geom, op.a.get("x_wpad")), 0, rt.det, None,
+                                               C.byref(splits), None) == 0
+            n_split += splits.value > 1
+    assert (n_split > 0) == (not deterministic), n_split
