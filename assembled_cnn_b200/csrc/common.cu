@@ -76,4 +76,67 @@ int scratch_free(void* p, cudaStream_t stream, const char* what) {
   return ACNN_OK;
 }
 
+static int g_num_sms = 0;
+int num_sms() {
+  if (g_num_sms == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+      (void)cudaGetLastError();   // no device (host-only queries): size for the H100's kMaxSms
+      g_num_sms = 0;
+    }
+    // at most kMaxSms: the partial statistics rows (one per CTA of an N tile) are sized for it
+    if (g_num_sms <= 0 || g_num_sms > kMaxSms) g_num_sms = kMaxSms;
+  }
+  return g_num_sms;
+}
+
+EncodeTiledFn g_encode_tiled = nullptr;
+EncodeIm2colFn g_encode_im2col = nullptr;
+int g_driver_version = 0;
+
+int load_driver_fns() {
+  if (g_encode_tiled && g_encode_im2col) return ACNN_OK;
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
+  if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || !fn) {
+    set_error("cuTensorMapEncodeTiled entry point unavailable (%s)", cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  g_encode_tiled = reinterpret_cast<EncodeTiledFn>(fn);
+  fn = nullptr;
+  e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &q);
+  if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || !fn) {
+    set_error("cuTensorMapEncodeIm2col entry point unavailable (%s)", cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  g_encode_im2col = reinterpret_cast<EncodeIm2colFn>(fn);
+  cudaDriverGetVersion(&g_driver_version);
+  return ACNN_OK;
+}
+
+CUtensorMapSwizzle swizzle_enum(int bytes) {
+  return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                      : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+}
+
+int make_map_2d(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld,
+                int box_rows, int box_cols) {
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base),
+                              dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              swizzle_enum(box_cols * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed (%d): rows=%lld cols=%lld ld=%lld box=%dx%d", (int)r,
+              (long long)rows, (long long)cols, (long long)ld, box_rows, box_cols);
+    return ACNN_ERR_CUDA;
+  }
+  return ACNN_OK;
+}
+
 }  // namespace acnn

@@ -62,6 +62,31 @@ inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
   (void)cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);   // errors: check_launch()
 }
 
+// SM count of the current device, at most kMaxSms (kMaxSms without a device: host-only queries).
+int num_sms();
+
+// ------------------------------------------------------------------------------------------
+// Tensor-map creation (driver entry points fetched lazily: libacnn.so does not link libcuda).
+// ------------------------------------------------------------------------------------------
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
+                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
+                                   const cuuint64_t*, const cuuint64_t*, const int*, const int*,
+                                   cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle,
+                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+extern EncodeTiledFn g_encode_tiled;
+extern EncodeIm2colFn g_encode_im2col;
+extern int g_driver_version;
+
+int load_driver_fns();
+CUtensorMapSwizzle swizzle_enum(int bytes);
+// bf16 matrix [rows][cols] (cols contiguous, row pitch ld elements); box = [box_rows][box_cols].
+int make_map_2d(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld,
+                int box_rows, int box_cols);
+
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -21,68 +21,6 @@
 
 namespace acnn {
 
-// ------------------------------------------------------------------------------------------
-// Tensor-map creation (driver entry points fetched lazily: libacnn.so does not link libcuda).
-// ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                   const cuuint64_t*, const cuuint64_t*, const int*, const int*,
-                                   cuuint32_t, cuuint32_t, const cuuint32_t*,
-                                   CUtensorMapInterleave, CUtensorMapSwizzle,
-                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn g_encode_tiled = nullptr;
-static EncodeIm2colFn g_encode_im2col = nullptr;
-static int g_driver_version = 0;
-
-static int load_driver_fns() {
-  if (g_encode_tiled && g_encode_im2col) return ACNN_OK;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
-  if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || !fn) {
-    set_error("cuTensorMapEncodeTiled entry point unavailable (%s)", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  g_encode_tiled = reinterpret_cast<EncodeTiledFn>(fn);
-  fn = nullptr;
-  e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &q);
-  if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || !fn) {
-    set_error("cuTensorMapEncodeIm2col entry point unavailable (%s)", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  g_encode_im2col = reinterpret_cast<EncodeIm2colFn>(fn);
-  cudaDriverGetVersion(&g_driver_version);
-  return ACNN_OK;
-}
-
-static CUtensorMapSwizzle swizzle_enum(int bytes) {
-  return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                      : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-}
-
-// bf16 matrix [rows][cols] (cols contiguous, row pitch ld elements); box = [box_rows][box_cols].
-static int make_map_2d(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                       int box_rows, int box_cols) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base),
-                              dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              swizzle_enum(box_cols * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d): rows=%lld cols=%lld ld=%lld box=%dx%d", (int)r,
-              (long long)rows, (long long)cols, (long long)ld, box_rows, box_cols);
-    return ACNN_ERR_CUDA;
-  }
-  return ACNN_OK;
-}
-
 // Element pitches of the input tensor: dense NHWC unless the geometry overrides them (used by the
 // space-to-depth stem, whose "pixels" are overlapping 4-pixel windows of a W-padded image).
 static void input_pitches(const acnn_conv_geom& g, int64_t* pix, int64_t* row, int64_t* img) {
@@ -1191,21 +1129,6 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
 // ------------------------------------------------------------------------------------------
 // Host launchers
 // ------------------------------------------------------------------------------------------
-static int g_num_sms = 0;
-static int num_sms() {
-  if (g_num_sms == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess ||
-        cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
-      (void)cudaGetLastError();   // no device (host-only queries): size for the H100's kMaxSms
-      g_num_sms = 0;
-    }
-    // at most kMaxSms: the partial statistics rows (one per CTA of an N tile) are sized for it
-    if (g_num_sms <= 0 || g_num_sms > kMaxSms) g_num_sms = kMaxSms;
-  }
-  return g_num_sms;
-}
-
 struct ConvMaps {
   CUtensorMap a[3], b[3], c, add, mask;
 };

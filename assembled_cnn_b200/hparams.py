@@ -39,6 +39,12 @@ DEFAULTS = {
     "no_downsample": False,
     "cls_loss_type": "softmax",
     "dataset_name": None,                 # :31 (None -> the ImageNet constants, as data_config)
+    # zero-shot retrieval evaluation (metric/recall_metric.py, model_fns.recall_at_k)
+    "zeroshot_eval": False,               # :273
+    "eval_similarity": "cosine",          # :91 ('cosine' | 'euclidean')
+    "recall_at_k": [1, 5],                # :288
+    "return_embedding": False,            # :27
+    "val_batch_size": 256,                # :39
     # official/utils/flags/_base.py:50-105, _performance.py:74-137
     "batch_size": 32,
     "train_epochs": 90,                   # main_classification.py:38
@@ -48,9 +54,19 @@ DEFAULTS = {
     "num_gpus": 1,
 }
 
-# functions/data_config.py:42-50
+# functions/data_config.py:22-148, keyed by get_config's names; the *_zeroshot / SOP / CUB entries
+# are the retrieval datasets of the zero-shot evaluation
 DATASETS = {
+    "food101": dict(num_classes=101, num_images={"train": 75750, "validation": 25250}),
     "imagenet": dict(num_classes=1001, num_images={"train": 1281167, "validation": 50000}),
+    "cub_200_2011": dict(num_classes=100, num_images={"train": 5864, "validation": 5924}),
+    "iFood2019": dict(num_classes=251, num_images={"train": 118475, "validation": 11994}),
+    "SOP": dict(num_classes=11318, num_images={"train": 59551, "validation": 60502}),
+    "oxford_flowers102": dict(num_classes=102, num_images={"train": 2040, "validation": 6149}),
+    "cars196": dict(num_classes=196, num_images={"train": 8144, "validation": 8041}),
+    "cars196_zeroshot": dict(num_classes=196, num_images={"train": 8054, "validation": 8131}),
+    "oxford_iiit_pet": dict(num_classes=37, num_images={"train": 3680, "validation": 3669}),
+    "fgvc_aircraft": dict(num_classes=100, num_images={"train": 6667, "validation": 3333}),
 }
 
 

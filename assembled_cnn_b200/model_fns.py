@@ -6,6 +6,7 @@ Mirrors (same names, argument meaning and error behaviour):
   * functions/model_fns.py:201-239   model_fn_cls(features, labels, mode, params)
   * nets/run_loop_classification.py:60-234  resnet_model_fn (loss assembly, train op)
   * functions/model_fns.py:36-95     learning_rate_with_decay ; :26-33 keep_prob_decay
+  * metric/recall_metric.py:13-180   recall_at_k (the zero-shot retrieval evaluation)
 plus `build_model(**flags)` (the name BASELINE.json uses; the reference has no such function).
 
 The reference builds a TF graph and lets the Estimator run it; here a call executes on the GPU:
@@ -24,7 +25,7 @@ import torch
 from . import _lib, dp
 from .hparams import DATASETS, DEFAULTS, params_from_flags
 from .plan import BLOCK_SIZES, ModelConfig, build_plan
-from .metrics import EvalMetrics
+from .metrics import EvalMetrics, RecallAtK
 from .runtime import Runtime
 from .native import NativeModel, NativeRuntime
 
@@ -613,3 +614,23 @@ def reset_metrics(params=None):
 
 
 model_fn_cls.reset_metrics = reset_metrics
+
+
+def recall_at_k(model, batches, num_val_images, recall_at_k=(1, 5), eval_similarity="cosine",
+                use_resnet_d=False, return_embedding=True, global_step=None):
+    """metric/recall_metric.py:13-180, the evaluation of `--zeroshot_eval`: embeds every batch of
+    `batches` (an iterable of (images [N,H,W,3], labels [N]); label -1 marks a distractor) with
+    `model(images, False, use_resnet_d=..., return_embedding=...)`, then Recall@K of every k in
+    `recall_at_k` over queries = non-distractor rows against the index = all rows (RecallAtK).
+    The similarity search runs in the model's dtype ('fp32': three bf16 planes per operand), as the
+    reference feeds fp32 or fp16 placeholders by `flags_obj.dtype`.
+    Returns {'recall_at_<k>': ..., 'global_step': global_step}."""
+    dev = torch.device(model.device)
+    metric = RecallAtK(recall_at_k, similarity=eval_similarity, dtype=model.dtype, device=dev)
+    for images, labels in batches:
+        emb = model(images, False, use_resnet_d=use_resnet_d, return_embedding=return_embedding)
+        metric.update(emb, labels)
+    assert metric.count == num_val_images, (metric.count, num_val_images)
+    out = {"recall_at_%d" % k: v for k, v in metric.result().items()}
+    out["global_step"] = global_step
+    return out

@@ -411,6 +411,38 @@ int acnn_sgd_momentum(float* w, const float* grad, float* acc, int64_t n,
 int acnn_sgd_scratch_floats(void);
 int acnn_fill_zero(void* p, int64_t bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Zero-shot retrieval (metric/recall_metric.py:98-123: l2_normalize / tf_simple_pairwise_distance,
+ * MatMul and tf.nn.top_k over the query x index similarity matrix, which is never materialised)
+ * ------------------------------------------------------------------------------------------- */
+/* For every query row q of Q[nq][d] (fp32): the k rows of X[nx][d] (fp32) with the largest similarity,
+ * sorted by (similarity descending, index ascending) -- tf.nn.top_k's order, lower index first on ties.
+ * metric 0 = cosine: rows l2-normalised first (tf.nn.l2_normalize: x * rsqrt(max(sum x^2, 1e-12)));
+ * metric 1 = euclidean: -((|q|^2 + |x|^2) - 2 q.x) on the raw rows (tf_simple_pairwise_distance,
+ * negated), the squared norms taken over the rounded operands.
+ * dtype ACNN_BF16: bf16 operands, fp32 accumulation; ACNN_F32: three bf16 planes per operand (as the
+ * conv GEMMs), whose six significant cross products are accumulated in fp32.
+ * out_idx int32 [nq][k], out_sim fp32 [nq][k].  Any d >= 1 (<= 2^24); 1 <= k <= 128 (k > 128:
+ * ACNN_ERR_UNSUPPORTED); k > nx, non-positive sizes, an unknown metric or dtype: ACNN_ERR_INVALID.
+ * All of these are checked before any CUDA call.  The result is the same bit for bit for every
+ * column-split count, grid and stream.  Only similarities above -inf are ranked: a row with fewer
+ * than k of them (a NaN or infinite input, or a squared distance that overflows fp32) is padded with
+ * (similarity -inf, index 2147483647) entries -- callers that index with out_idx must check for it.
+ * work: acnn_knn_work_bytes(...) bytes, caller-owned; every section starts at a 256-byte boundary:
+ *   Q' bf16 [nq][K'], X' bf16 [nx][K']  (K' = P * roundup(d, 64), zero-padded; P = 1 for bf16, 6 for
+ *        fp32: K' holds six d-segments so that one bf16 GEMM forms the six plane products, smallest
+ *        first -- Q' = (hi, mid, lo, hi, mid, hi), X' = (lo, mid, hi, mid, hi, hi))
+ *   |q|^2 fp32 [nq], |x|^2 fp32 [nx]   (of the rounded operands: bf16, or (hi + mid) + lo)
+ *   partial lists: similarity fp32 [8][nq][k], index int32 [8][nq][k]  (one per column split) */
+int acnn_knn_topk(const float* q, const float* x, int nq, int nx, int d, int k, int metric, int dtype,
+                  int32_t* out_idx, float* out_sim, void* work, int64_t work_bytes, void* stream);
+/* Bytes of the `work` argument (host only, callable without a GPU); -1 for invalid sizes. */
+int64_t acnn_knn_work_bytes(int nq, int nx, int d, int k, int dtype);
+/* Tuning knob of acnn_knn_topk (no effect on results): n > 0 forces n column splits, clamped to
+ * [1, min(8, ceil(nx / 128))]; 0 (default) = the cost model that fills the SMs.  Returns the previous
+ * setting. */
+int acnn_set_knn_splits(int n);
+
 #ifdef __cplusplus
 }
 #endif
