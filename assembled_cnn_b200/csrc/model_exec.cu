@@ -880,6 +880,22 @@ int acnn_set_inputs(acnn_model* m, const float* images, const int32_t* labels, c
   return ACNN_OK;
 }
 
+int acnn_set_images_u8(acnn_model* m, const uint8_t* images_dev, const float* mean3, void* stream) {
+  ACNN_REQUIRE(m && m->bound && images_dev && mean3, "acnn_set_images_u8: not bound / null");
+  const Plan& p = m->plan;
+  cudaPointerAttributes at{};
+  const cudaError_t e = cudaPointerGetAttributes(&at, images_dev);
+  if (e != cudaSuccess) {
+    set_error("acnn_set_images_u8: %s", cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+               "acnn_set_images_u8: images_dev must be device memory (stage host images in a device buffer)");
+  const Tensor& t = p.tensors[p.images];
+  return acnn_images_from_u8(images_dev, mean3, (float*)(m->ws + t.ws_offset), (int)t.shape[0], (int)t.shape[1],
+                             (int)t.shape[2], stream);
+}
+
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream) {
   ACNN_REQUIRE(m && m->bound && hp, "acnn_set_hparams: not bound / null");
   return memcpy_async(m->ws + m->hp_off, hp, 32, stream, "acnn_set_hparams");

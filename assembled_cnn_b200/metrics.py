@@ -5,6 +5,7 @@ sums).  They consume the logits the CUDA forward produced; a few tiny torch redu
 host-side bookkeeping, not part of the hot path."""
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 
@@ -163,3 +164,99 @@ class RecallAtK:
             # a row with fewer than k finite similarities (e.g. squared distances overflowing fp32)
             raise ValueError("RecallAtK: similarities are not finite; cannot rank the index")
         return recall_from_sorted_idx(idx, labels[is_query], labels, self.k_list)
+
+
+# --------------------------------------------------------------------------------------------------
+# ImageNet-C corruption error (mce/eval_robustness.py)
+# --------------------------------------------------------------------------------------------------
+# AlexNet's top-1 error on each corruption, pooled over the five severities (Hendrycks & Dietterich,
+# "Benchmarking Neural Network Robustness to Common Corruptions and Perturbations", ICLR 2019): the
+# normaliser of CE.  The 15 ImageNet-C corruptions, then the four extra ones, in the order of
+# ALEXNET_CE in mce/eval_robustness.py:91-97 -- the order the distortions are split over GPUs.
+ALEXNET_CE = {
+    "gaussian_noise": 0.8864, "shot_noise": 0.8945, "impulse_noise": 0.9226,
+    "defocus_blur": 0.8199, "glass_blur": 0.8263, "motion_blur": 0.7860, "zoom_blur": 0.7984,
+    "snow": 0.8668, "frost": 0.8266, "fog": 0.8193, "brightness": 0.5646,
+    "contrast": 0.8532, "elastic_transform": 0.6461, "pixelate": 0.7178, "jpeg_compression": 0.6065,
+    "speckle_noise": 0.8454, "gaussian_blur": 0.7871, "spatter": 0.7175, "saturate": 0.6583,
+}
+DISTORTIONS = tuple(ALEXNET_CE)
+
+
+def softmax_top1_count(logits, labels, correct, n_valid=None, pred=None):
+    """acnn_softmax_top1_count on the current stream: pred = the smallest index of the largest fp32
+    softmax probability of every row r < n_valid of `logits` (CUDA fp32 [B, NC], rows may be strided, as
+    a model's logits view is), -1 for a row with a non-finite logit; adds the rows with pred == labels[r]
+    to `correct` (a CUDA int64 tensor of one element).  Rows >= n_valid are not touched.  `pred` (int32
+    [B]) is allocated unless given; returns it."""
+    from . import _lib
+    lib = _lib.load()
+    if logits.dim() != 2 or logits.dtype != torch.float32 or logits.stride(1) != 1:
+        raise ValueError("logits must be a float32 [B, NC] tensor with unit column stride")
+    B, NC = logits.shape
+    n_valid = B if n_valid is None else int(n_valid)
+    if not (logits.is_cuda and labels.is_cuda and correct.is_cuda):
+        raise _lib.AcnnError("softmax_top1_count runs on the GPU: logits, labels and correct must be CUDA tensors")
+    if labels.dtype != torch.int32 or labels.numel() < B or not labels.is_contiguous():
+        raise ValueError("labels must be a contiguous int32 tensor of at least B = %d values" % B)
+    if correct.dtype != torch.int64 or correct.numel() != 1:
+        raise ValueError("correct must be an int64 tensor of one element")
+    if pred is None:
+        pred = torch.empty(B, dtype=torch.int32, device=logits.device)
+    stream = torch.cuda.current_stream(logits.device).cuda_stream
+    _lib.check(lib.acnn_softmax_top1_count(logits.data_ptr(), B, logits.stride(0), NC, labels.data_ptr(), n_valid,
+                                           pred.data_ptr(), correct.data_ptr(), stream), "acnn_softmax_top1_count")
+    return pred
+
+
+def corruption_error_result(correct, count):
+    """show_corruption_error (mce/eval_robustness.py:231-232,287-300) from the per-distortion counts
+    {distortion: int}: error = 1 - correct / count (pooled over the severities), ce = error /
+    ALEXNET_CE[d], mCE = mean of the 19 ce, mCE_unnormalized = mean of the 19 errors."""
+    out = {}
+    for d in DISTORTIONS:
+        if d not in count or count[d] <= 0:
+            # the reference asserts num_of_images > 0 for every distortion (:231)
+            raise ValueError("corruption error: no images evaluated for distortion %r" % d)
+        err = 1 - 1. * correct[d] / count[d]
+        out[d] = {"error": err, "ce": err / ALEXNET_CE[d]}
+    out["mCE"] = float(np.mean([out[d]["ce"] for d in DISTORTIONS]))
+    out["mCE_unnormalized"] = float(np.mean([out[d]["error"] for d in DISTORTIONS]))
+    return out
+
+
+class CorruptionError:
+    """Streaming corruption error of the reference's robustness evaluation (mce/eval_robustness.py,
+    --robustness_type ce).  `update(logits, labels, distortion, n_valid=None)` counts the correct top-1
+    predictions of a batch into a per-distortion device counter (acnn_softmax_top1_count: no host
+    synchronisation); `add_counts` takes counts made elsewhere (a captured CUDA graph, another device);
+    `result()` reads the counters once and returns {'<distortion>': {'error', 'ce'}, ..., 'mCE',
+    'mCE_unnormalized'}.  It refuses a result while a distortion has no images."""
+
+    def __init__(self, device="cuda"):
+        self.device = torch.device(device)
+        self.correct = torch.zeros(len(DISTORTIONS), dtype=torch.int64, device=self.device)
+        self.count = [0] * len(DISTORTIONS)
+
+    @staticmethod
+    def index(distortion):
+        if distortion not in ALEXNET_CE:
+            raise ValueError("unknown distortion %r (one of %s)" % (distortion, list(DISTORTIONS)))
+        return DISTORTIONS.index(distortion)
+
+    def update(self, logits, labels, distortion, n_valid=None):
+        k = self.index(distortion)
+        n = logits.shape[0] if n_valid is None else int(n_valid)
+        labels = torch.as_tensor(labels).to(self.device, torch.int32).contiguous()
+        softmax_top1_count(logits, labels, self.correct[k:k + 1], n)
+        self.count[k] += n
+
+    def add_counts(self, distortion, correct, count):
+        k = self.index(distortion)
+        self.correct[k] += int(correct)
+        self.count[k] += int(count)
+
+    def result(self):
+        correct = self.correct.tolist()
+        return corruption_error_result({d: correct[k] for k, d in enumerate(DISTORTIONS)},
+                                       {d: self.count[k] for k, d in enumerate(DISTORTIONS)})

@@ -7,6 +7,8 @@ Mirrors (same names, argument meaning and error behaviour):
   * nets/run_loop_classification.py:60-234  resnet_model_fn (loss assembly, train op)
   * functions/model_fns.py:36-95     learning_rate_with_decay ; :26-33 keep_prob_decay
   * metric/recall_metric.py:13-180   recall_at_k (the zero-shot retrieval evaluation)
+  * mce/eval_robustness.py:161-326   show_corruption_error (the ImageNet-C robustness evaluation) as
+                                     corruption_error
 plus `build_model(**flags)` (the name BASELINE.json uses; the reference has no such function).
 
 The reference builds a TF graph and lets the Estimator run it; here a call executes on the GPU:
@@ -633,4 +635,184 @@ def recall_at_k(model, batches, num_val_images, recall_at_k=(1, 5), eval_similar
     assert metric.count == num_val_images, (metric.count, num_val_images)
     out = {"recall_at_%d" % k: v for k, v in metric.result().items()}
     out["global_step"] = global_step
+    return out
+
+
+def _replica(model, device, use_resnet_d, batch, size):
+    """`model` itself on its device, else a Model of the same flags on `device` with its weights."""
+    if torch.device(device) == torch.device(model.device):
+        return model
+    src = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d)
+    names = list(src.plan.params) + list(src.plan.state)
+    rep = Model(dtype=model.dtype, seed=model.seed, device=device, deterministic=model.deterministic,
+                native=model.native, **model.cfg_kwargs)
+    rep.set_weights({n: src.get_tf(n).detach().float().cpu().clone() for n in names})
+    return rep
+
+
+class _CorruptionEvalDevice:
+    """The evaluation loop of one device: decoded batches go from a pinned uint8 ring to one of two
+    device slots on a copy stream, overlapped with the previous batch's forward; the u8 -> f32 input
+    conversion, the eval forward and the top-1 count run as one CUDA graph per (slot, valid rows)."""
+
+    RING = 3        # pinned host batches
+
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph):
+        from .imagenet_c import CHANNEL_MEANS
+        self.dev = torch.device(model.device)
+        torch.cuda.set_device(self.dev)
+        self.rt = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d)
+        self.batch, self.use_graph = batch, use_cuda_graph
+        self.logits = self.rt.t[self.rt.plan.meta["logits"]][:, :model.num_classes]
+        u8 = dict(dtype=torch.uint8)
+        self.host = [(torch.zeros(batch, size, size, 3, **u8).pin_memory(),
+                      torch.zeros(batch, dtype=torch.int32).pin_memory()) for _ in range(self.RING)]
+        self.host_free = [None] * self.RING
+        self.slots = [(torch.zeros(batch, size, size, 3, **u8, device=self.dev),
+                       torch.zeros(batch, dtype=torch.int32, device=self.dev)) for _ in range(2)]
+        self.slot_free = [None, None]
+        self.mean = torch.tensor(CHANNEL_MEANS, dtype=torch.float32, device=self.dev)
+        self.acc = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.pred = torch.zeros(batch, dtype=torch.int32, device=self.dev)
+        self.copy_stream = torch.cuda.Stream(self.dev)
+        self.graphs = {}
+        self.warm = False
+        self.k = 0
+
+    def _body(self, slot, n_valid):
+        from .metrics import softmax_top1_count
+        images, labels = self.slots[slot]
+        self.rt.set_images_u8(images, self.mean)
+        self.rt.run_forward()
+        softmax_top1_count(self.logits, labels, self.acc, n_valid, self.pred)
+
+    def _graph(self, slot, n_valid):
+        g = self.graphs.get((slot, n_valid))
+        if g is None:
+            main = torch.cuda.current_stream(self.dev)
+            s = torch.cuda.Stream(self.dev)
+            s.wait_stream(main)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.stream(s):
+                # thread_local: the other devices' threads keep allocating and launching meanwhile
+                with torch.cuda.graph(g, stream=s, capture_error_mode="thread_local"):
+                    self._body(slot, n_valid)
+            main.wait_stream(s)
+            self.graphs[(slot, n_valid)] = g
+        return g
+
+    def run_batch(self, images, labels):
+        """Evaluate one batch: `images` a list of uint8 [H, W, 3] arrays (<= batch), `labels` ints."""
+        n, h, slot = len(images), self.k % self.RING, self.k % 2
+        self.k += 1
+        if self.host_free[h] is not None:
+            self.host_free[h].synchronize()          # its previous host -> device copy has run
+        hu8, hlab = self.host[h]
+        for i, a in enumerate(images):
+            hu8[i].copy_(torch.from_numpy(a))
+        hlab[:n].copy_(torch.as_tensor(labels, dtype=torch.int32))
+        du8, dlab = self.slots[slot]
+        main, cs = torch.cuda.current_stream(self.dev), self.copy_stream
+        if self.slot_free[slot] is not None:
+            cs.wait_event(self.slot_free[slot])       # the batch before the previous one has read it
+        with torch.cuda.stream(cs):
+            du8.copy_(hu8, non_blocking=True)
+            dlab.copy_(hlab, non_blocking=True)
+            copied = torch.cuda.Event()
+            copied.record(cs)
+        self.host_free[h] = copied
+        main.wait_event(copied)
+        if self.use_graph and self.warm:
+            self._graph(slot, n).replay()
+        else:
+            self._body(slot, n)        # the first batch also loads every kernel before any capture
+            self.warm = True
+        ev = torch.cuda.Event()
+        ev.record(main)
+        self.slot_free[slot] = ev
+
+    def take_count(self):
+        """The device count of correct predictions since the last call (a device tensor; no sync)."""
+        c = self.acc.clone()
+        self.acc.zero_()
+        return c
+
+
+def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=224, label_offset=1,
+                     robustness_type="ce", devices=None, use_resnet_d=None, global_step=None,
+                     use_cuda_graph=True, num_workers=None):
+    """mce/eval_robustness.py (show_corruption_error, --robustness_type ce): the top-1 error of `model`
+    on every distortion of ALEXNET_CE, pooled over data_dir/<distortion>/<severity 1..5>/<synset>/*,
+    its AlexNet-normalised CE and their means.  Labels are synsets2idx[synset dir] + label_offset from
+    `label_file`; images must decode to image_size x image_size (RGB), fed as uint8 minus CHANNEL_MEANS.
+
+    Decoding runs on a pool of `num_workers` CPU threads (PIL); the device work of a batch (uint8 ->
+    fp32, eval forward in the model's dtype, softmax top-1 count) is one CUDA graph replay
+    (use_cuda_graph=False: the same launches, eager).  The last batch of a distortion is padded to
+    batch_size and its padding rows are masked.  `devices` (default: the model's device) split the
+    distortions as the reference's process() does; every device gets a replica with the model's weights.
+    Returns {'<distortion>': {'error', 'ce'}, ..., 'mCE', 'mCE_unnormalized'} (+ 'global_step')."""
+    import threading
+    from concurrent.futures import ThreadPoolExecutor
+    from . import imagenet_c
+    from .metrics import DISTORTIONS, CorruptionError
+    if robustness_type == "fr":
+        raise ValueError("not yet supported ({}".format(robustness_type))
+    if robustness_type != "ce":
+        raise ValueError("invalid type ({})".format(robustness_type))
+    if use_resnet_d is None:
+        use_resnet_d = getattr(model, "use_resnet_d", False)
+    synsets2idx = imagenet_c.get_synsets2idx(label_file)
+    # the whole tree is walked first: a missing directory or an unknown synset fails before any GPU work
+    work = {d: imagenet_c.distortion_images(data_dir, d, synsets2idx, label_offset) for d in DISTORTIONS}
+    empty = [d for d in DISTORTIONS if not work[d][0]]
+    if empty:
+        raise ValueError("robustness evaluation: no images for distortion(s) %s" % empty)
+    devices = [torch.device(d) for d in (devices or [model.device])]
+    quota = imagenet_c.distortion_quota(len(devices))
+    metric = CorruptionError(device=devices[0])
+    replicas = [_replica(model, d, use_resnet_d, batch_size, image_size) for d in devices]
+    pool = ThreadPoolExecutor(max_workers=num_workers or min(32, os.cpu_count() or 1))
+    results, errors = [None] * len(devices), []
+
+    def run(i):
+        try:
+            ev = _CorruptionEvalDevice(replicas[i], batch_size, image_size, use_resnet_d, use_cuda_graph)
+            batches = [(d, work[d][0][a:a + batch_size], work[d][1][a:a + batch_size])
+                       for d in quota[i] for a in range(0, len(work[d][0]), batch_size)]
+            decode = lambda files: [pool.submit(imagenet_c.decode_image, f, image_size) for f in files]
+            ahead = 4                                   # batches decoding ahead of the GPU
+            pending = [decode(b[1]) for b in batches[:ahead]]
+            counts = {}
+            for j, (d, files, labels) in enumerate(batches):
+                futs = pending.pop(0)
+                if j + ahead < len(batches):
+                    pending.append(decode(batches[j + ahead][1]))
+                ev.run_batch([f.result() for f in futs], labels)
+                if j + 1 == len(batches) or batches[j + 1][0] != d:
+                    counts[d] = ev.take_count()
+            torch.cuda.current_stream(ev.dev).synchronize()
+            results[i] = {d: int(c.item()) for d, c in counts.items()}
+        except BaseException as e:        # re-raised in the calling thread
+            errors.append(e)
+
+    try:
+        if len(devices) == 1:
+            run(0)
+        else:
+            threads = [threading.Thread(target=run, args=(i,)) for i in range(len(devices))]
+            for t in threads:
+                t.start()
+            for t in threads:
+                t.join()
+    finally:
+        pool.shutdown(wait=True, cancel_futures=True)
+    if errors:
+        raise errors[0]
+    for counts in results:
+        for d, c in counts.items():
+            metric.add_counts(d, c, len(work[d][0]))
+    out = metric.result()
+    if global_step is not None:
+        out["global_step"] = global_step
     return out

@@ -81,6 +81,7 @@ PROTOTYPES = {
     "acnn_set_loss_scale": (_i, [_vp, C.c_double]),
     "acnn_set_dropblock": (_i, [_vp, C.c_uint64, _i]),
     "acnn_set_inputs": (_i, [_vp] * 7),
+    "acnn_set_images_u8": (_i, [_vp] * 4),
     "acnn_set_hparams": (_i, [_vp, _vp, _vp]),
     "acnn_get_logits": (_i, [_vp, _vp, _vp]),
     "acnn_get_loss": (_i, [_vp, _vp, _vp]),
@@ -376,6 +377,14 @@ class NativeRuntime(_runtime_base()):
             _lib.check(self.lib.acnn_run_ops(h, ops[i].phase, ops[i].index, ops[j].index + 1, st),
                        "acnn_run_ops(%s)" % ops[i].kind)
             i = j + 1
+
+    def set_images_u8(self, images_u8, mean):
+        """acnn_set_images_u8: the "images" buffer = (float)images_u8 - mean[c], images_u8 a CUDA uint8
+        tensor [input_batch, H, W, 3] on this device, mean a float32 tensor of 3 (host or device)."""
+        from .runtime import _check_u8_images
+        _check_u8_images(images_u8, self.t[self.plan.meta["images"]], mean)
+        _lib.check(self.lib.acnn_set_images_u8(self.model.handle, images_u8.data_ptr(), mean.data_ptr(),
+                                               self.stream), "acnn_set_images_u8")
 
     def zero_step_buffers(self):
         _lib.check(self.lib.acnn_clear_step_buffers(self.model.handle, self.stream),

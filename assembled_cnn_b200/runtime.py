@@ -16,6 +16,17 @@ from .plan import Plan, Geom, Slot
 _TORCH_DTYPE = {"bf16": torch.bfloat16, "f32": torch.float32, "i32": torch.int32}
 
 
+def _check_u8_images(images_u8, images, mean):
+    """Arguments of set_images_u8: uint8 NHWC of the input buffer's shape on its device, float32 mean[3]."""
+    if images_u8.dtype != torch.uint8 or tuple(images_u8.shape) != tuple(images.shape) \
+            or images_u8.device != images.device or not images_u8.is_contiguous():
+        raise ValueError("images_u8 must be a contiguous uint8 tensor %s on %s, got %s %s on %s"
+                         % (tuple(images.shape), images.device, images_u8.dtype, tuple(images_u8.shape),
+                            images_u8.device))
+    if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
+        raise ValueError("mean must be a contiguous float32 tensor of 3 values")
+
+
 class Runtime:
     def __init__(self, plan: Plan, device="cuda:0", eps: float = 1e-5, share: "Runtime | None" = None,
                  deterministic: "bool | None" = None):
@@ -241,6 +252,15 @@ class Runtime:
                 getattr(self, "op_" + op.kind)(op)
         if forked:
             main.wait_stream(side)                   # join before the optimizer
+
+    def set_images_u8(self, images_u8, mean):
+        """The "images" buffer = (float)images_u8 - mean[c] (acnn_images_from_u8), images_u8 a CUDA uint8
+        tensor [input_batch, H, W, 3] on this device, mean a float32 tensor of 3 (host or device)."""
+        images = self.t[self.plan.meta["images"]]
+        _check_u8_images(images_u8, images, mean)
+        b, h, w, _ = images.shape
+        _lib.check(self.lib.acnn_images_from_u8(images_u8.data_ptr(), mean.data_ptr(), images.data_ptr(), b, h, w,
+                                                self.stream), "acnn_images_from_u8")
 
     def zero_step_buffers(self):
         st = self.stream

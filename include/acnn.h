@@ -443,6 +443,28 @@ int64_t acnn_knn_work_bytes(int nq, int nx, int d, int k, int dtype);
  * setting. */
 int acnn_set_knn_splits(int n);
 
+/* ---------------------------------------------------------------------------------------------
+ * Robustness evaluation (mce/eval_robustness.py: ImageNet-C corruption error)
+ * ------------------------------------------------------------------------------------------- */
+/* out fp32 NHWC [B,H,W,3] = (float)images[b,h,w,c] - mean[c], images uint8 NHWC [B,H,W,3] (DEVICE):
+ * the tf.cast + mean_image_subtraction of input_fn_imagenet_c (mce/eval_robustness.py:123-148), the same
+ * fp32 subtraction.  mean: float[3], a host or a device array (a device one is read by the kernel, a
+ * host one when the call enqueues).  images and out must be 16-byte aligned. */
+int acnn_images_from_u8(const uint8_t* images, const float* mean, float* out, int B, int H, int W,
+                        void* stream);
+/* tf.nn.top_k(tf.nn.softmax(logits), 1) and the top-1 count of mce/eval_robustness.py:186-187,214-229.
+ * logits fp32 [B][ld] (columns < NC are the classes), labels int32 [B].  For every row r < n_valid:
+ * p_j = expf(x_j - max) / sum (the sum in a fixed order), pred[r] = the SMALLEST j with the largest p_j
+ * (tf.nn.top_k's rule applied to the fp32 probabilities: two distinct logits whose probabilities round
+ * to the same float tie, and the lower index wins), and *correct += 1 when pred[r] == labels[r].
+ * A row with a NaN or infinite logit gets pred[r] = -1 and is never counted as correct.
+ * Rows >= n_valid are padding: neither pred nor the count is touched for them.  The count uses integer
+ * atomics, so the result is the same under CUDA-graph replay and on concurrent streams.
+ * Null pointers, B < 1, NC < 1, ld < NC, n_valid outside [0, B]: ACNN_ERR_INVALID before any CUDA call;
+ * n_valid = 0 launches nothing. */
+int acnn_softmax_top1_count(const float* logits, int B, int ld, int NC, const int32_t* labels, int n_valid,
+                            int32_t* pred, uint64_t* correct, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

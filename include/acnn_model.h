@@ -175,6 +175,11 @@ int acnn_set_dropblock(acnn_model* m, uint64_t seed, int feed_uniforms);
 /* Copies host OR device arrays (cudaMemcpyDefault) into the static input buffers; NULL skips one. */
 int acnn_set_inputs(acnn_model* m, const float* images, const int32_t* labels, const float* lam1,
                     const float* lam2, const float* teacher_logits, void* stream);
+/* "images" = (float)images_dev - mean3[c] (acnn_images_from_u8) from uint8 NHWC [input_batch,H,W,3]:
+ * a quarter of the bytes of the fp32 input to copy to the device, one extra pass on it.  images_dev
+ * must be a DEVICE array (the caller stages its own buffer; a host pointer is ACNN_ERR_INVALID);
+ * mean3: float[3], host or device. */
+int acnn_set_images_u8(acnn_model* m, const uint8_t* images_dev, const float* mean3, void* stream);
 /* float hp[8] as in acnn_model_sizes.hp_offset. */
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream);
 /* logits [batch, num_classes] fp32 (dense, ld = num_classes) / loss float[4] to a host or device array. */
