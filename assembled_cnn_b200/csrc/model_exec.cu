@@ -896,6 +896,25 @@ int acnn_set_images_u8(acnn_model* m, const uint8_t* images_dev, const float* me
                              (int)t.shape[2], stream);
 }
 
+int acnn_set_images_resized(acnn_model* m, const acnn_resize_desc* desc_dev, int n_valid, const float* mean3,
+                            void* stream) {
+  ACNN_REQUIRE(m && m->bound && desc_dev && mean3, "acnn_set_images_resized: not bound / null");
+  const Plan& p = m->plan;
+  const Tensor& t = p.tensors[p.images];
+  ACNN_REQUIRE(t.shape[1] == t.shape[2], "acnn_set_images_resized: the plan's input is %lldx%lld, not square",
+               (long long)t.shape[1], (long long)t.shape[2]);
+  cudaPointerAttributes at{};
+  const cudaError_t e = cudaPointerGetAttributes(&at, desc_dev);
+  if (e != cudaSuccess) {
+    set_error("acnn_set_images_resized: %s", cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+               "acnn_set_images_resized: desc_dev must be device memory");
+  return acnn_resize_crop_u8(desc_dev, (int)t.shape[0], n_valid, (int)t.shape[1], mean3,
+                             (float*)(m->ws + t.ws_offset), stream);
+}
+
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream) {
   ACNN_REQUIRE(m && m->bound && hp, "acnn_set_hparams: not bound / null");
   return memcpy_async(m->ws + m->hp_off, hp, 32, stream, "acnn_set_hparams");

@@ -45,6 +45,9 @@ DEFAULTS = {
     "recall_at_k": [1, 5],                # :288
     "return_embedding": False,            # :27
     "val_batch_size": 256,                # :39
+    # classification evaluation (model_fns.evaluate_classification)
+    "preprocessing_type": "imagenet",     # :128
+    "val_regex": "validation-*",          # :284
     # official/utils/flags/_base.py:50-105, _performance.py:74-137
     "batch_size": 32,
     "train_epochs": 90,                   # main_classification.py:38

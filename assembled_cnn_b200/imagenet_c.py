@@ -59,11 +59,18 @@ def distortion_quota(num_gpus, distortions=DISTORTIONS):
     return out
 
 
+def decode_rgb(src):
+    """uint8 [H, W, 3] of an encoded image at its own size: `src` a path or a binary file object (PIL,
+    converted to RGB; for a JPEG, libjpeg's ISLOW DCT, TF's INTEGER_ACCURATE).  Image.draft is never
+    used: it trades pixels for speed."""
+    from PIL import Image
+    with Image.open(src) as im:
+        return np.array(im.convert("RGB"), dtype=np.uint8)
+
+
 def decode_image(path, image_size):
     """uint8 [image_size, image_size, 3] of an image file (PIL, converted to RGB)."""
-    from PIL import Image
-    with Image.open(path) as im:
-        a = np.array(im.convert("RGB"), dtype=np.uint8)
+    a = decode_rgb(path)
     if a.shape != (image_size, image_size, 3):
         raise ValueError("robustness evaluation: %s is %dx%d, expected %dx%d"
                          % (path, a.shape[1], a.shape[0], image_size, image_size))

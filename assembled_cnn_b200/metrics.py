@@ -260,3 +260,70 @@ class CorruptionError:
         correct = self.correct.tolist()
         return corruption_error_result({d: correct[k] for k, d in enumerate(DISTORTIONS)},
                                        {d: self.count[k] for k, d in enumerate(DISTORTIONS)})
+
+
+# --------------------------------------------------------------------------------------------------
+# ImageNet classification evaluation (classifier.evaluate(input_fn_eval), nets/run_loop_classification.py)
+# --------------------------------------------------------------------------------------------------
+def classify_rows(logits, labels, n_valid=None, k=5, label_smoothing=0.0, out=None):
+    """acnn_classify_rows on the current stream, for the rows r < n_valid of `logits` (CUDA fp32 [B, NC],
+    rows may be strided, as a model's logits view is) and `labels` (CUDA int32): pred = tf.argmax,
+    conf = the largest softmax probability, hit_k = tf.nn.in_top_k(k), ce = the label-smoothed softmax
+    cross-entropy.  Rows >= n_valid are not written.  `out` (pred int32, conf fp32, hit_k int32, ce fp32,
+    each of at least B) is allocated unless given; returns it."""
+    from . import _lib
+    lib = _lib.load()
+    if logits.dim() != 2 or logits.dtype != torch.float32 or logits.stride(1) != 1:
+        raise ValueError("logits must be a float32 [B, NC] tensor with unit column stride")
+    B, NC = logits.shape
+    n_valid = B if n_valid is None else int(n_valid)
+    if not (logits.is_cuda and labels.is_cuda):
+        raise _lib.AcnnError("classify_rows runs on the GPU: logits and labels must be CUDA tensors")
+    if labels.dtype != torch.int32 or labels.numel() < B or not labels.is_contiguous():
+        raise ValueError("labels must be a contiguous int32 tensor of at least B = %d values" % B)
+    if out is None:
+        out = tuple(torch.empty(B, dtype=dt, device=logits.device)
+                    for dt in (torch.int32, torch.float32, torch.int32, torch.float32))
+    for t, dt in zip(out, (torch.int32, torch.float32, torch.int32, torch.float32)):
+        if t.dtype != dt or t.numel() < B or not t.is_contiguous() or t.device != logits.device:
+            raise ValueError("out must be contiguous (int32, float32, int32, float32) tensors of at least B = %d "
+                             "values on %s" % (B, logits.device))
+    pred, conf, hit, ce = out
+    stream = torch.cuda.current_stream(logits.device).cuda_stream
+    _lib.check(lib.acnn_classify_rows(logits.data_ptr(), B, logits.stride(0), NC, labels.data_ptr(), n_valid, int(k),
+                                      float(label_smoothing), pred.data_ptr(), conf.data_ptr(), hit.data_ptr(),
+                                      ce.data_ptr(), stream), "acnn_classify_rows")
+    return out
+
+
+def classification_result(pred, conf, hit_k, ce, labels, batch_sizes, num_thresholds=10):
+    """The eval metrics of nets/run_loop_classification.py:141-234 from the per-row results of a whole
+    evaluation (numpy arrays, rows in evaluation order), in float64:
+      accuracy        tf.metrics.accuracy(labels, argmax)
+      accuracy_top_5  tf.metrics.mean(in_top_k(5))
+      ece             metric/ece_metric.py:171-298: bins (lo, hi] over the float32 thresholds
+                      [-1e-7, 0.1, ..., 0.9, 1 + 1e-7], acc and confidence per bin over (1e-7 + count),
+                      weighted by count / total; a NaN confidence falls in no bin
+      cross_entropy   the mean over batches of each batch's mean `ce` -- tf.metrics.mean of the per-batch
+                      loss, unweighted, so a short last batch counts as one batch."""
+    pred, labels = np.asarray(pred, np.int64), np.asarray(labels, np.int64)
+    conf, ce = np.asarray(conf, np.float32), np.asarray(ce, np.float64)
+    hit = np.asarray(hit_k).astype(bool)
+    sizes = [int(b) for b in batch_sizes]
+    n = len(labels)
+    if not (len(pred) == len(conf) == len(hit) == len(ce) == n) or sum(sizes) != n or n == 0 or min(sizes) < 1:
+        raise ValueError("classification_result: per-row arrays of one length, batch sizes summing to it")
+    correct = pred == labels
+    eps = 1e-7
+    th = [0.0 - eps] + [(i + 1) * 1.0 / num_thresholds for i in range(num_thresholds - 1)] + [1.0 + eps]
+    th = np.asarray(th, np.float32)
+    inb = (conf[None, :] > th[:-1, None]) & (conf[None, :] <= th[1:, None])
+    cnt = inb.sum(1).astype(np.float64)
+    acc = (inb & correct[None, :]).sum(1) / (eps + cnt)
+    avg = (np.where(inb, conf[None, :].astype(np.float64), 0.0)).sum(1) / (eps + cnt)
+    with np.errstate(invalid="ignore"):      # no row in any bin: 0 / 0, NaN as in the reference
+        ece = float((cnt / cnt.sum() * np.abs(acc - avg)).sum())
+    bounds = np.cumsum([0] + sizes)
+    batch_ce = [ce[a:b].mean() for a, b in zip(bounds[:-1], bounds[1:])]
+    return {"accuracy": float(correct.mean()), "accuracy_top_5": float(hit.mean()), "ece": ece,
+            "cross_entropy": float(np.mean(batch_ce))}

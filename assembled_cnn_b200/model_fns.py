@@ -9,6 +9,8 @@ Mirrors (same names, argument meaning and error behaviour):
   * metric/recall_metric.py:13-180   recall_at_k (the zero-shot retrieval evaluation)
   * mce/eval_robustness.py:161-326   show_corruption_error (the ImageNet-C robustness evaluation) as
                                      corruption_error
+  * nets/run_loop_classification.py:397-402,446-448  classifier.evaluate(input_fn_eval) (the ImageNet
+                                     classification evaluation) as evaluate_classification
 plus `build_model(**flags)` (the name BASELINE.json uses; the reference has no such function).
 
 The reference builds a TF graph and lets the Estimator run it; here a call executes on the GPU:
@@ -650,10 +652,11 @@ def _replica(model, device, use_resnet_d, batch, size):
     return rep
 
 
-class _CorruptionEvalDevice:
-    """The evaluation loop of one device: decoded batches go from a pinned uint8 ring to one of two
-    device slots on a copy stream, overlapped with the previous batch's forward; the u8 -> f32 input
-    conversion, the eval forward and the top-1 count run as one CUDA graph per (slot, valid rows)."""
+class _EvalPipeline:
+    """The evaluation loop of one device: decoded batches go from a ring of pinned host buffers to one of
+    two device slots on a copy stream, overlapped with the previous batch's forward; the device work of
+    a batch (`_body`: input preparation, eval forward, metric kernel) runs as one CUDA graph per (slot,
+    valid rows).  A subclass fills a host buffer and enqueues its copy (`_stage`) and defines `_body`."""
 
     RING = 3        # pinned host batches
 
@@ -664,27 +667,13 @@ class _CorruptionEvalDevice:
         self.rt = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d)
         self.batch, self.use_graph = batch, use_cuda_graph
         self.logits = self.rt.t[self.rt.plan.meta["logits"]][:, :model.num_classes]
-        u8 = dict(dtype=torch.uint8)
-        self.host = [(torch.zeros(batch, size, size, 3, **u8).pin_memory(),
-                      torch.zeros(batch, dtype=torch.int32).pin_memory()) for _ in range(self.RING)]
         self.host_free = [None] * self.RING
-        self.slots = [(torch.zeros(batch, size, size, 3, **u8, device=self.dev),
-                       torch.zeros(batch, dtype=torch.int32, device=self.dev)) for _ in range(2)]
         self.slot_free = [None, None]
         self.mean = torch.tensor(CHANNEL_MEANS, dtype=torch.float32, device=self.dev)
-        self.acc = torch.zeros(1, dtype=torch.int64, device=self.dev)
-        self.pred = torch.zeros(batch, dtype=torch.int32, device=self.dev)
         self.copy_stream = torch.cuda.Stream(self.dev)
         self.graphs = {}
         self.warm = False
         self.k = 0
-
-    def _body(self, slot, n_valid):
-        from .metrics import softmax_top1_count
-        images, labels = self.slots[slot]
-        self.rt.set_images_u8(images, self.mean)
-        self.rt.run_forward()
-        softmax_top1_count(self.logits, labels, self.acc, n_valid, self.pred)
 
     def _graph(self, slot, n_valid):
         g = self.graphs.get((slot, n_valid))
@@ -702,22 +691,16 @@ class _CorruptionEvalDevice:
         return g
 
     def run_batch(self, images, labels):
-        """Evaluate one batch: `images` a list of uint8 [H, W, 3] arrays (<= batch), `labels` ints."""
+        """Evaluate one batch of len(images) <= batch rows."""
         n, h, slot = len(images), self.k % self.RING, self.k % 2
         self.k += 1
         if self.host_free[h] is not None:
             self.host_free[h].synchronize()          # its previous host -> device copy has run
-        hu8, hlab = self.host[h]
-        for i, a in enumerate(images):
-            hu8[i].copy_(torch.from_numpy(a))
-        hlab[:n].copy_(torch.as_tensor(labels, dtype=torch.int32))
-        du8, dlab = self.slots[slot]
         main, cs = torch.cuda.current_stream(self.dev), self.copy_stream
         if self.slot_free[slot] is not None:
             cs.wait_event(self.slot_free[slot])       # the batch before the previous one has read it
         with torch.cuda.stream(cs):
-            du8.copy_(hu8, non_blocking=True)
-            dlab.copy_(hlab, non_blocking=True)
+            self._stage(h, slot, images, labels)
             copied = torch.cuda.Event()
             copied.record(cs)
         self.host_free[h] = copied
@@ -731,11 +714,107 @@ class _CorruptionEvalDevice:
         ev.record(main)
         self.slot_free[slot] = ev
 
+
+class _CorruptionEvalDevice(_EvalPipeline):
+    """The robustness evaluation's loop: fixed-size uint8 batches; the u8 -> f32 input conversion, the
+    eval forward and the top-1 count run as one CUDA graph per (slot, valid rows)."""
+
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph):
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
+        u8 = dict(dtype=torch.uint8)
+        self.host = [(torch.zeros(batch, size, size, 3, **u8).pin_memory(),
+                      torch.zeros(batch, dtype=torch.int32).pin_memory()) for _ in range(self.RING)]
+        self.slots = [(torch.zeros(batch, size, size, 3, **u8, device=self.dev),
+                       torch.zeros(batch, dtype=torch.int32, device=self.dev)) for _ in range(2)]
+        self.acc = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.pred = torch.zeros(batch, dtype=torch.int32, device=self.dev)
+
+    def _stage(self, h, slot, images, labels):
+        """`images` a list of uint8 [H, W, 3] arrays, `labels` ints."""
+        hu8, hlab = self.host[h]
+        for i, a in enumerate(images):
+            hu8[i].copy_(torch.from_numpy(a))
+        hlab[:len(images)].copy_(torch.as_tensor(labels, dtype=torch.int32))
+        du8, dlab = self.slots[slot]
+        du8.copy_(hu8, non_blocking=True)
+        dlab.copy_(hlab, non_blocking=True)
+
+    def _body(self, slot, n_valid):
+        from .metrics import softmax_top1_count
+        images, labels = self.slots[slot]
+        self.rt.set_images_u8(images, self.mean)
+        self.rt.run_forward()
+        softmax_top1_count(self.logits, labels, self.acc, n_valid, self.pred)
+
     def take_count(self):
         """The device count of correct predictions since the last call (a device tensor; no sync)."""
         c = self.acc.clone()
         self.acc.zero_()
         return c
+
+
+class _ClassifyEvalDevice(_EvalPipeline):
+    """The classification evaluation's loop: decoded images of any sizes are packed into a growable
+    pinned uint8 buffer with one acnn_resize_desc per image; resize + crop + mean, the eval forward and
+    the per-row metrics (acnn_classify_rows) run as one CUDA graph per (slot, valid rows).  The per-row
+    results of every batch are appended to device arrays of `total` rows (`rows`), read once at the end."""
+
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_smoothing, total):
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
+        i32 = dict(dtype=torch.int32)
+        self.size, self.label_smoothing = size, float(label_smoothing)
+        # pinned image bytes (grown on demand), labels, descriptors
+        self.host = [[torch.empty(0, dtype=torch.uint8), torch.zeros(batch, **i32).pin_memory(),
+                      torch.zeros(32 * batch, dtype=torch.uint8).pin_memory()] for _ in range(self.RING)]
+        # device image bytes (allocated on the copy stream, grown on demand), labels, descriptors: a graph
+        # holds the descriptor table's address only, so the image bytes may move
+        self.slots = [[None, torch.zeros(batch, **i32, device=self.dev),
+                       torch.zeros(32 * batch, dtype=torch.uint8, device=self.dev)] for _ in range(2)]
+        kinds = (torch.int32, torch.float32, torch.int32, torch.float32)       # pred, conf, hit_5, ce
+        self.out = tuple(torch.zeros(batch, dtype=dt, device=self.dev) for dt in kinds)
+        self.rows = tuple(torch.zeros(total, dtype=dt, device=self.dev) for dt in kinds)
+        self.done = 0
+
+    @staticmethod
+    def _grown(buf, nbytes, **kw):
+        if buf is not None and buf.numel() >= nbytes:
+            return buf
+        return torch.empty(max(nbytes + nbytes // 4, 1), dtype=torch.uint8, **kw)
+
+    def _stage(self, h, slot, images, labels):
+        """`images` a list of (uint8 [H, W, 3] array, eval_geometry) pairs, `labels` ints."""
+        from .imagenet_eval import DESC_DTYPE, check_descriptors
+        n = len(images)
+        offs = np.cumsum([0] + [(a.nbytes + 15) // 16 * 16 for a, _ in images])
+        total = int(offs[-1])
+        hbuf, hlab, hdesc = self.host[h]
+        hbuf = self.host[h][0] = self._grown(hbuf, total, pin_memory=True)
+        dbuf = self.slots[slot][0] = self._grown(self.slots[slot][0], total, device=self.dev)
+        hnp, base = hbuf.numpy(), dbuf.data_ptr()
+        desc = hdesc.numpy().view(DESC_DTYPE)
+        for i, (a, (s, rh, rw, cy, cx)) in enumerate(images):
+            hnp[offs[i]:offs[i] + a.nbytes] = a.reshape(-1)
+            desc[i] = (base + int(offs[i]), a.shape[0], a.shape[1], rh, rw, cy, cx)
+        check_descriptors(desc, n, self.size)
+        hlab[:n].copy_(torch.as_tensor(labels, dtype=torch.int32))
+        _, dlab, ddesc = self.slots[slot]
+        dbuf[:total].copy_(hbuf[:total], non_blocking=True)
+        ddesc.copy_(hdesc, non_blocking=True)
+        dlab.copy_(hlab, non_blocking=True)
+
+    def _body(self, slot, n_valid):
+        from .metrics import classify_rows
+        _, labels, desc = self.slots[slot]
+        self.rt.set_images_resized(desc, n_valid, self.mean)
+        self.rt.run_forward()
+        classify_rows(self.logits, labels, n_valid, 5, self.label_smoothing, out=self.out)
+
+    def run_batch(self, images, labels):
+        super().run_batch(images, labels)
+        n = len(images)
+        for dst, src in zip(self.rows, self.out):
+            dst[self.done:self.done + n].copy_(src[:n])
+        self.done += n
 
 
 def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=224, label_offset=1,
@@ -816,3 +895,60 @@ def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=
     if global_step is not None:
         out["global_step"] = global_step
     return out
+
+
+def evaluate_classification(model, data_dir, *, val_regex="validation-*", preprocessing_type="imagenet",
+                            image_size=224, batch_size=256, label_smoothing=0.0, weight_decay=4e-5,
+                            use_resnet_d=None, global_step=None, use_cuda_graph=True, num_workers=None):
+    """classifier.evaluate(input_fn_eval) (nets/run_loop_classification.py:397-402,446-448): top-1 and
+    top-5 accuracy, ECE and loss of `model` on the TFRecord shards data_dir/val_regex
+    (image/encoded, image/class/label), each image given the reference's eval preprocessing for
+    `preprocessing_type` (imagenet_eval.eval_geometry: aspect-preserving TF bilinear resize, central
+    crop, - CHANNEL_MEANS).
+
+    Every shard is read and checked first: an empty glob, a corrupt record or a label outside
+    [0, num_classes) fails before any GPU work.  Decoding runs on a pool of `num_workers` CPU threads
+    (PIL); the device work of a batch (resize + crop from uint8, eval forward in the model's dtype,
+    acnn_classify_rows) is one CUDA graph replay (use_cuda_graph=False: the same launches, eager).  The
+    last batch is padded to batch_size and its padding rows are masked; the per-row results stay on the
+    device until the end.  loss = the mean over batches of the batch-mean label-smoothed cross-entropy
+    (a short last batch counts as one batch, as tf.metrics.mean of the per-batch loss does) +
+    l2_loss(weight_decay).  Returns {'accuracy', 'accuracy_top_5', 'ece', 'loss', 'global_step'}."""
+    from concurrent.futures import ThreadPoolExecutor
+    from . import imagenet_eval
+    from .metrics import classification_result
+    size, _ = imagenet_eval.eval_size(preprocessing_type, image_size)
+    if use_resnet_d is None:
+        use_resnet_d = getattr(model, "use_resnet_d", False)
+    records = []
+    for path in imagenet_eval.validation_files(data_dir, val_regex):
+        for label, offset, length in imagenet_eval.read_records(path):
+            if not 0 <= label < model.num_classes:
+                raise ValueError("classification evaluation: %s: label %d (image at byte offset %d) outside "
+                                 "[0, %d)" % (path, label, offset, model.num_classes))
+            records.append((path, offset, length, label))
+    if not records:
+        raise ValueError("classification evaluation: the shards under %s hold no record" % data_dir)
+    labels = np.array([r[3] for r in records], dtype=np.int64)
+    batches = [records[a:a + batch_size] for a in range(0, len(records), batch_size)]
+    ev = _ClassifyEvalDevice(model, batch_size, size, use_resnet_d, use_cuda_graph, label_smoothing,
+                             len(records))
+    pool = ThreadPoolExecutor(max_workers=num_workers or min(32, os.cpu_count() or 1))
+    decode = lambda recs: [pool.submit(imagenet_eval.decode_record, r[0], r[1], r[2], preprocessing_type,
+                                       image_size) for r in recs]
+    try:
+        ahead = 4                                   # batches decoding ahead of the GPU
+        pending = [decode(b) for b in batches[:ahead]]
+        for j, recs in enumerate(batches):
+            futs = pending.pop(0)
+            if j + ahead < len(batches):
+                pending.append(decode(batches[j + ahead]))
+            ev.run_batch([f.result() for f in futs], [r[3] for r in recs])
+        torch.cuda.current_stream(ev.dev).synchronize()
+    finally:
+        pool.shutdown(wait=True, cancel_futures=True)
+    pred, conf, hit, ce = (t.cpu().numpy() for t in ev.rows)
+    r = classification_result(pred, conf, hit, ce, labels, [len(b) for b in batches])
+    l2 = float(l2_loss(ev.rt, weight_decay))
+    return {"accuracy": r["accuracy"], "accuracy_top_5": r["accuracy_top_5"], "ece": r["ece"],
+            "loss": r["cross_entropy"] + l2, "global_step": global_step}

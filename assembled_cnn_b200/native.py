@@ -82,6 +82,7 @@ PROTOTYPES = {
     "acnn_set_dropblock": (_i, [_vp, C.c_uint64, _i]),
     "acnn_set_inputs": (_i, [_vp] * 7),
     "acnn_set_images_u8": (_i, [_vp] * 4),
+    "acnn_set_images_resized": (_i, [_vp, _vp, _i, _vp, _vp]),
     "acnn_set_hparams": (_i, [_vp, _vp, _vp]),
     "acnn_get_logits": (_i, [_vp, _vp, _vp]),
     "acnn_get_loss": (_i, [_vp, _vp, _vp]),
@@ -385,6 +386,15 @@ class NativeRuntime(_runtime_base()):
         _check_u8_images(images_u8, self.t[self.plan.meta["images"]], mean)
         _lib.check(self.lib.acnn_set_images_u8(self.model.handle, images_u8.data_ptr(), mean.data_ptr(),
                                                self.stream), "acnn_set_images_u8")
+
+    def set_images_resized(self, desc, n_valid, mean):
+        """acnn_set_images_resized: the "images" buffer from decoded uint8 images of any sizes (resize,
+        central crop, - mean[c]); desc a CUDA uint8 tensor of input_batch 32-byte acnn_resize_desc on
+        this device, validated by the caller; mean a float32 tensor of 3 (host or device)."""
+        from .runtime import _check_resize_args
+        _check_resize_args(desc, self.t[self.plan.meta["images"]], n_valid, mean)
+        _lib.check(self.lib.acnn_set_images_resized(self.model.handle, desc.data_ptr(), int(n_valid),
+                                                    mean.data_ptr(), self.stream), "acnn_set_images_resized")
 
     def zero_step_buffers(self):
         _lib.check(self.lib.acnn_clear_step_buffers(self.model.handle, self.stream),

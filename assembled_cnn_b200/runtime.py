@@ -27,6 +27,23 @@ def _check_u8_images(images_u8, images, mean):
         raise ValueError("mean must be a contiguous float32 tensor of 3 values")
 
 
+def _check_resize_args(desc, images, n_valid, mean):
+    """Arguments of set_images_resized: a square input buffer, B descriptors of 32 bytes on its device,
+    n_valid in [0, B], float32 mean[3].  Returns (B, S)."""
+    b, h, w, _ = images.shape
+    if h != w:
+        raise ValueError("set_images_resized needs a square input buffer, got %dx%d" % (h, w))
+    if desc.dtype != torch.uint8 or desc.numel() != 32 * b or desc.device != images.device \
+            or not desc.is_contiguous():
+        raise ValueError("desc must be a contiguous uint8 tensor of %d descriptors (%d bytes) on %s"
+                         % (b, 32 * b, images.device))
+    if not 0 <= int(n_valid) <= b:
+        raise ValueError("n_valid=%d outside [0, %d]" % (int(n_valid), b))
+    if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
+        raise ValueError("mean must be a contiguous float32 tensor of 3 values")
+    return b, h
+
+
 class Runtime:
     def __init__(self, plan: Plan, device="cuda:0", eps: float = 1e-5, share: "Runtime | None" = None,
                  deterministic: "bool | None" = None):
@@ -261,6 +278,16 @@ class Runtime:
         b, h, w, _ = images.shape
         _lib.check(self.lib.acnn_images_from_u8(images_u8.data_ptr(), mean.data_ptr(), images.data_ptr(), b, h, w,
                                                 self.stream), "acnn_images_from_u8")
+
+    def set_images_resized(self, desc, n_valid, mean):
+        """The "images" buffer [B, S, S, 3] from decoded uint8 images of any sizes (acnn_resize_crop_u8:
+        resize, central crop, - mean[c]).  desc: a CUDA uint8 tensor of B 32-byte acnn_resize_desc
+        (imagenet_eval.DESC_DTYPE) on this device, validated by the caller; rows >= n_valid are not
+        written; mean a float32 tensor of 3 (host or device)."""
+        images = self.t[self.plan.meta["images"]]
+        b, s = _check_resize_args(desc, images, n_valid, mean)
+        _lib.check(self.lib.acnn_resize_crop_u8(desc.data_ptr(), b, int(n_valid), s, mean.data_ptr(),
+                                                images.data_ptr(), self.stream), "acnn_resize_crop_u8")
 
     def zero_step_buffers(self):
         st = self.stream

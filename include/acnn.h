@@ -465,6 +465,48 @@ int acnn_images_from_u8(const uint8_t* images, const float* mean, float* out, in
 int acnn_softmax_top1_count(const float* logits, int B, int ld, int NC, const int32_t* labels, int n_valid,
                             int32_t* pred, uint64_t* correct, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Classification evaluation (classifier.evaluate(input_fn_eval), nets/run_loop_classification.py)
+ * ------------------------------------------------------------------------------------------- */
+/* One decoded image of a batch: uint8 RGB [src_h][src_w][3] at `src` (DEVICE), resized to
+ * [rsz_h][rsz_w] and cropped to the S x S window at (crop_y, crop_x).  32 bytes, the layout of
+ * imagenet_eval.DESC_DTYPE. */
+typedef struct acnn_resize_desc {
+  const uint8_t* src;
+  int32_t src_h, src_w;
+  int32_t rsz_h, rsz_w;
+  int32_t crop_y, crop_x;
+} acnn_resize_desc;
+/* out fp32 NHWC [B,S,S,3], row b < n_valid = central_crop(resize_bilinear(img_b, rsz_h, rsz_w), S, S)
+ * - mean[c]: the eval preprocessing of preprocessing/imagenet_preprocessing.py:295-313.  The resize is
+ * TF 1.14's legacy bilinear (align_corners = false, half_pixel_centers = false), bit for bit:
+ * scale = (float)src / rsz, in = i * scale, lower = max(floor(in), 0), upper = min(ceil(in), src - 1),
+ * lerp = in - floor(in), top = tl + (tr - tl) * x_lerp, bottom likewise, out = top + (bottom - top) *
+ * y_lerp, then - mean[c]; every step a separately rounded fp32 operation (no FMA).  Only the S x S
+ * pixels the crop keeps are computed, at resized coordinates (y + crop_y, x + crop_x).
+ * desc: a DEVICE array of B descriptors (a captured CUDA graph holds only its address, so the image
+ * buffers it points to may move between replays).  The descriptors are not checked here: the caller
+ * guarantees src_h, src_w >= 1, 0 <= crop_y <= rsz_h - S, 0 <= crop_x <= rsz_w - S.  mean: float[3],
+ * host or device.  Rows >= n_valid are not written.  Null pointers, B < 1, S < 1, n_valid outside
+ * [0, B], out not 4-byte or desc not 8-byte aligned: ACNN_ERR_INVALID before any CUDA call. */
+int acnn_resize_crop_u8(const acnn_resize_desc* desc, int B, int n_valid, int S, const float* mean, float* out,
+                        void* stream);
+/* Per-row results of the classification metrics for logits fp32 [B][ld] (columns < NC are the
+ * classes) and labels int32 [B], for every row r < n_valid (rows >= n_valid are not written):
+ *   pred[r]  = tf.argmax(logits): the smallest index of the largest logit;
+ *   conf[r]  = the largest softmax probability, 1 / sum_j expf(x_j - max) (the sum in a fixed order);
+ *   hit_k[r] = tf.nn.in_top_k(logits, label, k): 1 when fewer than k logits are strictly greater than
+ *              the label's (ties count as in), 0 when the label is outside [0, NC);
+ *   ce[r]    = -((1 - ls) log p[label] + ls / NC sum_j log p_j), tf.losses.softmax_cross_entropy with
+ *              label_smoothing = ls; NaN when the label is outside [0, NC).
+ * A row with a NaN or infinite logit gets pred = -1, conf = NaN, hit_k = 0, ce = NaN.  No atomics:
+ * the results are the same under CUDA-graph replay and on concurrent streams.  Null pointers, B < 1,
+ * NC < 1, ld < NC, n_valid outside [0, B], k < 1, a non-finite ls: ACNN_ERR_INVALID before any CUDA
+ * call; n_valid = 0 launches nothing. */
+int acnn_classify_rows(const float* logits, int B, int ld, int NC, const int32_t* labels, int n_valid, int k,
+                       float label_smoothing, int32_t* pred, float* conf, int32_t* hit_k, float* ce,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

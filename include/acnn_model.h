@@ -180,6 +180,12 @@ int acnn_set_inputs(acnn_model* m, const float* images, const int32_t* labels, c
  * must be a DEVICE array (the caller stages its own buffer; a host pointer is ACNN_ERR_INVALID);
  * mean3: float[3], host or device. */
 int acnn_set_images_u8(acnn_model* m, const uint8_t* images_dev, const float* mean3, void* stream);
+/* "images" [input_batch,S,S,3] from a batch of decoded uint8 images of any sizes through
+ * acnn_resize_crop_u8 (resize, central crop, - mean3[c]), S = the plan's H = W.  desc_dev: a DEVICE
+ * array of input_batch acnn_resize_desc (checked by the caller, see acnn_resize_crop_u8); rows >=
+ * n_valid are not written; mean3: float[3], host or device. */
+int acnn_set_images_resized(acnn_model* m, const acnn_resize_desc* desc_dev, int n_valid, const float* mean3,
+                            void* stream);
 /* float hp[8] as in acnn_model_sizes.hp_offset. */
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream);
 /* logits [batch, num_classes] fp32 (dense, ld = num_classes) / loss float[4] to a host or device array. */
