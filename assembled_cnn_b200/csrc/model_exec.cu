@@ -915,6 +915,24 @@ int acnn_set_images_resized(acnn_model* m, const acnn_resize_desc* desc_dev, int
                              (float*)(m->ws + t.ws_offset), stream);
 }
 
+int acnn_set_images_cropped(acnn_model* m, const acnn_crop_desc* desc_dev, const float* mean3, void* stream) {
+  ACNN_REQUIRE(m && m->bound && desc_dev && mean3, "acnn_set_images_cropped: not bound / null");
+  const Plan& p = m->plan;
+  const Tensor& t = p.tensors[p.images];
+  ACNN_REQUIRE(t.shape[1] == t.shape[2], "acnn_set_images_cropped: the plan's input is %lldx%lld, not square",
+               (long long)t.shape[1], (long long)t.shape[2]);
+  cudaPointerAttributes at{};
+  const cudaError_t e = cudaPointerGetAttributes(&at, desc_dev);
+  if (e != cudaSuccess) {
+    set_error("acnn_set_images_cropped: %s", cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+               "acnn_set_images_cropped: desc_dev must be device memory");
+  return acnn_crop_resize_u8(desc_dev, (int)t.shape[0], (int)t.shape[0], (int)t.shape[1], mean3,
+                             (float*)(m->ws + t.ws_offset), stream);
+}
+
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream) {
   ACNN_REQUIRE(m && m->bound && hp, "acnn_set_hparams: not bound / null");
   return memcpy_async(m->ws + m->hp_off, hp, 32, stream, "acnn_set_hparams");

@@ -48,6 +48,17 @@ DEFAULTS = {
     # classification evaluation (model_fns.evaluate_classification)
     "preprocessing_type": "imagenet",     # :128
     "val_regex": "validation-*",          # :284
+    # training from TFRecord shards (model_fns.train_and_evaluate)
+    "train_regex": "train-*",             # :280
+    "training_random_crop": True,         # :256
+    "autoaugment_type": None,             # :132 (only None: AutoAugment is not implemented)
+    "num_best_ckpt_to_keep": 3,           # :242
+    "keep_ckpt_every_eval": True,         # :246
+    "keep_checkpoint_max": 20,            # :249
+    "eval_only": False,                   # :252
+    "save_checkpoints_epochs": 1.0,       # :266
+    "ratio_fine_eval": 1.0,               # :269
+    "pretrained_model_checkpoint_path": None,   # :43
     # official/utils/flags/_base.py:50-105, _performance.py:74-137
     "batch_size": 32,
     "train_epochs": 90,                   # main_classification.py:38

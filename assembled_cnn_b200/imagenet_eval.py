@@ -93,12 +93,29 @@ def _fields(buf, pos, end):
         yield field, wt, v
 
 
-def parse_example(buf):
+def _float_list(buf, feature):
+    """float32 array of a Feature's float_list(2) -> value(1), packed (fixed32 run) or not."""
+    vals = []
+    for f, wt, v in _fields(buf, *feature):
+        if f == 2 and wt == 2:                       # FloatList
+            for f2, wt2, v2 in _fields(buf, *v):
+                if f2 == 1 and wt2 == 5:
+                    vals.append(bytes(buf[v2:v2 + 4]))
+                elif f2 == 1 and wt2 == 2:
+                    if (v2[1] - v2[0]) % 4:
+                        raise ValueError("packed FloatList of %d bytes" % (v2[1] - v2[0]))
+                    vals.append(bytes(buf[v2[0]:v2[1]]))
+    return np.frombuffer(b"".join(vals), dtype="<f4").astype(np.float32)
+
+
+def parse_example(buf, logits=False):
     """(label, (start, end) of the encoded image in buf) of a serialised tf.train.Example: the
     'image/class/label' int64 and 'image/encoded' bytes features (parse_example_proto).  Only the
     protobuf wire format is read: Example.features(1) -> Features.feature(1) map entries {key(1),
     value(2)} -> Feature.bytes_list(1) / int64_list(3) -> value(1).  A repeated key keeps its last
-    value, as protobuf's map parsing does."""
+    value, as protobuf's map parsing does.  logits=True appends the float32 values of the
+    'image/logit' FloatList (the knowledge-distillation teacher logits; empty when the feature is
+    absent, as tf.VarLenFeature)."""
     feats = {}
     for f, wt, v in _fields(buf, 0, len(buf)):
         if f != 1 or wt != 2:
@@ -112,7 +129,7 @@ def parse_example(buf):
                     key = bytes(buf[kv[0]:kv[1]])
                 elif f3 == 2 and wt3 == 2:
                     value = kv
-            if key in (b"image/encoded", b"image/class/label"):
+            if key in (b"image/encoded", b"image/class/label", b"image/logit"):
                 feats[key] = value
     if b"image/encoded" not in feats or b"image/class/label" not in feats:
         raise ValueError("Example without image/encoded or image/class/label")
@@ -135,15 +152,19 @@ def parse_example(buf):
         raise ValueError("image/encoded and image/class/label must hold one value each (got %d, %d)"
                          % (len(enc), len(labels)))
     label = labels[0] - (1 << 64) if labels[0] >= 1 << 63 else labels[0]
+    if logits:
+        lg = _float_list(buf, feats[b"image/logit"]) if feats.get(b"image/logit") else np.zeros(0, np.float32)
+        return label, enc[0], lg
     return label, enc[0]
 
 
-def read_records(path):
+def read_records(path, logits=False):
     """[(label, offset, length)] of every record of a TFRecord file: the label and the byte range of the
-    encoded image in the file.  A record is u64 length, u32 masked CRC32C of the length, the data, u32
-    masked CRC32C of the data.  The length's CRC is verified; the data's is not (a pure-Python CRC over the
-    6.4 GB of ImageNet validation JPEGs would take far longer than the evaluation).  A truncated or corrupt
-    record raises ValueError naming the file and the record's byte offset."""
+    encoded image in the file (logits=True: [(label, offset, length, float32 image/logit values)]).  A
+    record is u64 length, u32 masked CRC32C of the length, the data, u32 masked CRC32C of the data.  The
+    length's CRC is verified; the data's is not (a pure-Python CRC over the 6.4 GB of ImageNet validation
+    JPEGs would take far longer than the evaluation).  A truncated or corrupt record raises ValueError
+    naming the file and the record's byte offset."""
     with open(path, "rb") as f:
         data = f.read()
     out, pos, n = [], 0, len(data)
@@ -159,10 +180,11 @@ def read_records(path):
         if start + length + 4 > n:
             raise ValueError("%s: truncated record at byte offset %d" % (path, pos))
         try:
-            label, (a, b) = parse_example(memoryview(data)[start:start + length])
+            ex = parse_example(memoryview(data)[start:start + length], logits)
         except ValueError as e:
             raise ValueError("%s: bad tf.train.Example in the record at byte offset %d: %s" % (path, pos, e))
-        out.append((label, start + a, b - a))
+        label, (a, b) = ex[:2]
+        out.append((label, start + a, b - a) + tuple(ex[2:]))
         pos = start + length + 4
     return out
 

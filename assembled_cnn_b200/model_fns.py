@@ -289,7 +289,9 @@ class Trainer:
     get_train_op): owns the step's static buffers, the LR schedule and the CUDA graphs."""
 
     def __init__(self, model: Model, params: dict, height=224, width=224, *, use_cuda_graph=True,
-                 lam_seed=7):
+                 lam_seed=7, num_images=None):
+        """num_images: training images per epoch for the LR and keep-prob schedules (default: the
+        dataset's data_config count)."""
         p = params
         if p.get("cls_loss_type", "softmax") != "softmax":
             raise NotImplementedError("only cls_loss_type='softmax' is on the hot path")
@@ -306,15 +308,17 @@ class Trainer:
                                 label_smoothing=float(p.get("label_smoothing", 0.0)),
                                 use_dropblock=self.use_dropblock, kd_temp=self.kd_temp)
         ds = DATASETS[p.get("dataset_name") or "imagenet"]
+        if num_images is None:
+            num_images = ds["num_images"]["train"]
         # functions/model_fns.py:221-228: keep_prob decays linearly over the whole run
         self.keep_prob_fn = None
         if self.use_dropblock:
             kp0, kp1 = p["dropblock_kp"]
-            bpe = ds["num_images"]["train"] / p["batch_size"]
+            bpe = num_images / p["batch_size"]
             self.keep_prob_fn = keep_prob_decay(kp0, kp1, int(p["train_epochs"] * bpe))
         self.learning_rate_fn = learning_rate_with_decay(
             learning_rate_decay_type=p["learning_rate_decay_type"], batch_size=p["batch_size"],
-            batch_denom=p["batch_size"], num_images=ds["num_images"]["train"],
+            batch_denom=p["batch_size"], num_images=num_images,
             num_epochs_per_decay=p["num_epochs_per_decay"],
             learning_rate_decay_factor=p["learning_rate_decay_factor"],
             end_learning_rate=p["end_learning_rate"],
@@ -435,6 +439,19 @@ class Trainer:
         if images is self._stage_imgs:
             self._consumed = torch.cuda.Event()
             self._consumed.record(torch.cuda.current_stream(rt.dev))
+        return self._step(lam1, lam2, teacher_logits, keep_prob)
+
+    def train_step_cropped(self, desc, labels, mean, lam1=None, lam2=None, teacher_logits=None, keep_prob=None):
+        """train_step with the images made on the device from training crop windows: one
+        acnn_set_images_cropped launch (flip, resize to H x W, - mean) on the current stream, then the step.
+        desc: a CUDA uint8 tensor of input_batch 32-byte acnn_crop_desc (imagenet_train.CROP_DESC_DTYPE,
+        checked by the caller); labels int32 [input_batch]; the rest as train_step."""
+        self.rt.set_images_cropped(desc, mean)
+        self.labels_buf.copy_(labels, non_blocking=True)
+        return self._step(lam1, lam2, teacher_logits, keep_prob)
+
+    def _step(self, lam1, lam2, teacher_logits, keep_prob):
+        rt = self.rt
         if self.mixup_type:
             n = self.input_batch // 2
             if lam1 is None:
@@ -652,6 +669,27 @@ def _replica(model, device, use_resnet_d, batch, size):
     return rep
 
 
+def _grown(buf, nbytes, **kw):
+    if buf is not None and buf.numel() >= nbytes:
+        return buf
+    return torch.empty(max(nbytes + nbytes // 4, 1), dtype=torch.uint8, **kw)
+
+
+def _pack_u8(hbuf, dbuf, arrays, device):
+    """Packs uint8 arrays at 16-byte aligned offsets into the pinned host buffer `hbuf` and enqueues its copy
+    to the device buffer `dbuf` on the current stream; either buffer is replaced by a larger one when it is
+    too small (None: allocate).  Returns (hbuf, dbuf, the device address of each array)."""
+    offs = np.cumsum([0] + [(a.nbytes + 15) // 16 * 16 for a in arrays])
+    total = int(offs[-1])
+    hbuf = _grown(hbuf, total, pin_memory=True)
+    dbuf = _grown(dbuf, total, device=device)
+    hnp, base = hbuf.numpy(), dbuf.data_ptr()
+    for a, o in zip(arrays, offs):
+        hnp[o:o + a.nbytes] = a.reshape(-1)
+    dbuf[:total].copy_(hbuf[:total], non_blocking=True)
+    return hbuf, dbuf, [base + int(o) for o in offs[:-1]]
+
+
 class _EvalPipeline:
     """The evaluation loop of one device: decoded batches go from a ring of pinned host buffers to one of
     two device slots on a copy stream, overlapped with the previous batch's forward; the device work of
@@ -775,30 +813,19 @@ class _ClassifyEvalDevice(_EvalPipeline):
         self.rows = tuple(torch.zeros(total, dtype=dt, device=self.dev) for dt in kinds)
         self.done = 0
 
-    @staticmethod
-    def _grown(buf, nbytes, **kw):
-        if buf is not None and buf.numel() >= nbytes:
-            return buf
-        return torch.empty(max(nbytes + nbytes // 4, 1), dtype=torch.uint8, **kw)
-
     def _stage(self, h, slot, images, labels):
         """`images` a list of (uint8 [H, W, 3] array, eval_geometry) pairs, `labels` ints."""
         from .imagenet_eval import DESC_DTYPE, check_descriptors
         n = len(images)
-        offs = np.cumsum([0] + [(a.nbytes + 15) // 16 * 16 for a, _ in images])
-        total = int(offs[-1])
         hbuf, hlab, hdesc = self.host[h]
-        hbuf = self.host[h][0] = self._grown(hbuf, total, pin_memory=True)
-        dbuf = self.slots[slot][0] = self._grown(self.slots[slot][0], total, device=self.dev)
-        hnp, base = hbuf.numpy(), dbuf.data_ptr()
+        self.host[h][0], self.slots[slot][0], addrs = _pack_u8(hbuf, self.slots[slot][0], [a for a, _ in images],
+                                                              self.dev)
         desc = hdesc.numpy().view(DESC_DTYPE)
         for i, (a, (s, rh, rw, cy, cx)) in enumerate(images):
-            hnp[offs[i]:offs[i] + a.nbytes] = a.reshape(-1)
-            desc[i] = (base + int(offs[i]), a.shape[0], a.shape[1], rh, rw, cy, cx)
+            desc[i] = (addrs[i], a.shape[0], a.shape[1], rh, rw, cy, cx)
         check_descriptors(desc, n, self.size)
         hlab[:n].copy_(torch.as_tensor(labels, dtype=torch.int32))
         _, dlab, ddesc = self.slots[slot]
-        dbuf[:total].copy_(hbuf[:total], non_blocking=True)
         ddesc.copy_(hdesc, non_blocking=True)
         dlab.copy_(hlab, non_blocking=True)
 
@@ -952,3 +979,227 @@ def evaluate_classification(model, data_dir, *, val_regex="validation-*", prepro
     l2 = float(l2_loss(ev.rt, weight_decay))
     return {"accuracy": r["accuracy"], "accuracy_top_5": r["accuracy_top_5"], "ece": r["ece"],
             "loss": r["cross_entropy"] + l2, "global_step": global_step}
+
+
+class _TrainFeed:
+    """The training input's staging ring: per step, the crop windows packed into a growable pinned uint8
+    buffer with one acnn_crop_desc each, the labels and (KD) the teacher logits, copied to one of two
+    device slots on a copy stream while the previous step computes; `step` makes the images on the device
+    (Trainer.train_step_cropped) and runs the training step."""
+
+    RING = 3        # pinned host batches
+
+    def __init__(self, trainer, kd):
+        from .imagenet_c import CHANNEL_MEANS
+        self.tr, self.dev = trainer, trainer.rt.dev
+        n, nc = trainer.input_batch, trainer.model.num_classes
+        i32, f32 = dict(dtype=torch.int32), dict(dtype=torch.float32)
+        self.host = [[None, torch.zeros(n, **i32).pin_memory(), torch.zeros(32 * n, dtype=torch.uint8).pin_memory(),
+                      torch.zeros(n, nc, **f32).pin_memory() if kd else None] for _ in range(self.RING)]
+        # a step's graph holds no address of these: the image bytes may move when the buffer grows
+        self.slots = [[None, torch.zeros(n, **i32, device=self.dev),
+                       torch.zeros(32 * n, dtype=torch.uint8, device=self.dev),
+                       torch.zeros(n, nc, **f32, device=self.dev) if kd else None] for _ in range(2)]
+        self.mean = torch.tensor(CHANNEL_MEANS, dtype=torch.float32, device=self.dev)
+        self.copy_stream = torch.cuda.Stream(self.dev)
+        self.host_free = [None] * self.RING
+        self.slot_free = [None, None]
+        self.copied = [None, None]
+        self.staged = self.consumed = 0
+
+    def stage(self, windows, labels, teacher_logits=None):
+        """`windows` input_batch (uint8 [h, w, 3] array, flip) pairs, `labels` ints, `teacher_logits` float32
+        [input_batch, num_classes] with KD."""
+        from .imagenet_train import CROP_DESC_DTYPE, check_crop_descriptors
+        h, slot = self.staged % self.RING, self.staged % 2
+        self.staged += 1
+        if self.host_free[h] is not None:
+            self.host_free[h].synchronize()          # its previous host -> device copy has run
+        cs = self.copy_stream
+        if self.slot_free[slot] is not None:
+            cs.wait_event(self.slot_free[slot])       # the step before the previous one has read it
+        with torch.cuda.stream(cs):
+            hbuf, hlab, hdesc, hteach = self.host[h]
+            self.host[h][0], self.slots[slot][0], addrs = _pack_u8(hbuf, self.slots[slot][0],
+                                                                  [a for a, _ in windows], self.dev)
+            desc = hdesc.numpy().view(CROP_DESC_DTYPE)
+            for i, (a, flip) in enumerate(windows):
+                desc[i] = (addrs[i], a.shape[0], a.shape[1], int(flip), (0, 0, 0))
+            check_crop_descriptors(desc)
+            hlab.copy_(torch.as_tensor(labels, dtype=torch.int32))
+            _, dlab, ddesc, dteach = self.slots[slot]
+            ddesc.copy_(hdesc, non_blocking=True)
+            dlab.copy_(hlab, non_blocking=True)
+            if dteach is not None:
+                hteach.copy_(torch.as_tensor(teacher_logits, dtype=torch.float32))
+                dteach.copy_(hteach, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(cs)
+        self.host_free[h] = self.copied[slot] = ev
+
+    def step(self, lam1=None, lam2=None):
+        """The training step of the oldest staged batch; returns Trainer.train_step's loss tensor."""
+        slot = self.consumed % 2
+        self.consumed += 1
+        main = torch.cuda.current_stream(self.dev)
+        main.wait_event(self.copied[slot])
+        _, dlab, ddesc, dteach = self.slots[slot]
+        loss = self.tr.train_step_cropped(ddesc, dlab, self.mean, lam1=lam1, lam2=lam2, teacher_logits=dteach)
+        ev = torch.cuda.Event()
+        ev.record(main)
+        self.slot_free[slot] = ev
+        return loss
+
+
+def _prune_checkpoints(model_dir, keep):
+    """RunConfig(keep_checkpoint_max): only the `keep` newest model.ckpt-<step>.npz stay in model_dir."""
+    import glob
+    found = []
+    for f in glob.glob(os.path.join(model_dir, "model.ckpt-*.npz")):
+        try:
+            found.append((int(os.path.basename(f)[len("model.ckpt-"):-4]), f))
+        except ValueError:
+            continue
+    for _, f in sorted(found)[:max(len(found) - keep, 0)]:
+        os.remove(f)
+
+
+def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_threshold=None, max_train_steps=None,
+                       image_size=224, seed=0, use_cuda_graph=True, num_workers=None, **flags):
+    """resnet_main's train-and-evaluate loop (nets/run_loop_classification.py:389-489) over the TFRecord
+    shards data_dir/train_regex (training) and data_dir/val_regex (evaluation).  `flags` are hparams
+    names (params_from_flags); epochs_between_evals, stop_threshold and max_train_steps are the run loop's
+    flags of official/utils/flags (_base.py:51-63, _performance.py:96-97) with their defaults; image_size is
+    the `imagenet` preprocessing type's size.
+
+    Every training record is read and checked first (imagenet_train.read_train_records).  The latest
+    model.ckpt-<step> in model_dir is restored (weights, momentum slots, global_step), else
+    pretrained_model_checkpoint_path warm-starts the run (checkpoint.warm_start).  Cycles follow
+    imagenet_train.epoch_schedule from the restored step (one evaluation with eval_only or train_epochs = 0).
+    A cycle trains on imagenet_train.CycleStream (at most max_train_steps steps): PIL decoding of the crop
+    windows on a pool of `num_workers` CPU threads, _TrainFeed staging, acnn_set_images_cropped and the
+    Trainer's step (use_cuda_graph: one graph replay).  It saves model.ckpt-<global step> every
+    save_checkpoints_epochs epochs and at its end, keeping keep_checkpoint_max of them, then runs
+    evaluate_classification, CheckpointKeeper.save(accuracy) and stops at stop_threshold or once the global
+    step reaches train_epochs * int(num_images / batch_size).  The seed gives the initial weights, the
+    record order, the crop windows, the flips and the mixup lambdas (imagenet_train's counter-based
+    generators).  num_images is the number of records in the shards (the reference's data_config count).
+    Under torch.distributed every rank trains its slice of each global batch; rank 0 writes the
+    checkpoints and evaluates.  Returns the list of the cycles' evaluation results."""
+    from concurrent.futures import ThreadPoolExecutor
+    from . import imagenet_train as it
+    from .checkpoint import CheckpointKeeper, latest_checkpoint, restore, save_checkpoint, warm_start
+    from .imagenet_eval import eval_size
+    p = params_from_flags(**flags)
+    if p["autoaugment_type"] is not None:
+        raise NotImplementedError("autoaugment_type=%r: AutoAugment is not implemented; train with "
+                                  "autoaugment_type=None" % (p["autoaugment_type"],))
+    ds_name = p["dataset_name"] or "imagenet"
+    ds = DATASETS[ds_name]
+    size = it.train_size(p["preprocessing_type"], image_size)
+    eval_size(p["preprocessing_type"], image_size)
+    dist = torch.distributed.is_initialized()
+    world = torch.distributed.get_world_size() if dist else 1
+    rank = torch.distributed.get_rank() if dist else 0
+    kd = float(p["kd_temp"] or 0) > 0
+    records, counts = it.read_train_records(it.train_files(data_dir, p["train_regex"]), ds["num_classes"], kd)
+    num_images = len(records)
+    steps_per_epoch = int(num_images / p["batch_size"])
+    if steps_per_epoch < 1:
+        raise ValueError("training: %d records hold no batch of %d" % (num_images, p["batch_size"]))
+    dev = torch.device("cuda", torch.cuda.current_device())
+    model = Model(p["resnet_size"], p["data_format"], num_classes=ds["num_classes"],
+                  resnet_version=p["resnet_version"], zero_gamma=p["zero_gamma"],
+                  use_se_block=p["use_se_block"], use_sk_block=p["use_sk_block"],
+                  no_downsample=p["no_downsample"], anti_alias_filter_size=p["anti_alias_filter_size"],
+                  anti_alias_type=p["anti_alias_type"], bn_momentum=p["bn_momentum"],
+                  embedding_size=p["embedding_size"], pool_type=p["pool_type"], bl_alpha=p["bl_alpha"],
+                  bl_beta=p["bl_beta"], dtype=p["dtype"], loss_type=p["cls_loss_type"], seed=seed,
+                  device=str(dev))
+    model.use_resnet_d = bool(p["use_resnet_d"])
+    trainer = Trainer(model, p, size, size, use_cuda_graph=use_cuda_graph, num_images=num_images)
+    ckpt = latest_checkpoint(model_dir) if os.path.isdir(model_dir) else None
+    if ckpt:
+        restore(model, ckpt, trainer)
+    elif p["pretrained_model_checkpoint_path"]:
+        warm_start(model, p["pretrained_model_checkpoint_path"], trainer.global_step)
+    if p["eval_only"] or not p["train_epochs"]:
+        schedule, first = [0], 0
+    else:
+        args = (p["train_epochs"], epochs_between_evals, p["ratio_fine_eval"])
+        full = it.epoch_schedule(*args)
+        schedule = it.epoch_schedule(*args, cur_epoch=trainer.global_step // steps_per_epoch)
+        first = len(full) - len(schedule)          # the cycle index keys the cycle's randomness
+    total_train_steps = p["train_epochs"] * steps_per_epoch
+    save_steps = int(p["save_checkpoints_epochs"] * steps_per_epoch)
+    shuffle_buffer = it.SHUFFLE_BUFFER.get(ds_name, it.DEFAULT_SHUFFLE_BUFFER)
+    keeper = CheckpointKeeper(model_dir, p["num_best_ckpt_to_keep"], p["keep_ckpt_every_eval"], maximize=True) \
+        if rank == 0 else None
+
+    def save():
+        if rank == 0:
+            save_checkpoint(os.path.join(model_dir, "model.ckpt-%d" % trainer.global_step), model, trainer)
+            _prune_checkpoints(model_dir, p["keep_checkpoint_max"])
+
+    feed = _TrainFeed(trainer, kd)
+    n_lam = trainer.input_batch // 2
+    pool = ThreadPoolExecutor(max_workers=num_workers or min(32, os.cpu_count() or 1))
+    results = []
+    try:
+        for ci, epochs in enumerate(schedule):
+            c = first + ci
+            if epochs:
+                stream = it.CycleStream(counts, seed, c, epochs * (2 if trainer.mixup_type == 1 else 1),
+                                        shuffle_buffer, trainer.input_batch, world, rank)
+                steps = stream.steps if max_train_steps is None else min(stream.steps, max_train_steps)
+
+                def decode(t, c=c, stream=stream):
+                    return [(pool.submit(it.decode_window, *records[r][:3], seed, c, pos,
+                                         p["training_random_crop"]), r) for pos, r in stream.records(t)]
+                ahead = 4                               # steps decoding ahead of the GPU
+                pending = [decode(t) for t in range(min(ahead, steps))]
+
+                def stage(t):
+                    futs = pending.pop(0)
+                    if t + ahead < steps:
+                        pending.append(decode(t + ahead))
+                    teacher = np.stack([records[r][4] for _, r in futs]) if kd else None
+                    feed.stage([f.result() for f, _ in futs], [records[r][3] for _, r in futs], teacher)
+
+                if steps:
+                    stage(0)
+                for t in range(steps):
+                    lam1 = lam2 = None
+                    if trainer.mixup_type:
+                        lam = it.mixup_lambdas(seed, trainer.global_step, rank, 2 * n_lam).reshape(2, n_lam)
+                        lam1, lam2 = lam[0], (lam[1] if trainer.mixup_type == 2 else None)
+                    feed.step(lam1, lam2)
+                    if t + 1 < steps:
+                        stage(t + 1)
+                        if save_steps > 0 and trainer.global_step % save_steps == 0:
+                            save()
+                save()
+            if rank == 0:
+                if latest_checkpoint(model_dir) is None:
+                    raise ValueError("evaluation: no checkpoint in %s" % model_dir)
+                res = evaluate_classification(
+                    model, data_dir, val_regex=p["val_regex"], preprocessing_type=p["preprocessing_type"],
+                    image_size=image_size, batch_size=trainer.local_batch, label_smoothing=p["label_smoothing"],
+                    weight_decay=p["weight_decay"], global_step=trainer.global_step,
+                    use_cuda_graph=use_cuda_graph, num_workers=num_workers)
+                keeper.save(res["accuracy"], model_dir)
+            else:
+                res = None
+            if dist:
+                box = [res]
+                torch.distributed.broadcast_object_list(box, src=0)
+                res = box[0]
+            results.append(res)
+            if stop_threshold is not None and res["accuracy"] >= stop_threshold:
+                break
+            if res["global_step"] >= total_train_steps:
+                break
+    finally:
+        pool.shutdown(wait=True, cancel_futures=True)
+    torch.cuda.current_stream(dev).synchronize()
+    return results

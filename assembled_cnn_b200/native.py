@@ -83,6 +83,7 @@ PROTOTYPES = {
     "acnn_set_inputs": (_i, [_vp] * 7),
     "acnn_set_images_u8": (_i, [_vp] * 4),
     "acnn_set_images_resized": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "acnn_set_images_cropped": (_i, [_vp] * 4),
     "acnn_set_hparams": (_i, [_vp, _vp, _vp]),
     "acnn_get_logits": (_i, [_vp, _vp, _vp]),
     "acnn_get_loss": (_i, [_vp, _vp, _vp]),
@@ -395,6 +396,15 @@ class NativeRuntime(_runtime_base()):
         _check_resize_args(desc, self.t[self.plan.meta["images"]], n_valid, mean)
         _lib.check(self.lib.acnn_set_images_resized(self.model.handle, desc.data_ptr(), int(n_valid),
                                                     mean.data_ptr(), self.stream), "acnn_set_images_resized")
+
+    def set_images_cropped(self, desc, mean):
+        """acnn_set_images_cropped: every row of the "images" buffer from training crop windows (flip,
+        resize to S x S, - mean[c]); desc a CUDA uint8 tensor of input_batch 32-byte acnn_crop_desc on this
+        device, validated by the caller; mean a float32 tensor of 3 (host or device)."""
+        from .runtime import _check_crop_args
+        _check_crop_args(desc, self.t[self.plan.meta["images"]], mean)
+        _lib.check(self.lib.acnn_set_images_cropped(self.model.handle, desc.data_ptr(), mean.data_ptr(),
+                                                    self.stream), "acnn_set_images_cropped")
 
     def zero_step_buffers(self):
         _lib.check(self.lib.acnn_clear_step_buffers(self.model.handle, self.stream),

@@ -44,6 +44,21 @@ def _check_resize_args(desc, images, n_valid, mean):
     return b, h
 
 
+def _check_crop_args(desc, images, mean):
+    """Arguments of set_images_cropped: a square input buffer, B descriptors of 32 bytes on its device,
+    float32 mean[3].  Returns (B, S)."""
+    b, h, w, _ = images.shape
+    if h != w:
+        raise ValueError("set_images_cropped needs a square input buffer, got %dx%d" % (h, w))
+    if desc.dtype != torch.uint8 or desc.numel() != 32 * b or desc.device != images.device \
+            or not desc.is_contiguous():
+        raise ValueError("desc must be a contiguous uint8 tensor of %d descriptors (%d bytes) on %s"
+                         % (b, 32 * b, images.device))
+    if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
+        raise ValueError("mean must be a contiguous float32 tensor of 3 values")
+    return b, h
+
+
 class Runtime:
     def __init__(self, plan: Plan, device="cuda:0", eps: float = 1e-5, share: "Runtime | None" = None,
                  deterministic: "bool | None" = None):
@@ -288,6 +303,16 @@ class Runtime:
         b, s = _check_resize_args(desc, images, n_valid, mean)
         _lib.check(self.lib.acnn_resize_crop_u8(desc.data_ptr(), b, int(n_valid), s, mean.data_ptr(),
                                                 images.data_ptr(), self.stream), "acnn_resize_crop_u8")
+
+    def set_images_cropped(self, desc, mean):
+        """Every row of the "images" buffer [B, S, S, 3] from training crop windows (acnn_crop_resize_u8:
+        flip, resize to S x S, - mean[c]).  desc: a CUDA uint8 tensor of B 32-byte acnn_crop_desc
+        (imagenet_train.CROP_DESC_DTYPE) on this device, validated by the caller; mean a float32 tensor
+        of 3 (host or device)."""
+        images = self.t[self.plan.meta["images"]]
+        b, s = _check_crop_args(desc, images, mean)
+        _lib.check(self.lib.acnn_crop_resize_u8(desc.data_ptr(), b, b, s, mean.data_ptr(), images.data_ptr(),
+                                                self.stream), "acnn_crop_resize_u8")
 
     def zero_step_buffers(self):
         st = self.stream

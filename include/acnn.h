@@ -491,6 +491,28 @@ typedef struct acnn_resize_desc {
  * [0, B], out not 4-byte or desc not 8-byte aligned: ACNN_ERR_INVALID before any CUDA call. */
 int acnn_resize_crop_u8(const acnn_resize_desc* desc, int B, int n_valid, int S, const float* mean, float* out,
                         void* stream);
+/* One training crop window of a batch: uint8 RGB [h][w][3] at `src` (DEVICE), the window the host cut out
+ * of the decoded image (sample_distorted_bounding_box + decode_and_crop_jpeg), mirrored when flip != 0.
+ * 32 bytes, the layout of imagenet_train.CROP_DESC_DTYPE. */
+typedef struct acnn_crop_desc {
+  const uint8_t* src;
+  int32_t h, w;
+  int32_t flip;
+  int32_t reserved_[3];
+} acnn_crop_desc;
+/* out fp32 NHWC [B,S,S,3], row b < n_valid = resize_bilinear(flip_b ? mirror(window_b) : window_b, S, S)
+ * - mean[c]: the training preprocessing of preprocessing/imagenet_preprocessing.py:57-97,269-313 after the
+ * crop (random_flip_left_right, _resize_image, mean_image_subtraction).  The resize is TF 1.14's legacy
+ * bilinear with the independent scales (float)h / S and (float)w / S, every step a separately rounded fp32
+ * operation, as in acnn_resize_crop_u8; the result stays fp32.  The flip comes before the resize, whose
+ * sample grid is anchored at the left edge, so a mirrored window reads source columns w - 1 - lower and
+ * w - 1 - upper.  A 1 x 1 window (scale < 1, upsampling) is valid.
+ * desc: a DEVICE array of B descriptors (a captured CUDA graph holds only its address).  The descriptors
+ * are not checked here: the caller guarantees src != 0 and h, w >= 1.  mean: float[3], host or device.
+ * Rows >= n_valid are not written.  Null pointers, B < 1, S < 1, n_valid outside [0, B], out not 4-byte
+ * or desc not 8-byte aligned: ACNN_ERR_INVALID before any CUDA call. */
+int acnn_crop_resize_u8(const acnn_crop_desc* desc, int B, int n_valid, int S, const float* mean, float* out,
+                        void* stream);
 /* Per-row results of the classification metrics for logits fp32 [B][ld] (columns < NC are the
  * classes) and labels int32 [B], for every row r < n_valid (rows >= n_valid are not written):
  *   pred[r]  = tf.argmax(logits): the smallest index of the largest logit;

@@ -186,6 +186,12 @@ int acnn_set_images_u8(acnn_model* m, const uint8_t* images_dev, const float* me
  * n_valid are not written; mean3: float[3], host or device. */
 int acnn_set_images_resized(acnn_model* m, const acnn_resize_desc* desc_dev, int n_valid, const float* mean3,
                             void* stream);
+/* "images" [input_batch,S,S,3] from a batch of training crop windows through acnn_crop_resize_u8 (flip,
+ * resize to S x S, - mean3[c]), S = the plan's H = W.  Every one of the input_batch rows is written (a
+ * training batch has no padding).  desc_dev: a DEVICE array of input_batch acnn_crop_desc (checked by
+ * the caller, see acnn_crop_resize_u8; a host pointer is ACNN_ERR_INVALID); mean3: float[3], host or
+ * device. */
+int acnn_set_images_cropped(acnn_model* m, const acnn_crop_desc* desc_dev, const float* mean3, void* stream);
 /* float hp[8] as in acnn_model_sizes.hp_offset. */
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream);
 /* logits [batch, num_classes] fp32 (dense, ld = num_classes) / loss float[4] to a host or device array. */
