@@ -893,8 +893,7 @@ struct WgradParams {
   int stages_per_split;
   int splits;            // CTAs along the pixel range (gridDim.z)
   float* dw;
-  float* part;           // splits > 1: [splits][tiles][128 x BN] fp32 partial tiles
-  unsigned* counters;    // splits > 1: arrivals per tile (zeroed before the launch)
+  float* part;           // splits > 1: [splits][Cout][Ktot] fp32 partials (dw order), else null
 };
 
 constexpr int kWgPix = 64;   // default pixels per pipeline stage (4 wgmma K-steps); PIX = 128: 8 steps
@@ -1074,41 +1073,10 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     const int rl = cg * 64 + (warp & 3) * 16 + (lane >> 2);   // row inside the 128-row tile
     const int rb = m0 + rl;
     const int cq = (lane & 3) * 2;
-    __shared__ int s_last;
-    if (p.splits > 1) {
-      // split-K, ordered: every split stores its partial tile; the LAST split to arrive adds the
-      // partials in split order (the arrival order does not enter the sum)
-      const int tile = blockIdx.y * gridDim.x + blockIdx.x;
-      const size_t tiles = static_cast<size_t>(gridDim.x) * gridDim.y;
-      float* mine = p.part + (static_cast<size_t>(blockIdx.z) * tiles + tile) * (128 * BN);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<float2*>(mine + (rl + h * 8) * BN + j * 8 + cq) =
-              make_float2(acc[j * 4 + h * 2], acc[j * 4 + h * 2 + 1]);
-      __threadfence();
-      named_bar_sync(1, kConsumerThreads);
-      if (threadIdx.x == 128) s_last = atomicAdd(p.counters + tile, 1u) == static_cast<unsigned>(p.splits - 1);
-      named_bar_sync(1, kConsumerThreads);
-      if (!s_last) return;
-      __threadfence();
-      const float* first = p.part + static_cast<size_t>(tile) * (128 * BN);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float2 t = make_float2(0.f, 0.f);
-          for (int sp = 0; sp < p.splits; ++sp) {
-            const float2 v = __ldcg(reinterpret_cast<const float2*>(
-                first + sp * tiles * (128 * BN) + (rl + h * 8) * BN + j * 8 + cq));
-            t.x += v.x;
-            t.y += v.y;
-          }
-          acc[j * 4 + h * 2] = t.x;
-          acc[j * 4 + h * 2 + 1] = t.y;
-        }
-    }
+    // split-K: this split's partial goes to its own slice in dw order, summed in split order by
+    // wgrad_reduce_kernel.  Either way a warp's store covers 8 consecutive (tap,ci) rows of 4
+    // output channels: four full 32-byte sectors.
+    float* part = p.part ? p.part + static_cast<size_t>(blockIdx.z) * p.Cout * p.Ktot : nullptr;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -1117,13 +1085,41 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int co = co0 + j * 8 + cq + e;
-          // one add per dw element (the whole pixel range of this tile is summed above)
-          if (n < p.Ktot && co < p.Cout)
-            atomicAdd(p.dw + static_cast<size_t>(co) * p.Ktot + n, acc[j * 4 + h * 2 + e]);
+          if (n < p.Ktot && co < p.Cout) {
+            const size_t i = static_cast<size_t>(co) * p.Ktot + n;
+            if (part) part[i] = acc[j * 4 + h * 2 + e];
+            // one add per dw element (the whole pixel range of this tile is summed above)
+            else atomicAdd(p.dw + i, acc[j * 4 + h * 2 + e]);
+          }
         }
       }
     }
   }
+}
+
+// dw[i] += (((0 + part[0][i]) + part[1][i]) + ... + part[splits-1][i]): the ordered split-K sum,
+// one dw element per thread over the whole GPU.  Loads are issued kWgRedDepth splits ahead of the
+// (serial) adds so that each thread keeps that many L2 reads in flight.
+constexpr int kWgRedThreads = 128;
+constexpr int kWgRedDepth = 16;
+
+__global__ void __launch_bounds__(kWgRedThreads)
+wgrad_reduce_kernel(const float* __restrict__ part, float* dw, int64_t n, int splits) {
+  pdl_entry();
+  const int64_t i = blockIdx.x * static_cast<int64_t>(kWgRedThreads) + threadIdx.x;
+  if (i >= n) return;
+  const float* src = part + i;
+  float t = 0.f;
+  int s = 0;
+  for (; s + kWgRedDepth <= splits; s += kWgRedDepth) {
+    float v[kWgRedDepth];
+#pragma unroll
+    for (int u = 0; u < kWgRedDepth; ++u) v[u] = __ldcs(src + (s + u) * n);
+#pragma unroll
+    for (int u = 0; u < kWgRedDepth; ++u) t += v[u];
+  }
+  for (; s < splits; ++s) t += __ldcs(src + s * n);
+  dw[i] += t;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1500,13 +1496,16 @@ struct WgradMaps {
   CUtensorMap x[3], dy[3];
 };
 
-// fixed cost of one wgrad CTA (pipeline fill + atomic epilogue) in units of pipeline stages, for
-// the split-K cost model (0 = the "two waves of CTAs" rule); acnn_set_wgrad_overhead_stages
+// fixed cost of one wgrad CTA (pipeline fill + epilogue) in units of pipeline stages, for the
+// split-K cost model (0 = the "two waves of CTAs" rule); acnn_set_wgrad_overhead_stages.  With the
+// partials summed by wgrad_reduce_kernel, a sweep of forced split counts over the 43 wgrad
+// geometries of the c3 step (H100 80GB HBM3, 700 W) puts the layouts this value picks within
+// 0.11 ms per step of the fastest swept layout of every geometry, so it stays.
 static int g_wgrad_overhead_stages = 16;
 
-// Split-K partial tiles are bounded (the split count is capped to fit): 64 MiB per launch.
+// Split-K partials are bounded (the split count is capped so that the tile-padded partials of all
+// splits would fit): 64 MiB per launch.
 constexpr size_t kWgPartFloats = size_t(16) << 20;
-constexpr int kWgCounters = 1 << 16;
 
 // 0: the cost model picks the split count; n > 0: n splits, within the capacity caps
 // (acnn_set_wgrad_splits)
@@ -1555,10 +1554,10 @@ static int wgrad_plan(const acnn_conv_geom& g, int precision, int deterministic,
   // does not depend on which split finishes first.  deterministic: no split -- one add per dw
   // element.  One CTA per SM (384 threads with register accumulators).
   const int tiles = w->m_tiles * w->n_tiles;
-  // capacity: the partial tiles of all splits fit kWgPartFloats, one arrival counter per tile
+  // capacity: the partial tiles of all splits fit kWgPartFloats
   const int64_t tile_floats = (int64_t)tiles * 128 * bn;
   int cap = (int)std::min<int64_t>(w->stages_total, (int64_t)kWgPartFloats / tile_floats);
-  if (cap < 1 || tiles > kWgCounters) cap = 1;
+  if (cap < 1) cap = 1;
   const int max_splits = std::min(cap, w->stages_total >= 8 ? w->stages_total / 4 : 1);
   int splits;
   if (g_wgrad_splits > 0) {
@@ -1602,33 +1601,30 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int m_tiles, int n_t
     }
     attr_set = true;
   }
-  const int tiles = m_tiles * n_tiles;
   const int splits = p.splits;
+  const int64_t n = (int64_t)p.Cout * p.Ktot;
   p.part = nullptr;
-  p.counters = nullptr;
-  void* scratch = nullptr;
   if (splits > 1) {
-    // this launch's partial tiles + arrival counters, stream-ordered (per stream, capturable)
-    const size_t part_bytes = (size_t)splits * tiles * 128 * BN * sizeof(float);
-    int rc = scratch_alloc(&scratch, part_bytes + (size_t)tiles * sizeof(unsigned), stream, "wgrad");
+    // this launch's partials, stream-ordered (per stream, capturable)
+    void* scratch = nullptr;
+    int rc = scratch_alloc(&scratch, (size_t)splits * n * sizeof(float), stream, "wgrad");
     if (rc) return rc;
     p.part = static_cast<float*>(scratch);
-    p.counters = reinterpret_cast<unsigned*>(static_cast<char*>(scratch) + part_bytes);
-    if (cudaMemsetAsync(p.counters, 0, (size_t)tiles * sizeof(unsigned), stream) != cudaSuccess) {
-      set_error("wgrad: clearing the split counters: %s", cudaGetErrorString(cudaGetLastError()));
-      return ACNN_ERR_CUDA;
-    }
   }
   dim3 grid(m_tiles, n_tiles, splits);
   launch_k(kern, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, tm.x[0], tm.dy[0], tm.x[1],
            tm.x[2], tm.dy[1], tm.dy[2], p);
   count_launch();
-  const int rc = check_launch("wgrad_gemm_kernel");
-  if (scratch) {
-    const int rc2 = scratch_free(scratch, stream, "wgrad");
-    if (rc == ACNN_OK) return rc2;
+  int rc = check_launch("wgrad_gemm_kernel");
+  if (!p.part) return rc;
+  if (rc == ACNN_OK) {
+    launch_k(wgrad_reduce_kernel, dim3((unsigned)ceil_div64(n, kWgRedThreads)), dim3(kWgRedThreads),
+             0, stream, static_cast<const float*>(p.part), p.dw, n, splits);
+    count_launch();
+    rc = check_launch("wgrad_reduce_kernel");
   }
-  return rc;
+  const int rc2 = scratch_free(p.part, stream, "wgrad");
+  return rc ? rc : rc2;
 }
 
 template <int BN, int CW, bool IM2COL>

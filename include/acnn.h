@@ -75,12 +75,12 @@ int acnn_set_conv_out_bufs(int mode);
  * Returns the previous setting. */
 int acnn_set_wgrad_pixels(int pix);
 /* Tuning knob of the wgrad launcher's split-K choice (no effect on results beyond fp32 summation
- * order): the fixed cost of one CTA (pipeline fill + atomic epilogue) in pipeline stages used by the
+ * order): the fixed cost of one CTA (pipeline fill + epilogue) in pipeline stages used by the
  * cost model that picks the number of pixel splits (default 16); 0 = the "two waves of CTAs"
  * rule.  Returns the previous setting. */
 int acnn_set_wgrad_overhead_stages(int stages);
 /* Tuning knob of the wgrad launcher: n > 0 asks for n pixel splits, clamped to the capacity of the
- * partial-tile scratch (64 MiB, one arrival counter per tile) and to the number of pipeline stages;
+ * partial-tile scratch (64 MiB) and to the number of pipeline stages;
  * 0 (default) = the cost model above.  deterministic != 0 still runs one split.  Returns the previous
  * setting. */
 int acnn_set_wgrad_splits(int n);
@@ -146,8 +146,8 @@ int acnn_conv_dgrad(const acnn_conv_geom* g, const void* dy, const void* w_dgrad
                     int64_t w_plane_stride, void* stream);
 
 /* dw[Cout,kh,kw,Cin] (fp32) += sum_pixels x (*) dy  -- weight gradient, split-K over pixels: the
- * splits store partial tiles in a stream-ordered scratch of the launch (cudaMallocAsync on `stream`)
- * and the last split of a tile adds them to dw in split order (bit-reproducible).  dw must be zeroed
+ * splits store their partials in a stream-ordered scratch of the launch (cudaMallocAsync on `stream`)
+ * and a second kernel on `stream` adds them to dw in split order (bit-reproducible).  dw must be zeroed
  * (or hold the running sum) by the caller.  deterministic != 0: no split (one add per element).
  * precision 1: x and dy are 3-plane operands. */
 int acnn_conv_wgrad(const acnn_conv_geom* g, const void* x, const void* dy, float* dw,
