@@ -192,10 +192,10 @@ def crop_window(h, w, rng, use_random_crop=True):
 
 
 def jpeg_shape(buf):
-    """(height, width) from the image header (tf.image.extract_jpeg_shape): PIL's lazy open, no decoding."""
-    from PIL import Image
-    with Image.open(io.BytesIO(buf)) as im:
-        return im.size[1], im.size[0]
+    """(height, width) from the image header (tf.image.extract_jpeg_shape): the JPEG header parser of
+    acnn_jpeg_parse, or PIL's lazy open for the images it does not accept; no decoding."""
+    from .jpeg import jpeg_shape as shape
+    return shape(buf)
 
 
 def decode_window(path, offset, length, seed, cycle, position, use_random_crop=True):
@@ -210,6 +210,16 @@ def decode_window(path, offset, length, seed, cycle, position, use_random_crop=T
         raise ValueError("%s: the image at byte offset %d decodes to %s, its header says %dx%d"
                          % (path, offset, a.shape[:2], h, w))
     return np.ascontiguousarray(a[y:y + ch, x:x + cw]), flip
+
+
+def encoded_window(path, offset, length, seed, cycle, position, use_random_crop=True):
+    """(encoded bytes, (offset_y, offset_x, crop_h, crop_w), flip) of the record at path[offset:offset + length],
+    the example at `position` of cycle `cycle`: the window and flip decode_window would cut, left for the
+    device decoder (model_fns._TrainFeed.stage_encoded)."""
+    buf = read_encoded(path, offset, length)
+    h, w = jpeg_shape(buf)
+    y, x, ch, cw, flip = crop_window(h, w, example_rng(seed, cycle, position), use_random_crop)
+    return buf, (y, x, ch, cw), flip
 
 
 def check_crop_descriptors(desc):

@@ -766,16 +766,41 @@ class _CorruptionEvalDevice(_EvalPipeline):
                        torch.zeros(batch, dtype=torch.int32, device=self.dev)) for _ in range(2)]
         self.acc = torch.zeros(1, dtype=torch.int64, device=self.dev)
         self.pred = torch.zeros(batch, dtype=torch.int32, device=self.dev)
+        self.decoders, self._files = [None, None], None
 
     def _stage(self, h, slot, images, labels):
-        """`images` a list of uint8 [H, W, 3] arrays, `labels` ints."""
+        """`images` a list of uint8 [H, W, 3] arrays, `labels` ints; or, from run_batch_encoded, the files'
+        encoded bytes, decoded on the copy stream straight into the slot."""
         hu8, hlab = self.host[h]
-        for i, a in enumerate(images):
-            hu8[i].copy_(torch.from_numpy(a))
-        hlab[:len(images)].copy_(torch.as_tensor(labels, dtype=torch.int32))
         du8, dlab = self.slots[slot]
-        du8.copy_(hu8, non_blocking=True)
+        if self._files is None:
+            for i, a in enumerate(images):
+                hu8[i].copy_(torch.from_numpy(a))
+            du8.copy_(hu8, non_blocking=True)
+        else:
+            from . import imagenet_c, jpeg
+            files, S = self._files, du8.shape[1]
+            desc = jpeg.parse(images)
+            for i, d in enumerate(desc):      # a wrong size raises decode_image's error, as the PIL path does
+                if d["supported"] and (int(d["height"]), int(d["width"])) != (S, S):
+                    imagenet_c.decode_image(files[i], S)
+            if self.decoders[slot] is None:
+                self.decoders[slot] = jpeg.JpegDecoder(self.dev)
+            row = S * S * 3
+            self.decoders[slot].stage(images, None, torch.cuda.current_stream(self.dev),
+                                      fallback=lambda i: imagenet_c.decode_image(files[i], S),
+                                      out=du8.view(-1), out_offsets=np.arange(len(images), dtype=np.int64) * row)
+        hlab[:len(images)].copy_(torch.as_tensor(labels, dtype=torch.int32))
         dlab.copy_(hlab, non_blocking=True)
+
+    def run_batch_encoded(self, buffers, labels, files):
+        """run_batch from the encoded bytes of `files` (jpeg.JpegDecoder on the copy stream; PIL, through
+        imagenet_c.decode_image, for the images the device does not decode)."""
+        self._files = files
+        try:
+            self.run_batch(buffers, labels)
+        finally:
+            self._files = None
 
     def _body(self, slot, n_valid):
         from .metrics import softmax_top1_count
@@ -812,17 +837,28 @@ class _ClassifyEvalDevice(_EvalPipeline):
         self.out = tuple(torch.zeros(batch, dtype=dt, device=self.dev) for dt in kinds)
         self.rows = tuple(torch.zeros(total, dtype=dt, device=self.dev) for dt in kinds)
         self.done = 0
+        self.decoders, self._geometry = [None, None], None
 
     def _stage(self, h, slot, images, labels):
-        """`images` a list of (uint8 [H, W, 3] array, eval_geometry) pairs, `labels` ints."""
+        """`images` a list of (uint8 [H, W, 3] array, eval_geometry) pairs, `labels` ints; or, from
+        run_batch_encoded, encoded images, decoded on the copy stream."""
         from .imagenet_eval import DESC_DTYPE, check_descriptors
         n = len(images)
         hbuf, hlab, hdesc = self.host[h]
-        self.host[h][0], self.slots[slot][0], addrs = _pack_u8(hbuf, self.slots[slot][0], [a for a, _ in images],
-                                                              self.dev)
         desc = hdesc.numpy().view(DESC_DTYPE)
-        for i, (a, (s, rh, rw, cy, cx)) in enumerate(images):
-            desc[i] = (addrs[i], a.shape[0], a.shape[1], rh, rw, cy, cx)
+        if self._geometry is None:
+            self.host[h][0], self.slots[slot][0], addrs = _pack_u8(hbuf, self.slots[slot][0],
+                                                                  [a for a, _ in images], self.dev)
+            for i, (a, (s, rh, rw, cy, cx)) in enumerate(images):
+                desc[i] = (addrs[i], a.shape[0], a.shape[1], rh, rw, cy, cx)
+        else:
+            from . import jpeg
+            if self.decoders[slot] is None:
+                self.decoders[slot] = jpeg.JpegDecoder(self.dev)
+            placed = self.decoders[slot].stage(images, None, torch.cuda.current_stream(self.dev))
+            for i, (addr, ih, iw) in enumerate(placed):
+                s, rh, rw, cy, cx = self._geometry(ih, iw)
+                desc[i] = (addr, ih, iw, rh, rw, cy, cx)
         check_descriptors(desc, n, self.size)
         hlab[:n].copy_(torch.as_tensor(labels, dtype=torch.int32))
         _, dlab, ddesc = self.slots[slot]
@@ -836,12 +872,26 @@ class _ClassifyEvalDevice(_EvalPipeline):
         self.rt.run_forward()
         classify_rows(self.logits, labels, n_valid, 5, self.label_smoothing, out=self.out)
 
+    def run_batch_encoded(self, buffers, labels, geometry):
+        """run_batch from encoded images (jpeg.JpegDecoder on the copy stream; PIL for the images the device
+        does not decode); geometry(h, w) gives an image's imagenet_eval.eval_geometry."""
+        self._geometry = geometry
+        try:
+            self.run_batch(buffers, labels)
+        finally:
+            self._geometry = None
+
     def run_batch(self, images, labels):
         super().run_batch(images, labels)
         n = len(images)
         for dst, src in zip(self.rows, self.out):
             dst[self.done:self.done + n].copy_(src[:n])
         self.done += n
+
+
+def _read_file(path):
+    with open(path, "rb") as f:
+        return f.read()
 
 
 def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=224, label_offset=1,
@@ -886,7 +936,7 @@ def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=
             ev = _CorruptionEvalDevice(replicas[i], batch_size, image_size, use_resnet_d, use_cuda_graph)
             batches = [(d, work[d][0][a:a + batch_size], work[d][1][a:a + batch_size])
                        for d in quota[i] for a in range(0, len(work[d][0]), batch_size)]
-            decode = lambda files: [pool.submit(imagenet_c.decode_image, f, image_size) for f in files]
+            decode = lambda files: [pool.submit(_read_file, f) for f in files]
             ahead = 4                                   # batches decoding ahead of the GPU
             pending = [decode(b[1]) for b in batches[:ahead]]
             counts = {}
@@ -894,7 +944,7 @@ def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=
                 futs = pending.pop(0)
                 if j + ahead < len(batches):
                     pending.append(decode(batches[j + ahead][1]))
-                ev.run_batch([f.result() for f in futs], labels)
+                ev.run_batch_encoded([f.result() for f in futs], labels, files)
                 if j + 1 == len(batches) or batches[j + 1][0] != d:
                     counts[d] = ev.take_count()
             torch.cuda.current_stream(ev.dev).synchronize()
@@ -961,8 +1011,8 @@ def evaluate_classification(model, data_dir, *, val_regex="validation-*", prepro
     ev = _ClassifyEvalDevice(model, batch_size, size, use_resnet_d, use_cuda_graph, label_smoothing,
                              len(records))
     pool = ThreadPoolExecutor(max_workers=num_workers or min(32, os.cpu_count() or 1))
-    decode = lambda recs: [pool.submit(imagenet_eval.decode_record, r[0], r[1], r[2], preprocessing_type,
-                                       image_size) for r in recs]
+    decode = lambda recs: [pool.submit(imagenet_eval.read_encoded, r[0], r[1], r[2]) for r in recs]
+    geometry = lambda h, w: imagenet_eval.eval_geometry(h, w, preprocessing_type, image_size)
     try:
         ahead = 4                                   # batches decoding ahead of the GPU
         pending = [decode(b) for b in batches[:ahead]]
@@ -970,7 +1020,7 @@ def evaluate_classification(model, data_dir, *, val_regex="validation-*", prepro
             futs = pending.pop(0)
             if j + ahead < len(batches):
                 pending.append(decode(batches[j + ahead]))
-            ev.run_batch([f.result() for f in futs], [r[3] for r in recs])
+            ev.run_batch_encoded([f.result() for f in futs], [r[3] for r in recs], geometry)
         torch.cuda.current_stream(ev.dev).synchronize()
     finally:
         pool.shutdown(wait=True, cancel_futures=True)
@@ -1005,11 +1055,32 @@ class _TrainFeed:
         self.host_free = [None] * self.RING
         self.slot_free = [None, None]
         self.copied = [None, None]
+        self.decoders = [None, None]
         self.staged = self.consumed = 0
 
     def stage(self, windows, labels, teacher_logits=None):
         """`windows` input_batch (uint8 [h, w, 3] array, flip) pairs, `labels` ints, `teacher_logits` float32
         [input_batch, num_classes] with KD."""
+        def place(h, slot):
+            self.host[h][0], self.slots[slot][0], addrs = _pack_u8(self.host[h][0], self.slots[slot][0],
+                                                                  [a for a, _ in windows], self.dev)
+            return [(ad, a.shape[0], a.shape[1], flip) for ad, (a, flip) in zip(addrs, windows)]
+        self._stage(place, labels, teacher_logits)
+
+    def stage_encoded(self, items, labels, teacher_logits=None):
+        """As stage, from input_batch (encoded JPEG bytes, (y, x, h, w) window, flip) triples: the windows are
+        decoded on the copy stream (jpeg.JpegDecoder, one per slot; PIL's decode_rgb for the images the
+        device does not decode)."""
+        def place(h, slot):
+            from . import jpeg
+            if self.decoders[slot] is None:
+                self.decoders[slot] = jpeg.JpegDecoder(self.dev)
+            got = self.decoders[slot].stage([b for b, _, _ in items], np.array([w for _, w, _ in items], np.int32),
+                                            self.copy_stream)
+            return [(ad, hh, ww, flip) for (ad, hh, ww), (_, _, flip) in zip(got, items)]
+        self._stage(place, labels, teacher_logits)
+
+    def _stage(self, place, labels, teacher_logits):
         from .imagenet_train import CROP_DESC_DTYPE, check_crop_descriptors
         h, slot = self.staged % self.RING, self.staged % 2
         self.staged += 1
@@ -1019,12 +1090,11 @@ class _TrainFeed:
         if self.slot_free[slot] is not None:
             cs.wait_event(self.slot_free[slot])       # the step before the previous one has read it
         with torch.cuda.stream(cs):
-            hbuf, hlab, hdesc, hteach = self.host[h]
-            self.host[h][0], self.slots[slot][0], addrs = _pack_u8(hbuf, self.slots[slot][0],
-                                                                  [a for a, _ in windows], self.dev)
+            placed = place(h, slot)
+            _, hlab, hdesc, hteach = self.host[h]
             desc = hdesc.numpy().view(CROP_DESC_DTYPE)
-            for i, (a, flip) in enumerate(windows):
-                desc[i] = (addrs[i], a.shape[0], a.shape[1], int(flip), (0, 0, 0))
+            for i, (addr, wh, ww, flip) in enumerate(placed):
+                desc[i] = (addr, wh, ww, int(flip), (0, 0, 0))
             check_crop_descriptors(desc)
             hlab.copy_(torch.as_tensor(labels, dtype=torch.int32))
             _, dlab, ddesc, dteach = self.slots[slot]
@@ -1154,7 +1224,7 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                 steps = stream.steps if max_train_steps is None else min(stream.steps, max_train_steps)
 
                 def decode(t, c=c, stream=stream):
-                    return [(pool.submit(it.decode_window, *records[r][:3], seed, c, pos,
+                    return [(pool.submit(it.encoded_window, *records[r][:3], seed, c, pos,
                                          p["training_random_crop"]), r) for pos, r in stream.records(t)]
                 ahead = 4                               # steps decoding ahead of the GPU
                 pending = [decode(t) for t in range(min(ahead, steps))]
@@ -1164,7 +1234,7 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                     if t + ahead < steps:
                         pending.append(decode(t + ahead))
                     teacher = np.stack([records[r][4] for _, r in futs]) if kd else None
-                    feed.stage([f.result() for f, _ in futs], [records[r][3] for _, r in futs], teacher)
+                    feed.stage_encoded([f.result() for f, _ in futs], [records[r][3] for _, r in futs], teacher)
 
                 if steps:
                     stage(0)

@@ -529,6 +529,105 @@ int acnn_classify_rows(const float* logits, int B, int ld, int NC, const int32_t
                        float label_smoothing, int32_t* pred, float* conf, int32_t* hit_k, float* ce,
                        void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * JPEG decoding (the tf.image.decode_jpeg / PIL decode of every input pipeline), bit for bit equal to
+ * libjpeg's ISLOW IDCT, fancy upsampling and YCbCr->RGB, i.e. to PIL's Image.open(b).convert("RGB").
+ * Baseline and extended (SOF0 / SOF1) 8-bit Huffman JPEGs with one scan: grayscale, or 3-component
+ * YCbCr with luma sampling 1x1, 2x1, 1x2 or 2x2 and chroma 1x1, any restart interval.  Everything
+ * else is reported unsupported by acnn_jpeg_parse and is left to the caller (PIL).
+ * ------------------------------------------------------------------------------------------- */
+/* A Huffman table in decoding form: `look` maps the next 9 bits to (length << 8) | symbol (0: the
+ * code is longer than 9 bits); for longer codes, maxcode[l] is the largest code of length l (-1: none)
+ * and vals[valoff[l] + code] its symbol. */
+typedef struct acnn_jpeg_huff {
+  uint16_t look[512];
+  int32_t maxcode[18];
+  int32_t valoff[18];
+  uint8_t vals[256];
+} acnn_jpeg_huff;
+typedef struct acnn_jpeg_comp {
+  int32_t h, v;     /* sampling factors (1 x 1 for a grayscale image) */
+  int32_t tq;       /* quantisation table */
+  int32_t td, ta;   /* DC / AC Huffman tables */
+  int32_t blk0;     /* index of the component's first block inside an MCU */
+  int32_t dw, dh;   /* sample columns / rows: ceil(width * h / hmax), ceil(height * v / vmax) */
+} acnn_jpeg_comp;
+/* One parsed image (6368 bytes, the layout of jpeg.DESC_DTYPE), filled on the host by acnn_jpeg_parse and
+ * read by the device as it is. */
+typedef struct acnn_jpeg_desc {
+  int32_t supported;         /* 1: acnn_jpeg_decode handles the image; 0: see reason */
+  int32_t reason;            /* ACNN_JPEG_* code (acnn_jpeg_reason gives its text) */
+  int32_t height, width;     /* from the frame header, whenever one was read (0 otherwise) */
+  int32_t ncomp, hmax, vmax; /* 1 or 3 components; the largest sampling factors */
+  int32_t bpm;               /* blocks per MCU */
+  int32_t mcus_x, mcus_y;
+  int32_t restart_interval;  /* MCUs per restart interval; 0: none */
+  int32_t n_intervals;       /* restart markers in the scan + 1 */
+  int64_t ecs_offset;        /* the entropy-coded segment: bytes [ecs_offset, ecs_offset + ecs_length) */
+  int64_t ecs_length;        /*   of the image's buffer, restart markers included, stuffing not removed */
+  acnn_jpeg_comp comp[3];
+  int16_t quant[4][64];      /* natural order, as libjpeg's 16-bit multiplier table holds them */
+  acnn_jpeg_huff dc[2], ac[2];
+} acnn_jpeg_desc;
+#define ACNN_JPEG_OK 0
+#define ACNN_JPEG_NOT_JPEG 1        /* no SOI marker (PNG, ...) */
+#define ACNN_JPEG_TRUNCATED 2       /* the buffer ends inside the header */
+#define ACNN_JPEG_MALFORMED 3       /* a marker segment contradicts T.81 */
+#define ACNN_JPEG_PROCESS 4         /* progressive, lossless, hierarchical or arithmetic coding */
+#define ACNN_JPEG_PRECISION 5       /* not 8-bit samples */
+#define ACNN_JPEG_COLOR 6           /* not 1 component or 3 YCbCr components (CMYK, Adobe RGB, ...) */
+#define ACNN_JPEG_SAMPLING 7        /* sampling factors other than those above */
+#define ACNN_JPEG_LAYOUT 8          /* several scans, a scan order other than the frame's, tables >= 2,
+                                       DNL, fill bytes or misnumbered restart markers inside the scan, ... */
+#define ACNN_JPEG_SIZE 9            /* more than 89478485 pixels or a scan of 2^27 bytes or more */
+/* Text of an ACNN_JPEG_* code (host). */
+const char* acnn_jpeg_reason(int code);
+/* Parse the headers of n encoded images, image i at data + offsets[i], lengths[i] bytes (HOST memory):
+ * SOI ... SOS (DQT, DHT, SOF, DRI, APP0 JFIF, APP14 Adobe), then a scan of the entropy-coded segment for
+ * its restart markers and its end.  Every length and index is checked against the buffer; a malformed or
+ * unsupported image gets supported = 0 and a reason, and never makes the call fail.  Null pointers or
+ * n < 0: ACNN_ERR_INVALID. */
+int acnn_jpeg_parse(const uint8_t* data, const int64_t* offsets, const int64_t* lengths, int n,
+                    acnn_jpeg_desc* desc);
+/* Decode plan of one image of a batch (host, filled by acnn_jpeg_plan). */
+typedef struct acnn_jpeg_job {
+  int64_t src;           /* offset of the image's encoded bytes in `data` */
+  int64_t out;           /* offset of its uint8 [win_h][win_w][3] output in `out` (16-byte aligned) */
+  int32_t win_y, win_x, win_h, win_w;
+  int32_t active;        /* 0: unsupported, nothing runs for it and its status is ACNN_JPEG_ST_UNSUPPORTED */
+  int32_t max_sub;       /* capacity of the subsequence tables */
+  int32_t mcu_r0, mcu_r1, mcu_c0, mcu_c1;   /* MCU rows / columns the window and its upsampling context need */
+  int32_t stored_blocks; /* coefficient blocks kept: MCU rows 0 .. mcu_r1 */
+  int32_t idct_blocks;   /* blocks of MCU rows mcu_r0 .. mcu_r1, columns mcu_c0 .. mcu_c1 */
+  int64_t o_bits, o_intervals, o_subs, o_state, o_dirty, o_prefix, o_coef, o_plane[3];  /* into `work` */
+} acnn_jpeg_job;
+typedef struct acnn_jpeg_batch {
+  int64_t work_bytes;    /* size of `work` */
+  int64_t out_bytes;     /* size of `out` */
+  int64_t coef_begin, coef_end;   /* the coefficient span of `work` (zeroed by acnn_jpeg_decode) */
+  int32_t n, max_sub, max_idct_blocks, max_pixels;
+} acnn_jpeg_batch;
+/* Plan the decode of n parsed images (host): image i's encoded bytes at offsets[i] of the device buffer
+ * `data`, its crop window windows[i] = (y, x, h, w) (int32 [n][4], HOST; NULL: whole images).  Windows
+ * outside the image or empty: ACNN_ERR_INVALID.  Fills jobs[n] and *batch. */
+int acnn_jpeg_plan(const acnn_jpeg_desc* desc, const int64_t* offsets, const int32_t* windows, int n,
+                   acnn_jpeg_job* jobs, acnn_jpeg_batch* batch);
+/* Decode the batch planned by acnn_jpeg_plan into `out` (DEVICE, batch->out_bytes): the window of every
+ * active image as packed uint8 RGB, the same bytes as PIL's Image.open(b).convert("RGB") sliced to it.
+ * desc and jobs: DEVICE copies of the host arrays; batch: HOST.  work: DEVICE, batch->work_bytes bytes.
+ * status: DEVICE int32 [n], written with ACNN_JPEG_ST_* bits: an image with a non-zero status has
+ * undefined pixels in its window (and nothing outside it is written).  The entropy decode is the
+ * self-synchronising parallel Huffman decode of Weissenberger & Schmidt (one thread per 1024-bit
+ * subsequence of the unstuffed scan); restart markers are exact synchronisation points.  The kernels
+ * read no byte outside an image's entropy-coded segment. */
+#define ACNN_JPEG_ST_UNSUPPORTED 1
+#define ACNN_JPEG_ST_BAD_CODE 2       /* a bit pattern that is no code of its Huffman table */
+#define ACNN_JPEG_ST_OUT_OF_BITS 4    /* a restart interval or the scan ends inside an MCU */
+#define ACNN_JPEG_ST_MCU_COUNT 8      /* a restart interval or the scan holds the wrong number of MCUs */
+int acnn_jpeg_decode(const acnn_jpeg_desc* desc, const acnn_jpeg_job* jobs, const acnn_jpeg_batch* batch,
+                     const uint8_t* data, uint8_t* out, void* work, int64_t work_bytes, int32_t* status,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
