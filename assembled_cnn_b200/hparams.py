@@ -39,13 +39,13 @@ DEFAULTS = {
     "no_downsample": False,
     "cls_loss_type": "softmax",
     "dataset_name": None,                 # :31 (None -> the ImageNet constants, as data_config)
-    # zero-shot retrieval evaluation (metric/recall_metric.py, model_fns.recall_at_k)
-    "zeroshot_eval": False,               # :273
+    # zero-shot retrieval evaluation (metric/recall_metric.py; model_fns.evaluate_retrieval, recall_at_k)
+    "zeroshot_eval": False,               # :273 (train_and_evaluate: evaluate_retrieval, keep by recall_at_1)
     "eval_similarity": "cosine",          # :91 ('cosine' | 'euclidean')
-    "recall_at_k": [1, 5],                # :288
-    "return_embedding": False,            # :27
-    "val_batch_size": 256,                # :39
-    # classification evaluation (model_fns.evaluate_classification)
+    "recall_at_k": [1, 5],                # :288 (max + 1 <= 128; train_and_evaluate needs 1 in it)
+    "return_embedding": False,            # :27 (train_and_evaluate embeds with True, as the reference's loop)
+    "val_batch_size": 256,                # :39 (the retrieval evaluation's batch)
+    # classification and retrieval evaluation (model_fns.evaluate_classification, evaluate_retrieval)
     "preprocessing_type": "imagenet",     # :128
     "val_regex": "validation-*",          # :284
     # training from TFRecord shards (model_fns.train_and_evaluate)

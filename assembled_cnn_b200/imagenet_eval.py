@@ -1,7 +1,8 @@
 """The data side of the ImageNet classification evaluation (classifier.evaluate(input_fn_eval),
 nets/run_loop_classification.py:397-402,446-448): the validation shards, the TFRecord / tf.train.Example
 reader, the eval preprocessing geometry and the descriptors of acnn_resize_crop_u8.  The device side is
-model_fns.evaluate_classification.
+model_fns.evaluate_classification; the zero-shot retrieval evaluation (model_fns.evaluate_retrieval) reads
+the same shards with missing_label=-1.
 
   validation_files      utils/data_util.py:161-170      sorted(glob(data_dir/val_regex))
   read_records          utils/data_util.py:173-208      image/encoded and image/class/label of every record
@@ -54,7 +55,7 @@ def validation_files(data_dir, val_regex="validation-*"):
     """get_filenames(is_training=False): the shards matching data_dir/val_regex, sorted."""
     files = sorted(glob.glob(os.path.join(data_dir, val_regex)))
     if not files:
-        raise FileNotFoundError("classification evaluation: no file matches %s" % os.path.join(data_dir, val_regex))
+        raise FileNotFoundError("evaluation: no file matches %s" % os.path.join(data_dir, val_regex))
     return files
 
 
@@ -108,14 +109,16 @@ def _float_list(buf, feature):
     return np.frombuffer(b"".join(vals), dtype="<f4").astype(np.float32)
 
 
-def parse_example(buf, logits=False):
+def parse_example(buf, logits=False, missing_label=None):
     """(label, (start, end) of the encoded image in buf) of a serialised tf.train.Example: the
     'image/class/label' int64 and 'image/encoded' bytes features (parse_example_proto).  Only the
     protobuf wire format is read: Example.features(1) -> Features.feature(1) map entries {key(1),
     value(2)} -> Feature.bytes_list(1) / int64_list(3) -> value(1).  A repeated key keeps its last
     value, as protobuf's map parsing does.  logits=True appends the float32 values of the
     'image/logit' FloatList (the knowledge-distillation teacher logits; empty when the feature is
-    absent, as tf.VarLenFeature)."""
+    absent, as tf.VarLenFeature).  An Example without 'image/class/label' raises ValueError unless
+    missing_label is given, which is then its label (-1: the reference's default_value, the
+    distractor label of the retrieval evaluation)."""
     feats = {}
     for f, wt, v in _fields(buf, 0, len(buf)):
         if f != 1 or wt != 2:
@@ -131,14 +134,14 @@ def parse_example(buf, logits=False):
                     value = kv
             if key in (b"image/encoded", b"image/class/label", b"image/logit"):
                 feats[key] = value
-    if b"image/encoded" not in feats or b"image/class/label" not in feats:
+    if b"image/encoded" not in feats or (b"image/class/label" not in feats and missing_label is None):
         raise ValueError("Example without image/encoded or image/class/label")
     enc = []
     for f, wt, v in _fields(buf, *feats[b"image/encoded"]):
         if f == 1 and wt == 2:                       # BytesList
             enc += [v2 for f2, wt2, v2 in _fields(buf, *v) if f2 == 1 and wt2 == 2]
-    labels = []
-    for f, wt, v in _fields(buf, *feats[b"image/class/label"]):
+    labels = [] if b"image/class/label" in feats else [int(missing_label)]
+    for f, wt, v in _fields(buf, *feats.get(b"image/class/label", (0, 0))):
         if f == 3 and wt == 2:                       # Int64List, packed or not
             for f2, wt2, v2 in _fields(buf, *v):
                 if f2 == 1 and wt2 == 0:
@@ -158,9 +161,10 @@ def parse_example(buf, logits=False):
     return label, enc[0]
 
 
-def read_records(path, logits=False):
+def read_records(path, logits=False, missing_label=None):
     """[(label, offset, length)] of every record of a TFRecord file: the label and the byte range of the
-    encoded image in the file (logits=True: [(label, offset, length, float32 image/logit values)]).  A
+    encoded image in the file (logits=True: [(label, offset, length, float32 image/logit values)];
+    missing_label: the label of a record without one, as parse_example).  A
     record is u64 length, u32 masked CRC32C of the length, the data, u32 masked CRC32C of the data.  The
     length's CRC is verified; the data's is not (a pure-Python CRC over the 6.4 GB of ImageNet validation
     JPEGs would take far longer than the evaluation).  A truncated or corrupt record raises ValueError
@@ -180,7 +184,7 @@ def read_records(path, logits=False):
         if start + length + 4 > n:
             raise ValueError("%s: truncated record at byte offset %d" % (path, pos))
         try:
-            ex = parse_example(memoryview(data)[start:start + length], logits)
+            ex = parse_example(memoryview(data)[start:start + length], logits, missing_label)
         except ValueError as e:
             raise ValueError("%s: bad tf.train.Example in the record at byte offset %d: %s" % (path, pos, e))
         label, (a, b) = ex[:2]

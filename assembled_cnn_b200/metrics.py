@@ -67,6 +67,7 @@ class EvalMetrics:
 # --------------------------------------------------------------------------------------------------
 SIMILARITIES = {"cosine": 0, "euclidean": 1}
 DTYPES = {"bf16": 0, "fp32": 1}
+KNN_MAX_K = 128      # the largest k of acnn_knn_topk's per-row candidate lists (include/acnn.h)
 
 
 def knn_topk(query, index, k, similarity="cosine", dtype="bf16"):
@@ -154,16 +155,22 @@ class RecallAtK:
         return sum(int(e.shape[0]) for e in self.embeddings)
 
     def result(self):
-        feats = torch.cat(self.embeddings)
-        labels = torch.cat(self.labels)
-        if not bool(torch.isfinite(feats).all()):
-            raise ValueError("RecallAtK: the embeddings contain NaN or infinite values")
-        is_query = labels != -1
-        idx, _ = knn_topk(feats[is_query], feats, max(self.k_list) + 1, self.similarity, self.dtype)
-        if bool((idx >= feats.shape[0]).any()):
-            # a row with fewer than k finite similarities (e.g. squared distances overflowing fp32)
-            raise ValueError("RecallAtK: similarities are not finite; cannot rank the index")
-        return recall_from_sorted_idx(idx, labels[is_query], labels, self.k_list)
+        return recall_of_index(torch.cat(self.embeddings), torch.cat(self.labels), self.k_list, self.similarity,
+                               self.dtype)
+
+
+def recall_of_index(feats, labels, k_list=(1, 5), similarity="cosine", dtype="bf16"):
+    """RecallAtK's result for a whole index already on the device: feats fp32 [N, d], labels int64 [N]
+    (-1: a distractor).  One acnn_knn_topk with k = max(k_list) + 1 over queries = the rows whose label
+    != -1 against every row, then get_recall's rules.  Non-finite embeddings raise ValueError."""
+    if not bool(torch.isfinite(feats).all()):
+        raise ValueError("RecallAtK: the embeddings contain NaN or infinite values")
+    is_query = labels != -1
+    idx, _ = knn_topk(feats[is_query], feats, max(k_list) + 1, similarity, dtype)
+    if bool((idx >= feats.shape[0]).any()):
+        # a row with fewer than k finite similarities (e.g. squared distances overflowing fp32)
+        raise ValueError("RecallAtK: similarities are not finite; cannot rank the index")
+    return recall_from_sorted_idx(idx, labels[is_query], labels, k_list)
 
 
 # --------------------------------------------------------------------------------------------------

@@ -11,6 +11,8 @@ Mirrors (same names, argument meaning and error behaviour):
                                      corruption_error
   * nets/run_loop_classification.py:397-402,446-448  classifier.evaluate(input_fn_eval) (the ImageNet
                                      classification evaluation) as evaluate_classification
+  * metric/recall_metric.py:13-180 fed by functions/input_fns.py:148-165 (recall_at_k on the validation
+                                     shards, run by --zeroshot_eval) as evaluate_retrieval
 plus `build_model(**flags)` (the name BASELINE.json uses; the reference has no such function).
 
 The reference builds a TF graph and lets the Estimator run it; here a call executes on the GPU:
@@ -816,27 +818,23 @@ class _CorruptionEvalDevice(_EvalPipeline):
         return c
 
 
-class _ClassifyEvalDevice(_EvalPipeline):
-    """The classification evaluation's loop: decoded images of any sizes are packed into a growable
-    pinned uint8 buffer with one acnn_resize_desc per image; resize + crop + mean, the eval forward and
-    the per-row metrics (acnn_classify_rows) run as one CUDA graph per (slot, valid rows).  The per-row
-    results of every batch are appended to device arrays of `total` rows (`rows`), read once at the end."""
+class _ResizedEvalPipeline(_EvalPipeline):
+    """The input side of the evaluations over TFRecord shards: decoded images of any sizes are packed into a
+    growable pinned uint8 buffer with one acnn_resize_desc per image, or decoded on the device
+    (run_batch_encoded), and the batch's labels (`label_dtype`) go to the device slot with them; a subclass's
+    `_body` starts with rt.set_images_resized (resize + crop + mean)."""
 
-    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_smoothing, total):
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_dtype=torch.int32):
         super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
-        i32 = dict(dtype=torch.int32)
-        self.size, self.label_smoothing = size, float(label_smoothing)
+        lab = dict(dtype=label_dtype)
+        self.size = size
         # pinned image bytes (grown on demand), labels, descriptors
-        self.host = [[torch.empty(0, dtype=torch.uint8), torch.zeros(batch, **i32).pin_memory(),
+        self.host = [[torch.empty(0, dtype=torch.uint8), torch.zeros(batch, **lab).pin_memory(),
                       torch.zeros(32 * batch, dtype=torch.uint8).pin_memory()] for _ in range(self.RING)]
         # device image bytes (allocated on the copy stream, grown on demand), labels, descriptors: a graph
         # holds the descriptor table's address only, so the image bytes may move
-        self.slots = [[None, torch.zeros(batch, **i32, device=self.dev),
+        self.slots = [[None, torch.zeros(batch, **lab, device=self.dev),
                        torch.zeros(32 * batch, dtype=torch.uint8, device=self.dev)] for _ in range(2)]
-        kinds = (torch.int32, torch.float32, torch.int32, torch.float32)       # pred, conf, hit_5, ce
-        self.out = tuple(torch.zeros(batch, dtype=dt, device=self.dev) for dt in kinds)
-        self.rows = tuple(torch.zeros(total, dtype=dt, device=self.dev) for dt in kinds)
-        self.done = 0
         self.decoders, self._geometry = [None, None], None
 
     def _stage(self, h, slot, images, labels):
@@ -860,17 +858,10 @@ class _ClassifyEvalDevice(_EvalPipeline):
                 s, rh, rw, cy, cx = self._geometry(ih, iw)
                 desc[i] = (addr, ih, iw, rh, rw, cy, cx)
         check_descriptors(desc, n, self.size)
-        hlab[:n].copy_(torch.as_tensor(labels, dtype=torch.int32))
+        hlab[:n].copy_(torch.as_tensor(labels, dtype=hlab.dtype))
         _, dlab, ddesc = self.slots[slot]
         ddesc.copy_(hdesc, non_blocking=True)
         dlab.copy_(hlab, non_blocking=True)
-
-    def _body(self, slot, n_valid):
-        from .metrics import classify_rows
-        _, labels, desc = self.slots[slot]
-        self.rt.set_images_resized(desc, n_valid, self.mean)
-        self.rt.run_forward()
-        classify_rows(self.logits, labels, n_valid, 5, self.label_smoothing, out=self.out)
 
     def run_batch_encoded(self, buffers, labels, geometry):
         """run_batch from encoded images (jpeg.JpegDecoder on the copy stream; PIL for the images the device
@@ -881,11 +872,66 @@ class _ClassifyEvalDevice(_EvalPipeline):
         finally:
             self._geometry = None
 
+
+class _ClassifyEvalDevice(_ResizedEvalPipeline):
+    """The classification evaluation's loop: resize + crop + mean, the eval forward and the per-row metrics
+    (acnn_classify_rows) run as one CUDA graph per (slot, valid rows).  The per-row results of every batch
+    are appended to device arrays of `total` rows (`rows`), read once at the end."""
+
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_smoothing, total):
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
+        self.label_smoothing = float(label_smoothing)
+        kinds = (torch.int32, torch.float32, torch.int32, torch.float32)       # pred, conf, hit_5, ce
+        self.out = tuple(torch.zeros(batch, dtype=dt, device=self.dev) for dt in kinds)
+        self.rows = tuple(torch.zeros(total, dtype=dt, device=self.dev) for dt in kinds)
+        self.done = 0
+
+    def _body(self, slot, n_valid):
+        from .metrics import classify_rows
+        _, labels, desc = self.slots[slot]
+        self.rt.set_images_resized(desc, n_valid, self.mean)
+        self.rt.run_forward()
+        classify_rows(self.logits, labels, n_valid, 5, self.label_smoothing, out=self.out)
+
     def run_batch(self, images, labels):
         super().run_batch(images, labels)
         n = len(images)
         for dst, src in zip(self.rows, self.out):
             dst[self.done:self.done + n].copy_(src[:n])
+        self.done += n
+
+
+class _RetrievalEvalDevice(_ResizedEvalPipeline):
+    """The retrieval evaluation's loop: resize + crop + mean and the eval forward run as one CUDA graph per
+    (slot, valid rows), which also copies the slot's int64 labels beside the model's outputs.  After each
+    batch its valid rows are appended to the device index: `index` fp32 [total, d] (the embedding, else the
+    pooled features, with return_embedding; the logits without, as Model.__call__ returns) and `labels`
+    int64 [total]."""
+
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, return_embedding, total):
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph, label_dtype=torch.int64)
+        m = self.rt.plan.meta
+        if return_embedding:
+            self.feat = self.rt.t[m["embedding"] if "embedding" in m else m["pooled"]].reshape(batch, -1)
+        else:
+            self.feat = self.logits
+        self.batch_labels = torch.zeros(batch, dtype=torch.int64, device=self.dev)
+        self.index = torch.zeros(total, self.feat.shape[1], dtype=torch.float32, device=self.dev)
+        self.labels = torch.zeros(total, dtype=torch.int64, device=self.dev)
+        self.done = 0
+
+    def _body(self, slot, n_valid):
+        _, labels, desc = self.slots[slot]
+        self.rt.set_images_resized(desc, n_valid, self.mean)
+        self.rt.run_forward()
+        # the slot is refilled two batches later: its labels are read here, before the batch's event
+        self.batch_labels.copy_(labels)
+
+    def run_batch(self, images, labels):
+        super().run_batch(images, labels)
+        n = len(images)
+        self.index[self.done:self.done + n].copy_(self.feat[:n])
+        self.labels[self.done:self.done + n].copy_(self.batch_labels[:n])
         self.done += n
 
 
@@ -991,7 +1037,6 @@ def evaluate_classification(model, data_dir, *, val_regex="validation-*", prepro
     device until the end.  loss = the mean over batches of the batch-mean label-smoothed cross-entropy
     (a short last batch counts as one batch, as tf.metrics.mean of the per-batch loss does) +
     l2_loss(weight_decay).  Returns {'accuracy', 'accuracy_top_5', 'ece', 'loss', 'global_step'}."""
-    from concurrent.futures import ThreadPoolExecutor
     from . import imagenet_eval
     from .metrics import classification_result
     size, _ = imagenet_eval.eval_size(preprocessing_type, image_size)
@@ -1007,9 +1052,38 @@ def evaluate_classification(model, data_dir, *, val_regex="validation-*", prepro
     if not records:
         raise ValueError("classification evaluation: the shards under %s hold no record" % data_dir)
     labels = np.array([r[3] for r in records], dtype=np.int64)
-    batches = [records[a:a + batch_size] for a in range(0, len(records), batch_size)]
     ev = _ClassifyEvalDevice(model, batch_size, size, use_resnet_d, use_cuda_graph, label_smoothing,
                              len(records))
+    sizes = _feed_records(ev, records, batch_size, preprocessing_type, image_size, num_workers)
+    pred, conf, hit, ce = (t.cpu().numpy() for t in ev.rows)
+    r = classification_result(pred, conf, hit, ce, labels, sizes)
+    l2 = float(l2_loss(ev.rt, weight_decay))
+    return {"accuracy": r["accuracy"], "accuracy_top_5": r["accuracy_top_5"], "ece": r["ece"],
+            "loss": r["cross_entropy"] + l2, "global_step": global_step}
+
+
+def _check_recall_args(recall_at_k, eval_similarity):
+    """The k list and similarity of the retrieval evaluation, checked before any GPU work."""
+    from .metrics import KNN_MAX_K, SIMILARITIES
+    if eval_similarity not in SIMILARITIES:
+        raise NotImplementedError("eval_similarity must be one of %s" % sorted(SIMILARITIES))
+    k_list = tuple(int(k) for k in recall_at_k)
+    if not k_list or min(k_list) < 1:
+        raise ValueError("recall_at_k must be a non-empty list of positive k (got %r)" % (recall_at_k,))
+    if max(k_list) + 1 > KNN_MAX_K:
+        raise ValueError("recall_at_k: max(recall_at_k) + 1 = %d exceeds %d, the largest k of the fused top-k "
+                         "search (acnn_knn_topk)" % (max(k_list) + 1, KNN_MAX_K))
+    return k_list
+
+
+def _feed_records(ev, records, batch_size, preprocessing_type, image_size, num_workers):
+    """Runs the records [(path, offset, length, label)] through `ev` (a _ResizedEvalPipeline) in batches of
+    batch_size, in order: a pool of `num_workers` CPU threads reads the encoded images four batches ahead of
+    the GPU, ev.run_batch_encoded decodes and evaluates them.  Returns the batch sizes once the device is
+    done."""
+    from concurrent.futures import ThreadPoolExecutor
+    from . import imagenet_eval
+    batches = [records[a:a + batch_size] for a in range(0, len(records), batch_size)]
     pool = ThreadPoolExecutor(max_workers=num_workers or min(32, os.cpu_count() or 1))
     decode = lambda recs: [pool.submit(imagenet_eval.read_encoded, r[0], r[1], r[2]) for r in recs]
     geometry = lambda h, w: imagenet_eval.eval_geometry(h, w, preprocessing_type, image_size)
@@ -1024,11 +1098,60 @@ def evaluate_classification(model, data_dir, *, val_regex="validation-*", prepro
         torch.cuda.current_stream(ev.dev).synchronize()
     finally:
         pool.shutdown(wait=True, cancel_futures=True)
-    pred, conf, hit, ce = (t.cpu().numpy() for t in ev.rows)
-    r = classification_result(pred, conf, hit, ce, labels, [len(b) for b in batches])
-    l2 = float(l2_loss(ev.rt, weight_decay))
-    return {"accuracy": r["accuracy"], "accuracy_top_5": r["accuracy_top_5"], "ece": r["ece"],
-            "loss": r["cross_entropy"] + l2, "global_step": global_step}
+    return [len(b) for b in batches]
+
+
+def _retrieval_index(model, records, size, batch_size, preprocessing_type, image_size, return_embedding,
+                     use_resnet_d, use_cuda_graph, num_workers):
+    """The device index of evaluate_retrieval: (fp32 [N, d] outputs, int64 [N] labels) of the records
+    [(path, offset, length, label)], in order."""
+    ev = _RetrievalEvalDevice(model, batch_size, size, use_resnet_d, use_cuda_graph, return_embedding,
+                              len(records))
+    _feed_records(ev, records, batch_size, preprocessing_type, image_size, num_workers)
+    return ev.index, ev.labels
+
+
+def evaluate_retrieval(model, data_dir, *, val_regex="validation-*", preprocessing_type="imagenet",
+                       image_size=224, batch_size=256, recall_at_k=(1, 5), eval_similarity="cosine",
+                       return_embedding=True, use_resnet_d=None, global_step=None, use_cuda_graph=True,
+                       num_workers=None):
+    """The zero-shot retrieval evaluation of `--zeroshot_eval` (metric/recall_metric.py:13-180 fed by
+    input_fn_ir_eval, functions/input_fns.py:148-165): Recall@K of `model` on the TFRecord shards
+    data_dir/val_regex, each image given the eval preprocessing of `preprocessing_type` (as
+    evaluate_classification).  A record without image/class/label is a distractor (label -1, the
+    reference's default_value): it is in the index, never a query; any other int64 label is kept, so the
+    test classes of a zero-shot split need not lie in [0, num_classes).
+
+    Every shard is read and checked first, and so are the arguments: an empty glob, a corrupt record, an
+    unknown eval_similarity (NotImplementedError), an empty recall_at_k or max(recall_at_k) + 1 above the
+    fused search's 128 fail before any GPU work.  Decoding runs as in evaluate_classification; the device
+    work of a batch (resize + crop from uint8, eval forward in the model's dtype) is one CUDA graph replay
+    (use_cuda_graph=False: the same launches, eager), and its valid rows are copied into a device index
+    of every record: the embedding (return_embedding=True; the pooled features without an embedding layer)
+    or the logits, as Model.__call__(..., return_embedding) returns them.  Then one acnn_knn_topk in the
+    model's dtype, k = max(recall_at_k) + 1, queries = the rows whose label != -1 against every row, and
+    get_recall's rules (metrics.recall_of_index).  Returns {'recall_at_<k>': ..., 'global_step': ...}, as
+    recall_at_k does."""
+    from . import imagenet_eval
+    from .metrics import recall_of_index
+    k_list = _check_recall_args(recall_at_k, eval_similarity)
+    size, _ = imagenet_eval.eval_size(preprocessing_type, image_size)
+    if use_resnet_d is None:
+        use_resnet_d = getattr(model, "use_resnet_d", False)
+    records = [(path, offset, length, label)
+               for path in imagenet_eval.validation_files(data_dir, val_regex)
+               for label, offset, length in imagenet_eval.read_records(path, missing_label=-1)]
+    n_query = sum(r[3] != -1 for r in records)
+    if n_query == 0 or len(records) < max(k_list) + 1:
+        raise ValueError("retrieval evaluation: the shards under %s hold %d records, %d of them queries; it "
+                         "needs a query and at least max(recall_at_k) + 1 = %d records"
+                         % (data_dir, len(records), n_query, max(k_list) + 1))
+    index, labels = _retrieval_index(model, records, size, batch_size, preprocessing_type, image_size,
+                                     return_embedding, use_resnet_d, use_cuda_graph, num_workers)
+    out = {"recall_at_%d" % k: v for k, v in recall_of_index(index, labels, k_list, eval_similarity,
+                                                             model.dtype).items()}
+    out["global_step"] = global_step
+    return out
 
 
 class _TrainFeed:
@@ -1151,11 +1274,16 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     Trainer's step (use_cuda_graph: one graph replay).  It saves model.ckpt-<global step> every
     save_checkpoints_epochs epochs and at its end, keeping keep_checkpoint_max of them, then runs
     evaluate_classification, CheckpointKeeper.save(accuracy) and stops at stop_threshold or once the global
-    step reaches train_epochs * int(num_images / batch_size).  The seed gives the initial weights, the
+    step reaches train_epochs * int(num_images / batch_size).  With zeroshot_eval the evaluation is
+    evaluate_retrieval instead (batch val_batch_size, the recall_at_k, eval_similarity, preprocessing_type
+    and val_regex flags, return_embedding=True as the reference's loop passes it), and accuracy is replaced
+    by recall_at_1 for the keeper and stop_threshold (nets/run_loop_classification.py:439-448,476-480);
+    recall_at_k and eval_similarity are checked before any GPU work.  The seed gives the initial weights, the
     record order, the crop windows, the flips and the mixup lambdas (imagenet_train's counter-based
     generators).  num_images is the number of records in the shards (the reference's data_config count).
     Under torch.distributed every rank trains its slice of each global batch; rank 0 writes the
-    checkpoints and evaluates.  Returns the list of the cycles' evaluation results."""
+    checkpoints and evaluates.  Returns the list of the cycles' evaluation results (the recall dicts with
+    zeroshot_eval)."""
     from concurrent.futures import ThreadPoolExecutor
     from . import imagenet_train as it
     from .checkpoint import CheckpointKeeper, latest_checkpoint, restore, save_checkpoint, warm_start
@@ -1168,6 +1296,11 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     ds = DATASETS[ds_name]
     size = it.train_size(p["preprocessing_type"], image_size)
     eval_size(p["preprocessing_type"], image_size)
+    zeroshot = bool(p["zeroshot_eval"])
+    if zeroshot and 1 not in _check_recall_args(p["recall_at_k"], p["eval_similarity"]):
+        raise ValueError("zeroshot_eval ranks the checkpoints by recall_at_1: recall_at_k must hold 1 (got %r)"
+                         % (p["recall_at_k"],))
+    key = "recall_at_1" if zeroshot else "accuracy"
     dist = torch.distributed.is_initialized()
     world = torch.distributed.get_world_size() if dist else 1
     rank = torch.distributed.get_rank() if dist else 0
@@ -1252,12 +1385,20 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
             if rank == 0:
                 if latest_checkpoint(model_dir) is None:
                     raise ValueError("evaluation: no checkpoint in %s" % model_dir)
-                res = evaluate_classification(
-                    model, data_dir, val_regex=p["val_regex"], preprocessing_type=p["preprocessing_type"],
-                    image_size=image_size, batch_size=trainer.local_batch, label_smoothing=p["label_smoothing"],
-                    weight_decay=p["weight_decay"], global_step=trainer.global_step,
-                    use_cuda_graph=use_cuda_graph, num_workers=num_workers)
-                keeper.save(res["accuracy"], model_dir)
+                if zeroshot:
+                    # the reference's loop embeds with return_embedding=True whatever the flag says
+                    res = evaluate_retrieval(
+                        model, data_dir, val_regex=p["val_regex"], preprocessing_type=p["preprocessing_type"],
+                        image_size=image_size, batch_size=p["val_batch_size"], recall_at_k=p["recall_at_k"],
+                        eval_similarity=p["eval_similarity"], return_embedding=True,
+                        global_step=trainer.global_step, use_cuda_graph=use_cuda_graph, num_workers=num_workers)
+                else:
+                    res = evaluate_classification(
+                        model, data_dir, val_regex=p["val_regex"], preprocessing_type=p["preprocessing_type"],
+                        image_size=image_size, batch_size=trainer.local_batch, label_smoothing=p["label_smoothing"],
+                        weight_decay=p["weight_decay"], global_step=trainer.global_step,
+                        use_cuda_graph=use_cuda_graph, num_workers=num_workers)
+                keeper.save(res[key], model_dir)
             else:
                 res = None
             if dist:
@@ -1265,7 +1406,7 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                 torch.distributed.broadcast_object_list(box, src=0)
                 res = box[0]
             results.append(res)
-            if stop_threshold is not None and res["accuracy"] >= stop_threshold:
+            if stop_threshold is not None and res[key] >= stop_threshold:
                 break
             if res["global_step"] >= total_train_steps:
                 break
