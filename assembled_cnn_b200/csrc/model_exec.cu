@@ -933,6 +933,29 @@ int acnn_set_images_cropped(acnn_model* m, const acnn_crop_desc* desc_dev, const
                              (float*)(m->ws + t.ws_offset), stream);
 }
 
+int acnn_set_images_augmented(acnn_model* m, const acnn_crop_desc* desc_dev, const acnn_autoaugment_desc* aug_dev,
+                              uint8_t* work_dev, const float* mean3, void* stream) {
+  ACNN_REQUIRE(m && m->bound && desc_dev && aug_dev && work_dev && mean3, "acnn_set_images_augmented: not bound / null");
+  const Plan& p = m->plan;
+  const Tensor& t = p.tensors[p.images];
+  ACNN_REQUIRE(t.shape[1] == t.shape[2], "acnn_set_images_augmented: the plan's input is %lldx%lld, not square",
+               (long long)t.shape[1], (long long)t.shape[2]);
+  const void* ptrs[3] = {desc_dev, aug_dev, work_dev};
+  const char* names[3] = {"desc_dev", "aug_dev", "work_dev"};
+  for (int k = 0; k < 3; ++k) {
+    cudaPointerAttributes at{};
+    const cudaError_t e = cudaPointerGetAttributes(&at, ptrs[k]);
+    if (e != cudaSuccess) {
+      set_error("acnn_set_images_augmented: %s: %s", names[k], cudaGetErrorString(e));
+      return ACNN_ERR_CUDA;
+    }
+    ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
+                 "acnn_set_images_augmented: %s must be device memory", names[k]);
+  }
+  return acnn_crop_resize_autoaugment_u8(desc_dev, aug_dev, (int)t.shape[0], (int)t.shape[0], (int)t.shape[1],
+                                         mean3, work_dev, (float*)(m->ws + t.ws_offset), stream);
+}
+
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream) {
   ACNN_REQUIRE(m && m->bound && hp, "acnn_set_hparams: not bound / null");
   return memcpy_async(m->ws + m->hp_off, hp, 32, stream, "acnn_set_hparams");

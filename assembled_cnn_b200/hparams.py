@@ -51,7 +51,8 @@ DEFAULTS = {
     # training from TFRecord shards (model_fns.train_and_evaluate)
     "train_regex": "train-*",             # :280
     "training_random_crop": True,         # :256
-    "autoaugment_type": None,             # :132 (only None: AutoAugment is not implemented)
+    "autoaugment_type": None,             # :132 (only None in train_and_evaluate, which does not draw AutoAugment
+                                          # records yet; Trainer.train_step_cropped(augment=) runs it)
     "num_best_ckpt_to_keep": 3,           # :242
     "keep_ckpt_every_eval": True,         # :246
     "keep_checkpoint_max": 20,            # :249

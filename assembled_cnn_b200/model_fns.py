@@ -357,6 +357,7 @@ class Trainer:
         self._consumed = None
         self._stage_imgs = None
         self._stage_labs = None
+        self._aug_work = None
 
     @property
     def input_batch(self):
@@ -443,12 +444,23 @@ class Trainer:
             self._consumed.record(torch.cuda.current_stream(rt.dev))
         return self._step(lam1, lam2, teacher_logits, keep_prob)
 
-    def train_step_cropped(self, desc, labels, mean, lam1=None, lam2=None, teacher_logits=None, keep_prob=None):
+    def train_step_cropped(self, desc, labels, mean, lam1=None, lam2=None, teacher_logits=None, keep_prob=None,
+                           augment=None):
         """train_step with the images made on the device from training crop windows: one
         acnn_set_images_cropped launch (flip, resize to H x W, - mean) on the current stream, then the step.
         desc: a CUDA uint8 tensor of input_batch 32-byte acnn_crop_desc (imagenet_train.CROP_DESC_DTYPE,
-        checked by the caller); labels int32 [input_batch]; the rest as train_step."""
-        self.rt.set_images_cropped(desc, mean)
+        checked by the caller); labels int32 [input_batch]; the rest as train_step.
+        augment: None, or a CUDA uint8 tensor of input_batch 88-byte AutoAugment descriptors
+        (autoaugment.AUTOAUG_DESC_DTYPE, checked by the caller with check_autoaugment_descriptors); then the
+        images come from acnn_set_images_augmented instead, through a work buffer allocated on first use."""
+        if augment is None:
+            self.rt.set_images_cropped(desc, mean)
+        else:
+            if self._aug_work is None:
+                b, s = self.images_buf.shape[0], self.images_buf.shape[1]
+                self._aug_work = torch.empty(self.rt.lib.acnn_autoaugment_work_bytes(b, s), dtype=torch.uint8,
+                                             device=self.rt.dev)
+            self.rt.set_images_augmented(desc, augment, self._aug_work, mean)
         self.labels_buf.copy_(labels, non_blocking=True)
         return self._step(lam1, lam2, teacher_logits, keep_prob)
 

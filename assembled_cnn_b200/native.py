@@ -84,6 +84,7 @@ PROTOTYPES = {
     "acnn_set_images_u8": (_i, [_vp] * 4),
     "acnn_set_images_resized": (_i, [_vp, _vp, _i, _vp, _vp]),
     "acnn_set_images_cropped": (_i, [_vp] * 4),
+    "acnn_set_images_augmented": (_i, [_vp] * 6),
     "acnn_set_hparams": (_i, [_vp, _vp, _vp]),
     "acnn_get_logits": (_i, [_vp, _vp, _vp]),
     "acnn_get_loss": (_i, [_vp, _vp, _vp]),
@@ -405,6 +406,17 @@ class NativeRuntime(_runtime_base()):
         _check_crop_args(desc, self.t[self.plan.meta["images"]], mean)
         _lib.check(self.lib.acnn_set_images_cropped(self.model.handle, desc.data_ptr(), mean.data_ptr(),
                                                     self.stream), "acnn_set_images_cropped")
+
+    def set_images_augmented(self, desc, aug, work, mean):
+        """acnn_set_images_augmented: set_images_cropped with AutoAugment (the resized image truncated to
+        uint8, aug's two operations, - mean[c]); aug a CUDA uint8 tensor of input_batch 88-byte
+        acnn_autoaugment_desc (autoaugment.AUTOAUG_DESC_DTYPE), validated by the caller; work a CUDA uint8
+        tensor of acnn_autoaugment_work_bytes(input_batch, S) bytes."""
+        from .runtime import _check_augment_args
+        _check_augment_args(desc, aug, work, self.t[self.plan.meta["images"]], mean)
+        _lib.check(self.lib.acnn_set_images_augmented(self.model.handle, desc.data_ptr(), aug.data_ptr(),
+                                                      work.data_ptr(), mean.data_ptr(), self.stream),
+                   "acnn_set_images_augmented")
 
     def zero_step_buffers(self):
         _lib.check(self.lib.acnn_clear_step_buffers(self.model.handle, self.stream),

@@ -59,6 +59,21 @@ def _check_crop_args(desc, images, mean):
     return b, h
 
 
+def _check_augment_args(desc, aug, work, images, mean):
+    """Arguments of set_images_augmented: those of set_images_cropped, B descriptors of 88 bytes and a work
+    buffer of acnn_autoaugment_work_bytes(B, S) bytes, both uint8 on the input buffer's device.
+    Returns (B, S)."""
+    b, s = _check_crop_args(desc, images, mean)
+    if aug.dtype != torch.uint8 or aug.numel() != 88 * b or aug.device != images.device or not aug.is_contiguous():
+        raise ValueError("aug must be a contiguous uint8 tensor of %d AutoAugment descriptors (%d bytes) on %s"
+                         % (b, 88 * b, images.device))
+    need = _lib.load().acnn_autoaugment_work_bytes(b, s)
+    if work.dtype != torch.uint8 or work.numel() < need or work.device != images.device \
+            or not work.is_contiguous():
+        raise ValueError("work must be a contiguous uint8 tensor of at least %d bytes on %s" % (need, images.device))
+    return b, s
+
+
 class Runtime:
     def __init__(self, plan: Plan, device="cuda:0", eps: float = 1e-5, share: "Runtime | None" = None,
                  deterministic: "bool | None" = None):
@@ -313,6 +328,17 @@ class Runtime:
         b, s = _check_crop_args(desc, images, mean)
         _lib.check(self.lib.acnn_crop_resize_u8(desc.data_ptr(), b, b, s, mean.data_ptr(), images.data_ptr(),
                                                 self.stream), "acnn_crop_resize_u8")
+
+    def set_images_augmented(self, desc, aug, work, mean):
+        """set_images_cropped with AutoAugment (acnn_crop_resize_autoaugment_u8: flip, resize, clip and
+        truncate to uint8, aug's two operations, - mean[c]).  aug: a CUDA uint8 tensor of B 88-byte
+        acnn_autoaugment_desc (autoaugment.AUTOAUG_DESC_DTYPE) on this device, validated by the caller; work a
+        CUDA uint8 tensor of acnn_autoaugment_work_bytes(B, S) bytes."""
+        images = self.t[self.plan.meta["images"]]
+        b, s = _check_augment_args(desc, aug, work, images, mean)
+        _lib.check(self.lib.acnn_crop_resize_autoaugment_u8(desc.data_ptr(), aug.data_ptr(), b, b, s, mean.data_ptr(),
+                                                            work.data_ptr(), images.data_ptr(), self.stream),
+                   "acnn_crop_resize_autoaugment_u8")
 
     def zero_step_buffers(self):
         st = self.stream

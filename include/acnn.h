@@ -513,6 +513,48 @@ typedef struct acnn_crop_desc {
  * or desc not 8-byte aligned: ACNN_ERR_INVALID before any CUDA call. */
 int acnn_crop_resize_u8(const acnn_crop_desc* desc, int B, int n_valid, int S, const float* mean, float* out,
                         void* stream);
+/* AutoAugment (preprocessing/autoaugment.py distort_image_with_autoaugment) of one training image: the two
+ * operations of the sub-policy drawn for it, resolved on the host (assembled_cnn_b200/autoaugment.py).
+ * An operation that does not apply has op = ACNN_AA_IDENTITY.  Arguments per op:
+ *   POSTERIZE     i[0] = shift in [0, 7] (8 - bits, clamped as TF's shift ops do): (x >> i0) << i0
+ *   SOLARIZE      i[0] = threshold in [0, 255] (the uint8 constant):  x < i0 ? x : 255 - x
+ *   SOLARIZE_ADD  i[0] = addition >= 0:  x < 128 ? min(x + i0, 255) : x
+ *   COLOR, BRIGHTNESS, SHARPNESS, CONTRAST  f[0] = blend factor >= 0; CONTRAST i[0] = its grey in [0, 255]
+ *   ROTATE, SHEAR_X, SHEAR_Y, TRANSLATE_X, TRANSLATE_Y  f[0..5] = the projective transform t0..t5
+ *   CUTOUT        i[0] = centre row, i[1] = centre column, i[2] = pad size
+ * 88 bytes, the layout of autoaugment.AUTOAUG_DESC_DTYPE. */
+enum {
+  ACNN_AA_IDENTITY = 0, ACNN_AA_AUTOCONTRAST, ACNN_AA_EQUALIZE, ACNN_AA_INVERT, ACNN_AA_ROTATE, ACNN_AA_POSTERIZE,
+  ACNN_AA_SOLARIZE, ACNN_AA_SOLARIZE_ADD, ACNN_AA_COLOR, ACNN_AA_CONTRAST, ACNN_AA_BRIGHTNESS, ACNN_AA_SHARPNESS,
+  ACNN_AA_SHEAR_X, ACNN_AA_SHEAR_Y, ACNN_AA_TRANSLATE_X, ACNN_AA_TRANSLATE_Y, ACNN_AA_CUTOUT, ACNN_AA_NUM_OPS
+};
+typedef struct acnn_autoaugment_op {
+  int32_t op;
+  int32_t i[3];
+  float f[6];
+} acnn_autoaugment_op;
+typedef struct acnn_autoaugment_desc {
+  int32_t subpolicy;                 /* the drawn sub-policy (informational; the kernel does not read it) */
+  int32_t reserved_;
+  acnn_autoaugment_op slot[2];
+} acnn_autoaugment_desc;
+/* Bytes of the `work` buffer acnn_crop_resize_autoaugment_u8 needs for B images of S x S: two uint8 planes
+ * per image, each S*S*3 bytes rounded up to 16.  -1 for B < 1, S < 1 or a size that overflows. */
+int64_t acnn_autoaugment_work_bytes(int B, int S);
+/* out fp32 NHWC [B,S,S,3], row b < n_valid = (float)autoaugment(trunc(clip(resize(window_b), 0, 255)))
+ * - mean[c]: the training preprocessing of preprocessing/imagenet_preprocessing.py:269-313 with
+ * autoaugment_type set.  The resize is acnn_crop_resize_u8's, bit for bit; then clip_by_value(0, 255) and a
+ * truncating cast to uint8 (for every image, also when no operation applies), aug_b's two operations in
+ * order on the uint8 image, each float step a separately rounded fp32 operation, then the cast to fp32 and
+ * the mean.  One CTA per image; the image lives in two planes of `work` (DEVICE, acnn_autoaugment_work_bytes
+ * (B, S) bytes, 16-byte aligned); histograms and minima / maxima are integer shared-memory atomics, so the
+ * result does not depend on the order of execution.  desc, aug: DEVICE arrays of B descriptors, checked by
+ * the caller (acnn_crop_resize_u8; autoaugment.check_autoaugment_descriptors).  mean: float[3], host or
+ * device.  Rows >= n_valid are not written.  Null pointers, B < 1, S < 1, n_valid outside [0, B], out not
+ * 4-byte, desc or aug not 8-byte, work not 16-byte aligned: ACNN_ERR_INVALID before any CUDA call. */
+int acnn_crop_resize_autoaugment_u8(const acnn_crop_desc* desc, const acnn_autoaugment_desc* aug, int B,
+                                    int n_valid, int S, const float* mean, uint8_t* work, float* out,
+                                    void* stream);
 /* Per-row results of the classification metrics for logits fp32 [B][ld] (columns < NC are the
  * classes) and labels int32 [B], for every row r < n_valid (rows >= n_valid are not written):
  *   pred[r]  = tf.argmax(logits): the smallest index of the largest logit;

@@ -192,6 +192,12 @@ int acnn_set_images_resized(acnn_model* m, const acnn_resize_desc* desc_dev, int
  * the caller, see acnn_crop_resize_u8; a host pointer is ACNN_ERR_INVALID); mean3: float[3], host or
  * device. */
 int acnn_set_images_cropped(acnn_model* m, const acnn_crop_desc* desc_dev, const float* mean3, void* stream);
+/* acnn_set_images_cropped with AutoAugment: every row through acnn_crop_resize_autoaugment_u8 (flip, resize,
+ * clip and truncate to uint8, the two operations of aug_dev[b], - mean3[c]).  desc_dev, aug_dev: DEVICE
+ * arrays of input_batch descriptors, work_dev a DEVICE buffer of acnn_autoaugment_work_bytes(input_batch, S)
+ * bytes (host pointers are ACNN_ERR_INVALID); mean3: float[3], host or device. */
+int acnn_set_images_augmented(acnn_model* m, const acnn_crop_desc* desc_dev, const acnn_autoaugment_desc* aug_dev,
+                              uint8_t* work_dev, const float* mean3, void* stream);
 /* float hp[8] as in acnn_model_sizes.hp_offset. */
 int acnn_set_hparams(acnn_model* m, const float* hp, void* stream);
 /* logits [batch, num_classes] fp32 (dense, ld = num_classes) / loss float[4] to a host or device array. */
