@@ -259,19 +259,10 @@ crop_resize_autoaugment_kernel(const acnn_crop_desc* __restrict__ desc, const ac
   const float sy = __fdiv_rn((float)d.h, (float)S), sx = __fdiv_rn((float)d.w, (float)S);
   for (int p = threadIdx.x; p < n; p += kThreads) {
     const int y = p / S, x = p - y * S;
-    const Interp iy = legacy_interp(y, sy, d.h);
-    const Interp ix = legacy_interp(x, sx, d.w);
-    const int cl = d.flip ? d.w - 1 - ix.lo : ix.lo;
-    const int ch = d.flip ? d.w - 1 - ix.hi : ix.hi;
-    const uint8_t* top = d.src + (int64_t)iy.lo * d.w * 3;
-    const uint8_t* bot = d.src + (int64_t)iy.hi * d.w * 3;
-    const int xl = cl * 3, xh = ch * 3;
+    float v[3];
+    legacy_bilinear_rgb(d.src, d.h, d.w, sy, sx, y, x, d.flip != 0, v);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const float tv = lerp_rn((float)top[xl + c], (float)top[xh + c], ix.lerp);
-      const float uv = lerp_rn((float)bot[xl + c], (float)bot[xh + c], ix.lerp);
-      pa[p * 3 + c] = trunc_u8(lerp_rn(tv, uv, iy.lerp));
-    }
+    for (int c = 0; c < 3; ++c) pa[p * 3 + c] = trunc_u8(v[c]);
   }
   __syncthreads();
   // step 2: the two operations, ping-ponging between the planes; an identity slot costs nothing
@@ -319,18 +310,13 @@ int acnn_crop_resize_autoaugment_u8(const acnn_crop_desc* desc, const acnn_autoa
   ACNN_REQUIRE(((uintptr_t)aug & 7) == 0, "acnn_crop_resize_autoaugment_u8: aug must be 8-byte aligned");
   ACNN_REQUIRE(((uintptr_t)work & 15) == 0, "acnn_crop_resize_autoaugment_u8: work must be 16-byte aligned");
   ACNN_REQUIRE((int64_t)S * S <= INT32_MAX / 3, "acnn_crop_resize_autoaugment_u8: S=%d too large", S);
-  cudaPointerAttributes at{};
-  cudaError_t e = cudaPointerGetAttributes(&at, mean);
-  if (e != cudaSuccess) {
-    set_error("acnn_crop_resize_autoaugment_u8: mean: %s", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  const bool mean_on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
-  const float m0 = mean_on_device ? 0.f : mean[0], m1 = mean_on_device ? 0.f : mean[1],
-              m2 = mean_on_device ? 0.f : mean[2];
+  const float* mean_dev;
+  float m[3];
+  const int rc = resolve_mean("acnn_crop_resize_autoaugment_u8", mean, &mean_dev, m);
+  if (rc != ACNN_OK) return rc;
   if (n_valid == 0) return ACNN_OK;
   launch_k(crop_resize_autoaugment_kernel, dim3(n_valid), dim3(kThreads), 0, (cudaStream_t)stream, desc, aug, S,
-           aa_plane_bytes(S), mean_on_device ? mean : (const float*)nullptr, m0, m1, m2, work, out);
+           aa_plane_bytes(S), mean_dev, m[0], m[1], m[2], work, out);
   count_launch();
   return check_launch("crop_resize_autoaugment_u8");
 }

@@ -76,6 +76,19 @@ int scratch_free(void* p, cudaStream_t stream, const char* what) {
   return ACNN_OK;
 }
 
+int resolve_mean(const char* fn, const float* mean, const float** mean_dev, float m[3]) {
+  cudaPointerAttributes at{};
+  const cudaError_t e = cudaPointerGetAttributes(&at, mean);
+  if (e != cudaSuccess) {
+    set_error("%s: mean: %s", fn, cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  const bool on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+  *mean_dev = on_device ? mean : nullptr;
+  for (int c = 0; c < 3; ++c) m[c] = on_device ? 0.f : mean[c];
+  return ACNN_OK;
+}
+
 static int g_num_sms = 0;
 int num_sms() {
   if (g_num_sms == 0) {

@@ -33,6 +33,11 @@ int scratch_free(void* p, cudaStream_t stream, const char* what);
     }                                  \
   } while (0)
 
+// The float[3] `mean` argument of the entry point `fn`, host or device memory: device memory gives
+// *mean_dev = mean, host memory *mean_dev = nullptr and its values in m.  A failed pointer query is
+// reported as "<fn>: mean: <CUDA error>" (ACNN_ERR_CUDA).
+int resolve_mean(const char* fn, const float* mean, const float** mean_dev, float m[3]);
+
 // Programmatic dependent launch (PDL): every kernel of this library starts with
 // `griddepcontrol.launch_dependents; griddepcontrol.wait;` (pdl_entry() in vec.cuh / ptx.cuh), so a
 // kernel launched with the programmatic-stream-serialization attribute may be scheduled (CTAs

@@ -1,10 +1,17 @@
-// ImageNet classification evaluation (classifier.evaluate(input_fn_eval), nets/run_loop_classification.py):
-// the eval preprocessing of decoded images and the per-row metrics of the logits.
+// The input preprocessing of decoded uint8 images, for the evaluation and for training, and the per-row
+// metrics of the classification evaluation (classifier.evaluate(input_fn_eval),
+// nets/run_loop_classification.py).
 //
-//  * resize_crop_u8_kernel: aspect-preserving resize (TF 1.14's legacy bilinear, half_pixel_centers =
-//    false), central crop and mean subtraction of preprocessing/imagenet_preprocessing.py:158-226,295-313
-//    in one pass over a batch of images of different sizes.  Only the S x S pixels the crop keeps are
-//    computed: a resized pixel depends on its own coordinates only.
+//  * resample_u8: one pass over a batch of images of different sizes, resized with TF 1.14's legacy bilinear
+//    (half_pixel_centers = false), cropped to S x S, minus the channel means; one thread per output pixel.
+//    Only the S x S pixels the crop keeps are computed: a resized pixel depends on its own coordinates only.
+//    - resize_crop_u8_kernel: the eval preprocessing (aspect-preserving resize, central crop) of
+//      preprocessing/imagenet_preprocessing.py:158-226,295-313.
+//    - crop_resize_u8_kernel: the training preprocessing of a crop window (imagenet_preprocessing.py:57-97,
+//      269-313, is_training=True): random_flip_left_right, _resize_image to S x S with the independent
+//      scales (float)h / S and (float)w / S, mean_image_subtraction.  The crop itself
+//      (sample_distorted_bounding_box + decode_and_crop_jpeg) happens on the host: each descriptor points at
+//      the window's packed pixels.
 //  * classify_rows_kernel: tf.argmax(logits), the largest softmax probability, tf.nn.in_top_k and the
 //    label-smoothed softmax cross-entropy of every row (nets/run_loop_classification.py:141-234), one warp
 //    per row, no atomics.
@@ -16,10 +23,27 @@
 
 namespace acnn {
 
+// What the resampling reads of a descriptor: the source image, the resized size and the offset of the S x S
+// crop in it, and the flip.  A training window is resized to S x S and not cropped; an eval image is never
+// flipped.
+struct ResampleView {
+  const uint8_t* src;
+  int h, w, rsz_h, rsz_w, crop_y, crop_x;
+  bool flip;
+};
+
+__device__ __forceinline__ ResampleView view(const acnn_resize_desc& d, int) {
+  return {d.src, d.src_h, d.src_w, d.rsz_h, d.rsz_w, d.crop_y, d.crop_x, false};
+}
+
+__device__ __forceinline__ ResampleView view(const acnn_crop_desc& d, int S) {
+  return {d.src, d.h, d.w, S, S, 0, 0, d.flip != 0};
+}
+
 // grid (ceil(S*S / 256), n_valid): one thread per output pixel of one image.
-__global__ void __launch_bounds__(256)
-resize_crop_u8_kernel(const acnn_resize_desc* __restrict__ desc, int S, const float* __restrict__ mean_dev,
-                      float m0, float m1, float m2, float* __restrict__ out) {
+template <class Desc>
+__device__ __forceinline__ void resample_u8(const Desc* __restrict__ desc, int S, const float* __restrict__ mean_dev,
+                                            float m0, float m1, float m2, float* __restrict__ out) {
   pdl_entry();
   if (mean_dev) {
     m0 = mean_dev[0];
@@ -29,22 +53,29 @@ resize_crop_u8_kernel(const acnn_resize_desc* __restrict__ desc, int S, const fl
   const int b = blockIdx.y;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= S * S) return;
-  const acnn_resize_desc d = desc[b];
+  const Desc dd = desc[b];
+  const ResampleView d = view(dd, S);
   const int y = p / S, x = p - (p / S) * S;
   // scale = (float)in_size / out_size (CalculateResizeScale, align_corners = false)
-  const Interp iy = legacy_interp(y + d.crop_y, __fdiv_rn((float)d.src_h, (float)d.rsz_h), d.src_h);
-  const Interp ix = legacy_interp(x + d.crop_x, __fdiv_rn((float)d.src_w, (float)d.rsz_w), d.src_w);
-  const uint8_t* top = d.src + (int64_t)iy.lo * d.src_w * 3;
-  const uint8_t* bot = d.src + (int64_t)iy.hi * d.src_w * 3;
-  const int xl = ix.lo * 3, xh = ix.hi * 3;
+  float v[3];
+  legacy_bilinear_rgb(d.src, d.h, d.w, __fdiv_rn((float)d.h, (float)d.rsz_h), __fdiv_rn((float)d.w, (float)d.rsz_w),
+                      y + d.crop_y, x + d.crop_x, d.flip, v);
   const float mean[3] = {m0, m1, m2};
   float* o = out + ((int64_t)b * S * S + p) * 3;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const float t = lerp_rn((float)top[xl + c], (float)top[xh + c], ix.lerp);
-    const float u = lerp_rn((float)bot[xl + c], (float)bot[xh + c], ix.lerp);
-    o[c] = __fsub_rn(lerp_rn(t, u, iy.lerp), mean[c]);
-  }
+  for (int c = 0; c < 3; ++c) o[c] = __fsub_rn(v[c], mean[c]);
+}
+
+__global__ void __launch_bounds__(256)
+resize_crop_u8_kernel(const acnn_resize_desc* __restrict__ desc, int S, const float* __restrict__ mean_dev,
+                      float m0, float m1, float m2, float* __restrict__ out) {
+  resample_u8(desc, S, mean_dev, m0, m1, m2, out);
+}
+
+__global__ void __launch_bounds__(256)
+crop_resize_u8_kernel(const acnn_crop_desc* __restrict__ desc, int S, const float* __restrict__ mean_dev,
+                      float m0, float m1, float m2, float* __restrict__ out) {
+  resample_u8(desc, S, mean_dev, m0, m1, m2, out);
 }
 
 // One warp per row of logits [B][ld] (columns < NC are the classes).  Per-lane strided partial results,
@@ -126,30 +157,37 @@ classify_rows_kernel(const float* __restrict__ logits, int ld, int NC, const int
 
 using namespace acnn;
 
+// The argument checks and the launch of the entry point `fn` ("acnn_" + the launch's name).
+template <class Desc>
+static int launch_resample(void (*kernel)(const Desc*, int, const float*, float, float, float, float*), const char* fn,
+                           const Desc* desc, int B, int n_valid, int S, const float* mean, float* out, void* stream) {
+  ACNN_REQUIRE(desc && mean && out, "%s: null pointer", fn);
+  ACNN_REQUIRE(B > 0 && S > 0, "%s: bad shape B=%d S=%d", fn, B, S);
+  ACNN_REQUIRE(n_valid >= 0 && n_valid <= B, "%s: n_valid=%d outside [0, B=%d]", fn, n_valid, B);
+  ACNN_REQUIRE(((uintptr_t)out & 3) == 0, "%s: out must be 4-byte aligned", fn);
+  ACNN_REQUIRE(((uintptr_t)desc & 7) == 0, "%s: desc must be 8-byte aligned", fn);
+  ACNN_REQUIRE((int64_t)S * S <= INT32_MAX, "%s: S=%d too large", fn, S);
+  const float* mean_dev;
+  float m[3];
+  const int rc = resolve_mean(fn, mean, &mean_dev, m);
+  if (rc != ACNN_OK) return rc;
+  if (n_valid == 0) return ACNN_OK;
+  launch_k(kernel, dim3(ceil_div(S * S, 256), n_valid), dim3(256), 0, (cudaStream_t)stream, desc, S, mean_dev, m[0],
+           m[1], m[2], out);
+  count_launch();
+  return check_launch(fn + 5);
+}
+
 extern "C" {
 
 int acnn_resize_crop_u8(const acnn_resize_desc* desc, int B, int n_valid, int S, const float* mean, float* out,
                         void* stream) {
-  ACNN_REQUIRE(desc && mean && out, "acnn_resize_crop_u8: null pointer");
-  ACNN_REQUIRE(B > 0 && S > 0, "acnn_resize_crop_u8: bad shape B=%d S=%d", B, S);
-  ACNN_REQUIRE(n_valid >= 0 && n_valid <= B, "acnn_resize_crop_u8: n_valid=%d outside [0, B=%d]", n_valid, B);
-  ACNN_REQUIRE(((uintptr_t)out & 3) == 0, "acnn_resize_crop_u8: out must be 4-byte aligned");
-  ACNN_REQUIRE(((uintptr_t)desc & 7) == 0, "acnn_resize_crop_u8: desc must be 8-byte aligned");
-  ACNN_REQUIRE((int64_t)S * S <= INT32_MAX, "acnn_resize_crop_u8: S=%d too large", S);
-  cudaPointerAttributes at{};
-  cudaError_t e = cudaPointerGetAttributes(&at, mean);
-  if (e != cudaSuccess) {
-    set_error("acnn_resize_crop_u8: mean: %s", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  const bool mean_on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
-  const float m0 = mean_on_device ? 0.f : mean[0], m1 = mean_on_device ? 0.f : mean[1],
-              m2 = mean_on_device ? 0.f : mean[2];
-  if (n_valid == 0) return ACNN_OK;
-  launch_k(resize_crop_u8_kernel, dim3(ceil_div(S * S, 256), n_valid), dim3(256), 0, (cudaStream_t)stream, desc,
-           S, mean_on_device ? mean : (const float*)nullptr, m0, m1, m2, out);
-  count_launch();
-  return check_launch("resize_crop_u8");
+  return launch_resample(resize_crop_u8_kernel, "acnn_resize_crop_u8", desc, B, n_valid, S, mean, out, stream);
+}
+
+int acnn_crop_resize_u8(const acnn_crop_desc* desc, int B, int n_valid, int S, const float* mean, float* out,
+                        void* stream) {
+  return launch_resample(crop_resize_u8_kernel, "acnn_crop_resize_u8", desc, B, n_valid, S, mean, out, stream);
 }
 
 int acnn_classify_rows(const float* logits, int B, int ld, int NC, const int32_t* labels, int n_valid, int k,

@@ -571,6 +571,19 @@ int memcpy_async(void* dst, const void* src, int64_t bytes, void* stream, const 
   return ACNN_OK;
 }
 
+// The argument `name` of the entry point `fn` must be device (or managed) memory: the kernels read it.
+int require_device(const char* fn, const char* name, const void* p) {
+  cudaPointerAttributes at{};
+  const cudaError_t e = cudaPointerGetAttributes(&at, p);
+  if (e != cudaSuccess) {
+    set_error("%s: %s: %s", fn, name, cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged, "%s: %s must be device memory",
+               fn, name);
+  return ACNN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -883,14 +896,8 @@ int acnn_set_inputs(acnn_model* m, const float* images, const int32_t* labels, c
 int acnn_set_images_u8(acnn_model* m, const uint8_t* images_dev, const float* mean3, void* stream) {
   ACNN_REQUIRE(m && m->bound && images_dev && mean3, "acnn_set_images_u8: not bound / null");
   const Plan& p = m->plan;
-  cudaPointerAttributes at{};
-  const cudaError_t e = cudaPointerGetAttributes(&at, images_dev);
-  if (e != cudaSuccess) {
-    set_error("acnn_set_images_u8: %s", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
-               "acnn_set_images_u8: images_dev must be device memory (stage host images in a device buffer)");
+  const int rc = require_device("acnn_set_images_u8", "images_dev", images_dev);
+  if (rc != ACNN_OK) return rc;
   const Tensor& t = p.tensors[p.images];
   return acnn_images_from_u8(images_dev, mean3, (float*)(m->ws + t.ws_offset), (int)t.shape[0], (int)t.shape[1],
                              (int)t.shape[2], stream);
@@ -903,14 +910,8 @@ int acnn_set_images_resized(acnn_model* m, const acnn_resize_desc* desc_dev, int
   const Tensor& t = p.tensors[p.images];
   ACNN_REQUIRE(t.shape[1] == t.shape[2], "acnn_set_images_resized: the plan's input is %lldx%lld, not square",
                (long long)t.shape[1], (long long)t.shape[2]);
-  cudaPointerAttributes at{};
-  const cudaError_t e = cudaPointerGetAttributes(&at, desc_dev);
-  if (e != cudaSuccess) {
-    set_error("acnn_set_images_resized: %s", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
-               "acnn_set_images_resized: desc_dev must be device memory");
+  const int rc = require_device("acnn_set_images_resized", "desc_dev", desc_dev);
+  if (rc != ACNN_OK) return rc;
   return acnn_resize_crop_u8(desc_dev, (int)t.shape[0], n_valid, (int)t.shape[1], mean3,
                              (float*)(m->ws + t.ws_offset), stream);
 }
@@ -921,14 +922,8 @@ int acnn_set_images_cropped(acnn_model* m, const acnn_crop_desc* desc_dev, const
   const Tensor& t = p.tensors[p.images];
   ACNN_REQUIRE(t.shape[1] == t.shape[2], "acnn_set_images_cropped: the plan's input is %lldx%lld, not square",
                (long long)t.shape[1], (long long)t.shape[2]);
-  cudaPointerAttributes at{};
-  const cudaError_t e = cudaPointerGetAttributes(&at, desc_dev);
-  if (e != cudaSuccess) {
-    set_error("acnn_set_images_cropped: %s", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
-               "acnn_set_images_cropped: desc_dev must be device memory");
+  const int rc = require_device("acnn_set_images_cropped", "desc_dev", desc_dev);
+  if (rc != ACNN_OK) return rc;
   return acnn_crop_resize_u8(desc_dev, (int)t.shape[0], (int)t.shape[0], (int)t.shape[1], mean3,
                              (float*)(m->ws + t.ws_offset), stream);
 }
@@ -943,14 +938,8 @@ int acnn_set_images_augmented(acnn_model* m, const acnn_crop_desc* desc_dev, con
   const void* ptrs[3] = {desc_dev, aug_dev, work_dev};
   const char* names[3] = {"desc_dev", "aug_dev", "work_dev"};
   for (int k = 0; k < 3; ++k) {
-    cudaPointerAttributes at{};
-    const cudaError_t e = cudaPointerGetAttributes(&at, ptrs[k]);
-    if (e != cudaSuccess) {
-      set_error("acnn_set_images_augmented: %s: %s", names[k], cudaGetErrorString(e));
-      return ACNN_ERR_CUDA;
-    }
-    ACNN_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged,
-                 "acnn_set_images_augmented: %s must be device memory", names[k]);
+    const int rc = require_device("acnn_set_images_augmented", names[k], ptrs[k]);
+    if (rc != ACNN_OK) return rc;
   }
   return acnn_crop_resize_autoaugment_u8(desc_dev, aug_dev, (int)t.shape[0], (int)t.shape[0], (int)t.shape[1],
                                          mean3, work_dev, (float*)(m->ws + t.ws_offset), stream);

@@ -115,18 +115,13 @@ int acnn_images_from_u8(const uint8_t* images, const float* mean, float* out, in
   ACNN_REQUIRE(B > 0 && H > 0 && W > 0, "acnn_images_from_u8: bad shape [%d,%d,%d,3]", B, H, W);
   ACNN_REQUIRE(((uintptr_t)images & 15) == 0 && ((uintptr_t)out & 15) == 0,
                "acnn_images_from_u8: images and out must be 16-byte aligned");
-  cudaPointerAttributes at{};
-  cudaError_t e = cudaPointerGetAttributes(&at, mean);
-  if (e != cudaSuccess) {
-    set_error("acnn_images_from_u8: mean: %s", cudaGetErrorString(e));
-    return ACNN_ERR_CUDA;
-  }
-  const bool mean_on_device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
-  const float m0 = mean_on_device ? 0.f : mean[0], m1 = mean_on_device ? 0.f : mean[1],
-              m2 = mean_on_device ? 0.f : mean[2];
+  const float* mean_dev;
+  float m[3];
+  const int rc = resolve_mean("acnn_images_from_u8", mean, &mean_dev, m);
+  if (rc != ACNN_OK) return rc;
   const int64_t n = (int64_t)B * H * W * 3, n16 = n / 16;
   launch_k(images_from_u8_kernel, dim3(grid_for(n16 > 0 ? n16 : 1)), dim3(256), 0, (cudaStream_t)stream, images,
-           mean_on_device ? mean : (const float*)nullptr, m0, m1, m2, out, n16, n);
+           mean_dev, m[0], m[1], m[2], out, n16, n);
   count_launch();
   return check_launch("images_from_u8");
 }

@@ -22,6 +22,7 @@ import torch
 
 from . import _lib
 from .imagenet_c import decode_rgb
+from .staging import grow, pack_host, pack_u8
 
 DESC_BYTES = 6368
 # the head of include/acnn.h acnn_jpeg_desc (the tables follow)
@@ -109,15 +110,6 @@ def plan(desc, offsets, windows=None):
     return jobs, batch
 
 
-def _grow(buf, nbytes, device, pin=False):
-    if buf is not None and buf.numel() >= nbytes:
-        return buf
-    n = max(int(nbytes * 1.25), 4096)
-    if pin:
-        return torch.empty(n, dtype=torch.uint8, pin_memory=True)
-    return torch.empty(n, dtype=torch.uint8, device=device)
-
-
 def _window(a, w):
     if w is None:
         return a
@@ -142,7 +134,7 @@ class JpegDecoder:
 
     def _buf(self, key, nbytes, pin=False):
         store = self._h if pin else self._d
-        store[key] = _grow(store.get(key), nbytes, self.device, pin)
+        store[key] = grow(store.get(key), nbytes, self.device, pin)
         return store[key]
 
     def _enqueue(self, buffers, windows, stream, out=None, out_offsets=None):
@@ -202,21 +194,16 @@ class JpegDecoder:
                 res.append((None, a.shape[0], a.shape[1]))
         if slow:
             arrs = list(slow.values())
-            offs = np.cumsum([0] + [(a.nbytes + 15) // 16 * 16 for a in arrs])
-            hfb = self._buf("fallback", int(offs[-1]), pin=True)
-            hnp = hfb.numpy()
-            for a, o in zip(arrs, offs):
-                hnp[o:o + a.nbytes] = a.reshape(-1)
             with torch.cuda.stream(stream):
                 if out is None:
-                    dfb = self._buf("fallback", int(offs[-1]))
-                    dfb[:int(offs[-1])].copy_(hfb[:int(offs[-1])], non_blocking=True)
-                    base = [dfb.data_ptr() + int(o) for o in offs[:-1]]
+                    self._h["fallback"], self._d["fallback"], base = pack_u8(self._h.get("fallback"),
+                                                                             self._d.get("fallback"), arrs, self.device)
                 else:
+                    self._h["fallback"], offs = pack_host(self._h.get("fallback"), arrs)
                     base = []
                     for i, a, o in zip(slow, arrs, offs):
                         oo = int(out_offsets[i])
-                        out[oo:oo + a.nbytes].copy_(hfb[int(o):int(o) + a.nbytes], non_blocking=True)
+                        out[oo:oo + a.nbytes].copy_(self._h["fallback"][o:o + a.nbytes], non_blocking=True)
                         base.append(out.data_ptr() + oo)
                 done = torch.cuda.Event()
                 done.record(stream)

@@ -34,6 +34,7 @@ from .plan import BLOCK_SIZES, ModelConfig, build_plan
 from .metrics import EvalMetrics, RecallAtK
 from .runtime import Runtime
 from .native import NativeModel, NativeRuntime
+from .staging import StagingRing, pack_u8, read_ahead
 
 DEFAULT_VERSION = 1
 # dtype: 'bf16' = production path (bf16 storage, fp32 accumulation -- the analogue of the reference's
@@ -683,49 +684,21 @@ def _replica(model, device, use_resnet_d, batch, size):
     return rep
 
 
-def _grown(buf, nbytes, **kw):
-    if buf is not None and buf.numel() >= nbytes:
-        return buf
-    return torch.empty(max(nbytes + nbytes // 4, 1), dtype=torch.uint8, **kw)
+class _EvalPipeline(StagingRing):
+    """The evaluation loop of one device: each batch is staged from a ring of pinned host sets into one of two
+    device slots on the copy stream, overlapped with the previous batch's forward; the device work of a batch
+    (`_body`: input preparation, eval forward, metric kernel) runs as one CUDA graph per (slot, valid rows).
+    A subclass gives the host sets and slots, stages a batch's labels beside its images (`_fill`) and defines
+    `_body`."""
 
-
-def _pack_u8(hbuf, dbuf, arrays, device):
-    """Packs uint8 arrays at 16-byte aligned offsets into the pinned host buffer `hbuf` and enqueues its copy
-    to the device buffer `dbuf` on the current stream; either buffer is replaced by a larger one when it is
-    too small (None: allocate).  Returns (hbuf, dbuf, the device address of each array)."""
-    offs = np.cumsum([0] + [(a.nbytes + 15) // 16 * 16 for a in arrays])
-    total = int(offs[-1])
-    hbuf = _grown(hbuf, total, pin_memory=True)
-    dbuf = _grown(dbuf, total, device=device)
-    hnp, base = hbuf.numpy(), dbuf.data_ptr()
-    for a, o in zip(arrays, offs):
-        hnp[o:o + a.nbytes] = a.reshape(-1)
-    dbuf[:total].copy_(hbuf[:total], non_blocking=True)
-    return hbuf, dbuf, [base + int(o) for o in offs[:-1]]
-
-
-class _EvalPipeline:
-    """The evaluation loop of one device: decoded batches go from a ring of pinned host buffers to one of
-    two device slots on a copy stream, overlapped with the previous batch's forward; the device work of
-    a batch (`_body`: input preparation, eval forward, metric kernel) runs as one CUDA graph per (slot,
-    valid rows).  A subclass fills a host buffer and enqueues its copy (`_stage`) and defines `_body`."""
-
-    RING = 3        # pinned host batches
-
-    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph):
-        from .imagenet_c import CHANNEL_MEANS
-        self.dev = torch.device(model.device)
-        torch.cuda.set_device(self.dev)
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, host, slots):
+        torch.cuda.set_device(model.device)
+        super().__init__(torch.device(model.device), host, slots)
         self.rt = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d)
         self.batch, self.use_graph = batch, use_cuda_graph
         self.logits = self.rt.t[self.rt.plan.meta["logits"]][:, :model.num_classes]
-        self.host_free = [None] * self.RING
-        self.slot_free = [None, None]
-        self.mean = torch.tensor(CHANNEL_MEANS, dtype=torch.float32, device=self.dev)
-        self.copy_stream = torch.cuda.Stream(self.dev)
         self.graphs = {}
         self.warm = False
-        self.k = 0
 
     def _graph(self, slot, n_valid):
         g = self.graphs.get((slot, n_valid))
@@ -742,29 +715,17 @@ class _EvalPipeline:
             self.graphs[(slot, n_valid)] = g
         return g
 
-    def run_batch(self, images, labels):
-        """Evaluate one batch of len(images) <= batch rows."""
-        n, h, slot = len(images), self.k % self.RING, self.k % 2
-        self.k += 1
-        if self.host_free[h] is not None:
-            self.host_free[h].synchronize()          # its previous host -> device copy has run
-        main, cs = torch.cuda.current_stream(self.dev), self.copy_stream
-        if self.slot_free[slot] is not None:
-            cs.wait_event(self.slot_free[slot])       # the batch before the previous one has read it
-        with torch.cuda.stream(cs):
-            self._stage(h, slot, images, labels)
-            copied = torch.cuda.Event()
-            copied.record(cs)
-        self.host_free[h] = copied
-        main.wait_event(copied)
+    def _run(self, place, labels):
+        """Evaluate one batch of len(labels) <= batch rows, whose images place(h, slot) stages."""
+        n = len(labels)
+        self.push(lambda h, slot: self._fill(h, slot, place, labels))
+        slot = self.take()
         if self.use_graph and self.warm:
             self._graph(slot, n).replay()
         else:
             self._body(slot, n)        # the first batch also loads every kernel before any capture
             self.warm = True
-        ev = torch.cuda.Event()
-        ev.record(main)
-        self.slot_free[slot] = ev
+        self.release(slot)
 
 
 class _CorruptionEvalDevice(_EvalPipeline):
@@ -772,49 +733,45 @@ class _CorruptionEvalDevice(_EvalPipeline):
     eval forward and the top-1 count run as one CUDA graph per (slot, valid rows)."""
 
     def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph):
-        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
-        u8 = dict(dtype=torch.uint8)
-        self.host = [(torch.zeros(batch, size, size, 3, **u8).pin_memory(),
-                      torch.zeros(batch, dtype=torch.int32).pin_memory()) for _ in range(self.RING)]
-        self.slots = [(torch.zeros(batch, size, size, 3, **u8, device=self.dev),
-                       torch.zeros(batch, dtype=torch.int32, device=self.dev)) for _ in range(2)]
+        dev, u8 = torch.device(model.device), dict(dtype=torch.uint8)
+        host = [(torch.zeros(batch, size, size, 3, **u8).pin_memory(),
+                 torch.zeros(batch, dtype=torch.int32).pin_memory()) for _ in range(self.RING)]
+        slots = [(torch.zeros(batch, size, size, 3, **u8, device=dev),
+                  torch.zeros(batch, dtype=torch.int32, device=dev)) for _ in range(2)]
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph, host, slots)
         self.acc = torch.zeros(1, dtype=torch.int64, device=self.dev)
         self.pred = torch.zeros(batch, dtype=torch.int32, device=self.dev)
-        self.decoders, self._files = [None, None], None
 
-    def _stage(self, h, slot, images, labels):
-        """`images` a list of uint8 [H, W, 3] arrays, `labels` ints; or, from run_batch_encoded, the files'
-        encoded bytes, decoded on the copy stream straight into the slot."""
-        hu8, hlab = self.host[h]
-        du8, dlab = self.slots[slot]
-        if self._files is None:
+    def run_batch(self, images, labels):
+        """Evaluate uint8 [H, W, 3] arrays `images` with int `labels`."""
+        def place(h, slot):
+            hu8, du8 = self.host[h][0], self.slots[slot][0]
             for i, a in enumerate(images):
                 hu8[i].copy_(torch.from_numpy(a))
             du8.copy_(hu8, non_blocking=True)
-        else:
-            from . import imagenet_c, jpeg
-            files, S = self._files, du8.shape[1]
-            desc = jpeg.parse(images)
-            for i, d in enumerate(desc):      # a wrong size raises decode_image's error, as the PIL path does
-                if d["supported"] and (int(d["height"]), int(d["width"])) != (S, S):
-                    imagenet_c.decode_image(files[i], S)
-            if self.decoders[slot] is None:
-                self.decoders[slot] = jpeg.JpegDecoder(self.dev)
-            row = S * S * 3
-            self.decoders[slot].stage(images, None, torch.cuda.current_stream(self.dev),
-                                      fallback=lambda i: imagenet_c.decode_image(files[i], S),
-                                      out=du8.view(-1), out_offsets=np.arange(len(images), dtype=np.int64) * row)
-        hlab[:len(images)].copy_(torch.as_tensor(labels, dtype=torch.int32))
-        dlab.copy_(hlab, non_blocking=True)
+        self._run(place, labels)
 
     def run_batch_encoded(self, buffers, labels, files):
-        """run_batch from the encoded bytes of `files` (jpeg.JpegDecoder on the copy stream; PIL, through
-        imagenet_c.decode_image, for the images the device does not decode)."""
-        self._files = files
-        try:
-            self.run_batch(buffers, labels)
-        finally:
-            self._files = None
+        """run_batch from the encoded bytes of `files`, decoded on the copy stream straight into the slot
+        (jpeg.JpegDecoder; PIL, through imagenet_c.decode_image, for the images the device does not decode)."""
+        from . import imagenet_c, jpeg
+
+        def place(h, slot):
+            du8 = self.slots[slot][0]
+            S = du8.shape[1]
+            for i, d in enumerate(jpeg.parse(buffers)):   # a wrong size raises decode_image's error, as PIL's does
+                if d["supported"] and (int(d["height"]), int(d["width"])) != (S, S):
+                    imagenet_c.decode_image(files[i], S)
+            self.decoder(slot).stage(buffers, None, self.copy_stream,
+                                     fallback=lambda i: imagenet_c.decode_image(files[i], S),
+                                     out=du8.view(-1), out_offsets=np.arange(len(buffers), dtype=np.int64) * S * S * 3)
+        self._run(place, labels)
+
+    def _fill(self, h, slot, place, labels):
+        place(h, slot)
+        hlab, dlab = self.host[h][1], self.slots[slot][1]
+        hlab[:len(labels)].copy_(torch.as_tensor(labels, dtype=torch.int32))
+        dlab.copy_(hlab, non_blocking=True)
 
     def _body(self, slot, n_valid):
         from .metrics import softmax_top1_count
@@ -837,52 +794,43 @@ class _ResizedEvalPipeline(_EvalPipeline):
     `_body` starts with rt.set_images_resized (resize + crop + mean)."""
 
     def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_dtype=torch.int32):
-        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
-        lab = dict(dtype=label_dtype)
-        self.size = size
+        dev, lab = torch.device(model.device), dict(dtype=label_dtype)
         # pinned image bytes (grown on demand), labels, descriptors
-        self.host = [[torch.empty(0, dtype=torch.uint8), torch.zeros(batch, **lab).pin_memory(),
-                      torch.zeros(32 * batch, dtype=torch.uint8).pin_memory()] for _ in range(self.RING)]
+        host = [[None, torch.zeros(batch, **lab).pin_memory(), torch.zeros(32 * batch, dtype=torch.uint8).pin_memory()]
+                for _ in range(self.RING)]
         # device image bytes (allocated on the copy stream, grown on demand), labels, descriptors: a graph
         # holds the descriptor table's address only, so the image bytes may move
-        self.slots = [[None, torch.zeros(batch, **lab, device=self.dev),
-                       torch.zeros(32 * batch, dtype=torch.uint8, device=self.dev)] for _ in range(2)]
-        self.decoders, self._geometry = [None, None], None
+        slots = [[None, torch.zeros(batch, **lab, device=dev), torch.zeros(32 * batch, dtype=torch.uint8, device=dev)]
+                 for _ in range(2)]
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph, host, slots)
+        self.size = size
 
-    def _stage(self, h, slot, images, labels):
-        """`images` a list of (uint8 [H, W, 3] array, eval_geometry) pairs, `labels` ints; or, from
-        run_batch_encoded, encoded images, decoded on the copy stream."""
-        from .imagenet_eval import DESC_DTYPE, check_descriptors
-        n = len(images)
-        hbuf, hlab, hdesc = self.host[h]
-        desc = hdesc.numpy().view(DESC_DTYPE)
-        if self._geometry is None:
-            self.host[h][0], self.slots[slot][0], addrs = _pack_u8(hbuf, self.slots[slot][0],
-                                                                  [a for a, _ in images], self.dev)
-            for i, (a, (s, rh, rw, cy, cx)) in enumerate(images):
-                desc[i] = (addrs[i], a.shape[0], a.shape[1], rh, rw, cy, cx)
-        else:
-            from . import jpeg
-            if self.decoders[slot] is None:
-                self.decoders[slot] = jpeg.JpegDecoder(self.dev)
-            placed = self.decoders[slot].stage(images, None, torch.cuda.current_stream(self.dev))
-            for i, (addr, ih, iw) in enumerate(placed):
-                s, rh, rw, cy, cx = self._geometry(ih, iw)
-                desc[i] = (addr, ih, iw, rh, rw, cy, cx)
-        check_descriptors(desc, n, self.size)
-        hlab[:n].copy_(torch.as_tensor(labels, dtype=hlab.dtype))
-        _, dlab, ddesc = self.slots[slot]
-        ddesc.copy_(hdesc, non_blocking=True)
-        dlab.copy_(hlab, non_blocking=True)
+    def run_batch(self, images, labels):
+        """Evaluate (uint8 [H, W, 3] array, imagenet_eval.eval_geometry) pairs `images` with int `labels`."""
+        def place(h, slot):
+            self.host[h][0], self.slots[slot][0], addrs = pack_u8(self.host[h][0], self.slots[slot][0],
+                                                                 [a for a, _ in images], self.dev)
+            return [((addr, a.shape[0], a.shape[1]), g) for addr, (a, g) in zip(addrs, images)]
+        self._run(place, labels)
 
     def run_batch_encoded(self, buffers, labels, geometry):
         """run_batch from encoded images (jpeg.JpegDecoder on the copy stream; PIL for the images the device
         does not decode); geometry(h, w) gives an image's imagenet_eval.eval_geometry."""
-        self._geometry = geometry
-        try:
-            self.run_batch(buffers, labels)
-        finally:
-            self._geometry = None
+        def place(h, slot):
+            return [(p, geometry(p[1], p[2])) for p in self.decoder(slot).stage(buffers, None, self.copy_stream)]
+        self._run(place, labels)
+
+    def _fill(self, h, slot, place, labels):
+        from .imagenet_eval import DESC_DTYPE, check_descriptors
+        _, hlab, hdesc = self.host[h]
+        desc = hdesc.numpy().view(DESC_DTYPE)
+        for i, ((addr, ih, iw), (s, rh, rw, cy, cx)) in enumerate(place(h, slot)):
+            desc[i] = (addr, ih, iw, rh, rw, cy, cx)
+        check_descriptors(desc, len(labels), self.size)
+        hlab[:len(labels)].copy_(torch.as_tensor(labels, dtype=hlab.dtype))
+        _, dlab, ddesc = self.slots[slot]
+        ddesc.copy_(hdesc, non_blocking=True)
+        dlab.copy_(hlab, non_blocking=True)
 
 
 class _ClassifyEvalDevice(_ResizedEvalPipeline):
@@ -905,9 +853,9 @@ class _ClassifyEvalDevice(_ResizedEvalPipeline):
         self.rt.run_forward()
         classify_rows(self.logits, labels, n_valid, 5, self.label_smoothing, out=self.out)
 
-    def run_batch(self, images, labels):
-        super().run_batch(images, labels)
-        n = len(images)
+    def _run(self, place, labels):
+        super()._run(place, labels)
+        n = len(labels)
         for dst, src in zip(self.rows, self.out):
             dst[self.done:self.done + n].copy_(src[:n])
         self.done += n
@@ -939,9 +887,9 @@ class _RetrievalEvalDevice(_ResizedEvalPipeline):
         # the slot is refilled two batches later: its labels are read here, before the batch's event
         self.batch_labels.copy_(labels)
 
-    def run_batch(self, images, labels):
-        super().run_batch(images, labels)
-        n = len(images)
+    def _run(self, place, labels):
+        super()._run(place, labels)
+        n = len(labels)
         self.index[self.done:self.done + n].copy_(self.feat[:n])
         self.labels[self.done:self.done + n].copy_(self.batch_labels[:n])
         self.done += n
@@ -994,15 +942,10 @@ def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=
             ev = _CorruptionEvalDevice(replicas[i], batch_size, image_size, use_resnet_d, use_cuda_graph)
             batches = [(d, work[d][0][a:a + batch_size], work[d][1][a:a + batch_size])
                        for d in quota[i] for a in range(0, len(work[d][0]), batch_size)]
-            decode = lambda files: [pool.submit(_read_file, f) for f in files]
-            ahead = 4                                   # batches decoding ahead of the GPU
-            pending = [decode(b[1]) for b in batches[:ahead]]
             counts = {}
-            for j, (d, files, labels) in enumerate(batches):
-                futs = pending.pop(0)
-                if j + ahead < len(batches):
-                    pending.append(decode(batches[j + ahead][1]))
-                ev.run_batch_encoded([f.result() for f in futs], labels, files)
+            read = read_ahead(pool, [files for _, files, _ in batches], _read_file)
+            for j, ((d, files, labels), (_, buffers)) in enumerate(zip(batches, read)):
+                ev.run_batch_encoded(buffers, labels, files)
                 if j + 1 == len(batches) or batches[j + 1][0] != d:
                     counts[d] = ev.take_count()
             torch.cuda.current_stream(ev.dev).synchronize()
@@ -1097,16 +1040,10 @@ def _feed_records(ev, records, batch_size, preprocessing_type, image_size, num_w
     from . import imagenet_eval
     batches = [records[a:a + batch_size] for a in range(0, len(records), batch_size)]
     pool = ThreadPoolExecutor(max_workers=num_workers or min(32, os.cpu_count() or 1))
-    decode = lambda recs: [pool.submit(imagenet_eval.read_encoded, r[0], r[1], r[2]) for r in recs]
     geometry = lambda h, w: imagenet_eval.eval_geometry(h, w, preprocessing_type, image_size)
     try:
-        ahead = 4                                   # batches decoding ahead of the GPU
-        pending = [decode(b) for b in batches[:ahead]]
-        for j, recs in enumerate(batches):
-            futs = pending.pop(0)
-            if j + ahead < len(batches):
-                pending.append(decode(batches[j + ahead]))
-            ev.run_batch_encoded([f.result() for f in futs], [r[3] for r in recs], geometry)
+        for recs, buffers in read_ahead(pool, batches, lambda r: imagenet_eval.read_encoded(*r[:3])):
+            ev.run_batch_encoded(buffers, [r[3] for r in recs], geometry)
         torch.cuda.current_stream(ev.dev).synchronize()
     finally:
         pool.shutdown(wait=True, cancel_futures=True)
@@ -1166,39 +1103,29 @@ def evaluate_retrieval(model, data_dir, *, val_regex="validation-*", preprocessi
     return out
 
 
-class _TrainFeed:
+class _TrainFeed(StagingRing):
     """The training input's staging ring: per step, the crop windows packed into a growable pinned uint8
     buffer with one acnn_crop_desc each, the labels and (KD) the teacher logits, copied to one of two
-    device slots on a copy stream while the previous step computes; `step` makes the images on the device
+    device slots on the copy stream while the previous step computes; `step` makes the images on the device
     (Trainer.train_step_cropped) and runs the training step."""
 
-    RING = 3        # pinned host batches
-
     def __init__(self, trainer, kd):
-        from .imagenet_c import CHANNEL_MEANS
-        self.tr, self.dev = trainer, trainer.rt.dev
+        self.tr, dev = trainer, trainer.rt.dev
         n, nc = trainer.input_batch, trainer.model.num_classes
         i32, f32 = dict(dtype=torch.int32), dict(dtype=torch.float32)
-        self.host = [[None, torch.zeros(n, **i32).pin_memory(), torch.zeros(32 * n, dtype=torch.uint8).pin_memory(),
-                      torch.zeros(n, nc, **f32).pin_memory() if kd else None] for _ in range(self.RING)]
+        host = [[None, torch.zeros(n, **i32).pin_memory(), torch.zeros(32 * n, dtype=torch.uint8).pin_memory(),
+                 torch.zeros(n, nc, **f32).pin_memory() if kd else None] for _ in range(self.RING)]
         # a step's graph holds no address of these: the image bytes may move when the buffer grows
-        self.slots = [[None, torch.zeros(n, **i32, device=self.dev),
-                       torch.zeros(32 * n, dtype=torch.uint8, device=self.dev),
-                       torch.zeros(n, nc, **f32, device=self.dev) if kd else None] for _ in range(2)]
-        self.mean = torch.tensor(CHANNEL_MEANS, dtype=torch.float32, device=self.dev)
-        self.copy_stream = torch.cuda.Stream(self.dev)
-        self.host_free = [None] * self.RING
-        self.slot_free = [None, None]
-        self.copied = [None, None]
-        self.decoders = [None, None]
-        self.staged = self.consumed = 0
+        slots = [[None, torch.zeros(n, **i32, device=dev), torch.zeros(32 * n, dtype=torch.uint8, device=dev),
+                  torch.zeros(n, nc, **f32, device=dev) if kd else None] for _ in range(2)]
+        super().__init__(dev, host, slots)
 
     def stage(self, windows, labels, teacher_logits=None):
         """`windows` input_batch (uint8 [h, w, 3] array, flip) pairs, `labels` ints, `teacher_logits` float32
         [input_batch, num_classes] with KD."""
         def place(h, slot):
-            self.host[h][0], self.slots[slot][0], addrs = _pack_u8(self.host[h][0], self.slots[slot][0],
-                                                                  [a for a, _ in windows], self.dev)
+            self.host[h][0], self.slots[slot][0], addrs = pack_u8(self.host[h][0], self.slots[slot][0],
+                                                                 [a for a, _ in windows], self.dev)
             return [(ad, a.shape[0], a.shape[1], flip) for ad, (a, flip) in zip(addrs, windows)]
         self._stage(place, labels, teacher_logits)
 
@@ -1207,24 +1134,15 @@ class _TrainFeed:
         decoded on the copy stream (jpeg.JpegDecoder, one per slot; PIL's decode_rgb for the images the
         device does not decode)."""
         def place(h, slot):
-            from . import jpeg
-            if self.decoders[slot] is None:
-                self.decoders[slot] = jpeg.JpegDecoder(self.dev)
-            got = self.decoders[slot].stage([b for b, _, _ in items], np.array([w for _, w, _ in items], np.int32),
-                                            self.copy_stream)
+            got = self.decoder(slot).stage([b for b, _, _ in items], np.array([w for _, w, _ in items], np.int32),
+                                           self.copy_stream)
             return [(ad, hh, ww, flip) for (ad, hh, ww), (_, _, flip) in zip(got, items)]
         self._stage(place, labels, teacher_logits)
 
     def _stage(self, place, labels, teacher_logits):
         from .imagenet_train import CROP_DESC_DTYPE, check_crop_descriptors
-        h, slot = self.staged % self.RING, self.staged % 2
-        self.staged += 1
-        if self.host_free[h] is not None:
-            self.host_free[h].synchronize()          # its previous host -> device copy has run
-        cs = self.copy_stream
-        if self.slot_free[slot] is not None:
-            cs.wait_event(self.slot_free[slot])       # the step before the previous one has read it
-        with torch.cuda.stream(cs):
+
+        def fill(h, slot):
             placed = place(h, slot)
             _, hlab, hdesc, hteach = self.host[h]
             desc = hdesc.numpy().view(CROP_DESC_DTYPE)
@@ -1238,21 +1156,14 @@ class _TrainFeed:
             if dteach is not None:
                 hteach.copy_(torch.as_tensor(teacher_logits, dtype=torch.float32))
                 dteach.copy_(hteach, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(cs)
-        self.host_free[h] = self.copied[slot] = ev
+        self.push(fill)
 
     def step(self, lam1=None, lam2=None):
         """The training step of the oldest staged batch; returns Trainer.train_step's loss tensor."""
-        slot = self.consumed % 2
-        self.consumed += 1
-        main = torch.cuda.current_stream(self.dev)
-        main.wait_event(self.copied[slot])
+        slot = self.take()
         _, dlab, ddesc, dteach = self.slots[slot]
         loss = self.tr.train_step_cropped(ddesc, dlab, self.mean, lam1=lam1, lam2=lam2, teacher_logits=dteach)
-        ev = torch.cuda.Event()
-        ev.record(main)
-        self.slot_free[slot] = ev
+        self.release(slot)
         return loss
 
 
@@ -1368,21 +1279,18 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                                         shuffle_buffer, trainer.input_batch, world, rank)
                 steps = stream.steps if max_train_steps is None else min(stream.steps, max_train_steps)
 
-                def decode(t, c=c, stream=stream):
-                    return [(pool.submit(it.encoded_window, *records[r][:3], seed, c, pos,
-                                         p["training_random_crop"]), r) for pos, r in stream.records(t)]
-                ahead = 4                               # steps decoding ahead of the GPU
-                pending = [decode(t) for t in range(min(ahead, steps))]
+                def window(pos_r, c=c):
+                    pos, r = pos_r
+                    return it.encoded_window(*records[r][:3], seed, c, pos, p["training_random_crop"])
+                read = read_ahead(pool, map(stream.records, range(steps)), window)
 
-                def stage(t):
-                    futs = pending.pop(0)
-                    if t + ahead < steps:
-                        pending.append(decode(t + ahead))
-                    teacher = np.stack([records[r][4] for _, r in futs]) if kd else None
-                    feed.stage_encoded([f.result() for f, _ in futs], [records[r][3] for _, r in futs], teacher)
+                def stage():
+                    recs, items = next(read)
+                    teacher = np.stack([records[r][4] for _, r in recs]) if kd else None
+                    feed.stage_encoded(items, [records[r][3] for _, r in recs], teacher)
 
                 if steps:
-                    stage(0)
+                    stage()
                 for t in range(steps):
                     lam1 = lam2 = None
                     if trainer.mixup_type:
@@ -1390,7 +1298,7 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                         lam1, lam2 = lam[0], (lam[1] if trainer.mixup_type == 2 else None)
                     feed.step(lam1, lam2)
                     if t + 1 < steps:
-                        stage(t + 1)
+                        stage()
                         if save_steps > 0 and trainer.global_step % save_steps == 0:
                             save()
                 save()

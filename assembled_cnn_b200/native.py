@@ -393,8 +393,8 @@ class NativeRuntime(_runtime_base()):
         """acnn_set_images_resized: the "images" buffer from decoded uint8 images of any sizes (resize,
         central crop, - mean[c]); desc a CUDA uint8 tensor of input_batch 32-byte acnn_resize_desc on
         this device, validated by the caller; mean a float32 tensor of 3 (host or device)."""
-        from .runtime import _check_resize_args
-        _check_resize_args(desc, self.t[self.plan.meta["images"]], n_valid, mean)
+        from .runtime import _check_desc_args
+        _check_desc_args("set_images_resized", desc, self.t[self.plan.meta["images"]], mean, n_valid)
         _lib.check(self.lib.acnn_set_images_resized(self.model.handle, desc.data_ptr(), int(n_valid),
                                                     mean.data_ptr(), self.stream), "acnn_set_images_resized")
 
@@ -402,8 +402,8 @@ class NativeRuntime(_runtime_base()):
         """acnn_set_images_cropped: every row of the "images" buffer from training crop windows (flip,
         resize to S x S, - mean[c]); desc a CUDA uint8 tensor of input_batch 32-byte acnn_crop_desc on this
         device, validated by the caller; mean a float32 tensor of 3 (host or device)."""
-        from .runtime import _check_crop_args
-        _check_crop_args(desc, self.t[self.plan.meta["images"]], mean)
+        from .runtime import _check_desc_args
+        _check_desc_args("set_images_cropped", desc, self.t[self.plan.meta["images"]], mean)
         _lib.check(self.lib.acnn_set_images_cropped(self.model.handle, desc.data_ptr(), mean.data_ptr(),
                                                     self.stream), "acnn_set_images_cropped")
 

@@ -27,33 +27,18 @@ def _check_u8_images(images_u8, images, mean):
         raise ValueError("mean must be a contiguous float32 tensor of 3 values")
 
 
-def _check_resize_args(desc, images, n_valid, mean):
-    """Arguments of set_images_resized: a square input buffer, B descriptors of 32 bytes on its device,
-    n_valid in [0, B], float32 mean[3].  Returns (B, S)."""
+def _check_desc_args(method, desc, images, mean, n_valid=None):
+    """Arguments of set_images_resized / set_images_cropped (`method`): a square input buffer, B descriptors
+    of 32 bytes on its device, n_valid (when given) in [0, B], float32 mean[3].  Returns (B, S)."""
     b, h, w, _ = images.shape
     if h != w:
-        raise ValueError("set_images_resized needs a square input buffer, got %dx%d" % (h, w))
+        raise ValueError("%s needs a square input buffer, got %dx%d" % (method, h, w))
     if desc.dtype != torch.uint8 or desc.numel() != 32 * b or desc.device != images.device \
             or not desc.is_contiguous():
         raise ValueError("desc must be a contiguous uint8 tensor of %d descriptors (%d bytes) on %s"
                          % (b, 32 * b, images.device))
-    if not 0 <= int(n_valid) <= b:
+    if n_valid is not None and not 0 <= int(n_valid) <= b:
         raise ValueError("n_valid=%d outside [0, %d]" % (int(n_valid), b))
-    if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
-        raise ValueError("mean must be a contiguous float32 tensor of 3 values")
-    return b, h
-
-
-def _check_crop_args(desc, images, mean):
-    """Arguments of set_images_cropped: a square input buffer, B descriptors of 32 bytes on its device,
-    float32 mean[3].  Returns (B, S)."""
-    b, h, w, _ = images.shape
-    if h != w:
-        raise ValueError("set_images_cropped needs a square input buffer, got %dx%d" % (h, w))
-    if desc.dtype != torch.uint8 or desc.numel() != 32 * b or desc.device != images.device \
-            or not desc.is_contiguous():
-        raise ValueError("desc must be a contiguous uint8 tensor of %d descriptors (%d bytes) on %s"
-                         % (b, 32 * b, images.device))
     if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
         raise ValueError("mean must be a contiguous float32 tensor of 3 values")
     return b, h
@@ -63,7 +48,7 @@ def _check_augment_args(desc, aug, work, images, mean):
     """Arguments of set_images_augmented: those of set_images_cropped, B descriptors of 88 bytes and a work
     buffer of acnn_autoaugment_work_bytes(B, S) bytes, both uint8 on the input buffer's device.
     Returns (B, S)."""
-    b, s = _check_crop_args(desc, images, mean)
+    b, s = _check_desc_args("set_images_cropped", desc, images, mean)
     if aug.dtype != torch.uint8 or aug.numel() != 88 * b or aug.device != images.device or not aug.is_contiguous():
         raise ValueError("aug must be a contiguous uint8 tensor of %d AutoAugment descriptors (%d bytes) on %s"
                          % (b, 88 * b, images.device))
@@ -315,7 +300,7 @@ class Runtime:
         (imagenet_eval.DESC_DTYPE) on this device, validated by the caller; rows >= n_valid are not
         written; mean a float32 tensor of 3 (host or device)."""
         images = self.t[self.plan.meta["images"]]
-        b, s = _check_resize_args(desc, images, n_valid, mean)
+        b, s = _check_desc_args("set_images_resized", desc, images, mean, n_valid)
         _lib.check(self.lib.acnn_resize_crop_u8(desc.data_ptr(), b, int(n_valid), s, mean.data_ptr(),
                                                 images.data_ptr(), self.stream), "acnn_resize_crop_u8")
 
@@ -325,7 +310,7 @@ class Runtime:
         (imagenet_train.CROP_DESC_DTYPE) on this device, validated by the caller; mean a float32 tensor
         of 3 (host or device)."""
         images = self.t[self.plan.meta["images"]]
-        b, s = _check_crop_args(desc, images, mean)
+        b, s = _check_desc_args("set_images_cropped", desc, images, mean)
         _lib.check(self.lib.acnn_crop_resize_u8(desc.data_ptr(), b, b, s, mean.data_ptr(), images.data_ptr(),
                                                 self.stream), "acnn_crop_resize_u8")
 

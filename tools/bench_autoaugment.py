@@ -26,7 +26,8 @@ from assembled_cnn_b200 import _lib  # noqa: E402
 from assembled_cnn_b200 import autoaugment as A  # noqa: E402
 from assembled_cnn_b200 import imagenet_train as it  # noqa: E402
 from assembled_cnn_b200.hparams import params_from_flags  # noqa: E402
-from assembled_cnn_b200.model_fns import Trainer, _pack_u8, build_model  # noqa: E402
+from assembled_cnn_b200.model_fns import Trainer, build_model  # noqa: E402
+from assembled_cnn_b200.staging import pack_u8  # noqa: E402
 from bench_train_input import FLAGS, card, event_ms, windows  # noqa: E402
 
 SIZE, BATCH = 224, 256
@@ -34,7 +35,7 @@ SIZE, BATCH = 224, 256
 
 def device_inputs(B, policy, seed):
     wins = windows(B, seed)
-    hbuf, dbuf, addrs = _pack_u8(None, None, [w for w, _ in wins], torch.device("cuda"))
+    hbuf, dbuf, addrs = pack_u8(None, None, [w for w, _ in wins], torch.device("cuda"))
     desc = np.zeros(B, it.CROP_DESC_DTYPE)
     for i, (w, f) in enumerate(wins):
         desc[i] = (addrs[i], w.shape[0], w.shape[1], int(f), (0, 0, 0))

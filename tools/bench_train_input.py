@@ -69,9 +69,9 @@ def windows(n, seed):
 
 
 def bench_crop(B, a):
-    from assembled_cnn_b200.model_fns import _pack_u8
+    from assembled_cnn_b200.staging import pack_u8
     wins = windows(B, B)
-    hbuf, dbuf, addrs = _pack_u8(None, None, [w for w, _ in wins], torch.device("cuda"))   # dbuf: the pixels
+    hbuf, dbuf, addrs = pack_u8(None, None, [w for w, _ in wins], torch.device("cuda"))   # dbuf: the pixels
     desc = np.zeros(B, it.CROP_DESC_DTYPE)
     for i, (w, f) in enumerate(wins):
         desc[i] = (addrs[i], w.shape[0], w.shape[1], int(f), (0, 0, 0))
