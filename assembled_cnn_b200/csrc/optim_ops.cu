@@ -135,7 +135,11 @@ __global__ void s2d_wgrad_unpack_kernel(const float* __restrict__ dw2, float* __
   dw[i] = dw2[(((int64_t)co * k2 + r2) * k2 + s2) * 16 + (a * 2 + b) * 4 + c];
 }
 
-// l2_part: [gridDim.x + 1] floats of scratch; the last slot is the arrival counter (self-resetting)
+// l2_part: acnn_sgd_scratch_floats() floats of scratch: one partial per CTA, and the arrival counter
+// (self-resetting) in the LAST slot, whatever the grid: at slot gridDim.x a call with a smaller grid
+// than the previous one would read that call's partial sum as its counter and never finish the sum
+constexpr int kSgdMaxBlocks = kMaxSms * 8;
+
 __global__ void __launch_bounds__(256)
 sgd_momentum_kernel(float* __restrict__ w, const float* __restrict__ grad, float* __restrict__ acc,
                     int64_t n, const uint8_t* __restrict__ decay_flag, const float* __restrict__ hp,
@@ -177,7 +181,7 @@ sgd_momentum_kernel(float* __restrict__ w, const float* __restrict__ grad, float
     // the arrival order does not enter the sum
     __shared__ bool is_last;
     __shared__ float tsum[256];
-    unsigned int* counter = reinterpret_cast<unsigned int*>(l2_part + gridDim.x);
+    unsigned int* counter = reinterpret_cast<unsigned int*>(l2_part + kSgdMaxBlocks);
     if (threadIdx.x == 0) {
       float s = 0.f;
       for (int k = 0; k < 8; ++k) s += sh[k];
@@ -253,14 +257,14 @@ int acnn_s2d_wgrad_unpack(const float* dw2, float* dw, int Cout, int k, int pad,
   return check_launch("s2d_wgrad_unpack");
 }
 
-int acnn_sgd_scratch_floats(void) { return acnn::kMaxSms * 8 + 1; }
+int acnn_sgd_scratch_floats(void) { return acnn::kSgdMaxBlocks + 1; }
 
 int acnn_sgd_momentum(float* w, const float* grad, float* acc, int64_t n,
                       const uint8_t* decay_flag, const float* hp, float* l2_acc, float* scratch,
                       void* stream) {
   ACNN_REQUIRE(w && grad && acc && decay_flag && hp && n % 256 == 0 && (!l2_acc || scratch),
                "sgd_momentum: bad arguments (n must be a multiple of 256; l2_acc needs scratch)");
-  launch_k(sgd_momentum_kernel, dim3(grid_for(n / 4, 256, acnn::kMaxSms * 8)), dim3(256), 0,
+  launch_k(sgd_momentum_kernel, dim3(grid_for(n / 4, 256, acnn::kSgdMaxBlocks)), dim3(256), 0,
            (cudaStream_t)stream, w, grad, acc, n, decay_flag, hp, l2_acc, scratch);
   count_launch();
   return check_launch("sgd_momentum");
