@@ -47,10 +47,11 @@ def _parse_header(path: str = HEADER_PATH) -> dict:
     text = open(path).read()
     text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
     protos = {}
-    for m in re.finditer(r"(?:^|\n)\s*(const\s+char\s*\*|int64_t|int)\s+(acnn_\w+)\s*\(([^;{]*?)\)\s*;",
+    rets = {"int64_t": c_int64, "uint32_t": C.c_uint32, "int": c_int}
+    for m in re.finditer(r"(?:^|\n)\s*(const\s+char\s*\*|int64_t|uint32_t|int)\s+(acnn_\w+)\s*\(([^;{]*?)\)\s*;",
                          text):
         ret, name, args = m.group(1), m.group(2), m.group(3).strip()
-        res = C.c_char_p if "char" in ret else (c_int64 if ret == "int64_t" else c_int)
+        res = C.c_char_p if "char" in ret else rets[ret]
         argtypes = []
         if args and args != "void":
             for a in args.split(","):
@@ -63,6 +64,10 @@ def _parse_header(path: str = HEADER_PATH) -> dict:
                     argtypes.append(c_int64)
                 elif a.startswith("uint64_t"):
                     argtypes.append(C.c_uint64)
+                elif a.startswith("uint32_t"):
+                    argtypes.append(C.c_uint32)
+                elif a.startswith("size_t"):
+                    argtypes.append(C.c_size_t)
                 elif a.startswith("float"):
                     argtypes.append(c_float)
                 elif a.startswith("int"):

@@ -10,6 +10,11 @@ the same shards with missing_label=-1.
                         preprocessing/imagenet_preprocessing.py:100-119,158-226,295-313
                                                         _smallest_size_at_least, central_crop
 Decoding is imagenet_c.decode_rgb (PIL); the channel means are imagenet_c.CHANNEL_MEANS.
+
+The TFRecord writer of the knowledge-distillation shards (model_fns.extract_teacher_logits, the reference's
+datasets/build_imagenet_data.py --logits_file_path) is here too, so the record format lives in one module:
+write_record frames a record, add_float_feature adds a float feature to a serialised Example and
+FloatFeatureWriter copies whole files with one added to every record.
 """
 from __future__ import annotations
 
@@ -20,6 +25,7 @@ import struct
 
 import numpy as np
 
+from . import native
 from .imagenet_c import CHANNEL_MEANS, decode_rgb  # noqa: F401  (re-exported for the evaluation)
 
 # include/acnn.h acnn_resize_desc
@@ -27,27 +33,23 @@ DESC_DTYPE = np.dtype([("src", "<u8"), ("src_h", "<i4"), ("src_w", "<i4"), ("rsz
                        ("crop_y", "<i4"), ("crop_x", "<i4")])
 assert DESC_DTYPE.itemsize == 32
 
+# the knowledge-distillation teacher logits of a record (utils/data_util.py parse_record_sup)
+LOGIT_KEY = b"image/logit"
+
 # ------------------------------------------------------------------------------------------ CRC32C
-_CRC_TABLE = []
-for _n in range(256):
-    _c = _n
-    for _ in range(8):
-        _c = (_c >> 1) ^ 0x82F63B78 if _c & 1 else _c >> 1
-    _CRC_TABLE.append(_c)
+def crc32c(data, crc=0):
+    """CRC-32C (Castagnoli, reflected polynomial 0x82F63B78) of `data`, continued from `crc` (0 starts a
+    new one): libacnn's host acnn_crc32c."""
+    return native.crc32c(data, crc)
 
 
-def crc32c(data):
-    """CRC-32C (Castagnoli, reflected polynomial 0x82F63B78) of `data`."""
-    c = 0xFFFFFFFF
-    for b in data:
-        c = _CRC_TABLE[(c ^ b) & 0xFF] ^ (c >> 8)
-    return c ^ 0xFFFFFFFF
+def _mask(c):
+    return (((c >> 15) | (c << 17)) + 0xA282EAD8) & 0xFFFFFFFF
 
 
 def masked_crc32c(data):
     """The TFRecord checksum: the CRC rotated right by 15 bits plus 0xa282ead8."""
-    c = crc32c(data)
-    return (((c >> 15) | (c << 17)) + 0xA282EAD8) & 0xFFFFFFFF
+    return _mask(crc32c(data))
 
 
 # ---------------------------------------------------------------------------------------- TFRecord
@@ -166,12 +168,30 @@ def read_records(path, logits=False, missing_label=None):
     encoded image in the file (logits=True: [(label, offset, length, float32 image/logit values)];
     missing_label: the label of a record without one, as parse_example).  A
     record is u64 length, u32 masked CRC32C of the length, the data, u32 masked CRC32C of the data.  The
-    length's CRC is verified; the data's is not (a pure-Python CRC over the 6.4 GB of ImageNet validation
-    JPEGs would take far longer than the evaluation).  A truncated or corrupt record raises ValueError
-    naming the file and the record's byte offset."""
+    length's CRC is verified; the data's is not (FloatFeatureWriter verifies it when it copies a record).
+    A truncated or corrupt record raises ValueError naming the file and the record's byte offset."""
+    data = _read_file(path)
+    out = []
+    for pos, start, length in record_frames(data, path):
+        try:
+            ex = parse_example(memoryview(data)[start:start + length], logits, missing_label)
+        except ValueError as e:
+            raise ValueError("%s: bad tf.train.Example in the record at byte offset %d: %s" % (path, pos, e))
+        label, (a, b) = ex[:2]
+        out.append((label, start + a, b - a) + tuple(ex[2:]))
+    return out
+
+
+def _read_file(path):
     with open(path, "rb") as f:
-        data = f.read()
-    out, pos, n = [], 0, len(data)
+        return f.read()
+
+
+def record_frames(data, path):
+    """(byte offset, data start, data length) of every record of the TFRecord file contents `data`, in
+    order.  The length's CRC is verified: a truncated record or a corrupt length raises ValueError naming
+    `path` and the record's byte offset.  The data's CRC sits at data[start + length:][:4]."""
+    pos, n = 0, len(data)
     while pos < n:
         if pos + 12 > n:
             raise ValueError("%s: truncated record header at byte offset %d" % (path, pos))
@@ -183,14 +203,151 @@ def read_records(path, logits=False, missing_label=None):
         start = pos + 12
         if start + length + 4 > n:
             raise ValueError("%s: truncated record at byte offset %d" % (path, pos))
-        try:
-            ex = parse_example(memoryview(data)[start:start + length], logits, missing_label)
-        except ValueError as e:
-            raise ValueError("%s: bad tf.train.Example in the record at byte offset %d: %s" % (path, pos, e))
-        label, (a, b) = ex[:2]
-        out.append((label, start + a, b - a) + tuple(ex[2:]))
+        yield pos, start, length
         pos = start + length + 4
+
+
+# ------------------------------------------------------------------------------- TFRecord writer
+def write_record(f, pieces):
+    """Writes one TFRecord record to the binary file `f`: u64 length, masked CRC32C of the length, the data
+    (the bytes-like `pieces` back to back, not joined in memory), masked CRC32C of the data."""
+    head = struct.pack("<Q", sum(len(p) for p in pieces))
+    c = 0
+    for p in pieces:
+        c = crc32c(p, c)
+    f.write(head + struct.pack("<I", masked_crc32c(head)))
+    for p in pieces:
+        f.write(p)
+    f.write(struct.pack("<I", _mask(c)))
+
+
+def _encode_varint(v):
+    out = bytearray()
+    while v > 0x7F:
+        out.append((v & 0x7F) | 0x80)
+        v >>= 7
+    out.append(v)
+    return bytes(out)
+
+
+def _len_field(field, payload_len):
+    """The key and length of a length-delimited field (wire type 2) of payload_len bytes."""
+    return _encode_varint(field << 3 | 2) + _encode_varint(payload_len)
+
+
+def features_span(example, key):
+    """(start, end) of the Features message inside the serialised tf.train.Example `example`.  ValueError
+    unless the Example is exactly one `features` field, or when one of its map entries has `key`."""
+    fields = list(_fields(example, 0, len(example)))
+    if len(fields) != 1 or fields[0][:2] != (1, 2):
+        raise ValueError("the Example is not one features message")
+    span = fields[0][2]
+    for f, wt, entry in _fields(example, *span):
+        if f == 1 and wt == 2:
+            for f2, wt2, kv in _fields(example, *entry):
+                if f2 == 1 and wt2 == 2 and bytes(example[kv[0]:kv[1]]) == key:
+                    raise ValueError("the Example already holds %s" % key.decode())
+    return span
+
+
+def add_float_feature(example, key, values):
+    """The serialised tf.train.Example `example` with one more Features map entry, {key: Feature{float_list
+    {value: float32 `values`, packed}}}, as pieces for write_record: (the Example's key and new length, its
+    Features message as it is, the new entry).  The input's features keep their bytes and order, so a
+    protobuf parser reads the input's features plus the new one.  ValueError as features_span."""
+    a, b = features_span(example, key)
+    vals = np.ascontiguousarray(values, dtype="<f4").tobytes()
+    flist = _len_field(1, len(vals)) + vals                          # FloatList.value (packed)
+    feature = _len_field(2, len(flist)) + flist                      # Feature.float_list
+    entry = _len_field(1, len(key)) + key + _len_field(2, len(feature)) + feature
+    entry = _len_field(1, len(entry)) + entry                        # Features.feature map entry
+    return _len_field(1, (b - a) + len(entry)), example[a:b], entry  # Example.features
+
+
+def appendable_records(path, key):
+    """[(offset, length)] of the encoded image of every record of the TFRecord file `path`, each record
+    checked as add_float_feature's input (one features message without `key`) and as parse_example's (an
+    image/encoded; a missing label is allowed).  ValueError naming the file and the record's byte offset."""
+    data = _read_file(path)
+    out = []
+    for pos, start, length in record_frames(data, path):
+        ex = memoryview(data)[start:start + length]
+        try:
+            features_span(ex, key)
+            _, (a, b) = parse_example(ex, missing_label=-1)
+        except ValueError as e:
+            raise ValueError("%s: the record at byte offset %d: %s" % (path, pos, e))
+        out.append((start + a, b - a))
     return out
+
+
+class FloatFeatureWriter:
+    """Writes a copy of each TFRecord file of `jobs` [(input path, output path)] with one float feature
+    `key` added to every record (add_float_feature), fed the values record by record across the files in
+    order (`add`).  While a file is copied, the data CRC of each of its input records is verified (a
+    mismatch raises ValueError naming the file and the record's byte offset), so a fresh checksum never
+    covers corrupt bytes.  Each output is written under a hidden temporary name in its directory and
+    renamed once complete; `abort` removes the one being written.  One input file is held in memory."""
+
+    def __init__(self, jobs, key):
+        self.jobs, self.key = list(jobs), key
+        self.j, self.f = -1, None
+
+    def add(self, rows):
+        """Appends one record per row of the float32 [n, k] `rows` (copied before the call returns)."""
+        for row in np.asarray(rows, dtype=np.float32):
+            while self.f is None or self.i == len(self.frames):
+                self._next_file()
+            pos, start, length = self.frames[self.i]
+            src = self.jobs[self.j][0]
+            data = memoryview(self.data)[start:start + length]
+            (crc,) = struct.unpack("<I", self.data[start + length:start + length + 4])
+            if masked_crc32c(data) != crc:
+                raise ValueError("%s: corrupt record data at byte offset %d" % (src, pos))
+            try:
+                pieces = add_float_feature(data, self.key, row)
+            except ValueError as e:
+                raise ValueError("%s: the record at byte offset %d: %s" % (src, pos, e))
+            write_record(self.f, pieces)
+            self.i += 1
+
+    def close(self):
+        """Completes the files after the last one fed, which must hold no record."""
+        while self.f is None or self.i == len(self.frames):
+            if self.j + 1 == len(self.jobs):
+                break
+            self._next_file()
+        if self.f is not None and self.i < len(self.frames):
+            raise ValueError("%s: %d of its %d records were given values"
+                             % (self.jobs[self.j][0], self.i, len(self.frames)))
+        if self.f is not None:
+            self._finish()
+
+    def abort(self):
+        """Removes the output being written, if any."""
+        if self.f is not None:
+            self.f.close()
+            self.f = None
+            os.remove(self.tmp)
+
+    def _next_file(self):
+        if self.f is not None:
+            self._finish()
+        if self.j + 1 == len(self.jobs):
+            raise ValueError("more values than records in %s" % [s for s, _ in self.jobs])
+        self.j += 1
+        src, dst = self.jobs[self.j]
+        self.data = _read_file(src)
+        self.frames, self.i = list(record_frames(self.data, src)), 0
+        self.tmp = os.path.join(os.path.dirname(dst), ".%s.partial" % os.path.basename(dst))
+        self.f = open(self.tmp, "wb")
+
+    def _finish(self):
+        self.f.flush()
+        os.fsync(self.f.fileno())
+        self.f.close()
+        self.f = None
+        os.replace(self.tmp, self.jobs[self.j][1])
 
 
 def read_encoded(path, offset, length):

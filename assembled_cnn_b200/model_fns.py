@@ -13,6 +13,8 @@ Mirrors (same names, argument meaning and error behaviour):
                                      classification evaluation) as evaluate_classification
   * metric/recall_metric.py:13-180 fed by functions/input_fns.py:148-165 (recall_at_k on the validation
                                      shards, run by --zeroshot_eval) as evaluate_retrieval
+  * kd/extract_embeddings.py + datasets/build_imagenet_data.py --logits_file_path (the knowledge-
+                                     distillation shards) as extract_teacher_logits
 plus `build_model(**flags)` (the name BASELINE.json uses; the reference has no such function).
 
 The reference builds a TF graph and lets the Estimator run it; here a call executes on the GPU:
@@ -23,7 +25,7 @@ from __future__ import annotations
 
 import os
 import math
-from collections import namedtuple
+from collections import deque, namedtuple
 
 import numpy as np
 import torch
@@ -1101,6 +1103,131 @@ def evaluate_retrieval(model, data_dir, *, val_regex="validation-*", preprocessi
                                                              model.dtype).items()}
     out["global_step"] = global_step
     return out
+
+
+class _TeacherLogitsDevice(_ResizedEvalPipeline):
+    """The teacher-logits loop: resize + crop + mean, the eval forward and a copy of the logits into the slot's
+    output buffer run as one CUDA graph per (slot, valid rows).  The valid rows of each batch then go to a ring
+    of OUT_RING pinned host buffers on the copy stream, one batch late: after the next batch's input has been
+    enqueued there, so the copy never holds up that batch's decode.  `sink(rows)` gets each batch's float32
+    [n, num_classes] rows in order, only after their copy's event has completed; `finish` delivers the rest."""
+
+    OUT_RING = 3
+
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, sink):
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph)
+        nc = model.num_classes
+        self.out = [torch.zeros(batch, nc, dtype=torch.float32, device=self.dev) for _ in self.slots]
+        self.host_out = [torch.zeros(batch, nc, dtype=torch.float32).pin_memory() for _ in range(self.OUT_RING)]
+        self.sink = sink
+        self.last = None             # (slot, valid rows) of the batch whose copy is not enqueued yet
+        self.copies = 0
+        self.ready = deque()         # (event, pinned rows) of the enqueued copies not yet delivered
+
+    def _body(self, slot, n_valid):
+        _, _, desc = self.slots[slot]
+        self.rt.set_images_resized(desc, n_valid, self.mean)
+        self.rt.run_forward()
+        self.out[slot].copy_(self.logits)
+
+    def _run(self, place, labels):
+        super()._run(place, labels)
+        if self.last is not None:
+            self._copy_out(*self.last)
+        self.last = ((self.taken - 1) % len(self.slots), len(labels))
+
+    def _copy_out(self, slot, n):
+        # the slot's output is rewritten two batches later, after the copy stream reaches that batch's input
+        while len(self.ready) >= self.OUT_RING - 1:
+            self._deliver()
+        rows = self.host_out[self.copies % self.OUT_RING][:n]
+        self.copies += 1
+        cs = self.copy_stream
+        cs.wait_event(self.slot_free[slot])          # the batch's graph has run
+        with torch.cuda.stream(cs):
+            rows.copy_(self.out[slot][:n], non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(cs)
+        self.ready.append((ev, rows))
+
+    def _deliver(self):
+        ev, rows = self.ready.popleft()
+        ev.synchronize()
+        self.sink(rows.numpy())
+
+    def finish(self):
+        if self.last is not None:
+            self._copy_out(*self.last)
+            self.last = None
+        while self.ready:
+            self._deliver()
+
+
+def extract_teacher_logits(teacher, data_dir, out_dir, *, train_regex="train-*", val_regex="validation-*",
+                           preprocessing_type="imagenet", image_size=224, batch_size=256, shard_index=0,
+                           num_shards=1, dataset_name="imagenet", use_resnet_d=None, use_cuda_graph=True,
+                           num_workers=None):
+    """Knowledge-distillation shards from a trained teacher: the reference's kd/extract_embeddings.py followed
+    by datasets/build_imagenet_data.py --logits_file_path.  Every file of data_dir matching train_regex or
+    val_regex is copied to out_dir under its own name, its records in order, each record's Example keeping
+    its bytes and gaining 'image/logit', a float32 list of the teacher.num_classes fp32 logits that
+    teacher(x, training=False) returns for the record's image x after the eval preprocessing of
+    `preprocessing_type` / `image_size` (the teacher's, as evaluate_classification).  out_dir is then a data_dir
+    for train_and_evaluate(kd_temp > 0): the validation files get logits too, as the reference's evaluation
+    input asks for them whenever kd_temp > 0.
+
+    The sorted files are split round-robin over num_shards processes (the reference's --no_shard /
+    --total_num_shard, e.g. one process per GPU); this call writes those of shard_index.  Every shard is read
+    and checked first: an empty glob (FileNotFoundError), a corrupt record frame, a record that already
+    holds image/logit or is not one features message, a teacher whose num_classes is not that of
+    DATASETS[dataset_name], out_dir equal to data_dir and an output file that already exists raise
+    ValueError before any GPU work and before any output exists.  The device work is the classification
+    evaluation's (device JPEG decode with PIL as the fallback, resize + crop + mean, the eval forward in the
+    teacher's dtype, one CUDA graph replay per batch; use_cuda_graph=False: the same launches, eager), in
+    batches that run across file boundaries, padded only in the last one.  The host writes a record once its
+    batch's logits have reached pinned memory, verifying the input record's data CRC
+    (imagenet_eval.FloatFeatureWriter); each output appears complete, by rename, or not at all.  Host memory
+    holds a few batches and one input file.  Returns the paths written, in order."""
+    from . import imagenet_eval as ie
+    from .imagenet_train import train_files
+    if dataset_name not in DATASETS:
+        raise ValueError("extract_teacher_logits: unknown dataset_name %r" % (dataset_name,))
+    nc = DATASETS[dataset_name]["num_classes"]
+    if teacher.num_classes != nc:
+        raise ValueError("extract_teacher_logits: the teacher has %d classes; %s has %d"
+                         % (teacher.num_classes, dataset_name, nc))
+    if not 0 <= shard_index < num_shards:
+        raise ValueError("extract_teacher_logits: shard_index %d outside [0, num_shards = %d)"
+                         % (shard_index, num_shards))
+    if os.path.realpath(out_dir) == os.path.realpath(data_dir):
+        raise ValueError("extract_teacher_logits: out_dir is data_dir (%s); the inputs would be overwritten"
+                         % data_dir)
+    size, _ = ie.eval_size(preprocessing_type, image_size)
+    if use_resnet_d is None:
+        use_resnet_d = getattr(teacher, "use_resnet_d", False)
+    files = sorted(set(train_files(data_dir, train_regex)) | set(ie.validation_files(data_dir, val_regex)))
+    jobs, records = [], []
+    for path in files[shard_index::num_shards]:
+        dst = os.path.join(out_dir, os.path.basename(path))
+        if os.path.exists(dst):
+            raise ValueError("extract_teacher_logits: %s already exists" % dst)
+        records += [(path, offset, length, 0) for offset, length in ie.appendable_records(path, ie.LOGIT_KEY)]
+        jobs.append((path, dst))
+    os.makedirs(out_dir, exist_ok=True)
+    writer = ie.FloatFeatureWriter(jobs, ie.LOGIT_KEY)
+    ev = None
+    try:
+        if records:
+            ev = _TeacherLogitsDevice(teacher, batch_size, size, use_resnet_d, use_cuda_graph, writer.add)
+            _feed_records(ev, records, batch_size, preprocessing_type, image_size, num_workers)
+            ev.finish()
+        writer.close()
+    except BaseException:
+        if ev is not None:
+            torch.cuda.synchronize(ev.dev)      # no copy into the pinned ring outlives the call
+        writer.abort()
+        raise
+    return [dst for _, dst in jobs]
 
 
 class _TrainFeed(StagingRing):

@@ -3,7 +3,8 @@ by libacnn.so (csrc/model_plan.cu, csrc/model_exec.cu); this module only
 
   * fills `acnn_model_config` from the reference's constructor flags (functions/model_fns.py:141-157),
   * allocates the caller-owned device buffers as torch tensors and hands their pointers to acnn_bind,
-  * exposes the variables (TF names / layouts) and the static input / output buffers as torch views.
+  * exposes the variables (TF names / layouts) and the static input / output buffers as torch views,
+  * and wraps the host CRC-32C of include/acnn.h (crc32c) for the TFRecord reader and writer.
 
 `NativeModel` (plan + introspection) needs no GPU; `NativeRuntime` (execution) has no CPU path.
 plan.py / runtime.py remain as the op-by-op executor the parity tests drive in lockstep with the
@@ -14,6 +15,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 from collections import OrderedDict
+
+import numpy as np
 
 from . import _lib
 from .plan import ModelConfig, Param, Slot, Tensor
@@ -114,6 +117,13 @@ def lib():
             fn.restype, fn.argtypes = res, args
         _bound = l
     return _bound
+
+
+def crc32c(data, crc=0):
+    """acnn_crc32c: the CRC-32C of the bytes-like `data` (bytes, bytearray, memoryview; not copied),
+    continued from `crc`, a value this function returned (0 starts a new one)."""
+    buf = np.frombuffer(data, dtype=np.uint8)
+    return _lib.load().acnn_crc32c(buf.ctypes.data, buf.size, crc)
 
 
 def make_config(cfg: ModelConfig, batch, height, width, *, training=True, mixup_type=0,

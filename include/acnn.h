@@ -18,6 +18,7 @@
 #ifndef ACNN_H_
 #define ACNN_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -669,6 +670,15 @@ int acnn_jpeg_plan(const acnn_jpeg_desc* desc, const int64_t* offsets, const int
 int acnn_jpeg_decode(const acnn_jpeg_desc* desc, const acnn_jpeg_job* jobs, const acnn_jpeg_batch* batch,
                      const uint8_t* data, uint8_t* out, void* work, int64_t work_bytes, int32_t* status,
                      void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * TFRecord checksums (the writer of knowledge-distillation shards, model_fns.extract_teacher_logits)
+ * ------------------------------------------------------------------------------------------- */
+/* CRC-32C (Castagnoli, reflected polynomial 0x82F63B78) of n bytes of HOST memory at data, continued
+ * from crc, a CRC this function returned (0 starts a new one): acnn_crc32c(b, nb, acnn_crc32c(a, na, 0))
+ * is the CRC of a followed by b.  data may be NULL when n = 0.  On x86-64 it runs SSE4.2's crc32
+ * instruction.  No CUDA call; never fails. */
+uint32_t acnn_crc32c(const void* data, size_t n, uint32_t crc);
 
 #ifdef __cplusplus
 }
