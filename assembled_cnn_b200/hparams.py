@@ -57,6 +57,10 @@ DEFAULTS = {
     "keep_ckpt_every_eval": True,         # :246
     "keep_checkpoint_max": 20,            # :249
     "eval_only": False,                   # :252
+    # export (model_fns.export_model, train_and_evaluate(export_dir=...)); export_dir itself is a keyword of
+    # train_and_evaluate, as official/utils/flags/_base.py defines it outside hparams_config.py
+    "export_only": False,                 # :259 (no cycle: export the latest checkpoint)
+    "export_decoder_type": "jpeg",        # :262 ('jpeg': export_test runs after the export)
     "save_checkpoints_epochs": 1.0,       # :266
     "ratio_fine_eval": 1.0,               # :269
     "pretrained_model_checkpoint_path": None,   # :43

@@ -303,6 +303,40 @@ def classify_rows(logits, labels, n_valid=None, k=5, label_smoothing=0.0, out=No
     return out
 
 
+def predict_rows(logits, n_valid=None, out=None):
+    """acnn_predict_rows on the current stream, for the rows r < n_valid of `logits` (CUDA fp32 [B, NC], rows
+    may be strided, as a model's logits view is): the PREDICT dict of nets/run_loop_classification.py:126-130,
+    classes = tf.argmax (-1 for a row holding a NaN), probabilities = the softmax, probabilities_sigmoid =
+    the sigmoid.  Rows >= n_valid are not written.  `out` (classes int32 [>= B], probabilities and
+    probabilities_sigmoid fp32 [>= B, NC], contiguous) is allocated unless given; returns it."""
+    from . import _lib
+    lib = _lib.load()
+    if logits.dim() != 2 or logits.dtype != torch.float32 or logits.stride(1) != 1:
+        raise ValueError("logits must be a float32 [B, NC] tensor with unit column stride")
+    B, NC = logits.shape
+    n_valid = B if n_valid is None else int(n_valid)
+    if not logits.is_cuda:
+        raise _lib.AcnnError("predict_rows runs on the GPU: logits must be a CUDA tensor")
+    if out is None:
+        out = (torch.empty(B, dtype=torch.int32, device=logits.device),
+               torch.empty(B, NC, dtype=torch.float32, device=logits.device),
+               torch.empty(B, NC, dtype=torch.float32, device=logits.device))
+    classes, prob, sig = out
+    if classes.dtype != torch.int32 or classes.numel() < B or not classes.is_contiguous() \
+            or classes.device != logits.device:
+        raise ValueError("classes must be a contiguous int32 tensor of at least B = %d values on %s"
+                         % (B, logits.device))
+    for t in (prob, sig):
+        if t.dtype != torch.float32 or t.dim() != 2 or t.shape[0] < B or t.shape[1] != NC \
+                or not t.is_contiguous() or t.device != logits.device:
+            raise ValueError("probabilities must be contiguous float32 [>= %d, %d] tensors on %s"
+                             % (B, NC, logits.device))
+    stream = torch.cuda.current_stream(logits.device).cuda_stream
+    _lib.check(lib.acnn_predict_rows(logits.data_ptr(), B, logits.stride(0), NC, n_valid, classes.data_ptr(),
+                                     prob.data_ptr(), sig.data_ptr(), stream), "acnn_predict_rows")
+    return out
+
+
 def classification_result(pred, conf, hit_k, ce, labels, batch_sizes, num_thresholds=10):
     """The eval metrics of nets/run_loop_classification.py:141-234 from the per-row results of a whole
     evaluation (numpy arrays, rows in evaluation order), in float64:

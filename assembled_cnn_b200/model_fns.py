@@ -15,6 +15,8 @@ Mirrors (same names, argument meaning and error behaviour):
                                      shards, run by --zeroshot_eval) as evaluate_retrieval
   * kd/extract_embeddings.py + datasets/build_imagenet_data.py --logits_file_path (the knowledge-
                                      distillation shards) as extract_teacher_logits
+  * utils/export_utils.py:36-154     export_pb (the binary_input / preprocessed_input servables) and
+                                     export_test as export_model, load_servable / Servable, export_test
 plus `build_model(**flags)` (the name BASELINE.json uses; the reference has no such function).
 
 The reference builds a TF graph and lets the Estimator run it; here a call executes on the GPU:
@@ -1230,6 +1232,374 @@ def extract_teacher_logits(teacher, data_dir, out_dir, *, train_regex="train-*",
     return [dst for _, dst in jobs]
 
 
+# ------------------------------------------------------------------------------------------------ export
+# utils/export_utils.py: the servables export_pb writes under <export_dir>/<data_format>/
+SIGNATURES = ("binary_input", "preprocessed_input")
+SERVABLE_FORMAT = "assembled_cnn_b200.servable/1"
+EXPORT_DECODERS = ("jpeg", "webp")           # --export_decoder_type (hparams_config.py:262-264)
+PREDICT_OUTPUTS = ("classes", "probabilities", "probabilities_sigmoid")
+
+
+class _PredictDevice(_ResizedEvalPipeline):
+    """The servable's loop: resize + crop + mean, the eval forward, acnn_predict_rows and (with an embedding
+    output) a copy of the embedding run as one CUDA graph per (slot, valid rows), into one set of output
+    buffers.  After each batch, its valid rows go to a ring of OUT_RING pinned host sets on the current stream,
+    one copy per output, so the next batch's graph runs after them; `sink(arrays)` gets each batch's rows in
+    order, once their copy's event has completed.  run_images runs a batch of preprocessed images instead."""
+
+    OUT_RING = 3
+
+    def __init__(self, model, batch, size, use_resnet_d, embedding):
+        super().__init__(model, batch, size, use_resnet_d, True)
+        nc, m = model.num_classes, self.rt.plan.meta
+        self.out = [torch.zeros(batch, dtype=torch.int32, device=self.dev),
+                    torch.zeros(batch, nc, dtype=torch.float32, device=self.dev),
+                    torch.zeros(batch, nc, dtype=torch.float32, device=self.dev)]
+        self.feat = None
+        if embedding:
+            # Model.__call__(return_embedding=True): the embedding, else the pooled features
+            self.feat = self.rt.t[m["embedding"] if "embedding" in m else m["pooled"]].reshape(batch, -1)
+            self.out.append(torch.zeros(batch, self.feat.shape[1], dtype=torch.float32, device=self.dev))
+        self.images = self.rt.t[m["images"]]
+        self.host_out = [[torch.zeros(t.shape, dtype=t.dtype).pin_memory() for t in self.out]
+                         for _ in range(self.OUT_RING)]
+        self.copies = 0
+        self.pending = deque()       # (event, pinned set, rows) of the enqueued copies not yet delivered
+        self.sink = None
+
+    def _outputs(self, n_valid):
+        from .metrics import predict_rows
+        predict_rows(self.logits, n_valid, self.out[:3])
+        if self.feat is not None:
+            self.out[3].copy_(self.feat)
+
+    def _body(self, slot, n_valid):
+        _, _, desc = self.slots[slot]
+        self.rt.set_images_resized(desc, n_valid, self.mean)
+        self.rt.run_forward()
+        self._outputs(n_valid)
+
+    def _run(self, place, labels):
+        super()._run(place, labels)
+        self._copy_out(len(labels))
+
+    def run_images(self, images):
+        """The outputs of the float32 [n <= batch, S, S, 3] preprocessed `images` (eager launches)."""
+        n = images.shape[0]
+        self.images[:n].copy_(images)
+        self.rt.run_forward()
+        self._outputs(n)
+        self._copy_out(n)
+
+    def _copy_out(self, n):
+        while len(self.pending) >= self.OUT_RING:
+            self._deliver()
+        host = self.host_out[self.copies % self.OUT_RING]
+        self.copies += 1
+        for h, d in zip(host, self.out):
+            h[:n].copy_(d[:n], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.dev))
+        self.pending.append((ev, host, n))
+
+    def _deliver(self):
+        ev, host, n = self.pending.popleft()
+        ev.synchronize()
+        self.sink([h[:n].numpy() for h in host])
+
+    def finish(self):
+        while self.pending:
+            self._deliver()
+
+
+class Servable:
+    """An exported model (export_model / load_servable) or an in-memory `model` serving the PREDICT dict of
+    nets/run_loop_classification.py:126-130 for encoded images (predict, the reference's binary_input
+    SavedModel) or for preprocessed ones (predict_images, preprocessed_input).  Both methods return numpy
+    {'classes': int64 [n], 'probabilities': float32 [n, num_classes], 'probabilities_sigmoid': float32
+    [n, num_classes]} plus 'embedding' float32 [n, d] when the model has an embedding layer or was exported
+    with return_embedding (without an embedding layer, the pooled features, as Model.__call__ returns them).
+
+    The device work runs in chunks of max_batch images on the model's device; the first call builds it."""
+
+    def __init__(self, model, *, preprocessing_type="imagenet", image_size=224, use_resnet_d=None,
+                 return_embedding=False, max_batch=256, signature="binary_input", decoder_type="jpeg"):
+        from .imagenet_eval import eval_size
+        self.size, _ = eval_size(preprocessing_type, image_size)
+        if int(max_batch) < 1:
+            raise ValueError("max_batch must be >= 1 (got %r)" % (max_batch,))
+        self.model, self.max_batch = model, int(max_batch)
+        self.preprocessing_type, self.image_size = preprocessing_type, int(image_size)
+        self.use_resnet_d = bool(getattr(model, "use_resnet_d", False) if use_resnet_d is None else use_resnet_d)
+        self.embedding = bool(return_embedding) or model.cfg_kwargs["embedding_size"] > 0
+        self.signature, self.decoder_type = signature, decoder_type
+        self.outputs = PREDICT_OUTPUTS + (("embedding",) if self.embedding else ())
+        self._pipe = None
+
+    def _empty(self, n):
+        nc = self.model.num_classes
+        res = {"classes": np.zeros(n, np.int64), "probabilities": np.zeros((n, nc), np.float32),
+               "probabilities_sigmoid": np.zeros((n, nc), np.float32)}
+        if self.embedding:
+            res["embedding"] = None          # its width is the runtime's: set by the first delivery
+        return res
+
+    def _collect(self, n, work):
+        """Runs work(pipeline) and returns the outputs of its n rows, delivered in order."""
+        res, pos = self._empty(n), 0
+        if n == 0:
+            if self.embedding:
+                res["embedding"] = np.zeros((0, 0), np.float32)
+            return res
+        if self._pipe is None:
+            self._pipe = _PredictDevice(self.model, self.max_batch, self.size, self.use_resnet_d, self.embedding)
+        pipe = self._pipe
+
+        def sink(arrays):
+            nonlocal pos
+            k = len(arrays[0])
+            for name, a in zip(self.outputs, arrays):
+                if res[name] is None:
+                    res[name] = np.zeros((n,) + a.shape[1:], a.dtype)
+                res[name][pos:pos + k] = a
+            pos += k
+
+        pipe.sink = sink
+        try:
+            work(pipe)
+            pipe.finish()
+        except BaseException:
+            # a batch may be staged and not run: the next call starts a new pipeline
+            torch.cuda.synchronize(pipe.dev)
+            self._pipe = None
+            raise
+        assert pos == n, (pos, n)
+        return res
+
+    def predict(self, images):
+        """The PREDICT dict of a list of encoded images (bytes; any number).  Each is decoded on the device
+        where the device decoder handles it, by PIL otherwise, and given the eval preprocessing of the
+        servable's preprocessing_type (imagenet_eval.eval_geometry); a chunk's decode runs on the copy stream
+        while the previous chunk computes."""
+        from .imagenet_eval import eval_geometry
+        images = list(images)
+        for i, b in enumerate(images):
+            if not isinstance(b, (bytes, bytearray, memoryview)):
+                raise TypeError("predict: image %d is a %s, not encoded bytes" % (i, type(b).__name__))
+        images = [b if isinstance(b, bytes) else bytes(b) for b in images]
+        B = self.max_batch
+
+        def geometry(h, w):
+            return eval_geometry(h, w, self.preprocessing_type, self.image_size)
+
+        def work(pipe):
+            for a in range(0, len(images), B):
+                chunk = images[a:a + B]
+                pipe.run_batch_encoded(chunk, [0] * len(chunk), geometry)
+        return self._collect(len(images), work)
+
+    def predict_images(self, images):
+        """The PREDICT dict of float32 [n, S, S, 3] images already preprocessed (S: the eval size of the
+        servable's preprocessing_type), numpy or torch."""
+        x = torch.as_tensor(images)
+        S = self.size
+        if x.dim() != 4 or tuple(x.shape[1:]) != (S, S, 3):
+            raise ValueError("predict_images: images must be [n, %d, %d, 3] (got %s)" % (S, S, tuple(x.shape)))
+        x = x.to(torch.float32)
+        B = self.max_batch
+
+        def work(pipe):
+            for a in range(0, x.shape[0], B):
+                pipe.run_images(x[a:a + B])
+        return self._collect(x.shape[0], work)
+
+
+def _variable_names(cfg_kwargs, use_resnet_d, size):
+    """The variables (trainables, then BN moving statistics) of a model's plan, from the host plan."""
+    plan = build_plan(ModelConfig(use_resnet_d=bool(use_resnet_d), **cfg_kwargs), 1, size, size, training=False)
+    return list(plan.params) + list(plan.state)
+
+
+def _host_weights(model, use_resnet_d, size):
+    """float32 numpy arrays of every variable of `model`: its runtime's, or, before any runtime exists, the
+    ones given to set_weights (no GPU work); a model with neither gets its seed's initial weights."""
+    if bool(use_resnet_d) not in model._primary and model._pending_weights is not None:
+        pending = model._pending_weights
+        names = _variable_names(model.cfg_kwargs, use_resnet_d, size)
+        missing = [n for n in names if n not in pending]
+        if missing:
+            raise KeyError("export: the weights lack %d variable(s), e.g. %s" % (len(missing), missing[:3]))
+        return {n: torch.as_tensor(pending[n]).detach().float().cpu().numpy() for n in names}
+    if bool(use_resnet_d) not in model._primary:
+        model.runtime(1, size, size, training=False, use_resnet_d=use_resnet_d)
+    return {n: v.numpy() for n, v in model.get_weights(use_resnet_d).items()}
+
+
+def _partial(path):
+    return os.path.join(os.path.dirname(path), ".%s.partial" % os.path.basename(path))
+
+
+def export_model(model, export_dir, *, preprocessing_type, image_size, use_resnet_d=None, return_embedding=False,
+                 decoder_type="jpeg"):
+    """utils/export_utils.export_pb: writes the two servables of `model` as Estimator.export_savedmodel
+    lays them out, <export_dir>/channels_last/binary_input/<timestamp>/ (encoded images in, the eval
+    preprocessing of preprocessing_type / image_size) and <export_dir>/channels_last/preprocessed_input/
+    <timestamp>/ (float images in), and returns the two paths.  Each holds config.json (the model's
+    constructor flags, use_resnet_d, dtype, preprocessing_type, image_size, decoder_type, the signature's
+    input and outputs) and variables.npz (every variable in the checkpoint module's TF naming, without the
+    momentum slots or global_step).  load_servable reads them; TF SavedModels are not written (they cannot
+    be without TensorFlow).
+
+    An unknown preprocessing_type (NotImplementedError), an image_size that is not a positive int or gives
+    an eval size that is not a multiple of 32, an unknown decoder_type and an existing target (FileExistsError)
+    raise before anything is written and before any GPU work.  The weights are read from the model's runtime
+    (those given to set_weights when it has none yet: then no GPU work at all).  Each directory is written
+    under a hidden name beside its target and renamed when complete."""
+    import json
+    import time
+    from .imagenet_eval import eval_size
+    if isinstance(image_size, bool) or not isinstance(image_size, (int, np.integer)) or image_size < 1:
+        raise ValueError("export: image_size must be a positive int (got %r)" % (image_size,))
+    size, _ = eval_size(preprocessing_type, int(image_size))
+    if decoder_type not in EXPORT_DECODERS:
+        raise ValueError("export: decoder_type must be one of %s (got %r)" % (EXPORT_DECODERS, decoder_type))
+    if use_resnet_d is None:
+        use_resnet_d = getattr(model, "use_resnet_d", False)
+    stamp = str(int(time.time()))
+    targets = [os.path.join(export_dir, model.data_format, sig, stamp) for sig in SIGNATURES]
+    for t in targets:
+        if os.path.lexists(t) or os.path.lexists(_partial(t)):
+            raise FileExistsError("export: %s already exists" % t)
+    weights = _host_weights(model, use_resnet_d, size)
+    nc = model.num_classes
+    outputs = {"classes": "int64 [n]", "probabilities": "float32 [n, %d]" % nc,
+               "probabilities_sigmoid": "float32 [n, %d]" % nc}
+    if return_embedding or model.cfg_kwargs["embedding_size"] > 0:
+        outputs["embedding"] = "float32 [n, d]"
+    inputs = {"binary_input": "encoded images: bytes [n]",
+              "preprocessed_input": "float32 [n, %d, %d, 3], eval-preprocessed" % (size, size)}
+    written = []
+    try:
+        for sig, t in zip(SIGNATURES, targets):
+            tmp = _partial(t)
+            os.makedirs(tmp)
+            written.append(tmp)
+            config = {"format": SERVABLE_FORMAT, "signature": sig, "inputs": inputs[sig], "outputs": outputs,
+                      "model": dict(model.cfg_kwargs), "dtype": model.dtype, "use_resnet_d": bool(use_resnet_d),
+                      "data_format": model.data_format, "preprocessing_type": preprocessing_type,
+                      "image_size": int(image_size), "eval_size": size, "decoder_type": decoder_type,
+                      "return_embedding": bool(return_embedding), "variables": "variables.npz"}
+            with open(os.path.join(tmp, "variables.npz"), "wb") as f:
+                np.savez(f, **weights)
+                f.flush()
+                os.fsync(f.fileno())
+            with open(os.path.join(tmp, "config.json"), "w") as f:
+                json.dump(config, f, indent=1, sort_keys=True)
+        for tmp, t in zip(list(written), targets):
+            os.rename(tmp, t)
+            written.remove(tmp)
+    except BaseException:
+        import shutil
+        for tmp in written:
+            shutil.rmtree(tmp, ignore_errors=True)
+        raise
+    return targets[0], targets[1]
+
+
+def read_servable_config(path):
+    """The config.json of an exported servable directory, checked (ValueError) before anything is built."""
+    import json
+    fname = os.path.join(path, "config.json")
+    if not os.path.isfile(fname) or not os.path.isfile(os.path.join(path, "variables.npz")):
+        raise ValueError("%s is not an exported servable (config.json and variables.npz expected)" % path)
+    with open(fname) as f:
+        cfg = json.load(f)
+    keys = {"format", "signature", "model", "dtype", "use_resnet_d", "preprocessing_type", "image_size",
+            "decoder_type", "return_embedding"}
+    if not isinstance(cfg, dict) or cfg.get("format") != SERVABLE_FORMAT or not keys <= set(cfg) \
+            or cfg["signature"] not in SIGNATURES:
+        raise ValueError("%s: not a config.json of format %s" % (fname, SERVABLE_FORMAT))
+    return cfg
+
+
+def load_servable(path, *, device=None, max_batch=256):
+    """The Servable of a directory export_model wrote: a new Model of the directory's flags and dtype with
+    its variables (on `device`, default the current CUDA device).  Host work only: the device work starts
+    with the first predict."""
+    from .checkpoint import load_checkpoint
+    from .imagenet_eval import eval_size
+    cfg = read_servable_config(path)
+    size, _ = eval_size(cfg["preprocessing_type"], cfg["image_size"])
+    model = Model(dtype=cfg["dtype"], device=device or "cuda:%d" % torch.cuda.current_device(), **cfg["model"])
+    model.use_resnet_d = bool(cfg["use_resnet_d"])
+    weights = load_checkpoint(os.path.join(path, "variables.npz"))
+    names = _variable_names(model.cfg_kwargs, model.use_resnet_d, size)
+    missing = [n for n in names if n not in weights]
+    if missing:
+        raise ValueError("%s: variables.npz lacks %d variable(s), e.g. %s" % (path, len(missing), missing[:3]))
+    model.set_weights({n: torch.as_tensor(weights[n]) for n in names})
+    return Servable(model, preprocessing_type=cfg["preprocessing_type"], image_size=cfg["image_size"],
+                    use_resnet_d=model.use_resnet_d, return_embedding=cfg["return_embedding"], max_batch=max_batch,
+                    signature=cfg["signature"], decoder_type=cfg["decoder_type"])
+
+
+def export_recall_at_1(embedding, labels, device=None):
+    """Recall@1 of export_test's zero-shot branch (utils/export_utils.py:75-86): every row is a query
+    (distractors, label -1, included, and two distractors match), the index is every row but the query
+    itself (fill_diagonal(-10)), similarity the cosine of l2-normalised rows, and the nearest row is the
+    lowest index among equal similarities (np.argmax).  The search is one acnn_knn_topk with k = 2 in fp32
+    (three bf16 planes per operand); the query's own index is skipped."""
+    from .metrics import knn_topk
+    x = torch.as_tensor(np.asarray(embedding, np.float32)).to(device or "cuda")
+    labels = np.asarray(labels, np.int64)
+    n = x.shape[0]
+    if n < 2 or len(labels) != n:
+        raise ValueError("export_test: Recall@1 needs at least two rows with one label each (got %d rows, %d labels)"
+                         % (n, len(labels)))
+    if not bool(torch.isfinite(x).all()):
+        raise ValueError("export_test: the embeddings contain NaN or infinite values")
+    idx, _ = knn_topk(x, x, 2, "cosine", "fp32")
+    idx = idx.long().cpu().numpy()
+    if (idx >= n).any():
+        raise ValueError("export_test: similarities are not finite; cannot rank the index")
+    nearest = np.where(idx[:, 0] == np.arange(n), idx[:, 1], idx[:, 0])
+    return int((labels[nearest] == labels).sum()) / n
+
+
+def export_test(binary_dir, data_dir, *, val_regex="validation-*", batch_size=256, zeroshot=False):
+    """utils/export_utils.export_test: the exported binary_input servable at binary_dir re-reads the
+    validation shards data_dir/val_regex (a record without image/class/label has label -1) and scores
+    itself: the accuracy of `classes` against the labels, or with zeroshot Recall@1 of its `embedding`
+    (export_recall_at_1).  Writes binary_dir/model_performance.txt with the reference's message and returns
+    the metric.  A bad directory, an empty glob, a corrupt record and zeroshot on a servable without an
+    embedding output raise before any GPU work."""
+    from . import imagenet_eval as ie
+    sv = load_servable(binary_dir, max_batch=batch_size)
+    if zeroshot and not sv.embedding:
+        raise ValueError("export_test: zeroshot needs an embedding output; export with return_embedding=True")
+    per_file = [(path, ie.read_records(path, missing_label=-1)) for path in ie.validation_files(data_dir, val_regex)]
+    labels = np.array([r[0] for _, recs in per_file for r in recs], np.int64)
+    if len(labels) == 0:
+        raise ValueError("export_test: the shards under %s hold no record" % data_dir)
+    group = 8 * sv.max_batch
+    classes, emb = [], []
+    for path, recs in per_file:
+        data = ie._read_file(path)
+        for a in range(0, len(recs), group):
+            out = sv.predict([data[off:off + n] for _, off, n in recs[a:a + group]])
+            classes.append(out["classes"])
+            if zeroshot:
+                emb.append(out["embedding"])
+    if zeroshot:
+        metric = export_recall_at_1(np.concatenate(emb), labels, sv.model.device)
+    else:
+        metric = int((np.concatenate(classes) == labels).sum()) / len(labels)
+    msg = "IMPOTANT! Evaluation metric of exported saved_model.pb is {}".format(metric)
+    with open(os.path.join(binary_dir, "model_performance.txt"), "w") as fp:
+        fp.write(msg)
+    return metric
+
+
 class _TrainFeed(StagingRing):
     """The training input's staging ring: per step, the crop windows packed into a growable pinned uint8
     buffer with one acnn_crop_desc each, the labels and (KD) the teacher logits, copied to one of two
@@ -1307,8 +1677,24 @@ def _prune_checkpoints(model_dir, keep):
         os.remove(f)
 
 
+def cycle_schedule(p, epochs_between_evals, cur_epoch):
+    """(the training epochs of each train-and-evaluate cycle, the index of the first one) of resnet_main
+    (nets/run_loop_classification.py:457-468) for the params p, resumed at epoch cur_epoch: one evaluation with
+    eval_only or train_epochs = 0, no cycle with export_only, else imagenet_train.epoch_schedule from
+    cur_epoch.  The cycle index keys the cycle's randomness."""
+    from . import imagenet_train as it
+    if p["eval_only"] or not p["train_epochs"]:
+        return [0], 0
+    if p["export_only"]:
+        return [], 0
+    args = (p["train_epochs"], epochs_between_evals, p["ratio_fine_eval"])
+    full = it.epoch_schedule(*args)
+    schedule = it.epoch_schedule(*args, cur_epoch=cur_epoch)
+    return schedule, len(full) - len(schedule)
+
+
 def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_threshold=None, max_train_steps=None,
-                       image_size=224, seed=0, use_cuda_graph=True, num_workers=None, **flags):
+                       image_size=224, seed=0, use_cuda_graph=True, num_workers=None, export_dir=None, **flags):
     """resnet_main's train-and-evaluate loop (nets/run_loop_classification.py:389-489) over the TFRecord
     shards data_dir/train_regex (training) and data_dir/val_regex (evaluation).  `flags` are hparams
     names (params_from_flags); epochs_between_evals, stop_threshold and max_train_steps are the run loop's
@@ -1332,7 +1718,15 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     record order, the crop windows, the flips and the mixup lambdas (imagenet_train's counter-based
     generators).  num_images is the number of records in the shards (the reference's data_config count).
     Under torch.distributed every rank trains its slice of each global batch; rank 0 writes the
-    checkpoints and evaluates.  Returns the list of the cycles' evaluation results (the recall dicts with
+    checkpoints and evaluates.
+
+    With export_dir (official/utils/flags/_base.py's --export_dir), rank 0 exports the model after the last
+    cycle (export_model with the preprocessing_type, image_size and use_resnet_d flags; return_embedding with
+    return_embedding or zeroshot_eval) and, when export_decoder_type is 'jpeg', runs export_test on the binary
+    servable (batch val_batch_size, val_regex, zeroshot_eval), as nets/run_loop_classification.py:494-495.
+    export_only runs no cycle (unless eval_only or train_epochs = 0 ask for an evaluation, as the reference's
+    order has it) and exports the latest checkpoint of model_dir; it needs export_dir and a checkpoint, both
+    checked before any GPU work.  Returns the list of the cycles' evaluation results (the recall dicts with
     zeroshot_eval)."""
     from concurrent.futures import ThreadPoolExecutor
     from . import imagenet_train as it
@@ -1351,6 +1745,13 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
         raise ValueError("zeroshot_eval ranks the checkpoints by recall_at_1: recall_at_k must hold 1 (got %r)"
                          % (p["recall_at_k"],))
     key = "recall_at_1" if zeroshot else "accuracy"
+    if export_dir is not None and p["export_decoder_type"] not in EXPORT_DECODERS:
+        raise ValueError("export_decoder_type must be one of %s (got %r)" % (EXPORT_DECODERS, p["export_decoder_type"]))
+    if p["export_only"]:
+        if export_dir is None:
+            raise ValueError("export_only exports the latest checkpoint: give export_dir")
+        if not os.path.isdir(model_dir) or latest_checkpoint(model_dir) is None:
+            raise ValueError("export_only: no checkpoint in %s" % model_dir)
     dist = torch.distributed.is_initialized()
     world = torch.distributed.get_world_size() if dist else 1
     rank = torch.distributed.get_rank() if dist else 0
@@ -1376,13 +1777,7 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
         restore(model, ckpt, trainer)
     elif p["pretrained_model_checkpoint_path"]:
         warm_start(model, p["pretrained_model_checkpoint_path"], trainer.global_step)
-    if p["eval_only"] or not p["train_epochs"]:
-        schedule, first = [0], 0
-    else:
-        args = (p["train_epochs"], epochs_between_evals, p["ratio_fine_eval"])
-        full = it.epoch_schedule(*args)
-        schedule = it.epoch_schedule(*args, cur_epoch=trainer.global_step // steps_per_epoch)
-        first = len(full) - len(schedule)          # the cycle index keys the cycle's randomness
+    schedule, first = cycle_schedule(p, epochs_between_evals, trainer.global_step // steps_per_epoch)
     total_train_steps = p["train_epochs"] * steps_per_epoch
     save_steps = int(p["save_checkpoints_epochs"] * steps_per_epoch)
     shuffle_buffer = it.SHUFFLE_BUFFER.get(ds_name, it.DEFAULT_SHUFFLE_BUFFER)
@@ -1460,4 +1855,12 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     finally:
         pool.shutdown(wait=True, cancel_futures=True)
     torch.cuda.current_stream(dev).synchronize()
+    if export_dir is not None and rank == 0:
+        binary_dir, _ = export_model(model, export_dir, preprocessing_type=p["preprocessing_type"],
+                                     image_size=image_size, use_resnet_d=p["use_resnet_d"],
+                                     return_embedding=bool(p["return_embedding"] or zeroshot),
+                                     decoder_type=p["export_decoder_type"])
+        if p["export_decoder_type"] == "jpeg":
+            export_test(binary_dir, data_dir, val_regex=p["val_regex"], batch_size=p["val_batch_size"],
+                        zeroshot=zeroshot)
     return results

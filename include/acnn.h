@@ -571,6 +571,20 @@ int acnn_crop_resize_autoaugment_u8(const acnn_crop_desc* desc, const acnn_autoa
 int acnn_classify_rows(const float* logits, int B, int ld, int NC, const int32_t* labels, int n_valid, int k,
                        float label_smoothing, int32_t* pred, float* conf, int32_t* hit_k, float* ce,
                        void* stream);
+/* The PREDICT-mode `predictions` dict of nets/run_loop_classification.py:126-130 for logits fp32 [B][ld]
+ * (columns < NC are the classes), for every row r < n_valid (rows >= n_valid are not written):
+ *   classes[r]                   = tf.argmax(logits, 1): the smallest index of the largest logit.  An
+ *                                  infinite logit is an ordinary value (a row of -inf only gets 0); a row
+ *                                  holding a NaN gets -1.  (acnn_softmax_top1_count gives -1 for any
+ *                                  non-finite logit: its rule is about the probabilities, not the logits.)
+ *   probabilities[r][j]          = expf(x_j - max) / sum_j expf(x_j - max), the sum in a fixed order;
+ *                                  a row with +inf, or only -inf, gives NaN as tf.nn.softmax does;
+ *   probabilities_sigmoid[r][j]  = 1 / (1 + expf(-x_j)).
+ * probabilities and probabilities_sigmoid are dense [B][NC].  One CTA per row, no atomics: the results are
+ * the same under CUDA-graph replay and on concurrent streams.  Null pointers, B < 1, NC < 1, ld < NC,
+ * n_valid outside [0, B]: ACNN_ERR_INVALID before any CUDA call; n_valid = 0 launches nothing. */
+int acnn_predict_rows(const float* logits, int B, int ld, int NC, int n_valid, int32_t* classes, float* probabilities,
+                      float* probabilities_sigmoid, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * JPEG decoding (the tf.image.decode_jpeg / PIL decode of every input pipeline), bit for bit equal to
