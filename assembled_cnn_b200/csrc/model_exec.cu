@@ -1004,6 +1004,30 @@ int acnn_step(acnn_model* m, void* stream) {
   if (rc == ACNN_OK) rc = acnn_sgd_step(m, stream);
   return rc;
 }
+int acnn_replica_accumulate_model(acnn_model* m, int phase, float* acc_grads, float* state_base, float* acc_state,
+                                  int64_t lo, int64_t hi, int replicas, void* stream) {
+  ACNN_REQUIRE(m && m->bound && m->grads, "acnn_replica_accumulate_model: not bound for training");
+  const Plan& p = m->plan;
+  ACNN_REQUIRE(replicas >= 2, "acnn_replica_accumulate_model: replicas=%d (needs at least 2)", replicas);
+  ACNN_REQUIRE(lo >= 0 && lo <= hi && hi <= p.param_elems,
+               "acnn_replica_accumulate_model: [lo, hi) = [%lld, %lld) outside [0, %lld)", (long long)lo,
+               (long long)hi, (long long)p.param_elems);
+  const float scale = 1.0f / (float)replicas;
+  if (phase == ACNN_REPLICA_SAVE)
+    return acnn_replica_accumulate(phase, nullptr, nullptr, state_base, nullptr, m->state, 0, 0, p.state_elems, scale,
+                                   stream);
+  const bool with_state = lo == 0;   // the moving statistics and the loss go with the range that starts at 0
+  int rc = acnn_replica_accumulate(phase, acc_grads, m->grads, state_base, acc_state, m->state, lo, hi,
+                                   with_state ? p.state_elems : 0, scale, stream);
+  if (rc == ACNN_OK && with_state && p.loss.buf != BUF_NONE) {
+    ACNN_REQUIRE(acc_state, "acnn_replica_accumulate_model: null acc_state");
+    rc = acnn_replica_accumulate(phase, nullptr, nullptr, nullptr, acc_state + p.state_elems,
+                                 (float*)(m->ws + m->zero_off + 4 * p.loss.offset), 0, 0, ACNN_REPLICA_LOSS_FLOATS,
+                                 scale, stream);
+  }
+  return rc;
+}
+
 int acnn_run_ops(acnn_model* m, int phase, int first, int last, void* stream) {
   ACNN_REQUIRE(m && phase >= 0 && phase <= 2, "acnn_run_ops: bad phase %d", phase);
   return run_range(m, phase == 0 ? m->fwd : (phase == 1 ? m->bwd : m->upd), first, last, stream);

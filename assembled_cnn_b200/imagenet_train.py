@@ -321,6 +321,18 @@ class CycleStream:
         return [(p, int(self._epoch(p // self.n)[p % self.n])) for p in self.positions(t)]
 
 
+def replica_streams(counts, seed, cycle, epochs, shuffle_buffer, input_batch, world=1, rank=0, replicas=1):
+    """The CycleStreams of the `replicas` replicas q = rank * replicas + r of process `rank`: each gets what rank
+    q of a world * replicas run gets, so the data does not depend on how the replicas are split over processes."""
+    return [CycleStream(counts, seed, cycle, epochs, shuffle_buffer, input_batch, world * replicas, rank * replicas + r)
+            for r in range(replicas)]
+
+
+def replica_mixup_lambdas(seed, global_step, rank, replicas, n):
+    """float32 [replicas, n]: row r holds mixup_lambdas of replica q = rank * replicas + r."""
+    return np.stack([mixup_lambdas(seed, global_step, rank * replicas + r, n) for r in range(replicas)])
+
+
 def epoch_schedule(train_epochs, epochs_between_evals, ratio_fine_eval, cur_epoch=0):
     """The epochs of each train-and-evaluate cycle (nets/run_loop_classification.py:453-467 and
     utils/config_utils.py:71-96 get_epoch_schedule): cycles of epochs_between_evals epochs, the last one

@@ -291,12 +291,26 @@ def build_model(**flags) -> Model:
     return model
 
 
+def check_replicas_per_device(replicas_per_device):
+    """replicas_per_device must be an integer >= 1 (ValueError otherwise); returns it as an int."""
+    r = replicas_per_device
+    if isinstance(r, bool) or not isinstance(r, (int, np.integer)) or r < 1:
+        raise ValueError("replicas_per_device must be an integer >= 1 (got %r)" % (r,))
+    return int(r)
+
+
 class Trainer:
-    """One data-parallel replica of the training step (resnet_model_fn's TRAIN branch +
-    get_train_op): owns the step's static buffers, the LR schedule and the CUDA graphs."""
+    """The data-parallel replicas of the training step this process runs (resnet_model_fn's TRAIN branch +
+    get_train_op): owns the step's static buffers, the LR schedule and the CUDA graphs.
+
+    replicas_per_device = R > 1 runs R replicas one after another on this device (micro-steps), each a full
+    forward + backward of batch_size / (world * R) examples from the same moving statistics, as R GPUs of a
+    MirroredStrategy run would: the gradients are summed in replica order, the updated moving statistics and
+    the reported loss averaged (acnn_replica_accumulate), then one SGD step with grad_scale 1 / (world * R *
+    loss_scale).  The reference's --num_gpus=N is world * replicas_per_device = N."""
 
     def __init__(self, model: Model, params: dict, height=224, width=224, *, use_cuda_graph=True,
-                 lam_seed=7, num_images=None):
+                 lam_seed=7, num_images=None, replicas_per_device=1):
         """num_images: training images per epoch for the LR and keep-prob schedules (default: the
         dataset's data_config count)."""
         p = params
@@ -304,8 +318,9 @@ class Trainer:
             raise NotImplementedError("only cls_loss_type='softmax' is on the hot path")
         self.model = model
         self.p = p
+        self.replicas = check_replicas_per_device(replicas_per_device)
         self.world = torch.distributed.get_world_size() if torch.distributed.is_initialized() else 1
-        self.local_batch = per_device_batch_size(p["batch_size"], self.world)
+        self.local_batch = per_device_batch_size(p["batch_size"], self.world * self.replicas)
         self.mixup_type = int(p.get("mixup_type", 0))
         self.kd_temp = float(p.get("kd_temp", 0) or 0)
         self.use_dropblock = bool(p.get("use_dropblock", False))
@@ -355,6 +370,9 @@ class Trainer:
         if self.world > 1:
             self._buckets = dp.grad_buckets(self.rt.plan)
             self._segments = dp.backward_segments(self.rt.plan, self._buckets)
+        # several replicas: the accumulators (empty between global steps) and one graph per (phase, range)
+        self._acc_bufs = self.rt.replica_buffers() if self.replicas > 1 else None
+        self._acc_graphs = {}
         # input double-buffering: prefetch() copies the NEXT batch host->device on a side stream
         # while the current step computes; train_step() then takes it with a device-side copy
         self._copy_stream = torch.cuda.Stream(self.rt.dev)
@@ -376,6 +394,8 @@ class Trainer:
         # a real forward/backward, so the BN moving statistics it updated are put back
         state_backup = rt.state.clone()
         self._fwd_bwd()
+        if self.replicas > 1:     # SAVE only writes the (empty) state_base
+            rt.replica_accumulate(rt.REPLICA_SAVE, self._acc_bufs, 0, rt.plan.param_elems, self.replicas)
         torch.cuda.synchronize()
         rt.state.copy_(state_backup)
         s = torch.cuda.Stream(rt.dev)
@@ -398,8 +418,36 @@ class Trainer:
                 with torch.cuda.graph(g, stream=s):
                     fn()
                 graphs.append(g)
+            for key in self._accumulate_variants():
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, stream=s):
+                    rt.replica_accumulate(key[0], self._acc_bufs, key[1], key[2], self.replicas)
+                self._acc_graphs[key] = g
         torch.cuda.current_stream(rt.dev).wait_stream(s)
         self._graphs = graphs
+
+    def _accumulate_variants(self):
+        """(phase, lo, hi) of every accumulate call of a global step: none with one replica; SAVE, FIRST and
+        MIDDLE over the whole gradient buffer; LAST over it, or per gradient bucket with data parallelism."""
+        if self.replicas == 1:
+            return []
+        n, rt = self.rt.plan.param_elems, self.rt
+        last = [(0, n)] if self.world == 1 else [(lo, hi) for lo, hi, _ in self._buckets]
+        return [(rt.REPLICA_SAVE, 0, n), (rt.REPLICA_FIRST, 0, n), (rt.REPLICA_MIDDLE, 0, n)] + \
+            [(rt.REPLICA_LAST, lo, hi) for lo, hi in last]
+
+    def _accumulate(self, phase, lo, hi):
+        if self.use_graph:
+            self._acc_graphs[(phase, lo, hi)].replay()
+        else:
+            self.rt.replica_accumulate(phase, self._acc_bufs, lo, hi, self.replicas)
+
+    def _phase(self, r):
+        """The accumulate phase after micro-step r (None with one replica)."""
+        rt = self.rt
+        if self.replicas == 1:
+            return None
+        return rt.REPLICA_FIRST if r == 0 else (rt.REPLICA_LAST if r == self.replicas - 1 else rt.REPLICA_MIDDLE)
 
     def _fwd_bwd(self):
         rt = self.rt
@@ -413,8 +461,9 @@ class Trainer:
         stream; the following train_step(None, None) consumes them.  Lets the PCIe transfer of
         step i+1 overlap the compute of step i."""
         if self._stage_imgs is None:
-            self._stage_imgs = torch.empty_like(self.images_buf)
-            self._stage_labs = torch.empty_like(self.labels_buf)
+            n = self.replicas * self.input_batch
+            self._stage_imgs = self.images_buf.new_empty((n,) + tuple(self.images_buf.shape[1:]))
+            self._stage_labs = self.labels_buf.new_empty((n,))
         cs = self._copy_stream
         # the staging buffers may still be read by the previous step's device-side copy (and only
         # by that: waiting for the whole main stream would serialise the transfer behind the step)
@@ -432,9 +481,10 @@ class Trainer:
         """images fp32 [input_batch,H,W,3] and int32 labels [input_batch] (pinned host or device),
         or None to consume the batch given to prefetch().  teacher_logits fp32 [input_batch, classes]
         when kd_temp > 0 (the second half of the reference's KD label tensor).  keep_prob overrides
-        the DropBlock schedule for this step.
-        Returns the device tensor [cross_entropy, l2_loss(, kd_loss)] of this replica (read it with
-        .tolist() -- that read is the only host sync of the step)."""
+        the DropBlock schedule for this step.  With R = replicas_per_device > 1, images, labels and
+        teacher_logits hold R * input_batch rows, replica-major, and lam1 / lam2 are [R, input_batch / 2].
+        Returns the device tensor [cross_entropy, l2_loss(, kd_loss)] of this process (the mean over its
+        replicas; read it with .tolist() -- that read is the only host sync of the step)."""
         rt = self.rt
         if images is None:
             if self._staged is None:
@@ -442,12 +492,19 @@ class Trainer:
             torch.cuda.current_stream(rt.dev).wait_event(self._staged)
             self._staged = None
             images, labels = self._stage_imgs, self._stage_labs
-        self.images_buf.copy_(images, non_blocking=True)
-        self.labels_buf.copy_(labels, non_blocking=True)
-        if images is self._stage_imgs:
-            self._consumed = torch.cuda.Event()
-            self._consumed.record(torch.cuda.current_stream(rt.dev))
-        return self._step(lam1, lam2, teacher_logits, keep_prob)
+        n = self.input_batch
+        if self.replicas > 1 and (images.shape[0] != self.replicas * n or labels.shape[0] != self.replicas * n):
+            raise ValueError("train_step: images and labels need %d x %d rows, got %d and %d"
+                             % (self.replicas, n, images.shape[0], labels.shape[0]))
+
+        def load(r):
+            rows = slice(r * n, (r + 1) * n)
+            self.images_buf.copy_(images[rows] if self.replicas > 1 else images, non_blocking=True)
+            self.labels_buf.copy_(labels[rows] if self.replicas > 1 else labels, non_blocking=True)
+            if images is self._stage_imgs and r == self.replicas - 1:
+                self._consumed = torch.cuda.Event()
+                self._consumed.record(torch.cuda.current_stream(rt.dev))
+        return self._step(load, lam1, lam2, teacher_logits, keep_prob)
 
     def train_step_cropped(self, desc, labels, mean, lam1=None, lam2=None, teacher_logits=None, keep_prob=None,
                            augment=None):
@@ -457,34 +514,51 @@ class Trainer:
         checked by the caller); labels int32 [input_batch]; the rest as train_step.
         augment: None, or a CUDA uint8 tensor of input_batch 88-byte AutoAugment descriptors
         (autoaugment.AUTOAUG_DESC_DTYPE, checked by the caller with check_autoaugment_descriptors); then the
-        images come from acnn_set_images_augmented instead, through a work buffer allocated on first use."""
-        if augment is None:
-            self.rt.set_images_cropped(desc, mean)
-        else:
-            if self._aug_work is None:
-                b, s = self.images_buf.shape[0], self.images_buf.shape[1]
-                self._aug_work = torch.empty(self.rt.lib.acnn_autoaugment_work_bytes(b, s), dtype=torch.uint8,
-                                             device=self.rt.dev)
-            self.rt.set_images_augmented(desc, augment, self._aug_work, mean)
-        self.labels_buf.copy_(labels, non_blocking=True)
-        return self._step(lam1, lam2, teacher_logits, keep_prob)
+        images come from acnn_set_images_augmented instead, through a work buffer allocated on first use.
+        With R = replicas_per_device > 1, desc, labels, augment and teacher_logits hold R * input_batch rows,
+        replica-major, and lam1 / lam2 are [R, input_batch / 2]."""
+        n, R = self.input_batch, self.replicas
+        if R > 1 and (desc.numel() != 32 * R * n or labels.shape[0] != R * n
+                      or (augment is not None and augment.numel() != 88 * R * n)):
+            raise ValueError("train_step_cropped: desc, labels (and augment) need %d x %d rows" % (R, n))
+        if augment is not None and self._aug_work is None:
+            b, s = self.images_buf.shape[0], self.images_buf.shape[1]
+            self._aug_work = torch.empty(self.rt.lib.acnn_autoaugment_work_bytes(b, s), dtype=torch.uint8,
+                                         device=self.rt.dev)
 
-    def _step(self, lam1, lam2, teacher_logits, keep_prob):
-        rt = self.rt
+        def rows(t, width, r):
+            return t[r * n * width:(r + 1) * n * width] if R > 1 else t
+
+        def load(r):
+            if augment is None:
+                self.rt.set_images_cropped(rows(desc, 32, r), mean)
+            else:
+                self.rt.set_images_augmented(rows(desc, 32, r), rows(augment, 88, r), self._aug_work, mean)
+            self.labels_buf.copy_(rows(labels, 1, r), non_blocking=True)
+        return self._step(load, lam1, lam2, teacher_logits, keep_prob)
+
+    def _micro_inputs(self, r, lam1, lam2, teacher_logits):
+        """The mixup lambdas and teacher logits of micro-step r (drawn from self.rng when not given)."""
+        R, n = self.replicas, self.input_batch
+
+        def lam(given, buf):
+            v = self.rng.beta(0.2, 0.2, n // 2).astype(np.float32) if given is None \
+                else torch.as_tensor(given).reshape(R, n // 2)[r]
+            buf.copy_(torch.as_tensor(v, dtype=torch.float32), non_blocking=True)
         if self.mixup_type:
-            n = self.input_batch // 2
-            if lam1 is None:
-                lam1 = torch.from_numpy(self.rng.beta(0.2, 0.2, n).astype(np.float32))
-            self.lam1_buf.copy_(torch.as_tensor(lam1, dtype=torch.float32), non_blocking=True)
+            lam(lam1, self.lam1_buf)
             if self.mixup_type == 2:
-                if lam2 is None:
-                    lam2 = torch.from_numpy(self.rng.beta(0.2, 0.2, n).astype(np.float32))
-                self.lam2_buf.copy_(torch.as_tensor(lam2, dtype=torch.float32), non_blocking=True)
+                lam(lam2, self.lam2_buf)
         if self.kd_temp > 0:
-            if teacher_logits is None:
-                raise ValueError("kd_temp > 0: train_step needs teacher_logits")
-            self.teacher_buf.copy_(torch.as_tensor(teacher_logits, dtype=torch.float32),
-                                   non_blocking=True)
+            t = torch.as_tensor(teacher_logits, dtype=torch.float32)
+            self.teacher_buf.copy_(t[r * n:(r + 1) * n] if R > 1 else t, non_blocking=True)
+
+    def _step(self, load, lam1, lam2, teacher_logits, keep_prob):
+        rt = self.rt
+        if self.kd_temp > 0 and teacher_logits is None:
+            raise ValueError("kd_temp > 0: train_step needs teacher_logits")
+        if self.kd_temp > 0 and self.replicas > 1 and teacher_logits.shape[0] != self.replicas * self.input_batch:
+            raise ValueError("train_step: teacher_logits need %d x %d rows" % (self.replicas, self.input_batch))
         lr = self.learning_rate_fn(self.global_step)
         slot = self.global_step % len(self._hp_ring)
         if self._hp_events[slot] is not None:
@@ -493,7 +567,7 @@ class Trainer:
         hp[0] = lr
         hp[1] = self.p["momentum"]
         hp[2] = self.p["weight_decay"]
-        hp[3] = 1.0 / (self.world * self.loss_scale)
+        hp[3] = 1.0 / (self.world * self.replicas * self.loss_scale)
         if keep_prob is None:
             keep_prob = self.keep_prob_fn(self.global_step) if self.keep_prob_fn else 1.0
         hp[4] = keep_prob
@@ -502,15 +576,24 @@ class Trainer:
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(rt.dev))
         self._hp_events[slot] = ev
-        if self.use_graph and self._graphs is None:
-            self._capture()
-        if self.world == 1:
-            if self.use_graph:
-                self._graphs[0].replay()
+        for r in range(self.replicas):
+            load(r)
+            self._micro_inputs(r, lam1, lam2, teacher_logits)
+            if r == 0:
+                if self.use_graph and self._graphs is None:
+                    self._capture()
+                if self.replicas > 1:
+                    self._accumulate(rt.REPLICA_SAVE, 0, rt.plan.param_elems)
+            phase = self._phase(r)
+            if self.world == 1:
+                if self.use_graph:
+                    self._graphs[0].replay()
+                else:
+                    self._fwd_bwd()
+                if phase is not None:
+                    self._accumulate(phase, 0, rt.plan.param_elems)
             else:
-                self._fwd_bwd()
-        else:
-            self._fwd_bwd_allreduce()
+                self._fwd_bwd_allreduce(phase)
         if self.use_graph:
             self._graphs[-1].replay()
         else:
@@ -528,12 +611,15 @@ class Trainer:
         updates are MEAN-aggregated (official/utils/misc/distribution_utils.py:24-45)."""
         dp.average_moving_statistics(self.rt.state, self.world)
 
-    def _fwd_bwd_allreduce(self):
+    def _fwd_bwd_allreduce(self, phase=None):
         """forward + backward with the gradient all-reduce overlapped: the backward is cut into
         segments (each its own CUDA graph), and as soon as a segment has produced the last gradient
         of a bucket that bucket is all-reduced asynchronously on NCCL's stream while the next
-        segment computes (assembled_cnn_b200/dp.py)."""
+        segment computes (assembled_cnn_b200/dp.py).  With several replicas per device (phase = the
+        accumulate phase of this micro-step) only the last micro-step all-reduces, each bucket right
+        after its LAST accumulation; the earlier ones accumulate the whole buffer after the backward."""
         rt = self.rt
+        reduce = phase is None or phase == rt.REPLICA_LAST
         works, k = [], 0
         for ev in dp.schedule(self._buckets, self._segments):
             if ev[0] == "run":
@@ -544,10 +630,14 @@ class Trainer:
                         rt.run_forward()
                     rt.run(rt.plan.backward[ev[1]:ev[2]])
                 k += 1
-            else:
+            elif reduce:
+                if phase is not None:
+                    self._accumulate(phase, ev[1], ev[2])
                 works.append(dp.all_reduce_bucket(rt.grads, ev[1], ev[2], async_op=True))
         for w in works:
             w.wait()            # stream-level wait: the update runs after every bucket
+        if not reduce:
+            self._accumulate(phase, 0, rt.plan.param_elems)
 
 
 _TRAINERS = {}
@@ -1604,11 +1694,12 @@ class _TrainFeed(StagingRing):
     """The training input's staging ring: per step, the crop windows packed into a growable pinned uint8
     buffer with one acnn_crop_desc each, the labels and (KD) the teacher logits, copied to one of two
     device slots on the copy stream while the previous step computes; `step` makes the images on the device
-    (Trainer.train_step_cropped) and runs the training step."""
+    (Trainer.train_step_cropped) and runs the training step.  With several replicas per device a staged batch
+    holds the replicas' micro-batches one after another (replicas_per_device x input_batch examples)."""
 
     def __init__(self, trainer, kd):
         self.tr, dev = trainer, trainer.rt.dev
-        n, nc = trainer.input_batch, trainer.model.num_classes
+        n, nc = trainer.replicas * trainer.input_batch, trainer.model.num_classes
         i32, f32 = dict(dtype=torch.int32), dict(dtype=torch.float32)
         host = [[None, torch.zeros(n, **i32).pin_memory(), torch.zeros(32 * n, dtype=torch.uint8).pin_memory(),
                  torch.zeros(n, nc, **f32).pin_memory() if kd else None] for _ in range(self.RING)]
@@ -1618,8 +1709,8 @@ class _TrainFeed(StagingRing):
         super().__init__(dev, host, slots)
 
     def stage(self, windows, labels, teacher_logits=None):
-        """`windows` input_batch (uint8 [h, w, 3] array, flip) pairs, `labels` ints, `teacher_logits` float32
-        [input_batch, num_classes] with KD."""
+        """`windows` replicas x input_batch (uint8 [h, w, 3] array, flip) pairs, `labels` ints, `teacher_logits`
+        float32 [replicas x input_batch, num_classes] with KD."""
         def place(h, slot):
             self.host[h][0], self.slots[slot][0], addrs = pack_u8(self.host[h][0], self.slots[slot][0],
                                                                  [a for a, _ in windows], self.dev)
@@ -1627,7 +1718,7 @@ class _TrainFeed(StagingRing):
         self._stage(place, labels, teacher_logits)
 
     def stage_encoded(self, items, labels, teacher_logits=None):
-        """As stage, from input_batch (encoded JPEG bytes, (y, x, h, w) window, flip) triples: the windows are
+        """As stage, from replicas x input_batch (encoded JPEG bytes, (y, x, h, w) window, flip) triples: the windows are
         decoded on the copy stream (jpeg.JpegDecoder, one per slot; PIL's decode_rgb for the images the
         device does not decode)."""
         def place(h, slot):
@@ -1694,7 +1785,8 @@ def cycle_schedule(p, epochs_between_evals, cur_epoch):
 
 
 def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_threshold=None, max_train_steps=None,
-                       image_size=224, seed=0, use_cuda_graph=True, num_workers=None, export_dir=None, **flags):
+                       image_size=224, seed=0, use_cuda_graph=True, num_workers=None, export_dir=None,
+                       replicas_per_device=1, **flags):
     """resnet_main's train-and-evaluate loop (nets/run_loop_classification.py:389-489) over the TFRecord
     shards data_dir/train_regex (training) and data_dir/val_regex (evaluation).  `flags` are hparams
     names (params_from_flags); epochs_between_evals, stop_threshold and max_train_steps are the run loop's
@@ -1726,7 +1818,13 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     servable (batch val_batch_size, val_regex, zeroshot_eval), as nets/run_loop_classification.py:494-495.
     export_only runs no cycle (unless eval_only or train_epochs = 0 ask for an evaluation, as the reference's
     order has it) and exports the latest checkpoint of model_dir; it needs export_dir and a checkpoint, both
-    checked before any GPU work.  Returns the list of the cycles' evaluation results (the recall dicts with
+    checked before any GPU work.
+
+    replicas_per_device = R runs R data-parallel replicas on each device (Trainer's micro-steps): the reference's
+    --num_gpus=N is world * R = N.  Replica q = rank * R + r reads what rank q of a world * R run reads
+    (imagenet_train.replica_streams, replica_mixup_lambdas); each global step stages the R micro-batches together.
+    R >= 1 and batch_size divisible by world * R are checked before any GPU work.  The evaluation runs at the
+    per-replica batch.  Returns the list of the cycles' evaluation results (the recall dicts with
     zeroshot_eval)."""
     from concurrent.futures import ThreadPoolExecutor
     from . import imagenet_train as it
@@ -1755,6 +1853,8 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     dist = torch.distributed.is_initialized()
     world = torch.distributed.get_world_size() if dist else 1
     rank = torch.distributed.get_rank() if dist else 0
+    R = check_replicas_per_device(replicas_per_device)
+    per_device_batch_size(p["batch_size"], world * R)
     kd = float(p["kd_temp"] or 0) > 0
     records, counts = it.read_train_records(it.train_files(data_dir, p["train_regex"]), ds["num_classes"], kd)
     num_images = len(records)
@@ -1771,7 +1871,8 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                   bl_beta=p["bl_beta"], dtype=p["dtype"], loss_type=p["cls_loss_type"], seed=seed,
                   device=str(dev))
     model.use_resnet_d = bool(p["use_resnet_d"])
-    trainer = Trainer(model, p, size, size, use_cuda_graph=use_cuda_graph, num_images=num_images)
+    trainer = Trainer(model, p, size, size, use_cuda_graph=use_cuda_graph, num_images=num_images,
+                      replicas_per_device=R)
     ckpt = latest_checkpoint(model_dir) if os.path.isdir(model_dir) else None
     if ckpt:
         restore(model, ckpt, trainer)
@@ -1797,14 +1898,18 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
         for ci, epochs in enumerate(schedule):
             c = first + ci
             if epochs:
-                stream = it.CycleStream(counts, seed, c, epochs * (2 if trainer.mixup_type == 1 else 1),
-                                        shuffle_buffer, trainer.input_batch, world, rank)
-                steps = stream.steps if max_train_steps is None else min(stream.steps, max_train_steps)
+                streams = it.replica_streams(counts, seed, c, epochs * (2 if trainer.mixup_type == 1 else 1),
+                                             shuffle_buffer, trainer.input_batch, world, rank, R)
+                n_steps = streams[0].steps
+                steps = n_steps if max_train_steps is None else min(n_steps, max_train_steps)
 
                 def window(pos_r, c=c):
                     pos, r = pos_r
                     return it.encoded_window(*records[r][:3], seed, c, pos, p["training_random_crop"])
-                read = read_ahead(pool, map(stream.records, range(steps)), window)
+
+                def step_records(t):
+                    return [pr for s in streams for pr in s.records(t)]
+                read = read_ahead(pool, map(step_records, range(steps)), window)
 
                 def stage():
                     recs, items = next(read)
@@ -1816,8 +1921,8 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                 for t in range(steps):
                     lam1 = lam2 = None
                     if trainer.mixup_type:
-                        lam = it.mixup_lambdas(seed, trainer.global_step, rank, 2 * n_lam).reshape(2, n_lam)
-                        lam1, lam2 = lam[0], (lam[1] if trainer.mixup_type == 2 else None)
+                        lam = it.replica_mixup_lambdas(seed, trainer.global_step, rank, R, 2 * n_lam).reshape(R, 2, n_lam)
+                        lam1, lam2 = lam[:, 0], (lam[:, 1] if trainer.mixup_type == 2 else None)
                     feed.step(lam1, lam2)
                     if t + 1 < steps:
                         stage()

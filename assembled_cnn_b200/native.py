@@ -97,6 +97,7 @@ PROTOTYPES = {
     "acnn_backward_range": (_i, [_vp, _i, _i, _vp]),
     "acnn_sgd_step": (_i, [_vp, _vp]),
     "acnn_step": (_i, [_vp, _vp]),
+    "acnn_replica_accumulate_model": (_i, [_vp, _i, _vp, _vp, _vp, _i64, _i64, _i, _vp]),
     "acnn_run_ops": (_i, [_vp, _i, _i, _i, _vp]),
     "acnn_clear_step_buffers": (_i, [_vp, _vp]),
     "acnn_op_kind": (C.c_char_p, [_vp, _i, _i]),
@@ -440,3 +441,10 @@ class NativeRuntime(_runtime_base()):
 
     def run_step(self):
         _lib.check(self.lib.acnn_step(self.model.handle, self.stream), "acnn_step")
+
+    def replica_accumulate(self, phase, bufs, lo, hi, replicas):
+        """acnn_replica_accumulate_model over this handle's grads [lo, hi), state and loss."""
+        acc_g, base, acc_s = bufs
+        _lib.check(self.lib.acnn_replica_accumulate_model(self.model.handle, phase, acc_g.data_ptr(), base.data_ptr(),
+                                                          acc_s.data_ptr(), lo, hi, replicas, self.stream),
+                   "acnn_replica_accumulate_model")

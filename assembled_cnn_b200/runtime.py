@@ -341,6 +341,36 @@ class Runtime:
         self.run(self.plan.backward)
         self.run(self.plan.update)
 
+    # ---------------------------------------------------------------- several replicas per device
+    REPLICA_SAVE, REPLICA_FIRST, REPLICA_MIDDLE, REPLICA_LAST = 0, 1, 2, 3     # acnn.h ACNN_REPLICA_*
+    REPLICA_LOSS_FLOATS = 4                                                    # acnn_model.h
+
+    def replica_buffers(self):
+        """The device accumulators of several replicas per device: (acc_grads [param_elems], state_base
+        [state_elems], acc_state [state_elems + REPLICA_LOSS_FLOATS], the tail summing the loss)."""
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        ns = self.plan.state_elems
+        return (torch.zeros(self.plan.param_elems, **f32), torch.zeros(max(ns, 1), **f32),
+                torch.zeros(ns + self.REPLICA_LOSS_FLOATS, **f32))
+
+    def replica_accumulate(self, phase, bufs, lo, hi, replicas):
+        """acnn_replica_accumulate_model's phase on this runtime's grads [lo, hi), state and loss (the state and
+        the loss with the range that starts at 0), through the op-level acnn_replica_accumulate."""
+        acc_g, base, acc_s = bufs
+        ns, scale, st = self.plan.state_elems, 1.0 / replicas, self.stream
+        if phase == self.REPLICA_SAVE:
+            _lib.check(self.lib.acnn_replica_accumulate(phase, None, None, base.data_ptr(), None, self.state.data_ptr(),
+                                                        0, 0, ns, scale, st), "acnn_replica_accumulate")
+            return
+        with_state = lo == 0
+        _lib.check(self.lib.acnn_replica_accumulate(phase, acc_g.data_ptr(), self.grads.data_ptr(), base.data_ptr(),
+                                                    acc_s.data_ptr(), self.state.data_ptr(), lo, hi,
+                                                    ns if with_state else 0, scale, st), "acnn_replica_accumulate")
+        if with_state and "loss" in self.plan.meta:
+            _lib.check(self.lib.acnn_replica_accumulate(
+                phase, None, None, None, acc_s.data_ptr() + 4 * ns, self.slot_view(self.plan.meta["loss"]).data_ptr(),
+                0, 0, self.REPLICA_LOSS_FLOATS, scale, st), "acnn_replica_accumulate")
+
     def capture(self, train=True):
         """Capture one full step (or forward) into a CUDA graph; inputs are read from the static
         input buffers (plan.meta['images'] ...), hyper-parameters from the device `hp` vector."""

@@ -412,6 +412,26 @@ int acnn_sgd_momentum(float* w, const float* grad, float* acc, int64_t n,
 int acnn_sgd_scratch_floats(void);
 int acnn_fill_zero(void* p, int64_t bytes, void* stream);
 
+/* Several data-parallel replicas run one after another on one device (micro-steps r = 0 .. R-1 of one
+ * global step, each a full forward + backward from the same moving statistics).  One fused pass per
+ * micro-step over the gradient range [lo, hi) (grads and acc_grads at the same offsets) and the first
+ * n_state floats of the state buffers, in fp32, element by element:
+ *   SAVE   (before micro-step 0)        state_base = state; the gradients are not touched
+ *   FIRST  (after micro-step 0)         acc = g;        acc_state = state;        state = state_base
+ *   MIDDLE (after micro-steps 1 .. R-2) acc = acc + g;  acc_state = acc_state + state;  state = state_base
+ *   LAST   (after micro-step R-1)       g = acc + g;    state = (acc_state + state) * state_scale
+ * so the gradient ends as ((g0 + g1) + g2) + ... and, with state_scale = 1/R, the state as the mean of the
+ * R updated copies summed in replica order.  state_base may be NULL outside SAVE: the state is then left
+ * as it is (a buffer the next micro-step clears itself, such as the loss).  No atomics; any alignment
+ * (16-byte vectors where the pointers of a part share their alignment).  Capturable. */
+#define ACNN_REPLICA_SAVE 0
+#define ACNN_REPLICA_FIRST 1
+#define ACNN_REPLICA_MIDDLE 2
+#define ACNN_REPLICA_LAST 3
+int acnn_replica_accumulate(int phase, float* acc_grads, float* grads, float* state_base, float* acc_state,
+                            float* state, int64_t lo, int64_t hi, int64_t n_state, float state_scale,
+                            void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Zero-shot retrieval (metric/recall_metric.py:98-123: l2_normalize / tf_simple_pairwise_distance,
  * MatMul and tf.nn.top_k over the query x index similarity matrix, which is never materialised)

@@ -213,6 +213,19 @@ int acnn_backward(acnn_model* m, void* stream);  /* all gradients into the flat 
 int acnn_backward_range(acnn_model* m, int first, int last, void* stream);
 int acnn_sgd_step(acnn_model* m, void* stream);  /* weight decay + momentum + L2 loss, from hp */
 int acnn_step(acnn_model* m, void* stream);      /* forward + loss + backward + sgd_step */
+/* Several data-parallel replicas per device (acnn_replica_accumulate of acnn.h over this handle's grads,
+ * state and loss): a global step of R = `replicas` replicas is
+ *   SAVE; for r in 0 .. R-1: forward, loss, backward, then FIRST (r = 0) | MIDDLE | LAST (r = R-1); sgd_step
+ * with hp[3] (grad_scale) = 1 / (R * loss_scale).  The gradient part covers [lo, hi) of grads; the moving
+ * statistics and the loss go with the call whose range starts at lo = 0, so a data-parallel host can close
+ * each gradient bucket right before its all-reduce.  After LAST: grads = g0 + g1 + ... in replica order, state
+ * and loss = the mean of the R copies (sum in replica order, times 1/R in fp32).  SAVE ignores lo / hi.
+ * Caller-owned device accumulators: acc_grads param_elems floats (same offsets as grads), state_base
+ * state_elems floats, acc_state state_elems + ACNN_REPLICA_LOSS_FLOATS floats (the tail sums the loss).
+ * They hold nothing between global steps. */
+#define ACNN_REPLICA_LOSS_FLOATS 4
+int acnn_replica_accumulate_model(acnn_model* m, int phase, float* acc_grads, float* state_base, float* acc_state,
+                                  int64_t lo, int64_t hi, int replicas, void* stream);
 /* Any op range of a phase (0 forward incl. loss ops, 1 backward, 2 update): profiling / tests.
  * Does not clear the step buffers (acnn_clear_step_buffers does). */
 int acnn_run_ops(acnn_model* m, int phase, int first, int last, void* stream);
