@@ -303,6 +303,50 @@ def classify_rows(logits, labels, n_valid=None, k=5, label_smoothing=0.0, out=No
     return out
 
 
+# The layout of struct acnn_train_metrics (include/acnn.h).
+TRAIN_METRICS_DTYPE = np.dtype([("rows", "<i8"), ("top1", "<i8"), ("top5", "<i8"), ("bin_count", "<i8", 10),
+                                ("bin_correct", "<i8", 10), ("bin_conf", "<f8", 10), ("step_rows", "<i8"),
+                                ("step_conf", "<f8")])
+
+
+def train_metrics_buffer(device):
+    """A zeroed device accumulator for train_metrics_accumulate (uint8, TRAIN_METRICS_DTYPE's size)."""
+    return torch.zeros(TRAIN_METRICS_DTYPE.itemsize, dtype=torch.uint8, device=device)
+
+
+def train_metrics_accumulate(rows, labels, acc, n=None, step_begin=True):
+    """acnn_train_metrics_accumulate on the current stream: adds the rows r < n (default: all) of classify_rows'
+    (pred, conf, hit_k, ce) `rows` (k = 5) and the CUDA int32 `labels` to the accumulator `acc`
+    (train_metrics_buffer); step_begin clears its per-step fields first."""
+    from . import _lib
+    lib = _lib.load()
+    pred, conf, hit = rows[:3]
+    n = pred.numel() if n is None else int(n)
+    for t, dt in ((pred, torch.int32), (conf, torch.float32), (hit, torch.int32), (labels, torch.int32)):
+        if t.dtype != dt or t.numel() < n or not t.is_contiguous() or not t.is_cuda:
+            raise ValueError("pred, conf, hit_k and labels must be contiguous CUDA (int32, float32, int32, int32) "
+                             "tensors of at least n = %d values" % n)
+    if acc.dtype != torch.uint8 or acc.numel() != TRAIN_METRICS_DTYPE.itemsize or not acc.is_cuda:
+        raise ValueError("acc must be a CUDA uint8 tensor of %d bytes (train_metrics_buffer)" % TRAIN_METRICS_DTYPE.itemsize)
+    stream = torch.cuda.current_stream(acc.device).cuda_stream
+    _lib.check(lib.acnn_train_metrics_accumulate(pred.data_ptr(), conf.data_ptr(), hit.data_ptr(), labels.data_ptr(),
+                                                 n, int(bool(step_begin)), acc.data_ptr(), stream),
+               "acnn_train_metrics_accumulate")
+
+
+def train_metric_values(record, mixup=False):
+    """The training summaries of an accumulator read back to the host (a TRAIN_METRICS_DTYPE record):
+    sup/pred_prob = the step's mean confidence and, without mixup, train_accuracy, train_accuracy_top_5 and
+    train_ece over the rows since the last reset (with mixup the labels are mixed and they are not defined)."""
+    out = {"sup/pred_prob": float(record["step_conf"]) / max(int(record["step_rows"]), 1)}
+    if not mixup:
+        rows = max(int(record["rows"]), 1)
+        out["train_accuracy"] = int(record["top1"]) / rows
+        out["train_accuracy_top_5"] = int(record["top5"]) / rows
+        out["train_ece"] = ece_from_bins(record["bin_count"], record["bin_correct"], record["bin_conf"])
+    return out
+
+
 def predict_rows(logits, n_valid=None, out=None):
     """acnn_predict_rows on the current stream, for the rows r < n_valid of `logits` (CUDA fp32 [B, NC], rows
     may be strided, as a model's logits view is): the PREDICT dict of nets/run_loop_classification.py:126-130,
@@ -337,6 +381,26 @@ def predict_rows(logits, n_valid=None, out=None):
     return out
 
 
+ECE_EPS = 1e-7
+
+
+def ece_thresholds(num_thresholds=10):
+    """The bin thresholds of metric/ece_metric.py as Python floats: [-1e-7, 1/n, ..., (n-1)/n, 1 + 1e-7]
+    (the bins compare float32 confidences with their float32 roundings)."""
+    return [0.0 - ECE_EPS] + [(i + 1) * 1.0 / num_thresholds for i in range(num_thresholds - 1)] + [1.0 + ECE_EPS]
+
+
+def ece_from_bins(count, correct, conf_sum):
+    """metric/ece_metric.py's ECE from per-bin counts, correct counts and confidence sums, in float64: acc and
+    confidence per bin over (1e-7 + count), weighted by count / total.  With no row in any bin it is 0 / 0,
+    NaN as in the reference."""
+    cnt = np.asarray(count).astype(np.float64)
+    acc = np.asarray(correct) / (ECE_EPS + cnt)
+    avg = np.asarray(conf_sum, np.float64) / (ECE_EPS + cnt)
+    with np.errstate(invalid="ignore"):
+        return float((cnt / cnt.sum() * np.abs(acc - avg)).sum())
+
+
 def classification_result(pred, conf, hit_k, ce, labels, batch_sizes, num_thresholds=10):
     """The eval metrics of nets/run_loop_classification.py:141-234 from the per-row results of a whole
     evaluation (numpy arrays, rows in evaluation order), in float64:
@@ -355,15 +419,10 @@ def classification_result(pred, conf, hit_k, ce, labels, batch_sizes, num_thresh
     if not (len(pred) == len(conf) == len(hit) == len(ce) == n) or sum(sizes) != n or n == 0 or min(sizes) < 1:
         raise ValueError("classification_result: per-row arrays of one length, batch sizes summing to it")
     correct = pred == labels
-    eps = 1e-7
-    th = [0.0 - eps] + [(i + 1) * 1.0 / num_thresholds for i in range(num_thresholds - 1)] + [1.0 + eps]
-    th = np.asarray(th, np.float32)
+    th = np.asarray(ece_thresholds(num_thresholds), np.float32)
     inb = (conf[None, :] > th[:-1, None]) & (conf[None, :] <= th[1:, None])
-    cnt = inb.sum(1).astype(np.float64)
-    acc = (inb & correct[None, :]).sum(1) / (eps + cnt)
-    avg = (np.where(inb, conf[None, :].astype(np.float64), 0.0)).sum(1) / (eps + cnt)
-    with np.errstate(invalid="ignore"):      # no row in any bin: 0 / 0, NaN as in the reference
-        ece = float((cnt / cnt.sum() * np.abs(acc - avg)).sum())
+    ece = ece_from_bins(inb.sum(1), (inb & correct[None, :]).sum(1),
+                        (np.where(inb, conf[None, :].astype(np.float64), 0.0)).sum(1))
     bounds = np.cumsum([0] + sizes)
     batch_ce = [ce[a:b].mean() for a, b in zip(bounds[:-1], bounds[1:])]
     return {"accuracy": float(correct.mean()), "accuracy_top_5": float(hit.mean()), "ece": ece,

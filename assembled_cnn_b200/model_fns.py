@@ -307,10 +307,18 @@ class Trainer:
     forward + backward of batch_size / (world * R) examples from the same moving statistics, as R GPUs of a
     MirroredStrategy run would: the gradients are summed in replica order, the updated moving statistics and
     the reported loss averaged (acnn_replica_accumulate), then one SGD step with grad_scale 1 / (world * R *
-    loss_scale).  The reference's --num_gpus=N is world * replicas_per_device = N."""
+    loss_scale).  The reference's --num_gpus=N is world * replicas_per_device = N.
+
+    train_metrics=True accumulates the training summaries' metrics on the device (acnn_classify_rows and
+    acnn_train_metrics_accumulate after every micro-step's backward, on the current stream; no host read):
+    the top-1 / top-5 hits and the ECE bins since reset_train_metrics(), and the step's rows and confidence
+    sum (`train_metrics`, a TRAIN_METRICS_DTYPE record).  Only rank 0 accumulates, over the rows of all its
+    micro-steps -- the whole global batch with one process.  Other ranks launch nothing and nothing is
+    all-reduced, so summaries never add a collective to the step.  With mixup the labels are mixed and only
+    the step's confidence is meaningful."""
 
     def __init__(self, model: Model, params: dict, height=224, width=224, *, use_cuda_graph=True,
-                 lam_seed=7, num_images=None, replicas_per_device=1):
+                 lam_seed=7, num_images=None, replicas_per_device=1, train_metrics=False):
         """num_images: training images per epoch for the LR and keep-prob schedules (default: the
         dataset's data_config count)."""
         p = params
@@ -381,6 +389,33 @@ class Trainer:
         self._stage_imgs = None
         self._stage_labs = None
         self._aug_work = None
+        self._metrics = self._metric_rows = None
+        rank = torch.distributed.get_rank() if torch.distributed.is_initialized() else 0
+        if train_metrics and rank == 0:
+            from .metrics import train_metrics_buffer
+            self._metrics = train_metrics_buffer(self.rt.dev)
+            self._metric_rows = tuple(torch.empty(self.local_batch, dtype=dt, device=self.rt.dev)
+                                      for dt in (torch.int32, torch.float32, torch.int32, torch.float32))
+
+    @property
+    def train_metrics(self):
+        """The device accumulator of the training metrics (uint8 [280], metrics.TRAIN_METRICS_DTYPE), or None
+        when this Trainer does not accumulate them."""
+        return self._metrics
+
+    def reset_train_metrics(self):
+        """Zero the accumulator, on the current stream."""
+        if self._metrics is not None:
+            self._metrics.zero_()
+
+    def _accumulate_metrics(self, r):
+        """classify_rows (k = 5) and acnn_train_metrics_accumulate on micro-step r's logits and labels, which
+        the next micro-step overwrites."""
+        from .metrics import classify_rows, train_metrics_accumulate
+        B = self.local_batch
+        logits = self.rt.t[self.rt.plan.meta["logits"]][:B, :self.model.num_classes]
+        classify_rows(logits, self.labels_buf, k=5, out=self._metric_rows)
+        train_metrics_accumulate(self._metric_rows, self.labels_buf, self._metrics, B, step_begin=r == 0)
 
     @property
     def input_batch(self):
@@ -594,6 +629,8 @@ class Trainer:
                     self._accumulate(phase, 0, rt.plan.param_elems)
             else:
                 self._fwd_bwd_allreduce(phase)
+            if self._metrics is not None:
+                self._accumulate_metrics(r)
         if self.use_graph:
             self._graphs[-1].replay()
         else:
@@ -996,7 +1033,7 @@ def _read_file(path):
 
 def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=224, label_offset=1,
                      robustness_type="ce", devices=None, use_resnet_d=None, global_step=None,
-                     use_cuda_graph=True, num_workers=None):
+                     use_cuda_graph=True, num_workers=None, summary_dir=None):
     """mce/eval_robustness.py (show_corruption_error, --robustness_type ce): the top-1 error of `model`
     on every distortion of ALEXNET_CE, pooled over data_dir/<distortion>/<severity 1..5>/<synset>/*,
     its AlexNet-normalised CE and their means.  Labels are synsets2idx[synset dir] + label_offset from
@@ -1007,15 +1044,19 @@ def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=
     (use_cuda_graph=False: the same launches, eager).  The last batch of a distortion is padded to
     batch_size and its padding rows are masked.  `devices` (default: the model's device) split the
     distortions as the reference's process() does; every device gets a replica with the model's weights.
+    With summary_dir, the mCE is written there as a scalar at global_step (0 when it is None), as
+    mce/eval_robustness.py:305-315 does; the directory is made (or refused with ValueError) before any work.
     Returns {'<distortion>': {'error', 'ce'}, ..., 'mCE', 'mCE_unnormalized'} (+ 'global_step')."""
     import threading
     from concurrent.futures import ThreadPoolExecutor
     from . import imagenet_c
     from .metrics import DISTORTIONS, CorruptionError
+    from .summary import SummaryWriter, check_summary_dir
     if robustness_type == "fr":
         raise ValueError("not yet supported ({}".format(robustness_type))
     if robustness_type != "ce":
         raise ValueError("invalid type ({})".format(robustness_type))
+    summary_dir = check_summary_dir(summary_dir)
     if use_resnet_d is None:
         use_resnet_d = getattr(model, "use_resnet_d", False)
     synsets2idx = imagenet_c.get_synsets2idx(label_file)
@@ -1064,6 +1105,12 @@ def corruption_error(model, data_dir, label_file, *, batch_size=128, image_size=
         for d, c in counts.items():
             metric.add_counts(d, c, len(work[d][0]))
     out = metric.result()
+    if summary_dir is not None:
+        w = SummaryWriter(summary_dir)
+        try:
+            w.add_scalars(global_step or 0, [("mCE", out["mCE"])])
+        finally:
+            w.close()
     if global_step is not None:
         out["global_step"] = global_step
     return out
@@ -1786,7 +1833,7 @@ def cycle_schedule(p, epochs_between_evals, cur_epoch):
 
 def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_threshold=None, max_train_steps=None,
                        image_size=224, seed=0, use_cuda_graph=True, num_workers=None, export_dir=None,
-                       replicas_per_device=1, **flags):
+                       replicas_per_device=1, save_summary_steps=None, **flags):
     """resnet_main's train-and-evaluate loop (nets/run_loop_classification.py:389-489) over the TFRecord
     shards data_dir/train_regex (training) and data_dir/val_regex (evaluation).  `flags` are hparams
     names (params_from_flags); epochs_between_evals, stop_threshold and max_train_steps are the run loop's
@@ -1824,12 +1871,22 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     --num_gpus=N is world * R = N.  Replica q = rank * R + r reads what rank q of a world * R run reads
     (imagenet_train.replica_streams, replica_mixup_lambdas); each global step stages the R micro-batches together.
     R >= 1 and batch_size divisible by world * R are checked before any GPU work.  The evaluation runs at the
-    per-replica batch.  Returns the list of the cycles' evaluation results (the recall dicts with
-    zeroshot_eval)."""
+    per-replica batch.
+
+    save_summary_steps = N (RunConfig's save_summary_steps; None, the default, writes nothing) makes rank 0
+    write the training summaries to model_dir/events.out.tfevents.* on the first step of each cycle and every
+    N-th step after it, at the global step the step ran with, log one line per summary to the
+    "assembled_cnn_b200" logger at INFO, and write every numeric entry of each evaluation result to
+    model_dir/eval/ (summary.TrainSummaries: the metrics are accumulated on the device and read back without a
+    per-step host synchronisation).  Anything but None or an integer >= 1 raises before any GPU work.
+
+    Returns the list of the cycles' evaluation results (the recall dicts with zeroshot_eval)."""
     from concurrent.futures import ThreadPoolExecutor
     from . import imagenet_train as it
     from .checkpoint import CheckpointKeeper, latest_checkpoint, restore, save_checkpoint, warm_start
     from .imagenet_eval import eval_size
+    from .summary import SummaryWriter, TrainSummaries, check_save_summary_steps, is_summary_step, numeric_scalars
+    summary_every = check_save_summary_steps(save_summary_steps)
     p = params_from_flags(**flags)
     if p["autoaugment_type"] is not None:
         raise NotImplementedError("autoaugment_type=%r: AutoAugment is not implemented; train with "
@@ -1871,8 +1928,9 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                   bl_beta=p["bl_beta"], dtype=p["dtype"], loss_type=p["cls_loss_type"], seed=seed,
                   device=str(dev))
     model.use_resnet_d = bool(p["use_resnet_d"])
+    summarize = summary_every is not None and rank == 0
     trainer = Trainer(model, p, size, size, use_cuda_graph=use_cuda_graph, num_images=num_images,
-                      replicas_per_device=R)
+                      replicas_per_device=R, train_metrics=summarize)
     ckpt = latest_checkpoint(model_dir) if os.path.isdir(model_dir) else None
     if ckpt:
         restore(model, ckpt, trainer)
@@ -1885,10 +1943,15 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     keeper = CheckpointKeeper(model_dir, p["num_best_ckpt_to_keep"], p["keep_ckpt_every_eval"], maximize=True) \
         if rank == 0 else None
 
+    summaries = TrainSummaries(model_dir, trainer) if summarize else None
+    eval_writer = None
+
     def save():
         if rank == 0:
             save_checkpoint(os.path.join(model_dir, "model.ckpt-%d" % trainer.global_step), model, trainer)
             _prune_checkpoints(model_dir, p["keep_checkpoint_max"])
+            if summaries is not None:       # the checkpoint has read the weights: the ring has completed
+                summaries.drain()
 
     feed = _TrainFeed(trainer, kd)
     n_lam = trainer.input_batch // 2
@@ -1918,12 +1981,20 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
 
                 if steps:
                     stage()
+                if summaries is not None:
+                    summaries.begin_cycle()
+                cycle_first = trainer.global_step
                 for t in range(steps):
                     lam1 = lam2 = None
                     if trainer.mixup_type:
                         lam = it.replica_mixup_lambdas(seed, trainer.global_step, rank, R, 2 * n_lam).reshape(R, 2, n_lam)
                         lam1, lam2 = lam[:, 0], (lam[:, 1] if trainer.mixup_type == 2 else None)
-                    feed.step(lam1, lam2)
+                    step = trainer.global_step
+                    loss = feed.step(lam1, lam2)
+                    if summaries is not None:
+                        if is_summary_step(step, cycle_first, summary_every):
+                            summaries.record(loss, step, trainer.last_lr, trainer.last_keep_prob)
+                        summaries.poll()
                     if t + 1 < steps:
                         stage()
                         if save_steps > 0 and trainer.global_step % save_steps == 0:
@@ -1946,6 +2017,10 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
                         weight_decay=p["weight_decay"], global_step=trainer.global_step,
                         use_cuda_graph=use_cuda_graph, num_workers=num_workers)
                 keeper.save(res[key], model_dir)
+                if summarize:
+                    if eval_writer is None:
+                        eval_writer = SummaryWriter(os.path.join(model_dir, "eval"))
+                    eval_writer.add_scalars(res["global_step"], numeric_scalars(res))
             else:
                 res = None
             if dist:
@@ -1960,6 +2035,10 @@ def train_and_evaluate(data_dir, model_dir, *, epochs_between_evals=1, stop_thre
     finally:
         pool.shutdown(wait=True, cancel_futures=True)
     torch.cuda.current_stream(dev).synchronize()
+    if summaries is not None:
+        summaries.close()
+    if eval_writer is not None:
+        eval_writer.close()
     if export_dir is not None and rank == 0:
         binary_dir, _ = export_model(model, export_dir, preprocessing_type=p["preprocessing_type"],
                                      image_size=image_size, use_resnet_d=p["use_resnet_d"],

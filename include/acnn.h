@@ -607,6 +607,34 @@ int acnn_predict_rows(const float* logits, int B, int ld, int NC, int n_valid, i
                       float* probabilities_sigmoid, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Training-batch metrics (the training summaries of nets/run_loop_classification.py:146-227)
+ * ------------------------------------------------------------------------------------------- */
+/* Device accumulator of the training metrics (280 bytes, the layout of metrics.TRAIN_METRICS_DTYPE);
+ * zeroed by the caller.  Streaming fields, kept until the caller zeroes them again: */
+#define ACNN_ECE_BINS 10
+typedef struct acnn_train_metrics {
+  int64_t rows;                            /* rows accumulated */
+  int64_t top1;                            /* rows with pred == label (pred = -1 is wrong) */
+  int64_t top5;                            /* rows with hit_k != 0 */
+  int64_t bin_count[ACNN_ECE_BINS];        /* rows whose confidence falls in bin b */
+  int64_t bin_correct[ACNN_ECE_BINS];      /*   ... and whose pred == label */
+  double bin_conf[ACNN_ECE_BINS];          /*   the sum of their confidences */
+  /* per-step fields, cleared by the call with step_begin != 0: */
+  int64_t step_rows;
+  double step_conf;                        /* the sum of conf over the step's rows (NaN rows included) */
+} acnn_train_metrics;
+/* Adds the rows r < n of one micro-step to *m, from acnn_classify_rows' pred, conf and hit_k (k = 5) and the
+ * labels int32 [n].  Bins are (lo, hi] over the float32 thresholds [-1e-7, 0.1, ..., 0.9, 1 + 1e-7], as
+ * metrics.classification_result; a NaN confidence falls in no bin.  Counts are int64.  Every fp64 sum has one
+ * order: row r goes to lane r % 256, each lane adds its rows in ascending order to 0.0, lane partials are
+ * combined by the tree  p[i] = p[i] + p[i + s]  for s = 128, 64, ..., 1 (i < s), and the field then becomes
+ * field + p[0] (step_conf: p[0] when step_begin != 0).  One CTA, no atomics: the same bits on every replay
+ * and stream.  Capturable.  Null pointers, n < 1, m not 8-byte aligned: ACNN_ERR_INVALID before any CUDA
+ * call. */
+int acnn_train_metrics_accumulate(const int32_t* pred, const float* conf, const int32_t* hit_k, const int32_t* labels,
+                                  int n, int step_begin, acnn_train_metrics* m, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * JPEG decoding (the tf.image.decode_jpeg / PIL decode of every input pipeline), bit for bit equal to
  * libjpeg's ISLOW IDCT, fancy upsampling and YCbCr->RGB, i.e. to PIL's Image.open(b).convert("RGB").
  * Baseline and extended (SOF0 / SOF1) 8-bit Huffman JPEGs with one scan: grayscale, or 3-component
