@@ -973,18 +973,6 @@ static void set_sk_attr(const void* kern) {
 
 using namespace acnn;
 
-#define ACNN_DTYPE_OK(dt) ((dt) == ACNN_BF16 || (dt) == ACNN_F32)
-#define ACNN_BY_DTYPE(dt, ...)      \
-  do {                              \
-    if ((dt) == ACNN_F32) {         \
-      using T = float;              \
-      __VA_ARGS__;                  \
-    } else {                        \
-      using T = bf16;               \
-      __VA_ARGS__;                  \
-    }                               \
-  } while (0)
-
 template <class T>
 static void launch_bn_act(cudaStream_t st, const void* a, const float* scale_a, const float* shift_a,
                           const void* b, const float* scale_b, const float* shift_b, int b_mode,

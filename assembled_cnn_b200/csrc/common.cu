@@ -135,12 +135,12 @@ CUtensorMapSwizzle swizzle_enum(int bytes) {
 }
 
 int make_map_2d(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                int box_rows, int box_cols) {
+                int box_rows, int box_cols, CUtensorMapDataType dt) {
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base),
+  CUresult r = g_encode_tiled(m, dt, 2, const_cast<void*>(base),
                               dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                               swizzle_enum(box_cols * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -88,9 +88,11 @@ extern int g_driver_version;
 
 int load_driver_fns();
 CUtensorMapSwizzle swizzle_enum(int bytes);
-// bf16 matrix [rows][cols] (cols contiguous, row pitch ld elements); box = [box_rows][box_cols].
+// 16-bit (bf16 unless dt says fp16) matrix [rows][cols] (cols contiguous, row pitch ld elements);
+// box = [box_rows][box_cols].
 int make_map_2d(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                int box_rows, int box_cols);
+                int box_rows, int box_cols,
+                CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }

@@ -38,7 +38,7 @@ static bool is_plain(const acnn_conv_geom& g) {
 // bf16 NHWC tensor [B][H][W][C]; one load = `pixels` consecutive output pixels x `cw` channels of
 // one filter tap.  The bounding box of base pixels is [-pad_lo, dim + pad_hi - (k-1)).
 static int make_map_im2col(CUtensorMap* m, const void* base, const acnn_conv_geom& g, int cw,
-                           int pixels) {
+                           int pixels, CUtensorMapDataType dt) {
   int64_t pix, row, img;
   input_pitches(g, &pix, &row, &img);
   cuuint64_t dims[4] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.B};
@@ -46,7 +46,7 @@ static int make_map_im2col(CUtensorMap* m, const void* base, const acnn_conv_geo
   int lower[2] = {-g.pad_w_lo, -g.pad_h_lo};
   int upper[2] = {g.pad_w_hi - (g.kw - 1), g.pad_h_hi - (g.kh - 1)};
   cuuint32_t estr[4] = {1, (cuuint32_t)g.stride, (cuuint32_t)g.stride, 1};
-  CUresult r = g_encode_im2col(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base),
+  CUresult r = g_encode_im2col(m, dt, 4, const_cast<void*>(base),
                                dims, strides, lower, upper, (cuuint32_t)cw, (cuuint32_t)pixels,
                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(cw * 2),
                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -162,7 +162,7 @@ __device__ __forceinline__ int staged_offset(int r, int c) {
 // consumers run the epilogue); each consumer warpgroup accumulates 64 rows x BN in registers with
 // wgmma, keeping one k-block of MMAs in flight, and releases a stage as soon as the MMAs that read
 // it have completed.
-template <int BN, int CW, bool IM2COL, int NP, bool CG2>
+template <int BN, int CW, bool IM2COL, int NP, bool CG2, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAdd,
@@ -394,10 +394,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 const uint64_t db = db0 + ((pb * Cfg::kBBytes + (j * kKSteps + ks) * 32) >> 4);
                 const uint32_t accum = (j | ks | (small ? t : 0)) ? 1u : static_cast<uint32_t>(kb != 0);
                 if constexpr (NP == 3) {
-                  if (small) Wgmma<BN>::template mma<0, 0>(acc2, da, db, accum);
-                  else Wgmma<BN>::template mma<0, 0>(acc, da, db, accum);
+                  if (small) WgmmaOp<BN, F16>::type::template mma<0, 0>(acc2, da, db, accum);
+                  else WgmmaOp<BN, F16>::type::template mma<0, 0>(acc, da, db, accum);
                 } else {
-                  Wgmma<BN>::template mma<0, 0>(acc, da, db, accum);
+                  WgmmaOp<BN, F16>::type::template mma<0, 0>(acc, da, db, accum);
                 }
               }
             }
@@ -448,12 +448,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const int r = r0 + h * 8;
             float v0 = acc[j * 4 + h * 2] + b0, v1 = acc[j * 4 + h * 2 + 1] + b1;
             const int off = staged_offset<kSubW>(r, c);
-            if (p.has_add) bf16x2_add(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
+            if (p.has_add) x2_add<F16>(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
             // ReLU mask of the destination tensor: 0xffff per bf16 half that is > 0, applied to the
             // packed bf16 output (zeroing the half == zeroing the fp32 value before rounding)
             if (p.out_f32) {
               if (p.has_mask) {
-                const uint32_t k2 = bf16x2_gt0_mask(*reinterpret_cast<const uint32_t*>(s_mask + off));
+                const uint32_t k2 = x2_gt0_mask<F16>(*reinterpret_cast<const uint32_t*>(s_mask + off));
                 if (!(k2 & 0xffffu)) v0 = 0.f;
                 if (!(k2 >> 16)) v1 = 0.f;
               }
@@ -462,8 +462,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                                            static_cast<size_t>(m0 + r) * p.Cout + nh + c) =
                     make_float2(v0, v1);
             } else {
-              uint32_t pk = pack_bf16x2(v0, v1);
-              if (p.has_mask) pk &= bf16x2_gt0_mask(*reinterpret_cast<const uint32_t*>(s_mask + off));
+              uint32_t pk = pack_x2<F16>(v0, v1);
+              if (p.has_mask) pk &= x2_gt0_mask<F16>(*reinterpret_cast<const uint32_t*>(s_mask + off));
               *reinterpret_cast<uint32_t*>(s_out + off) = pk;
             }
           }
@@ -498,7 +498,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
             for (int e = 0; e < 4; ++e)
-              bf16x2_sum_sq(acc_s[hf][2 * e], acc_q[hf][2 * e], acc_s[hf][2 * e + 1],
+              x2_sum_sq<F16>(acc_s[hf][2 * e], acc_q[hf][2 * e], acc_s[hf][2 * e + 1],
                             acc_q[hf][2 * e + 1], w4[e]);
           }
         }
@@ -606,7 +606,7 @@ struct PatchIter {
   }
 };
 
-template <int BN, int CW>
+template <int BN, int CW, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAdd,
@@ -766,7 +766,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int t = 0; t < 9; ++t)
 #pragma unroll
             for (int ks = 0; ks < kKSteps; ++ks)
-              Wgmma<BN>::template mma<0, 0>(
+              WgmmaOp<BN, F16>::type::template mma<0, 0>(
                   acc, a_st + ((((t / 3) * kHaloW + (t % 3)) * kRowB + ks * 32) >> 4),
                   b_st + ((t * Cfg::kBTile + ks * 32) >> 4), (t | ks) ? 1u : static_cast<uint32_t>(kc != 0));
           wgmma_commit();
@@ -784,7 +784,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const uint64_t b_tap = b_desc0 + ((sb * Cfg::kBTile) >> 4);
 #pragma unroll
             for (int ks = 0; ks < kKSteps; ++ks)
-              Wgmma<BN>::template mma<0, 0>(acc, a_tap + ((ks * 32) >> 4), b_tap + ((ks * 32) >> 4),
+              WgmmaOp<BN, F16>::type::template mma<0, 0>(acc, a_tap + ((ks * 32) >> 4), b_tap + ((ks * 32) >> 4),
                                             (kc | t | ks) ? 1u : 0u);
             wgmma_commit();
             wgmma_fence_operand(acc);
@@ -816,9 +816,9 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int r = r0 + h * 8;
           float v0 = acc[j * 4 + h * 2], v1 = acc[j * 4 + h * 2 + 1];
           const int off = staged_offset<kSubW>(r, c);
-          if (p.has_add) bf16x2_add(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
-          uint32_t pk = pack_bf16x2(v0, v1);
-          if (p.has_mask) pk &= bf16x2_gt0_mask(*reinterpret_cast<const uint32_t*>(s_mask + off));
+          if (p.has_add) x2_add<F16>(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
+          uint32_t pk = pack_x2<F16>(v0, v1);
+          if (p.has_mask) pk &= x2_gt0_mask<F16>(*reinterpret_cast<const uint32_t*>(s_mask + off));
           *reinterpret_cast<uint32_t*>(s_out + off) = pk;
         }
       }
@@ -845,7 +845,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
           for (int e = 0; e < 4; ++e)
-            bf16x2_sum_sq(acc_s[2 * e], acc_q[2 * e], acc_s[2 * e + 1], acc_q[2 * e + 1], w4[e]);
+            x2_sum_sq<F16>(acc_s[2 * e], acc_q[2 * e], acc_s[2 * e + 1], acc_q[2 * e + 1], w4[e]);
         }
       }
     }
@@ -916,7 +916,7 @@ struct WgradCfg {
 // CW: channel width of one im2col chunk of x (16/32/64), CWB: channel width of one dy chunk.
 // Both operands are MN-major in shared memory (the pixel index is the GEMM K dimension): one pixel
 // row = width*2 bytes, 8-row groups SBO apart, column blocks (64/32/16 channels) LBO apart.
-template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX>
+template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX, bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmDY,
                   const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
@@ -1046,10 +1046,10 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           const uint64_t db = db0 + ((pb * Cfg::kBBytes + ks * 16 * CWB * 2) >> 4);
           const uint32_t accum = (it | ks | (small ? t : 0)) ? 1u : 0u;
           if constexpr (NP == 3) {
-            if (small) Wgmma<BN>::template mma<1, 1>(acc2, da, db, accum);
-            else Wgmma<BN>::template mma<1, 1>(acc, da, db, accum);
+            if (small) WgmmaOp<BN, F16>::type::template mma<1, 1>(acc2, da, db, accum);
+            else WgmmaOp<BN, F16>::type::template mma<1, 1>(acc, da, db, accum);
           } else {
-            Wgmma<BN>::template mma<1, 1>(acc, da, db, accum);
+            WgmmaOp<BN, F16>::type::template mma<1, 1>(acc, da, db, accum);
           }
         }
       }
@@ -1141,12 +1141,12 @@ static int g_conv_mtiles_mode = -1;
 // by default: c3 step on an H100 SXM at 700 W, 80.3 ms with pairs against 61.3 ms without
 static int g_conv_pairs = 0;
 
-template <int BN, int CW, bool IM2COL, int NP, bool CG2 = false>
+template <int BN, int CW, bool IM2COL, int NP, bool CG2 = false, bool F16 = false>
 static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per_n,
                             cudaStream_t stream) {
   using Cfg = FpropCfg<BN, NP>;
   static bool attr_set = false;
-  auto kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2>;
+  auto kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2, F16>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          kSmemBudget + 2048);
@@ -1217,24 +1217,29 @@ static ConvTiling conv_tiling(int M, int Cout, int Ktot, int cw, bool has_add, b
   return t;
 }
 
-template <int BN, int NP>
+template <int BN, int NP, bool F16 = false>
 static int dispatch_conv_cw(int cw, bool im2col, const ConvMaps& tm, const ConvGemmParams& p,
                             int per_n, cudaStream_t s) {
   if (im2col) {
-    if (cw == 64) return launch_conv_gemm<BN, 64, true, NP>(tm, p, per_n, s);
-    if (cw == 32) return launch_conv_gemm<BN, 32, true, NP>(tm, p, per_n, s);
-    return launch_conv_gemm<BN, 16, true, NP>(tm, p, per_n, s);
+    if (cw == 64) return launch_conv_gemm<BN, 64, true, NP, false, F16>(tm, p, per_n, s);
+    if (cw == 32) return launch_conv_gemm<BN, 32, true, NP, false, F16>(tm, p, per_n, s);
+    return launch_conv_gemm<BN, 16, true, NP, false, F16>(tm, p, per_n, s);
   }
-  if (cw == 64) return launch_conv_gemm<BN, 64, false, NP>(tm, p, per_n, s);
-  if (cw == 32) return launch_conv_gemm<BN, 32, false, NP>(tm, p, per_n, s);
-  return launch_conv_gemm<BN, 16, false, NP>(tm, p, per_n, s);
+  if (cw == 64) return launch_conv_gemm<BN, 64, false, NP, false, F16>(tm, p, per_n, s);
+  if (cw == 32) return launch_conv_gemm<BN, 32, false, NP, false, F16>(tm, p, per_n, s);
+  return launch_conv_gemm<BN, 16, false, NP, false, F16>(tm, p, per_n, s);
 }
 
+// f16: fp16 operands and output (ACNN_F16), one plane, the bf16 path's tiles
 template <int BN>
-static int dispatch_conv_gemm(const ConvTiling& t, int np, int cw, bool im2col, const ConvMaps& tm,
-                              const ConvGemmParams& p, cudaStream_t s) {
+static int dispatch_conv_gemm(const ConvTiling& t, int np, bool f16, int cw, bool im2col,
+                              const ConvMaps& tm, const ConvGemmParams& p, cudaStream_t s) {
   if constexpr (BN == 128) {
     if (t.pair) {     // full-width (64-channel) chunks only: bounds the instantiation count
+      if (f16) {
+        if (im2col) return launch_conv_gemm<128, 64, true, 1, true, true>(tm, p, t.per_n, s);
+        return launch_conv_gemm<128, 64, false, 1, true, true>(tm, p, t.per_n, s);
+      }
       if (im2col) return launch_conv_gemm<128, 64, true, 1, true>(tm, p, t.per_n, s);
       return launch_conv_gemm<128, 64, false, 1, true>(tm, p, t.per_n, s);
     }
@@ -1242,6 +1247,7 @@ static int dispatch_conv_gemm(const ConvTiling& t, int np, int cw, bool im2col, 
   if constexpr (BN <= 128) {
     if (np == 3) return dispatch_conv_cw<BN, 3>(cw, im2col, tm, p, t.per_n, s);
   }
+  if (f16) return dispatch_conv_cw<BN, 1, true>(cw, im2col, tm, p, t.per_n, s);
   return dispatch_conv_cw<BN, 1>(cw, im2col, tm, p, t.per_n, s);
 }
 
@@ -1327,12 +1333,12 @@ static int halo_per_n(const acnn_conv_geom& g) {
 }
 
 static int make_map_4d(CUtensorMap* m, const void* base, int C, int W, int H, int B, int box_c,
-                       int box_w, int box_h) {
+                       int box_w, int box_h, CUtensorMapDataType dt) {
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
   cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims,
+  CUresult r = g_encode_tiled(m, dt, 4, const_cast<void*>(base), dims,
                               strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                               swizzle_enum(box_c * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -1344,13 +1350,14 @@ static int make_map_4d(CUtensorMap* m, const void* base, int C, int W, int H, in
   return ACNN_OK;
 }
 
-template <int BN, int CW>
+template <int BN, int CW, bool F16>
 static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* w, void* y,
                             float* ch_part, const void* add_src, const void* mask_src,
                             cudaStream_t stream) {
   using Cfg = HaloCfg<BN, CW>;
   static bool attr_set = false;
-  auto kern = conv_halo_kernel<BN, CW>;
+  auto kern = conv_halo_kernel<BN, CW, F16>;
+  const CUtensorMapDataType dt = F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          kSmemBudget + 2048);
@@ -1376,16 +1383,16 @@ static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* 
   ACNN_REQUIRE(p.b_slots >= 2, "conv (halo): shared memory does not fit");
   const int smem = hp.smem;
   CUtensorMap tmA, tmB, tmC, tmAdd, tmMask;
-  int rc = make_map_4d(&tmA, x, g.Cin, g.W, g.H, g.B, CW, kHaloW, kHaloH);
+  int rc = make_map_4d(&tmA, x, g.Cin, g.W, g.H, g.B, CW, kHaloW, kHaloH, dt);
   if (rc) return rc;
-  if ((rc = make_map_2d(&tmB, w, g.Cout, 9 * g.Cin, 9 * g.Cin, BN, CW))) return rc;
-  if ((rc = make_map_4d(&tmC, y, g.Cout, g.W, g.H, g.B, Cfg::kSubW, kPatchW, kPatchH))) return rc;
+  if ((rc = make_map_2d(&tmB, w, g.Cout, 9 * g.Cin, 9 * g.Cin, BN, CW, dt))) return rc;
+  if ((rc = make_map_4d(&tmC, y, g.Cout, g.W, g.H, g.B, Cfg::kSubW, kPatchW, kPatchH, dt))) return rc;
   tmAdd = tmMask = tmC;
   if (add_src && (rc = make_map_4d(&tmAdd, add_src, g.Cout, g.W, g.H, g.B, Cfg::kSubW, kPatchW,
-                                   kPatchH)))
+                                   kPatchH, dt)))
     return rc;
   if (mask_src && (rc = make_map_4d(&tmMask, mask_src, g.Cout, g.W, g.H, g.B, Cfg::kSubW, kPatchW,
-                                    kPatchH)))
+                                    kPatchH, dt)))
     return rc;
   launch_k(kern, dim3(halo_per_n(g) * p.n_tiles), dim3(kThreads), smem, stream, tmA, tmB, tmC,
            tmAdd, tmMask, p);
@@ -1393,26 +1400,28 @@ static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* 
   return check_launch("conv_halo_kernel");
 }
 
+template <bool F16>
 static int conv_halo_host(const acnn_conv_geom& g, const void* x, const void* w, void* y,
                           float* ch_part, const void* add_src, const void* mask_src,
                           cudaStream_t stream) {
   const int bn = halo_bn(g.Cout);
   const bool c64 = g.Cin % 64 == 0;
   if (bn == 128) {
-    return c64 ? launch_conv_halo<128, 64>(g, x, w, y, ch_part, add_src, mask_src, stream)
-               : launch_conv_halo<128, 32>(g, x, w, y, ch_part, add_src, mask_src, stream);
+    return c64 ? launch_conv_halo<128, 64, F16>(g, x, w, y, ch_part, add_src, mask_src, stream)
+               : launch_conv_halo<128, 32, F16>(g, x, w, y, ch_part, add_src, mask_src, stream);
   }
   if (bn == 64) {
-    return c64 ? launch_conv_halo<64, 64>(g, x, w, y, ch_part, add_src, mask_src, stream)
-               : launch_conv_halo<64, 32>(g, x, w, y, ch_part, add_src, mask_src, stream);
+    return c64 ? launch_conv_halo<64, 64, F16>(g, x, w, y, ch_part, add_src, mask_src, stream)
+               : launch_conv_halo<64, 32, F16>(g, x, w, y, ch_part, add_src, mask_src, stream);
   }
-  return c64 ? launch_conv_halo<32, 64>(g, x, w, y, ch_part, add_src, mask_src, stream)
-             : launch_conv_halo<32, 32>(g, x, w, y, ch_part, add_src, mask_src, stream);
+  return c64 ? launch_conv_halo<32, 64, F16>(g, x, w, y, ch_part, add_src, mask_src, stream)
+             : launch_conv_halo<32, 32, F16>(g, x, w, y, ch_part, add_src, mask_src, stream);
 }
 
 // precision 0: x / w are bf16.  precision 1 (fp32 parity mode): x and w each are THREE consecutive
 // bf16 planes (acnn_split3 / acnn_prep_weights with planes = 3), plane p of x at x + p * numel(x),
 // plane p of w at w + p * w_plane_stride elements; y must be fp32 (out_f32), no fused epilogue.
+// precision ACNN_F16: x / w (and y, add, mask unless out_f32) are fp16, on the bf16 path's tiles.
 static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w, void* y,
                           float* ch_part, const void* add_src, const void* mask_src,
                           const float* bias, int out_f32, int precision, int64_t w_plane_stride,
@@ -1422,8 +1431,9 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   ACNN_REQUIRE(g.Cout % 32 == 0, "conv: Cout=%d must be a multiple of 32", g.Cout);
   ACNN_REQUIRE(g.stride >= 1 && g.kh >= 1 && g.kw >= 1, "conv: bad kernel/stride");
   ACNN_REQUIRE(!(ch_part && out_f32), "conv: statistics only with bf16 output");
-  ACNN_REQUIRE(precision == 0 || precision == 1, "conv: precision must be 0 (bf16) or 1 (fp32)");
-  ACNN_REQUIRE(precision == 0 || (out_f32 && !add_src && !mask_src && !ch_part && w_plane_stride > 0),
+  ACNN_REQUIRE(precision == ACNN_BF16 || precision == ACNN_F32 || precision == ACNN_F16,
+               "conv: precision must be 0 (bf16), 1 (fp32) or 3 (fp16)");
+  ACNN_REQUIRE(precision != ACNN_F32 || (out_f32 && !add_src && !mask_src && !ch_part && w_plane_stride > 0),
                "conv: the fp32 (3-plane) mode needs fp32 output, a weight plane stride and no "
                "fused add / mask / statistics epilogue");
   int Ho, Wo;
@@ -1432,12 +1442,14 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
                "conv: padding / filter exceed the TMA im2col corner range");
   int rc = load_driver_fns();
   if (rc) return rc;
-  if (use_halo(g, precision ? 3 : 1, out_f32 != 0, bias != nullptr, add_src != nullptr,
-               mask_src != nullptr))
-    return conv_halo_host(g, x, w, y, ch_part, add_src, mask_src, stream);
+  const int np = precision == ACNN_F32 ? 3 : 1;
+  const bool f16 = precision == ACNN_F16;
+  if (use_halo(g, np, out_f32 != 0, bias != nullptr, add_src != nullptr, mask_src != nullptr))
+    return f16 ? conv_halo_host<true>(g, x, w, y, ch_part, add_src, mask_src, stream)
+               : conv_halo_host<false>(g, x, w, y, ch_part, add_src, mask_src, stream);
   const bool plain = is_plain(g);
   const int cw = chunk_width(g.Cin);
-  const int np = precision ? 3 : 1;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   ConvGemmParams p;
   p.M = g.B * Ho * Wo;
   p.Cout = g.Cout;
@@ -1469,13 +1481,13 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
     const __nv_bfloat16* xp = static_cast<const __nv_bfloat16*>(x) + pl * x_plane;
     const __nv_bfloat16* wp = static_cast<const __nv_bfloat16*>(w) + pl * w_plane_stride;
     if (plain) {
-      rc = make_map_2d(&tm.a[pl], xp, p.M, g.Cin, g.Cin, kBM, cw);
+      rc = make_map_2d(&tm.a[pl], xp, p.M, g.Cin, g.Cin, kBM, cw, dt);
     } else {
-      rc = make_map_im2col(&tm.a[pl], xp, g, cw, kBM);
+      rc = make_map_im2col(&tm.a[pl], xp, g, cw, kBM, dt);
     }
     if (rc) return rc;
     rc = make_map_2d(&tm.b[pl], wp, g.Cout, p.Ktot, p.Ktot, t.pair ? bn / 2 : bn,
-                     p.Ktot >= 64 ? 64 : p.Ktot);
+                     p.Ktot >= 64 ? 64 : p.Ktot, dt);
     if (rc) return rc;
   }
   for (int pl = np; pl < 3; ++pl) {   // placeholders
@@ -1484,12 +1496,12 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   }
   tm.c = tm.add = tm.mask = tm.b[0];   // placeholders when unused
   const int subw = bn < 64 ? bn : 64;
-  if (!out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw))) return rc;
-  if (add_src && (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw))) return rc;
-  if (mask_src && (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw))) return rc;
-  if (bn == 128) return dispatch_conv_gemm<128>(t, np, cw, !plain, tm, p, stream);
-  if (bn == 64) return dispatch_conv_gemm<64>(t, np, cw, !plain, tm, p, stream);
-  return dispatch_conv_gemm<32>(t, np, cw, !plain, tm, p, stream);
+  if (!out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
+  if (add_src && (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
+  if (mask_src && (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
+  if (bn == 128) return dispatch_conv_gemm<128>(t, np, f16, cw, !plain, tm, p, stream);
+  if (bn == 64) return dispatch_conv_gemm<64>(t, np, f16, cw, !plain, tm, p, stream);
+  return dispatch_conv_gemm<32>(t, np, f16, cw, !plain, tm, p, stream);
 }
 
 struct WgradMaps {
@@ -1533,10 +1545,11 @@ struct WgradPlan {
 
 static int wgrad_plan(const acnn_conv_geom& g, int precision, int deterministic, WgradPlan* w) {
   ACNN_REQUIRE(g.Cin % 16 == 0 && g.Cout % 32 == 0, "wgrad: Cin %% 16 / Cout %% 32 required");
-  ACNN_REQUIRE(precision == 0 || precision == 1, "wgrad: precision must be 0 (bf16) or 1 (fp32)");
+  ACNN_REQUIRE(precision == ACNN_BF16 || precision == ACNN_F32 || precision == ACNN_F16,
+               "wgrad: precision must be 0 (bf16), 1 (fp32) or 3 (fp16)");
   int Ho, Wo;
   ACNN_REQUIRE(out_hw(g, &Ho, &Wo), "wgrad: empty output");
-  const int np = precision ? 3 : 1;
+  const int np = precision == ACNN_F32 ? 3 : 1;
   w->P = g.B * Ho * Wo;
   int bn = g.Cout >= 256 ? 256 : (g.Cout >= 128 ? 128 : (g.Cout >= 64 ? 64 : 32));
   if (np == 3 && bn > 128) bn = 128;   // three operand planes per stage: smem
@@ -1586,12 +1599,12 @@ static int wgrad_plan(const acnn_conv_geom& g, int precision, int deterministic,
   return ACNN_OK;
 }
 
-template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX = kWgPix>
+template <int BN, int CW, int CWB, bool IM2COL, int NP, int PIX = kWgPix, bool F16 = false>
 static int launch_wgrad(const WgradMaps& tm, WgradParams p, int m_tiles, int n_tiles,
                         cudaStream_t stream) {
   using Cfg = WgradCfg<BN, NP, PIX>;
   static bool attr_set = false;
-  auto kern = wgrad_gemm_kernel<BN, CW, CWB, IM2COL, NP, PIX>;
+  auto kern = wgrad_gemm_kernel<BN, CW, CWB, IM2COL, NP, PIX, F16>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
@@ -1627,10 +1640,10 @@ static int launch_wgrad(const WgradMaps& tm, WgradParams p, int m_tiles, int n_t
   return rc ? rc : rc2;
 }
 
-template <int BN, int CW, bool IM2COL>
+template <int BN, int CW, bool IM2COL, bool F16>
 static int dispatch_wgrad_cwb(int cwb, int np, const WgradMaps& tm, const WgradParams& p, int mt,
                               int nt, cudaStream_t s) {
-  if constexpr (BN <= 128) {
+  if constexpr (BN <= 128 && !F16) {
     if (np == 3) {
       if constexpr (BN >= 64) {
         if (cwb == 64) return launch_wgrad<BN, CW, 64, IM2COL, 3>(tm, p, mt, nt, s);
@@ -1641,32 +1654,33 @@ static int dispatch_wgrad_cwb(int cwb, int np, const WgradMaps& tm, const WgradP
   if constexpr (BN >= 64) {
     if (cwb == 64) {
       if constexpr (BN <= 128) {
-        if (p.pix == 128) return launch_wgrad<BN, CW, 64, IM2COL, 1, 128>(tm, p, mt, nt, s);
+        if (p.pix == 128) return launch_wgrad<BN, CW, 64, IM2COL, 1, 128, F16>(tm, p, mt, nt, s);
       }
-      return launch_wgrad<BN, CW, 64, IM2COL, 1>(tm, p, mt, nt, s);
+      return launch_wgrad<BN, CW, 64, IM2COL, 1, kWgPix, F16>(tm, p, mt, nt, s);
     }
   }
   if constexpr (BN <= 128) {
-    if (p.pix == 128) return launch_wgrad<BN, CW, 32, IM2COL, 1, 128>(tm, p, mt, nt, s);
+    if (p.pix == 128) return launch_wgrad<BN, CW, 32, IM2COL, 1, 128, F16>(tm, p, mt, nt, s);
   }
-  return launch_wgrad<BN, CW, 32, IM2COL, 1>(tm, p, mt, nt, s);
+  return launch_wgrad<BN, CW, 32, IM2COL, 1, kWgPix, F16>(tm, p, mt, nt, s);
 }
 
-template <int BN, bool IM2COL>
+template <int BN, bool IM2COL, bool F16>
 static int dispatch_wgrad_cw(int cw, int cwb, int np, const WgradMaps& tm, const WgradParams& p,
                              int mt, int nt, cudaStream_t s) {
-  if (cw == 64) return dispatch_wgrad_cwb<BN, 64, IM2COL>(cwb, np, tm, p, mt, nt, s);
-  if (cw == 32) return dispatch_wgrad_cwb<BN, 32, IM2COL>(cwb, np, tm, p, mt, nt, s);
-  return dispatch_wgrad_cwb<BN, 16, IM2COL>(cwb, np, tm, p, mt, nt, s);
+  if (cw == 64) return dispatch_wgrad_cwb<BN, 64, IM2COL, F16>(cwb, np, tm, p, mt, nt, s);
+  if (cw == 32) return dispatch_wgrad_cwb<BN, 32, IM2COL, F16>(cwb, np, tm, p, mt, nt, s);
+  return dispatch_wgrad_cwb<BN, 16, IM2COL, F16>(cwb, np, tm, p, mt, nt, s);
 }
 
-template <bool IM2COL>
+// F16: fp16 operands (ACNN_F16), one plane, the bf16 path's tiles
+template <bool IM2COL, bool F16>
 static int dispatch_wgrad(int bn, int cw, int cwb, int np, const WgradMaps& tm, const WgradParams& p,
                           int mt, int nt, cudaStream_t s) {
-  if (bn == 256) return dispatch_wgrad_cw<256, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
-  if (bn == 128) return dispatch_wgrad_cw<128, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
-  if (bn == 64) return dispatch_wgrad_cw<64, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
-  return dispatch_wgrad_cw<32, IM2COL>(cw, cwb, np, tm, p, mt, nt, s);
+  if (bn == 256) return dispatch_wgrad_cw<256, IM2COL, F16>(cw, cwb, np, tm, p, mt, nt, s);
+  if (bn == 128) return dispatch_wgrad_cw<128, IM2COL, F16>(cw, cwb, np, tm, p, mt, nt, s);
+  if (bn == 64) return dispatch_wgrad_cw<64, IM2COL, F16>(cw, cwb, np, tm, p, mt, nt, s);
+  return dispatch_wgrad_cw<32, IM2COL, F16>(cw, cwb, np, tm, p, mt, nt, s);
 }
 
 static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* dy, float* dw,
@@ -1679,7 +1693,9 @@ static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* d
   int Ho, Wo;
   out_hw(g, &Ho, &Wo);
   const bool plain = is_plain(g);
-  const int np = precision ? 3 : 1;
+  const int np = precision == ACNN_F32 ? 3 : 1;
+  const bool f16 = precision == ACNN_F16;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   WgradParams p;
   p.P = w.P;
   p.Cout = g.Cout;
@@ -1703,12 +1719,12 @@ static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* d
   for (int pl = 0; pl < np; ++pl) {
     const __nv_bfloat16* xp = static_cast<const __nv_bfloat16*>(x) + pl * x_plane;
     const __nv_bfloat16* dp = static_cast<const __nv_bfloat16*>(dy) + pl * dy_plane;
-    rc = make_map_2d(&tm.dy[pl], dp, p.P, g.Cout, g.Cout, p.pix, cwb);
+    rc = make_map_2d(&tm.dy[pl], dp, p.P, g.Cout, g.Cout, p.pix, cwb, dt);
     if (rc) return rc;
     if (plain) {
-      rc = make_map_2d(&tm.x[pl], xp, p.P, g.Cin, g.Cin, p.pix, cw);
+      rc = make_map_2d(&tm.x[pl], xp, p.P, g.Cin, g.Cin, p.pix, cw, dt);
     } else {
-      rc = make_map_im2col(&tm.x[pl], xp, g, cw, p.pix);
+      rc = make_map_im2col(&tm.x[pl], xp, g, cw, p.pix, dt);
     }
     if (rc) return rc;
   }
@@ -1716,8 +1732,12 @@ static int conv_wgrad_host(const acnn_conv_geom& g, const void* x, const void* d
     tm.x[pl] = tm.x[0];
     tm.dy[pl] = tm.dy[0];
   }
-  if (plain) return dispatch_wgrad<false>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
-  return dispatch_wgrad<true>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
+  if (f16) {
+    if (plain) return dispatch_wgrad<false, true>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
+    return dispatch_wgrad<true, true>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
+  }
+  if (plain) return dispatch_wgrad<false, false>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
+  return dispatch_wgrad<true, false>(w.bn, cw, cwb, np, tm, p, w.m_tiles, w.n_tiles, stream);
 }
 
 }  // namespace acnn
@@ -1852,7 +1872,7 @@ int acnn_conv_dgrad(const acnn_conv_geom* g, const void* dy, const void* w_dgrad
   t.pad_w_hi = g->kw - 1 - g->pad_w_hi;
   t.x_pix_stride = t.x_row_pitch = t.x_img_pitch = t.reserved_ = 0;
   return acnn::conv_gemm_host(t, dy, w_dgrad, dx, nullptr, add_src, mask_src, nullptr,
-                              precision ? 1 : 0, precision, w_plane_stride,
+                              precision == ACNN_F32 ? 1 : 0, precision, w_plane_stride,
                               static_cast<cudaStream_t>(stream));
 }
 

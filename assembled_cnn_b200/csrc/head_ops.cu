@@ -269,18 +269,6 @@ kd_teacher_labels_kernel(const float* __restrict__ tl, const int32_t* __restrict
 
 using namespace acnn;
 
-#define ACNN_DTYPE_OK(dt) ((dt) == ACNN_BF16 || (dt) == ACNN_F32)
-#define ACNN_BY_DTYPE(dt, ...)      \
-  do {                              \
-    if ((dt) == ACNN_F32) {         \
-      using T = float;              \
-      __VA_ARGS__;                  \
-    } else {                        \
-      using T = bf16;               \
-      __VA_ARGS__;                  \
-    }                               \
-  } while (0)
-
 extern "C" {
 
 int acnn_dropblock_scratch_floats(int H, int W, int C, int block_size) {

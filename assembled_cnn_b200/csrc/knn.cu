@@ -3,7 +3,8 @@
 // epilogue, so it never reaches HBM.
 //
 //   knn_prep_kernel : l2-normalised (cosine) or raw rows -> bf16 operands (or six plane segments in
-//                     the fp32 mode), zero-padded to a multiple of 64 in d, and their squared norms.
+//                     the fp32 mode, or fp16 operands in the fp16 mode), zero-padded to a multiple of
+//                     64 in d, and their squared norms.
 //   knn_topk_kernel : a CTA owns 128 query rows and walks a range of 128-column index tiles.  Warp 0
 //                     is the TMA producer of an mbarrier ring (the organisation of conv_gemm_kernel);
 //                     two consumer warpgroups accumulate 64 rows x 128 columns each in registers.
@@ -21,6 +22,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.h"
 #include "ptx.cuh"
@@ -67,10 +69,11 @@ __device__ __forceinline__ bool beats(float s1, int i1, float s2, int i2) {
   return s1 > s2 || (s1 == s2 && i1 < i2);
 }
 
-// One warp per row of Q and X.
+// One warp per row of Q and X.  E = bf16 (one plane, or six plane segments) or __half (one plane).
+template <class E>
 __global__ void __launch_bounds__(256)
 knn_prep_kernel(const float* __restrict__ q, const float* __restrict__ x, int nq, int nx, int d,
-                int dp, int planes, int cosine, bf16* __restrict__ qp, bf16* __restrict__ xp,
+                int dp, int planes, int cosine, E* __restrict__ qp, E* __restrict__ xp,
                 float* __restrict__ qn, float* __restrict__ xn) {
   pdl_wait();
   const int lane = threadIdx.x & 31;
@@ -79,7 +82,7 @@ knn_prep_kernel(const float* __restrict__ q, const float* __restrict__ x, int nq
   const bool is_q = r < nq;
   const int row = is_q ? r : r - nq;
   const float* src = (is_q ? q : x) + (int64_t)row * d;
-  bf16* dst = (is_q ? qp : xp) + (int64_t)row * dp * planes;
+  E* dst = (is_q ? qp : xp) + (int64_t)row * dp * planes;
   float scale = 1.f;
   if (cosine) {
     float ss = 0.f;
@@ -89,24 +92,32 @@ knn_prep_kernel(const float* __restrict__ q, const float* __restrict__ x, int nq
   float nrm = 0.f;
   for (int i = lane; i < dp; i += 32) {
     const float v = i < d ? src[i] * scale : 0.f;
-    const bf16 h = __float2bfloat16_rn(v);
-    if (planes == 1) {
+    if constexpr (std::is_same<E, __half>::value) {
+      // fp16 operands: round to nearest even (beyond +-65504: inf, then an unranked row)
+      const __half h = __float2half_rn(v);
       dst[i] = h;
-      const float r0 = __bfloat162float(h);
+      const float r0 = __half2float(h);
       nrm = fmaf(r0, r0, nrm);
     } else {
-      // v = hi + mid + lo (24 mantissa bits), the split of acnn_split3
-      const float r1 = v - __bfloat162float(h);
-      const bf16 m = __float2bfloat16_rn(r1);
-      const bf16 l = __float2bfloat16_rn(r1 - __bfloat162float(m));
-      const float rv = (__bfloat162float(h) + __bfloat162float(m)) + __bfloat162float(l);
-      nrm = fmaf(rv, rv, nrm);
-      // segments of the six plane products, smallest first: lo*hi, mid*mid, hi*lo, mid*hi,
-      // hi*mid, hi*hi (Q' = hi mid lo hi mid hi, X' = lo mid hi mid hi hi)
-      const bf16 seg_q[6] = {h, m, l, h, m, h};
-      const bf16 seg_x[6] = {l, m, h, m, h, h};
+      const bf16 h = __float2bfloat16_rn(v);
+      if (planes == 1) {
+        dst[i] = h;
+        const float r0 = __bfloat162float(h);
+        nrm = fmaf(r0, r0, nrm);
+      } else {
+        // v = hi + mid + lo (24 mantissa bits), the split of acnn_split3
+        const float r1 = v - __bfloat162float(h);
+        const bf16 m = __float2bfloat16_rn(r1);
+        const bf16 l = __float2bfloat16_rn(r1 - __bfloat162float(m));
+        const float rv = (__bfloat162float(h) + __bfloat162float(m)) + __bfloat162float(l);
+        nrm = fmaf(rv, rv, nrm);
+        // segments of the six plane products, smallest first: lo*hi, mid*mid, hi*lo, mid*hi,
+        // hi*mid, hi*hi (Q' = hi mid lo hi mid hi, X' = lo mid hi mid hi hi)
+        const bf16 seg_q[6] = {h, m, l, h, m, h};
+        const bf16 seg_x[6] = {l, m, h, m, h, h};
 #pragma unroll
-      for (int s = 0; s < 6; ++s) dst[i + (int64_t)s * dp] = is_q ? seg_q[s] : seg_x[s];
+        for (int s = 0; s < 6; ++s) dst[i + (int64_t)s * dp] = is_q ? seg_q[s] : seg_x[s];
+      }
     }
   }
   nrm = warp_sum(nrm);
@@ -174,6 +185,7 @@ __device__ int merge_row(int lane, const float* bs, const int* bi, int nb, float
   return n;
 }
 
+template <bool F16>
 __global__ void __launch_bounds__(kThreads, 1)
 knn_topk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmX,
                 const KnnParams p) {
@@ -288,7 +300,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint64_t db0 = b_desc0 + ((stage * kStageBytes) >> 4);
 #pragma unroll
         for (int ks = 0; ks < kStageK / 16; ++ks)
-          Wgmma<kCols>::template mma<0, 0>(acc, da0 + ((ks * 32) >> 4), db0 + ((ks * 32) >> 4),
+          WgmmaOp<kCols, F16>::type::template mma<0, 0>(acc, da0 + ((ks * 32) >> 4), db0 + ((ks * 32) >> 4),
                                            (ks | kb) ? 1u : 0u);
         wgmma_commit();
         wgmma_fence_operand(acc);
@@ -483,7 +495,8 @@ int knn_check(int nq, int nx, int d, int k, int metric, int dtype) {
   ACNN_REQUIRE(nq > 0 && nx > 0 && d > 0 && d <= (1 << 24) && k >= 1,
                "knn_topk: bad sizes nq=%d nx=%d d=%d k=%d", nq, nx, d, k);
   ACNN_REQUIRE(metric == 0 || metric == 1, "knn_topk: unknown metric %d", metric);
-  ACNN_REQUIRE(dtype == ACNN_BF16 || dtype == ACNN_F32, "knn_topk: unknown dtype %d", dtype);
+  ACNN_REQUIRE(dtype == ACNN_BF16 || dtype == ACNN_F32 || dtype == ACNN_F16, "knn_topk: unknown dtype %d",
+               dtype);
   if (k > kMaxK) {
     set_error("knn_topk: k=%d > %d is not supported", k, kMaxK);
     return ACNN_ERR_UNSUPPORTED;
@@ -519,28 +532,36 @@ int acnn_knn_topk(const float* q, const float* x, int nq, int nx, int d, int k, 
                (long long)work_bytes, (long long)l.total);
   ACNN_REQUIRE(reinterpret_cast<uintptr_t>(work) % 256 == 0, "knn_topk: work must be 256-byte aligned");
   if ((rc = load_driver_fns())) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(knn_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         kSmemBytes);
+  // fp16 mode (ACNN_F16): fp16 operands, wgmma .f16.f16, fp32 accumulation; the rest is shared
+  const bool f16 = dtype == ACNN_F16;
+  auto* topk = f16 ? knn_topk_kernel<true> : knn_topk_kernel<false>;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[f16]) {
+    cudaError_t e = cudaFuncSetAttribute(topk, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(knn_topk): %s", cudaGetErrorString(e));
       return ACNN_ERR_CUDA;
     }
-    attr_set = true;
+    attr_set[f16] = true;
   }
   uint8_t* w = static_cast<uint8_t*>(work);
-  bf16* qp = reinterpret_cast<bf16*>(w + l.q);
-  bf16* xp = reinterpret_cast<bf16*>(w + l.x);
   float* qn = reinterpret_cast<float*>(w + l.qn);
   float* xn = reinterpret_cast<float*>(w + l.xn);
   CUtensorMap tmQ, tmX;
-  if ((rc = make_map_2d(&tmQ, qp, nq, l.kp, l.kp, kRows, kStageK))) return rc;
-  if ((rc = make_map_2d(&tmX, xp, nx, l.kp, l.kp, kCols, kStageK))) return rc;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  if ((rc = make_map_2d(&tmQ, w + l.q, nq, l.kp, l.kp, kRows, kStageK, dt))) return rc;
+  if ((rc = make_map_2d(&tmX, w + l.x, nx, l.kp, l.kp, kCols, kStageK, dt))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
-  launch_k(knn_prep_kernel, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, l.dp,
-           l.planes, metric == 0 ? 1 : 0, qp, xp, qn, xn);
+  if (f16) {
+    launch_k(knn_prep_kernel<__half>, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, l.dp,
+             l.planes, metric == 0 ? 1 : 0, reinterpret_cast<__half*>(w + l.q),
+             reinterpret_cast<__half*>(w + l.x), qn, xn);
+  } else {
+    launch_k(knn_prep_kernel<bf16>, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, l.dp,
+             l.planes, metric == 0 ? 1 : 0, reinterpret_cast<bf16*>(w + l.q), reinterpret_cast<bf16*>(w + l.x),
+             qn, xn);
+  }
   if ((rc = check_launch("knn_prep_kernel"))) return rc;
 
   KnnParams p;
@@ -558,7 +579,7 @@ int acnn_knn_topk(const float* q, const float* x, int nq, int nx, int d, int k, 
   p.xn = xn;
   p.part_sim = reinterpret_cast<float*>(w + l.ps);
   p.part_idx = reinterpret_cast<int*>(w + l.pi);
-  launch_k(knn_topk_kernel, dim3(q_blocks, splits), dim3(kThreads), kSmemBytes, st, tmQ, tmX, p);
+  launch_k(topk, dim3(q_blocks, splits), dim3(kThreads), kSmemBytes, st, tmQ, tmX, p);
   if ((rc = check_launch("knn_topk_kernel"))) return rc;
 
   launch_k(knn_merge_kernel, dim3(ceil_div(nq, 128)), dim3(128), 0, st, p.part_sim, p.part_idx, nq,

@@ -43,7 +43,7 @@ int64_t ws_round(int64_t b) { return (std::max<int64_t>(b, 256) + kWsAlign - 1) 
 void layout(acnn_model* m) {
   Plan& p = m->plan;
   m->planes = p.cfg.fp32 ? 3 : 1;
-  m->adt = p.cfg.fp32 ? ACNN_F32 : ACNN_BF16;
+  m->adt = p.cfg.fp32 ? ACNN_F32 : (p.cfg.fp16 ? ACNN_F16 : ACNN_BF16);
   m->det = p.cfg.deterministic < 0 ? (p.cfg.fp32 ? 1 : 0) : (p.cfg.deterministic ? 1 : 0);
   m->loss_scale = p.cfg.loss_scale;
   // weight descriptor table + weight-decay flags (one byte per 256 elements)
@@ -172,6 +172,7 @@ acnn_model::Launch resolve(acnn_model* m, const Op& op) {
     const int n = m->n_descs, planes = m->planes;
     void *wf = m->w_fprop, *wd = m->w_dgrad;
     const int64_t fs = p.param_elems, ds = std::max<int64_t>(p.dgrad_elems, 1);
+    if (adt == ACNN_F16) return [=](void* st) { return acnn_prep_weights_f16(master, descs, n, wf, wd, st); };
     return [=](void* st) { return acnn_prep_weights(master, descs, n, wf, wd, planes, fs, ds, st); };
   }
   if (k == "split3") {
@@ -616,7 +617,8 @@ int acnn_create(const acnn_model_config* c, acnn_model** out) {
   ACNN_REQUIRE(c->struct_size == (int32_t)sizeof(acnn_model_config),
                "acnn_create: acnn_model_config.struct_size %d != %d (header / library mismatch)", c->struct_size,
                (int)sizeof(acnn_model_config));
-  ACNN_REQUIRE(c->dtype == ACNN_BF16 || c->dtype == ACNN_F32, "dtype must be one of: ('bf16', 'fp32')");
+  ACNN_REQUIRE(c->dtype == ACNN_BF16 || c->dtype == ACNN_F32 || c->dtype == ACNN_F16,
+               "dtype must be one of: ('bf16', 'fp32', 'fp16')");
   auto term = [](const char* s, size_t n) { return std::string(s, strnlen(s, n)); };
   Config k;
   k.resnet_size = c->resnet_size;
@@ -643,6 +645,7 @@ int acnn_create(const acnn_model_config* c, acnn_model** out) {
   k.mixup_type = c->mixup_type;
   k.with_loss = c->with_loss;
   k.fp32 = c->dtype == ACNN_F32;
+  k.fp16 = c->dtype == ACNN_F16;
   k.use_dropblock = c->use_dropblock;
   k.deterministic = c->deterministic;
   k.fuse_bn_pairs = c->fuse_bn_pairs;

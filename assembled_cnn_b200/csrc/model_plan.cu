@@ -817,7 +817,7 @@ void Builder::run() {
   if (use_dropblock_ && c.use_se_block) fail(ACNN_ERR_UNSUPPORTED, "use_dropblock together with use_se_block");
   kd_temp_ = training_ ? c.kd_temp : 0.0;
   fp32_ = c.fp32;
-  adt_ = fp32_ ? ACNN_F32 : ACNN_BF16;
+  adt_ = fp32_ ? ACNN_F32 : (c.fp16 ? ACNN_F16 : ACNN_BF16);
   if (c.height % 32 || c.width % 32 || c.height <= 0 || c.width <= 0)
     fail(ACNN_ERR_INVALID, "input size must be a multiple of 32 (got %dx%d)", c.height, c.width);
   if (c.mixup_type < 0 || c.mixup_type > 2) fail(ACNN_ERR_INVALID, "mixup_type must be 0, 1 or 2");
@@ -1147,7 +1147,7 @@ std::string Plan::dump() const {
   meta["num_classes"] = fmt_int(cfg.num_classes);
   meta["ld_logits"] = fmt_int(ld_logits);
   meta["bn_momentum"] = fmt_flt(cfg.bn_momentum);
-  meta["dtype"] = cfg.fp32 ? "fp32" : "bf16";
+  meta["dtype"] = cfg.fp32 ? "fp32" : (cfg.fp16 ? "fp16" : "bf16");
   meta["use_dropblock"] = fmt_int(cfg.use_dropblock && cfg.training);
   meta["kd_temp"] = fmt_flt(cfg.training ? cfg.kd_temp : 0.0);
   meta["input_batch"] = fmt_int(input_batch);
@@ -1183,7 +1183,7 @@ std::string Plan::dump() const {
     }
   for (const auto& t : tensors)
     out += "tensor " + t.name + " shape=" + fmt_ints(t.shape) + " dtype=" +
-           (t.dtype == ACNN_BF16 ? "bf16" : (t.dtype == ACNN_F32 ? "f32" : "i32")) + " relu=" +
+           (t.dtype == ACNN_BF16 ? "bf16" : (t.dtype == ACNN_F32 ? "f32" : (t.dtype == ACNN_F16 ? "f16" : "i32"))) + " relu=" +
            fmt_int(t.relu) + "\n";
   const std::pair<const char*, const std::vector<Op>*> lists[] = {
       {"F", &forward}, {"B", &backward}, {"U", &update}};

@@ -55,13 +55,13 @@ inline int64_t numel(const Shape& s) {
 struct Tensor {
   std::string name;
   Shape shape;
-  int dtype = ACNN_BF16;   // ACNN_BF16 | ACNN_F32 | ACNN_I32
+  int dtype = ACNN_BF16;   // ACNN_BF16 | ACNN_F32 | ACNN_F16 | ACNN_I32
   bool relu = false;       // output of a ReLU: its gradient gets masked by (t > 0)
   int consumers = 0;       // forward readers that will send a gradient back
   int contribs = 0;
   int grad = -1;           // tensor holding the accumulated gradient so far
   int64_t ws_offset = 0;   // bytes inside the workspace (set by layout())
-  int64_t bytes() const { return numel(shape) * (dtype == ACNN_BF16 ? 2 : 4); }
+  int64_t bytes() const { return numel(shape) * (dtype == ACNN_BF16 || dtype == ACNN_F16 ? 2 : 4); }
 };
 
 struct Variable {
@@ -128,6 +128,7 @@ struct Config {
   int mixup_type = 0;
   bool with_loss = true;
   bool fp32 = false, use_dropblock = false;
+  bool fp16 = false;   // the bf16 plan with fp16 activation storage (ACNN_F16); exclusive with fp32
   int deterministic = -1;
   bool fuse_bn_pairs = true;
   double label_smoothing = 0, kd_temp = 0, loss_scale = 1;

@@ -1,4 +1,4 @@
-// Parameter handling: bf16 operand copies of the fp32 master weights (fprop + dgrad layouts), the
+// Parameter handling: bf16 / fp16 operand copies of the fp32 master weights (fprop + dgrad layouts), the
 // space-to-depth stem weight transform, and the fused weight-decay + momentum SGD step over the
 // flat parameter buffer.  nets/optimizer_setting.py:23-38, nets/run_loop_classification.py:166-179.
 #include "common.h"
@@ -15,6 +15,10 @@ __device__ __forceinline__ void split3(float v, bf16& h, bf16& m, bf16& l) {
   const float r1 = v - __bfloat162float(h);      // exact
   m = __float2bfloat16_rn(r1);
   l = __float2bfloat16_rn(r1 - __bfloat162float(m));
+}
+// fp16 weight copies (ACNN_F16): one plane, round to nearest even
+__device__ __forceinline__ void store_planes(f16* base, int64_t idx, float v, int, int64_t) {
+  base[idx] = __float2half_rn(v);
 }
 __device__ __forceinline__ void store_planes(bf16* base, int64_t idx, float v, int planes,
                                              int64_t plane_stride) {
@@ -51,9 +55,10 @@ split3_kernel(const float* __restrict__ x, bf16* __restrict__ planes, int64_t nv
   }
 }
 
+template <class E>
 __global__ void __launch_bounds__(256)
 prep_weights_kernel(const float* __restrict__ master, const acnn_weight_desc* __restrict__ descs,
-                    bf16* __restrict__ w_fprop, bf16* __restrict__ w_dgrad, int planes,
+                    E* __restrict__ w_fprop, E* __restrict__ w_dgrad, int planes,
                     int64_t fprop_plane_stride, int64_t dgrad_plane_stride) {
   pdl_wait();   // multi-wave grid: an early trigger would let the next kernel's CTAs take SM slots from this one
   __shared__ float tile[32][33];
@@ -219,10 +224,20 @@ int acnn_prep_weights(const float* master, const acnn_weight_desc* descs, int n,
   ACNN_REQUIRE(master && descs && w_fprop && n > 0 && n < 65536 && (planes == 1 || planes == 3),
                "prep_weights: bad arguments");
   dim3 grid(96, n, 1);
-  launch_k(prep_weights_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, master, descs,
+  launch_k(prep_weights_kernel<bf16>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, master, descs,
            (bf16*)w_fprop, (bf16*)w_dgrad, planes, fprop_plane_stride, dgrad_plane_stride);
   count_launch();
   return check_launch("prep_weights");
+}
+
+int acnn_prep_weights_f16(const float* master, const acnn_weight_desc* descs, int n, void* w_fprop,
+                          void* w_dgrad, void* stream) {
+  ACNN_REQUIRE(master && descs && w_fprop && n > 0 && n < 65536, "prep_weights_f16: bad arguments");
+  dim3 grid(96, n, 1);
+  launch_k(prep_weights_kernel<f16>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, master, descs,
+           (f16*)w_fprop, (f16*)w_dgrad, 1, (int64_t)0, (int64_t)0);
+  count_launch();
+  return check_launch("prep_weights_f16");
 }
 
 int acnn_split3(const float* x, void* planes, int64_t n, void* stream) {
@@ -235,11 +250,14 @@ int acnn_split3(const float* x, void* planes, int64_t n, void* stream) {
 
 int acnn_s2d_weight_pack(const float* w, void* w2, int Cout, int k, int pad, int k2, int pad2,
                          int dtype, void* stream) {
-  ACNN_REQUIRE(w && w2 && (dtype == ACNN_BF16 || dtype == ACNN_F32), "s2d_weight_pack: bad argument");
+  ACNN_REQUIRE(w && w2 && ACNN_DTYPE_OK(dtype), "s2d_weight_pack: bad argument");
   const int64_t n = (int64_t)Cout * k2 * k2 * 16;
   if (dtype == ACNN_F32) {
     launch_k(s2d_weight_pack_kernel<float>, dim3((int)ceil_div64(n, 256)), dim3(256), 0,
              (cudaStream_t)stream, w, (float*)w2, Cout, k, pad, k2, pad2);
+  } else if (dtype == ACNN_F16) {
+    launch_k(s2d_weight_pack_kernel<f16>, dim3((int)ceil_div64(n, 256)), dim3(256), 0,
+             (cudaStream_t)stream, w, (f16*)w2, Cout, k, pad, k2, pad2);
   } else {
     launch_k(s2d_weight_pack_kernel<bf16>, dim3((int)ceil_div64(n, 256)), dim3(256), 0,
              (cudaStream_t)stream, w, (bf16*)w2, Cout, k, pad, k2, pad2);

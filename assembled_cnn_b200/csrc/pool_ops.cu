@@ -671,19 +671,6 @@ ce_finalize_kernel(const float* __restrict__ loss_rows, const float* __restrict_
 
 using namespace acnn;
 
-// Storage type of the activation tensors of a call: ACNN_BF16 (production) or ACNN_F32 (parity mode).
-#define ACNN_DTYPE_OK(dt) ((dt) == ACNN_BF16 || (dt) == ACNN_F32)
-#define ACNN_BY_DTYPE(dt, ...)      \
-  do {                              \
-    if ((dt) == ACNN_F32) {         \
-      using T = float;              \
-      __VA_ARGS__;                  \
-    } else {                        \
-      using T = bf16;               \
-      __VA_ARGS__;                  \
-    }                               \
-  } while (0)
-
 template <class T>
 static void launch_avgpool_bwd(dim3 grid, cudaStream_t st, const void* dout, void* dx,
                                const void* add_src, const void* mask_src, int H, int W, int C, int k,

@@ -1,6 +1,7 @@
 // 16-byte vector helpers for the HBM-bound NHWC bf16 kernels (8 channels per thread).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -22,6 +23,7 @@ __device__ __forceinline__ void pdl_entry() {
 #endif
 
 typedef __nv_bfloat16 bf16;
+typedef __half f16;
 
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   const uint32_t w[4] = {u.x, u.y, u.z, u.w};
@@ -61,9 +63,38 @@ __device__ __forceinline__ void storef8(float* p, const float (&f)[8]) {
 __device__ __forceinline__ void load8(const float* p, float (&f)[8]) { loadf8(p, f); }
 __device__ __forceinline__ void store8(float* p, const float (&f)[8]) { storef8(p, f); }
 
+// fp16 activation storage (acnn.h ACNN_F16): exact widening, round-to-nearest-even narrowing
+// (values beyond the fp16 range become +-inf).
+__device__ __forceinline__ void unpack8_f16(const uint4& u, float (&f)[8]) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+    f[2 * i] = t.x;
+    f[2 * i + 1] = t.y;
+  }
+}
+__device__ __forceinline__ uint4 pack8_f16(const float (&f)[8]) {
+  uint32_t w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    __half2 h = __floats2half2_rn(f[2 * i], f[2 * i + 1]);
+    w[i] = *reinterpret_cast<uint32_t*>(&h);
+  }
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+__device__ __forceinline__ void load8(const f16* p, float (&f)[8]) {
+  unpack8_f16(__ldg(reinterpret_cast<const uint4*>(p)), f);
+}
+__device__ __forceinline__ void store8(f16* p, const float (&f)[8]) {
+  *reinterpret_cast<uint4*>(p) = pack8_f16(f);
+}
+
 __device__ __forceinline__ void store1(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ void store1(f16* p, float v) { *p = __float2half_rn(v); }
 __device__ __forceinline__ void store1(float* p, float v) { *p = v; }
 __device__ __forceinline__ float load1(const bf16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ float load1(const f16* p) { return __half2float(*p); }
 __device__ __forceinline__ float load1(const float* p) { return *p; }
 
 // Raw 8-element vector of an activation tensor: loads can be issued back to back (batched ahead
@@ -80,6 +111,17 @@ struct V8<bf16> {
   __device__ __forceinline__ void zero() { r = make_uint4(0, 0, 0, 0); }
   __device__ __forceinline__ void unpack(float (&f)[8]) const { unpack8(r, f); }
   __device__ __forceinline__ void st(bf16* p) const { *reinterpret_cast<uint4*>(p) = r; }
+};
+template <>
+struct V8<f16> {
+  uint4 r;
+  __device__ __forceinline__ void ld(const f16* p) { r = __ldg(reinterpret_cast<const uint4*>(p)); }
+  __device__ __forceinline__ void lds(const uint8_t* base, int elem) {
+    r = *reinterpret_cast<const uint4*>(base + (size_t)elem * 2);
+  }
+  __device__ __forceinline__ void zero() { r = make_uint4(0, 0, 0, 0); }
+  __device__ __forceinline__ void unpack(float (&f)[8]) const { unpack8_f16(r, f); }
+  __device__ __forceinline__ void st(f16* p) const { *reinterpret_cast<uint4*>(p) = r; }
 };
 template <>
 struct V8<float> {
@@ -129,6 +171,23 @@ __device__ __forceinline__ void grad_epilogue(float (&v)[8], const T* add_src,
       if (!(m[i] > 0.f)) v[i] = 0.f;
   }
 }
+
+// Storage types of the `dtype` argument of the elementwise / reduction entry points (acnn.h), and
+// the dispatch that instantiates a launch on the matching element type T.
+#define ACNN_DTYPE_OK(dt) ((dt) == ACNN_BF16 || (dt) == ACNN_F32 || (dt) == ACNN_F16)
+#define ACNN_BY_DTYPE(dt, ...)      \
+  do {                              \
+    if ((dt) == ACNN_F32) {         \
+      using T = float;              \
+      __VA_ARGS__;                  \
+    } else if ((dt) == ACNN_F16) {  \
+      using T = f16;                \
+      __VA_ARGS__;                  \
+    } else {                        \
+      using T = bf16;               \
+      __VA_ARGS__;                  \
+    }                               \
+  } while (0)
 
 // cap of the grid-stride elementwise kernels' grids (acnn_set_stream_grid_cap; common.cu)
 extern int g_stream_grid_cap;

@@ -67,8 +67,8 @@ DEFAULTS = {
     # official/utils/flags/_base.py:50-105, _performance.py:74-137
     "batch_size": 32,
     "train_epochs": 90,                   # main_classification.py:38
-    "dtype": "bf16",                      # reference enum is fp32|fp16; bf16 added
-    "loss_scale": 1,
+    "dtype": "bf16",                      # reference enum is fp32|fp16; bf16 added (the default here)
+    "loss_scale": None,                   # None: the dtype's default, get_loss_scale (fp16: 128, else 1)
     "data_format": "channels_last",       # NHWC is the only layout of this implementation
     "num_gpus": 1,
 }
@@ -96,3 +96,18 @@ def params_from_flags(**overrides) -> dict:
     p = dict(DEFAULTS)
     p.update(overrides)
     return p
+
+
+# official/utils/flags/_performance.py:28-44 DTYPE_MAP: the static loss scale of a dtype when --loss_scale is
+# not given (bf16 keeps the full fp32 exponent range and needs none)
+DEFAULT_LOSS_SCALE = {"fp16": 128, "fp32": 1, "bf16": 1}
+
+
+def get_loss_scale(loss_scale, dtype):
+    """official/utils/flags/_performance.py:39-42 get_loss_scale: an explicit loss_scale wins, otherwise the
+    dtype's default (fp16: 128; bf16 / fp32: 1).  0 counts as 1 (no scaling)."""
+    if dtype not in DEFAULT_LOSS_SCALE:
+        raise ValueError("dtype must be one of: {}".format(tuple(DEFAULT_LOSS_SCALE)))
+    if loss_scale is None:
+        return float(DEFAULT_LOSS_SCALE[dtype])
+    return float(loss_scale or 1)

@@ -66,7 +66,7 @@ class EvalMetrics:
 # Zero-shot retrieval (metric/recall_metric.py:13-228)
 # --------------------------------------------------------------------------------------------------
 SIMILARITIES = {"cosine": 0, "euclidean": 1}
-DTYPES = {"bf16": 0, "fp32": 1}
+DTYPES = {"bf16": 0, "fp32": 1, "fp16": 3}     # acnn.h ACNN_BF16 / ACNN_F32 / ACNN_F16
 KNN_MAX_K = 128      # the largest k of acnn_knn_topk's per-row candidate lists (include/acnn.h)
 
 
@@ -75,7 +75,7 @@ def knn_topk(query, index, k, similarity="cosine", dtype="bf16"):
     with the largest similarity -- (indices int32 [nq, k], similarities fp32 [nq, k]) sorted by
     similarity descending, lower index first on ties (tf.nn.top_k's order).  'cosine' l2-normalises
     the rows, 'euclidean' is the negated squared distance; dtype 'bf16' runs bf16 operands, 'fp32'
-    three bf16 planes per operand.  Enqueued on the current stream; no similarity matrix is stored."""
+    three bf16 planes per operand, 'fp16' fp16 operands (the reference's fp16 search).  Enqueued on the current stream; no similarity matrix is stored."""
     from . import _lib
     lib = _lib.load()
     if similarity not in SIMILARITIES:

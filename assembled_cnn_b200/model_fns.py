@@ -33,7 +33,7 @@ import numpy as np
 import torch
 
 from . import _lib, dp
-from .hparams import DATASETS, DEFAULTS, params_from_flags
+from .hparams import DATASETS, DEFAULTS, get_loss_scale, params_from_flags
 from .plan import BLOCK_SIZES, ModelConfig, build_plan
 from .metrics import EvalMetrics, RecallAtK
 from .runtime import Runtime
@@ -41,12 +41,15 @@ from .native import NativeModel, NativeRuntime
 from .staging import StagingRing, pack_u8, read_ahead
 
 DEFAULT_VERSION = 1
-# dtype: 'bf16' = production path (bf16 storage, fp32 accumulation -- the analogue of the reference's
-# fp16 mode); 'fp32' = the reference's default (nets/resnet_model.py:30-33,
-# official/utils/flags/_performance.py:29-32): fp32 storage, 3-way bf16-split wgmma GEMMs,
-# bit-reproducible reductions -- the mode the 1e-3 parity tests run in.  'fp16' has no H100
-# counterpart here (bf16 replaces it) and is rejected.
-ALLOWED_TYPES = ("bf16", "fp32")
+# dtype: 'bf16' = production path (bf16 storage, fp32 accumulation; the default); 'fp32' = the reference's
+# default (nets/resnet_model.py:30-33, official/utils/flags/_performance.py:29-32): fp32 storage, 3-way
+# bf16-split wgmma GEMMs, bit-reproducible reductions -- the mode the 1e-3 parity tests run in; 'fp16' =
+# the reference's --dtype=fp16 (nets/resnet_model.py:251-303): fp32 variables read as fp16, fp16
+# activation / gradient storage, wgmma .f16.f16 GEMMs with fp32 accumulation, fp32 logits and loss, and a
+# static loss scale of 128 unless loss_scale is given (hparams.get_loss_scale).  fp16 keeps 10 mantissa
+# bits where bf16 keeps 7, at the same tensor-core rate, but only 5 exponent bits: values above 65504
+# become inf (as TF's cast does; nothing skips the step).
+ALLOWED_TYPES = ("bf16", "fp32", "fp16")
 
 # tf.estimator.ModeKeys values
 TRAIN, EVAL, PREDICT = "train", "eval", "infer"
@@ -358,7 +361,8 @@ class Trainer:
             warmup_epochs=p["lr_warmup_epochs"])
         self.global_step = 0
         self.rng = np.random.default_rng(lam_seed)
-        self.loss_scale = float(p.get("loss_scale", 1) or 1)
+        # the reference's get_loss_scale: an explicit loss_scale wins, else 128 for fp16 and 1 otherwise
+        self.loss_scale = get_loss_scale(p.get("loss_scale"), model.dtype)
         self.rt.loss_scale = self.loss_scale
         self.use_graph = use_cuda_graph
         self._graphs = None

@@ -21,7 +21,9 @@ import numpy as np
 from . import _lib
 from .plan import ModelConfig, Param, Slot, Tensor
 
-_DT = {0: "bf16", 1: "f32", 2: "i32"}
+_DT = {0: "bf16", 1: "f32", 2: "i32", 3: "f16"}
+# model dtype <-> acnn_model_config.dtype (ACNN_BF16 / ACNN_F32 / ACNN_F16)
+_CFG_DTYPE = {"bf16": 0, "fp32": 1, "fp16": 3}
 
 
 class Config(C.Structure):
@@ -130,8 +132,8 @@ def crc32c(data, crc=0):
 def make_config(cfg: ModelConfig, batch, height, width, *, training=True, mixup_type=0,
                 label_smoothing=0.0, with_loss=True, dtype="bf16", use_dropblock=False, kd_temp=0.0,
                 deterministic=None, loss_scale=1.0, eps=1e-5) -> Config:
-    if dtype not in ("bf16", "fp32"):
-        raise ValueError("dtype must be one of: ('bf16', 'fp32')")
+    if dtype not in _CFG_DTYPE:
+        raise ValueError("dtype must be one of: ('bf16', 'fp32', 'fp16')")
     c = Config()
     lib().acnn_model_config_init(C.byref(c))
     for k in ("resnet_size", "num_classes", "resnet_version", "embedding_size",
@@ -147,7 +149,7 @@ def make_config(cfg: ModelConfig, batch, height, width, *, training=True, mixup_
     c.bn_momentum, c.bn_epsilon = float(cfg.bn_momentum), float(eps)
     c.batch, c.height, c.width = int(batch), int(height), int(width)
     c.training, c.mixup_type, c.with_loss = int(bool(training)), int(mixup_type), int(bool(with_loss))
-    c.dtype = 1 if dtype == "fp32" else 0
+    c.dtype = _CFG_DTYPE[dtype]
     c.use_dropblock = int(bool(use_dropblock))
     c.deterministic = -1 if deterministic is None else int(bool(deterministic))
     c.fuse_bn_pairs = int(os.environ.get("ACNN_FUSE_BN_PAIRS", "1") == "1")
@@ -211,7 +213,7 @@ class NativeModel:
                          mixup_type=c.mixup_type if c.training else 0,
                          label_smoothing=c.label_smoothing, num_classes=c.num_classes,
                          ld_logits=s.ld_logits, bn_momentum=c.bn_momentum,
-                         dtype="fp32" if c.dtype == 1 else "bf16",
+                         dtype={v: k for k, v in _CFG_DTYPE.items()}[c.dtype],
                          use_dropblock=bool(c.use_dropblock and c.training),
                          kd_temp=c.kd_temp if c.training else 0.0, input_batch=s.input_batch,
                          dropblock_u=[])
@@ -300,19 +302,20 @@ class NativeRuntime(_runtime_base()):
         self.bn_momentum = c.bn_momentum
         self.training = bool(c.training)
         self.fp32 = c.dtype == 1
-        self.adt = 1 if self.fp32 else 0
+        self.adt = c.dtype                   # ACNN_BF16 / ACNN_F32 / ACNN_F16
         self.planes = 3 if self.fp32 else 1
+        wdt = torch.float16 if self.adt == 3 else torch.bfloat16
         self.det = int(self.fp32 if c.deterministic < 0 else bool(c.deterministic))
         f32 = dict(dtype=torch.float32, device=self.dev)
         if share is not None:
             if share.plan.param_elems != s.param_elems or share.plan.state_elems != s.state_elems \
-                    or share.fp32 != self.fp32:
+                    or share.adt != self.adt:
                 raise ValueError("NativeRuntime(share=...): parameter layouts differ")
             self.params, self.state, self.w_fprop = share.params, share.state, share.w_fprop
         else:
             self.params = torch.zeros(s.param_elems, **f32)
             self.state = torch.zeros(max(s.state_elems, 1), **f32)
-            self.w_fprop = torch.zeros(s.w_fprop_elems, dtype=torch.bfloat16, device=self.dev)
+            self.w_fprop = torch.zeros(s.w_fprop_elems, dtype=wdt, device=self.dev)
             for p in model.state.values():
                 if p.kind == "moving_variance":
                     self.state[p.offset:p.offset + p.size] = 1.0
@@ -320,7 +323,7 @@ class NativeRuntime(_runtime_base()):
             self.grads = torch.zeros(s.param_elems, **f32)
             self.momentum = share.momentum if (share is not None and share.momentum is not None) \
                 else torch.zeros(s.param_elems, **f32)
-            self.w_dgrad = torch.zeros(s.w_dgrad_elems, dtype=torch.bfloat16, device=self.dev)
+            self.w_dgrad = torch.zeros(s.w_dgrad_elems, dtype=wdt, device=self.dev)
         else:
             self.grads = self.momentum = self.w_dgrad = None
         self.workspace = torch.zeros(s.workspace_bytes, dtype=torch.uint8, device=self.dev)
@@ -332,7 +335,8 @@ class NativeRuntime(_runtime_base()):
         self.zero = view(s.zero_offset, max(s.zero_bytes, 4), torch.float32)
         self.work = view(s.work_offset, max(s.work_bytes, 4), torch.float32)
         self.decay_flags = view(s.decay_flags_offset, max(s.param_elems // 256, 1), torch.uint8)
-        tdt = {"bf16": (torch.bfloat16, 2), "f32": (torch.float32, 4), "i32": (torch.int32, 4)}
+        tdt = {"bf16": (torch.bfloat16, 2), "f32": (torch.float32, 4), "f16": (torch.float16, 2),
+               "i32": (torch.int32, 4)}
         self.t = {}
         for name, t in model.tensors.items():
             dt, esz = tdt[t.dtype]

@@ -255,12 +255,14 @@ class PlanBuilder:
         # (bn_backward2; ACNN_FUSE_BN_PAIRS=0 keeps the separate kernels for A/B runs)
         self.fuse_bn_pairs = os.environ.get("ACNN_FUSE_BN_PAIRS", "1") == "1"
         self._identity_bns = {}
-        if dtype not in ("bf16", "fp32"):
-            raise ValueError("dtype must be one of: ('bf16', 'fp32')")
+        if dtype not in ("bf16", "fp32", "fp16"):
+            raise ValueError("dtype must be one of: ('bf16', 'fp32', 'fp16')")
         # fp32 = the reference's default dtype (nets/resnet_model.py:30-33): fp32 activation storage,
-        # conv GEMMs on 3-way bf16-split operands, deterministic reductions -- the parity mode
+        # conv GEMMs on 3-way bf16-split operands, deterministic reductions -- the parity mode.
+        # fp16 = the reference's --dtype=fp16 (nets/resnet_model.py:251-303): the bf16 plan, op for op,
+        # with fp16 activation / gradient storage and fp16 GEMM operands
         self.fp32 = dtype == "fp32"
-        self.adt = "f32" if self.fp32 else "bf16"
+        self.adt = {"bf16": "bf16", "fp32": "f32", "fp16": "f16"}[dtype]
         self._planes = {}
         if height % 32 or width % 32:
             raise ValueError("input size must be a multiple of 32 (got %dx%d)" % (height, width))

@@ -13,7 +13,9 @@ import torch
 from . import _lib
 from .plan import Plan, Geom, Slot
 
-_TORCH_DTYPE = {"bf16": torch.bfloat16, "f32": torch.float32, "i32": torch.int32}
+_TORCH_DTYPE = {"bf16": torch.bfloat16, "f32": torch.float32, "f16": torch.float16, "i32": torch.int32}
+# plan dtype -> (ACNN_* storage type of the activations, torch dtype of the weight operand copies)
+_ACNN_DTYPE = {"bf16": (0, torch.bfloat16), "fp32": (1, torch.bfloat16), "fp16": (3, torch.float16)}
 
 
 def _check_u8_images(images_u8, images, mean):
@@ -74,7 +76,8 @@ class Runtime:
         self.training = plan.meta["training"]
         # fp32 plan = parity mode: fp32 activations, 3-plane GEMM operands, deterministic reductions
         self.fp32 = plan.meta.get("dtype", "bf16") == "fp32"
-        self.adt = 1 if self.fp32 else 0               # ACNN_F32 / ACNN_BF16
+        # ACNN_BF16 / ACNN_F32 / ACNN_F16 (the reference's fp16: fp16 activations and GEMM operands)
+        self.adt, wdt = _ACNN_DTYPE[plan.meta.get("dtype", "bf16")]
         self.planes = 3 if self.fp32 else 1
         # deterministic: also the split-K of wgrad and of the small SK / SE GEMMs is disabled (one add
         # per output element).  Every reduction is ordered in both modes (split-K partials are summed
@@ -84,14 +87,13 @@ class Runtime:
         if share is not None:
             # same model, another batch shape / mode: the variables are shared, not copied
             if share.plan.param_elems != plan.param_elems or share.plan.state_elems != plan.state_elems \
-                    or share.fp32 != self.fp32:
+                    or share.adt != self.adt:
                 raise ValueError("Runtime(share=...): parameter layouts differ")
             self.params, self.state, self.w_fprop = share.params, share.state, share.w_fprop
         else:
             self.params = torch.zeros(plan.param_elems, **f32)
             self.state = torch.zeros(max(plan.state_elems, 1), **f32)
-            self.w_fprop = torch.zeros(self.planes * plan.param_elems, dtype=torch.bfloat16,
-                                       device=self.dev)
+            self.w_fprop = torch.zeros(self.planes * plan.param_elems, dtype=wdt, device=self.dev)
         self.zero = torch.zeros(max(plan.zero_elems, 1), **f32)
         self.work = torch.zeros(max(plan.work_elems, 1), **f32)
         if self.training:
@@ -100,8 +102,7 @@ class Runtime:
                 self.momentum = share.momentum
             else:
                 self.momentum = torch.zeros(plan.param_elems, **f32)
-            self.w_dgrad = torch.zeros(self.planes * max(plan.dgrad_elems, 1), dtype=torch.bfloat16,
-                                       device=self.dev)
+            self.w_dgrad = torch.zeros(self.planes * max(plan.dgrad_elems, 1), dtype=wdt, device=self.dev)
         else:
             self.grads = self.momentum = self.w_dgrad = None
         # device hyper-parameters: lr, momentum, wd, grad_scale, dropblock keep_prob, global step
@@ -386,7 +387,11 @@ class Runtime:
 
     # ---------------------------------------------------------------- forward ops
     def op_prep_weights(self, op):
-        if self.n_descs:
+        if self.n_descs and self.adt == 3:
+            self._chk(self.lib.acnn_prep_weights_f16(
+                self.params.data_ptr(), self.descs.data_ptr(), self.n_descs, self.w_fprop.data_ptr(),
+                self.w_dgrad.data_ptr() if self.w_dgrad is not None else None, self.stream), op)
+        elif self.n_descs:
             self._chk(self.lib.acnn_prep_weights(
                 self.params.data_ptr(), self.descs.data_ptr(), self.n_descs,
                 self.w_fprop.data_ptr(),

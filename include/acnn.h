@@ -33,9 +33,14 @@ extern "C" {
 /* Storage type of the activation tensors of a call (`dtype` arguments): bf16 is the production
  * path; fp32 is the parity mode (the reference's own default dtype, nets/resnet_model.py:30-33):
  * fp32 activations, every elementwise / reduction kernel instantiated on float, and the conv GEMMs
- * run on operands split into three bf16 planes (`precision` = 1 below). */
+ * run on operands split into three bf16 planes (`precision` = 1 below).  fp16 is the reference's
+ * --dtype=fp16 (nets/resnet_model.py:251-303): fp16 activations and gradients (round to nearest
+ * even, overflow to inf), fp32 accumulation wherever the bf16 path accumulates in fp32, and the conv
+ * GEMMs on fp16 operands (`precision` = ACNN_F16 below, wgmma .f16.f16, the bf16 path's tiles).
+ * 2 is not a storage type. */
 #define ACNN_BF16 0
 #define ACNN_F32 1
+#define ACNN_F16 3
 
 /* Library / environment ------------------------------------------------------------------- */
 const char* acnn_last_error(void);
@@ -124,6 +129,8 @@ typedef struct acnn_conv_geom {
  *                                     to zero); parts = acnn_conv_stats_parts(g); acnn_bn_finalize
  *                                     adds the rows in a fixed order (bit-reproducible)
  * out_f32 != 0 stores y as fp32 (logits), else bf16.  Requires Cin % 16 == 0, Cout % 32 == 0.
+ * precision ACNN_F16 (3): x, w, add_src, mask_src and a 16-bit y are fp16 instead of bf16 (the
+ * statistics are of the fp16-rounded output); everything else as precision 0.
  * precision 0: x, w bf16.  precision 1 (fp32 parity mode): x and w are each three consecutive bf16
  * planes hi / mid / lo of an fp32 tensor (acnn_split3, acnn_prep_weights(planes = 3)); plane p of x
  * starts at x + p * numel(x), plane p of w at w + p * w_plane_stride elements; the six significant
@@ -141,7 +148,8 @@ int acnn_conv_stats_parts(const acnn_conv_geom* g);
  * of tf.layers.conv2d the reference gets from tf.gradients, nets/optimizer_setting.py:30).
  * w_dgrad is [Cin][kh][kw][Cout] with taps already flipped (acnn_prep_weights writes it).
  * Same optional add_src / mask_src epilogue as acnn_conv_fprop (shapes of dx).  precision 1: dy and
- * w_dgrad are 3-plane operands, dx is fp32 and no epilogue may be fused. */
+ * w_dgrad are 3-plane operands, dx is fp32 and no epilogue may be fused.  precision ACNN_F16: dy,
+ * w_dgrad, dx, add_src and mask_src are fp16. */
 int acnn_conv_dgrad(const acnn_conv_geom* g, const void* dy, const void* w_dgrad, void* dx,
                     const void* add_src, const void* mask_src, int precision,
                     int64_t w_plane_stride, void* stream);
@@ -150,7 +158,7 @@ int acnn_conv_dgrad(const acnn_conv_geom* g, const void* dy, const void* w_dgrad
  * splits store their partials in a stream-ordered scratch of the launch (cudaMallocAsync on `stream`)
  * and a second kernel on `stream` adds them to dw in split order (bit-reproducible).  dw must be zeroed
  * (or hold the running sum) by the caller.  deterministic != 0: no split (one add per element).
- * precision 1: x and dy are 3-plane operands. */
+ * precision 1: x and dy are 3-plane operands.  precision ACNN_F16: x and dy are fp16. */
 int acnn_conv_wgrad(const acnn_conv_geom* g, const void* x, const void* dy, float* dw,
                     int precision, int deterministic, void* stream);
 /* The split layout acnn_conv_wgrad(g, ..., precision, deterministic, ...) would launch with the
@@ -394,6 +402,10 @@ typedef struct acnn_weight_desc {
 int acnn_prep_weights(const float* master, const acnn_weight_desc* descs, int n, void* w_fprop,
                       void* w_dgrad, int planes, int64_t fprop_plane_stride,
                       int64_t dgrad_plane_stride, void* stream);
+/* The same with ONE fp16 copy of each layout (ACNN_F16: the fp32 master read as fp16, rounded to
+ * nearest even; a weight beyond the fp16 range becomes +-inf). */
+int acnn_prep_weights_f16(const float* master, const acnn_weight_desc* descs, int n, void* w_fprop,
+                          void* w_dgrad, void* stream);
 /* Stem: master [Cout][k][k][3] fp32 -> bf16 [Cout][k2][k2][16] for the space-to-depth input
  * (k2 taps, see acnn_pack_input); and the inverse gather-add for its gradient. */
 int acnn_s2d_weight_pack(const float* w, void* w2, int Cout, int k, int pad, int k2, int pad2,
@@ -442,7 +454,10 @@ int acnn_replica_accumulate(int phase, float* acc_grads, float* grads, float* st
  * metric 1 = euclidean: -((|q|^2 + |x|^2) - 2 q.x) on the raw rows (tf_simple_pairwise_distance,
  * negated), the squared norms taken over the rounded operands.
  * dtype ACNN_BF16: bf16 operands, fp32 accumulation; ACNN_F32: three bf16 planes per operand (as the
- * conv GEMMs), whose six significant cross products are accumulated in fp32.
+ * conv GEMMs), whose six significant cross products are accumulated in fp32; ACNN_F16: fp16 operands
+ * (round to nearest even; a row with an entry beyond +-65504 after the normalisation gets an infinite
+ * operand and is not ranked), fp32 accumulation -- the reference's fp16 search
+ * (metric/recall_metric.py:68-73).
  * out_idx int32 [nq][k], out_sim fp32 [nq][k].  Any d >= 1 (<= 2^24); 1 <= k <= 128 (k > 128:
  * ACNN_ERR_UNSUPPORTED); k > nx, non-positive sizes, an unknown metric or dtype: ACNN_ERR_INVALID.
  * All of these are checked before any CUDA call.  The result is the same bit for bit for every
@@ -450,10 +465,10 @@ int acnn_replica_accumulate(int phase, float* acc_grads, float* grads, float* st
  * than k of them (a NaN or infinite input, or a squared distance that overflows fp32) is padded with
  * (similarity -inf, index 2147483647) entries -- callers that index with out_idx must check for it.
  * work: acnn_knn_work_bytes(...) bytes, caller-owned; every section starts at a 256-byte boundary:
- *   Q' bf16 [nq][K'], X' bf16 [nx][K']  (K' = P * roundup(d, 64), zero-padded; P = 1 for bf16, 6 for
+ *   Q' bf16 [nq][K'], X' bf16 [nx][K']  (fp16 for ACNN_F16; K' = P * roundup(d, 64), zero-padded; P = 1 for bf16 / fp16, 6 for
  *        fp32: K' holds six d-segments so that one bf16 GEMM forms the six plane products, smallest
  *        first -- Q' = (hi, mid, lo, hi, mid, hi), X' = (lo, mid, hi, mid, hi, hi))
- *   |q|^2 fp32 [nq], |x|^2 fp32 [nx]   (of the rounded operands: bf16, or (hi + mid) + lo)
+ *   |q|^2 fp32 [nq], |x|^2 fp32 [nx]   (of the rounded operands: bf16 / fp16, or (hi + mid) + lo)
  *   partial lists: similarity fp32 [8][nq][k], index int32 [8][nq][k]  (one per column split) */
 int acnn_knn_topk(const float* q, const float* x, int nq, int nx, int d, int k, int metric, int dtype,
                   int32_t* out_idx, float* out_sim, void* work, int64_t work_bytes, void* stream);

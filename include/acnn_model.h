@@ -66,7 +66,7 @@ typedef struct acnn_model_config {
   int32_t training;               /* 1: batch statistics + backward + SGD; 0: moving statistics */
   int32_t mixup_type;             /* 0 | 1 (input batch = 2*batch) | 2 */
   int32_t with_loss;              /* eval: also run the loss ops */
-  int32_t dtype;                  /* ACNN_BF16 | ACNN_F32 (parity mode) */
+  int32_t dtype;                  /* ACNN_BF16 | ACNN_F32 (parity mode) | ACNN_F16 (the reference's fp16) */
   int32_t use_dropblock;
   int32_t deterministic;          /* -1: only in the fp32 mode; 0 / 1 */
   int32_t fuse_bn_pairs;          /* 1 (default): one backward pass for the two BNs of a projection block */
@@ -84,9 +84,10 @@ void acnn_destroy(acnn_model* m);
 typedef struct acnn_model_sizes {
   int64_t param_elems;     /* fp32 elements of params / grads / momentum (tensors 256-aligned) */
   int64_t state_elems;     /* fp32 elements of the BN moving statistics buffer */
-  int64_t dgrad_elems;     /* bf16 elements of one plane of the dgrad-layout weight copies */
-  int64_t w_fprop_elems;   /* bf16 elements the caller allocates for w_fprop (planes * param_elems) */
-  int64_t w_dgrad_elems;   /* bf16 elements the caller allocates for w_dgrad (training only) */
+  int64_t dgrad_elems;     /* 16-bit elements of one plane of the dgrad-layout weight copies */
+  int64_t w_fprop_elems;   /* 16-bit (bf16, fp16 in ACNN_F16) elements the caller allocates for w_fprop
+                              (planes * param_elems) */
+  int64_t w_dgrad_elems;   /* 16-bit elements the caller allocates for w_dgrad (training only) */
   int64_t workspace_bytes;
   /* byte offsets inside the workspace of the pieces a host reads or writes directly */
   int64_t hp_offset;          /* float[8]: lr, momentum, weight_decay, grad_scale, dropblock keep_prob,
@@ -136,7 +137,7 @@ int acnn_variable_unpack(const acnn_model* m, int i, const float* stored, float*
 #define ACNN_I32 2
 typedef struct acnn_tensor_info {
   char name[64];
-  int32_t dtype;           /* ACNN_BF16 | ACNN_F32 | ACNN_I32 */
+  int32_t dtype;           /* ACNN_BF16 | ACNN_F32 | ACNN_F16 | ACNN_I32 */
   int32_t rank;
   int64_t shape[5];
   int64_t offset;          /* bytes, inside the workspace */
