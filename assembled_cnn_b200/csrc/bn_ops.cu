@@ -252,7 +252,7 @@ bn_bwd_reduce_kernel(const T* __restrict__ g, const T* __restrict__ y,
   float acc[2][8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[0][i] = acc[1][i] = 0.f;
-  // 4 rows per trip.  The loads are unconditional (row index clamped, contribution zeroed) so
+  // 4 rows per trip.  The loads are unconditional (row index clamped, the duplicate row skipped) so
   // that all 8 of them are issued back to back: 8 x 16 B in flight per thread.
   const int64_t step = (int64_t)gridDim.x * RPB;
   for (int64_t r0 = (int64_t)blockIdx.x * RPB + rsub; r0 < M; r0 += 4 * step) {
@@ -267,12 +267,13 @@ bn_bwd_reduce_kernel(const T* __restrict__ g, const T* __restrict__ y,
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int64_t r = r0 + u * step;
-      const float valid = r < M ? 1.f : 0.f;
+      // skipped, not multiplied by 0: an inf in the clamped row would add 0 * inf = NaN
+      if (r >= M) continue;
       float gv[8], yv[8];
       gq[u].unpack(gv);
       yq[u].unpack(yv);
       if (gate || addbc) {
-        const int64_t bimg = (r < M ? r : M - 1) / HW;
+        const int64_t bimg = r / HW;
         if (gate) {
           float t[8];
           loadf8(gate + bimg * C + c0, t);
@@ -288,9 +289,8 @@ bn_bwd_reduce_kernel(const T* __restrict__ g, const T* __restrict__ y,
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float gg = gv[i] * valid;
-        acc[0][i] += gg;
-        acc[1][i] += gg * ((yv[i] - mu[i]) * rs[i]);
+        acc[0][i] += gv[i];
+        acc[1][i] += gv[i] * ((yv[i] - mu[i]) * rs[i]);
       }
     }
   }
@@ -335,18 +335,16 @@ bn_bwd_reduce2_kernel(const T* __restrict__ g, const T* __restrict__ ya, const T
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      const int64_t r = r0 + u * step;
-      const float valid = r < M ? 1.f : 0.f;
+      if (r0 + u * step >= M) continue;     // the clamped duplicate row (see bn_bwd_reduce_kernel)
       float gv[8], av[8], bv[8];
       gq[u].unpack(gv);
       aq[u].unpack(av);
       bq[u].unpack(bv);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float gg = gv[i] * valid;
-        acc_a[0][i] += gg;
-        acc_a[1][i] += gg * ((av[i] - mua[i]) * rsa[i]);
-        acc_b[1][i] += gg * ((bv[i] - mub[i]) * rsb[i]);
+        acc_a[0][i] += gv[i];
+        acc_a[1][i] += gv[i] * ((av[i] - mua[i]) * rsa[i]);
+        acc_b[1][i] += gv[i] * ((bv[i] - mub[i]) * rsb[i]);
       }
     }
   }
@@ -540,8 +538,9 @@ image_reduce_kernel(const T* __restrict__ p0, const T* __restrict__ p1,
       loadf8(shift + f + c0, h1);
     }
   }
-  // U rows per trip: all loads of a trip are issued before any math (row clamped, contribution
-  // zeroed), since only ~1.7 CTAs of 256 threads are resident per SM (grid = images)
+  // U rows per trip: all loads of a trip are issued before any math (row clamped, the duplicate
+  // row skipped -- not multiplied by 0, which turns an inf in it into NaN), since only ~1.7 CTAs of
+  // 256 threads are resident per SM (grid = images)
   constexpr int U = (MODE == 1 || MODE == 3) ? 4 : 1;   // measured: batching only pays with 3 loads/row
   for (int rb = rsub; rb < HW; rb += U * RPB) {
     V8<T> qa[U], qb[U], qc[U];
@@ -556,7 +555,7 @@ image_reduce_kernel(const T* __restrict__ p0, const T* __restrict__ p1,
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      const float valid = (rb + u * RPB) < HW ? 1.f : 0.f;
+      if (rb + u * RPB >= HW) continue;
       if (MODE == 0 || MODE == 1) {
         float y0[8], y1[8], dv[8];
         qa[u].unpack(y0);
@@ -566,7 +565,7 @@ image_reduce_kernel(const T* __restrict__ p0, const T* __restrict__ p1,
         for (int i = 0; i < 8; ++i) {
           const float u0 = fmaxf(fmaf(y0[i], s0[i], h0[i]), 0.f);
           const float u1 = fmaxf(fmaf(y1[i], s1[i], h1[i]), 0.f);
-          acc[i] += valid * ((MODE == 0) ? (u0 + u1) : dv[i] * (u0 - u1));
+          acc[i] += (MODE == 0) ? (u0 + u1) : __fmul_rn(dv[i], u0 - u1);
         }
       } else if (MODE == 2 || MODE == 3) {
         float yv[8], gv[8];
@@ -575,13 +574,14 @@ image_reduce_kernel(const T* __restrict__ p0, const T* __restrict__ p1,
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const float t = fmaf(yv[i], s0[i], h0[i]);
-          acc[i] += valid * ((MODE == 2) ? t : gv[i] * t);
+          // g * t is rounded before the add (__fmul_rn: never contracted into an fma)
+          acc[i] += (MODE == 2) ? t : __fmul_rn(gv[i], t);
         }
       } else {
         float xv[8];
         qa[u].unpack(xv);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] += valid * xv[i];
+        for (int i = 0; i < 8; ++i) acc[i] += xv[i];
       }
     }
   }

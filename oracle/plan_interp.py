@@ -7,7 +7,16 @@ adjoints taken by autograd where that is the definition), so that
   * on CPU, the whole plan -- topology, gradient accumulation, parameter order -- is checked
     against the autograd oracle (oracle/model.py) without a GPU, and
   * on the GPU box, each CUDA kernel and the whole step are checked against it, optionally with the
-    same bf16 rounding points as the CUDA path (`emulate_bf16=True`).
+    same storage rounding points as the CUDA path (`emulate_storage=True`).
+
+Storage emulation: every stored 16-bit tensor is rounded to its own declared type -- "bf16" to
+bfloat16, "f16" to float16 -- and the conv weights (GEMM operands, `wq`) to the plan's element type
+(plan.meta["dtype"]), each with round to nearest even and overflow to inf, as torch's .bfloat16() /
+.half() do.  fp32 tensors and fp32 plans are never rounded.  `emulate_bf16` is the older name of
+`emulate_storage` and means the same (on a bf16 plan every 16-bit tensor is "bf16").
+`emulate_storage` may also name one 16-bit type ("bf16" or "f16") that every 16-bit tensor and weight
+is rounded to instead of its own: a deliberately wrong emulation, for tests that show the choice of
+type is visible.
 """
 from __future__ import annotations
 
@@ -27,11 +36,21 @@ def _nhwc(x):
     return x.permute(0, 2, 3, 1)
 
 
+_ROUND = {"bf16": torch.bfloat16, "f16": torch.float16}
+_ELEMENT_TYPE = {"bf16": "bf16", "fp16": "f16", "fp32": "f32"}
+
+
 class PlanInterpreter:
-    def __init__(self, plan, dtype=torch.float32, emulate_bf16=False, eps=1e-5):
+    def __init__(self, plan, dtype=torch.float32, emulate_storage=False, eps=1e-5, emulate_bf16=None):
         self.plan = plan
         self.dtype = dtype
-        self.emu = emulate_bf16
+        if emulate_bf16 is not None:
+            emulate_storage = emulate_storage or emulate_bf16
+        if emulate_storage not in (False, True, "bf16", "f16"):
+            raise ValueError("emulate_storage must be a bool, 'bf16' or 'f16'")
+        self.emu = bool(emulate_storage)
+        self.emu_as = emulate_storage if isinstance(emulate_storage, str) else None
+        self.adt = _ELEMENT_TYPE[plan.meta.get("dtype", "bf16")]
         self.eps = eps
         self.t = {}                                   # activation tensors by name
         self.params = torch.zeros(plan.param_elems, dtype=dtype)
@@ -86,16 +105,21 @@ class PlanInterpreter:
         return buf[s.offset:s.offset + s.size]
 
     # ---------------------------------------------------------------- helpers
+    def round_to(self, value, tdt):
+        """value rounded to the 16-bit storage type tdt ("bf16" / "f16"; anything else: unchanged)."""
+        if not self.emu or tdt not in _ROUND:
+            return value
+        return value.to(_ROUND[self.emu_as or tdt]).to(self.dtype)
+
     def store(self, name, value):
         t = self.plan.tensors[name]
-        value = value.to(self.dtype)
-        if self.emu and t.dtype == "bf16":
-            value = value.bfloat16().to(self.dtype)
+        value = self.round_to(value.to(self.dtype), t.dtype)
         assert tuple(value.shape) == tuple(t.shape), (name, value.shape, t.shape)
         self.t[name] = value
 
     def wq(self, w):
-        return w.bfloat16().to(self.dtype) if self.emu else w
+        """A conv / dense weight as the GEMM reads it: rounded to the plan's element type."""
+        return self.round_to(w, self.adt)
 
     def _conv(self, x, w_ohwi, g):
         xp = F.pad(_nchw(x), (g.pad_w_lo, g.pad_w_hi, g.pad_h_lo, g.pad_h_hi))

@@ -9,6 +9,11 @@ of bf16 data cancel (BN backward sums), 1e-4 otherwise.
 
 The fp32 parity mode (dtype='fp32': fp32 storage, 3-plane wgmma GEMMs) runs the same lock-step
 against the exact fp32 interpreter with every tensor at 2e-5 and the reductions at 2e-4.
+
+The fp16 mode (dtype='fp16': fp16 storage, f16 wgmma GEMMs) runs it against the float64 interpreter
+rounding every stored tensor and GEMM weight to fp16 (tests/test_fp16_lockstep_gpu.py): fp16 tensors
+at 2^-10 (one fp16 ulp at the top of the range), everything else as in the bf16 mode.  `loss_scale`
+runs the backward at a static loss scale (the reference's fp16 recipes use 128).
 """
 import os
 import sys
@@ -21,6 +26,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 BF16_TOL = 2.0 ** -7
+F16_TOL = 2.0 ** -10
 F32_TOL = 2e-3
 
 
@@ -106,7 +112,11 @@ def _err(got, ref):
 
 
 def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbose=False,
-             dtype="bf16", use_dropblock=False, kd_temp=0.0, keep_prob=0.9):
+             dtype="bf16", use_dropblock=False, kd_temp=0.0, keep_prob=0.9, loss_scale=1.0,
+             emulate_storage=True, plan_hook=None):
+    """Returns (failures, worst error per 'op.kind:output kind').  emulate_storage is passed to the
+    interpreter of the 16-bit modes (a type name there makes it round to the wrong type on purpose);
+    plan_hook(plan, runtime) runs once before the first op."""
     H, W = (HW, HW) if isinstance(HW, int) else HW
     from oracle import model as M, plan_interp as PI
     from assembled_cnn_b200.plan import ModelConfig, build_plan
@@ -114,7 +124,9 @@ def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbo
 
     cfg = ModelConfig(use_resnet_d=use_resnet_d, **cfg_kw)
     fp32 = dtype == "fp32"
-    bf16_tol, f32_tol = (2e-5, 2e-4) if fp32 else (BF16_TOL, F32_TOL)
+    # tensors by their storage type; fp32 slots, gradients and partial rows
+    t_tol = {"bf16": 2e-5, "f32": 2e-5} if fp32 else {"bf16": BF16_TOL, "f16": F16_TOL, "f32": 1e-4}
+    f32_tol = 2e-4 if fp32 else F32_TOL
     plan = build_plan(cfg, B, H, W, training=training, mixup_type=mix, label_smoothing=0.1,
                       dtype=dtype, use_dropblock=use_dropblock, kd_temp=kd_temp)
     _, vs = M.build(seed=42, input_hw=64, use_resnet_d=use_resnet_d, **cfg_kw)
@@ -126,14 +138,22 @@ def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbo
             vs.vars[n] = 0.1 * torch.randn(vs.vars[n].shape, generator=g)
         elif n.endswith("moving_variance"):
             vs.vars[n] = 0.5 + torch.rand(vs.vars[n].shape, generator=g)
-    it = PI.PlanInterpreter(plan, dtype=torch.float64 if fp32 else torch.float32,
-                            emulate_bf16=not fp32)
+    # fp16: float64 with the fp16 roundings at the store points (fp16 x fp16 products are exact in
+    # fp32, so what remains is fp32 summation order and one storage rounding)
+    it = PI.PlanInterpreter(plan, dtype=torch.float32 if dtype == "bf16" else torch.float64,
+                            emulate_storage=False if fp32 else emulate_storage)
     rt = Runtime(plan)
     it.set_weights(vs.vars)
     rt.set_weights(vs.vars)
     hp = dict(lr=0.05, momentum=0.9, weight_decay=1e-4, keep_prob=keep_prob)
     it.hp.update(hp)
     rt.set_hparams(**hp)
+    # static loss scale: the loss gradient is scaled by it, the SGD step unscales the gradients
+    it.hp.update(grad_scale=loss_scale, sgd_grad_scale=1.0 / loss_scale)
+    rt.loss_scale = loss_scale
+    rt.set_hparams(grad_scale=1.0 / loss_scale)
+    if plan_hook is not None:
+        plan_hook(plan, rt)
     rt.dropblock_feed = True          # masks from the fed uniforms (identical on both sides)
     m = plan.meta
     Bin = m["input_batch"]
@@ -166,7 +186,7 @@ def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbo
             kind = out[0]
             if kind == "t":
                 ref, got = it.t[out[1]], rt.t[out[1]]
-                tol = bf16_tol if plan.tensors[out[1]].dtype == "bf16" else (2e-5 if fp32 else 1e-4)
+                tol = t_tol[plan.tensors[out[1]].dtype]
                 force = lambda r=ref, gt=got: gt.copy_(r)
             elif kind == "slot":
                 ref, got = it.slot(out[1]), rt.slot_view(out[1])

@@ -20,6 +20,8 @@ there); each one is shown sharp enough by tests/test_stream_ops_cpu.py.
   acnn_sk_gap / _bwd_gate          test_sk_plan_shapes             test_sk_edges                    restated            reduction per image
   acnn_sk_combine                  test_sk_plan_shapes             test_sk_edges                    restated (sk_attention) elementwise, 5 ops
   acnn_sk_bn_bwd_reduce / _apply   test_sk_plan_shapes             test_sk_edges                    restated            reduction per slab / 6 ops
+  acnn_se_gap                      test_se_reductions_plan_shapes  test_se_reductions_edges         restated            reduction per image
+  acnn_se_bwd_gate                 (both in tests/test_image_reduce_ops_gpu.py, bf16 / fp16 / fp32)  restated            reduction per image
   acnn_blurpool_fwd / _bwd         test_blurpool_plan_shapes       test_blurpool_edges              anti_aliased_downsample  filt^2 chain
   acnn_avgpool_fwd / _bwd          test_avgpool_plan_shapes        test_avgpool_edges               restated, = avg_pool_bl / _resnet_d  k^2 chain
   acnn_maxpool_fwd / _bwd          test_maxpool_production         test_maxpool_edges               restated, = max_pool_same  exact / k^2 chain
