@@ -14,7 +14,8 @@ Decoding is imagenet_c.decode_rgb (PIL); the channel means are imagenet_c.CHANNE
 The TFRecord writer of the knowledge-distillation shards (model_fns.extract_teacher_logits, the reference's
 datasets/build_imagenet_data.py --logits_file_path) is here too, so the record format lives in one module:
 write_record frames a record, add_float_feature adds a float feature to a serialised Example and
-FloatFeatureWriter copies whole files with one added to every record.
+FloatFeatureWriter copies whole files with one added to every record.  serialize_example writes a whole
+Example (the dataset builders, build_data).
 """
 from __future__ import annotations
 
@@ -233,6 +234,34 @@ def _encode_varint(v):
 def _len_field(field, payload_len):
     """The key and length of a length-delimited field (wire type 2) of payload_len bytes."""
     return _encode_varint(field << 3 | 2) + _encode_varint(payload_len)
+
+
+def serialize_example(features):
+    """A serialised tf.train.Example of `features` {key: (kind, values)}, kind 'bytes' (a list of bytes),
+    'int64' or 'float' (a list of numbers; float32 on the wire).  The map entries go in key order and the
+    numeric lists packed, as proto3 writes them; an empty list still sets the Feature's kind, as
+    tf.train.Feature(float_list=tf.train.FloatList(value=[])) does."""
+    entries = []
+    for key in sorted(features):
+        kind, values = features[key]
+        kb = key.encode() if isinstance(key, str) else key
+        if kind == "bytes":
+            body = b"".join(_len_field(1, len(v)) + v for v in values)
+            feature = _len_field(1, len(body)) + body                       # Feature.bytes_list
+        elif kind == "float":
+            vals = np.asarray(values, dtype="<f4").tobytes()
+            body = _len_field(1, len(vals)) + vals if vals else b""
+            feature = _len_field(2, len(body)) + body                       # Feature.float_list
+        elif kind == "int64":
+            vals = b"".join(_encode_varint(int(v) & 0xFFFFFFFFFFFFFFFF) for v in values)
+            body = _len_field(1, len(vals)) + vals if vals else b""
+            feature = _len_field(3, len(body)) + body                       # Feature.int64_list
+        else:
+            raise ValueError("unknown feature kind %r of %s" % (kind, key))
+        entry = _len_field(1, len(kb)) + kb + _len_field(2, len(feature)) + feature
+        entries.append(_len_field(1, len(entry)) + entry)                   # Features.feature map entry
+    feats = b"".join(entries)
+    return _len_field(1, len(feats)) + feats                                 # Example.features
 
 
 def features_span(example, key):
