@@ -36,7 +36,6 @@ from . import _lib, dp
 from .hparams import DATASETS, DEFAULTS, get_loss_scale, params_from_flags
 from .plan import BLOCK_SIZES, ModelConfig, build_plan
 from .metrics import EvalMetrics, RecallAtK
-from .runtime import Runtime
 from .native import NativeModel, NativeRuntime
 from .staging import StagingRing, pack_u8, read_ahead
 
@@ -138,7 +137,7 @@ class Model:
                  zero_gamma=False, use_se_block=False, use_sk_block=False, bn_momentum=0.997,
                  embedding_size=0, anti_alias_filter_size=0, anti_alias_type="", pool_type="gap",
                  loss_type="softmax", bl_alpha=2, bl_beta=4, *, seed=42, device="cuda:0",
-                 deterministic=None, native=None):
+                 deterministic=None):
         if data_format not in (None, "channels_last"):
             raise ValueError("this implementation is NHWC only (data_format='channels_last')")
         if dtype not in ALLOWED_TYPES:
@@ -161,17 +160,13 @@ class Model:
         # None: bit-reproducible steps in the fp32 mode only; True: also in bf16 (wgrad and the SE
         # fc GEMMs run without split-K -- slower); every other reduction is ordered in both modes
         self.deterministic = deterministic
-        # True (default): the layer plan is built and executed inside libacnn.so through the model-level
-        # C ABI (include/acnn_model.h, native.NativeRuntime); False (ACNN_NATIVE_PLAN=0): the Python plan
-        # + per-op ctypes executor the lockstep parity tests drive (same plan, text-for-text)
-        self.native = (os.environ.get("ACNN_NATIVE_PLAN", "1") != "0") if native is None else bool(native)
-        self._runtimes = {}          # (B, H, W, training, use_resnet_d, mixup, ls) -> Runtime
-        self._primary = {}           # use_resnet_d -> Runtime owning the parameters
+        self._runtimes = {}          # (B, H, W, training, use_resnet_d, mixup, ls) -> NativeRuntime
+        self._primary = {}           # use_resnet_d -> NativeRuntime owning the parameters
         self._pending_weights = None
 
     # ---------------------------------------------------------------- runtimes / parameters
     def runtime(self, batch, height, width, *, training, use_resnet_d=False, mixup_type=0,
-                label_smoothing=0.0, with_loss=False, use_dropblock=False, kd_temp=0.0) -> Runtime:
+                label_smoothing=0.0, with_loss=False, use_dropblock=False, kd_temp=0.0) -> NativeRuntime:
         key = (batch, height, width, bool(training), bool(use_resnet_d), mixup_type,
                float(label_smoothing), bool(with_loss or training), bool(use_dropblock and training),
                float(kd_temp) if training else 0.0)
@@ -182,13 +177,9 @@ class Model:
                         with_loss=with_loss, dtype=self.dtype, use_dropblock=use_dropblock,
                         kd_temp=kd_temp)
             prim = self._primary.get(bool(use_resnet_d))
-            if self.native:
-                rt = NativeRuntime(NativeModel(cfg, batch, height, width,
-                                               deterministic=self.deterministic, **step),
-                                   self.device, share=prim)
-            else:
-                rt = Runtime(build_plan(cfg, batch, height, width, **step), self.device, share=prim,
-                             deterministic=self.deterministic)
+            # the layer plan is built and executed inside libacnn.so (include/acnn_model.h)
+            rt = NativeRuntime(NativeModel(cfg, batch, height, width, deterministic=self.deterministic, **step),
+                               self.device, share=prim)
             if prim is None:
                 self._primary[bool(use_resnet_d)] = rt
                 if self._pending_weights is not None:
@@ -198,7 +189,7 @@ class Model:
             self._runtimes[key] = rt
         return rt
 
-    def init_weights(self, rt: Runtime):
+    def init_weights(self, rt: NativeRuntime):
         """The reference's initializers: variance_scaling (truncated normal, fan-in) for conv /
         SK / SE kernels (nets/model_helper.py:77), glorot-uniform dense kernel, zero bias
         (nets/resnet_model.py:595-597), gamma 1 (0 with zero_gamma on block-final BNs), beta 0."""
@@ -285,7 +276,7 @@ def build_model(**flags) -> Model:
         "resnet_size", "data_format", "num_classes", "resnet_version", "dtype", "no_downsample",
         "zero_gamma", "use_se_block", "use_sk_block", "bn_momentum", "embedding_size",
         "anti_alias_filter_size", "anti_alias_type", "pool_type", "loss_type", "bl_alpha",
-        "bl_beta", "seed", "device", "deterministic", "native")}
+        "bl_beta", "seed", "device", "deterministic")}
     if flags:
         raise TypeError("build_model: unknown flag(s) %s" % sorted(flags))
     ctor.setdefault("resnet_size", DEFAULTS["resnet_size"])
@@ -491,9 +482,7 @@ class Trainer:
     def _fwd_bwd(self):
         rt = self.rt
         rt.run_forward()
-        # (a second stream for the wgrad GEMMs: Runtime.run(..., overlap_wgrad=True); off by default,
-        # every kernel already spans the GPU)
-        rt.run(rt.plan.backward, overlap_wgrad=os.environ.get("ACNN_OVERLAP_WGRAD", "0") == "1")
+        rt.run(rt.plan.backward)
 
     def prefetch(self, images, labels):
         """Start the host->device copy of the next step's inputs (pinned host tensors) on a side
@@ -684,7 +673,7 @@ class Trainer:
 _TRAINERS = {}
 
 
-def l2_loss(rt: Runtime, weight_decay: float):
+def l2_loss(rt: NativeRuntime, weight_decay: float):
     """weight_decay * sum over the decayed variables of |v|^2 / 2 (run_loop_classification.py:
     166-177), from the flat master buffer and its per-256-element decay flags.  TRAIN gets the same
     number from the SGD kernel; this is the EVAL-mode path (a reduction over 42 M floats, once per
@@ -814,7 +803,7 @@ def _replica(model, device, use_resnet_d, batch, size):
     src = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d)
     names = list(src.plan.params) + list(src.plan.state)
     rep = Model(dtype=model.dtype, seed=model.seed, device=device, deterministic=model.deterministic,
-                native=model.native, **model.cfg_kwargs)
+                **model.cfg_kwargs)
     rep.set_weights({n: src.get_tf(n).detach().float().cpu().clone() for n in names})
     return rep
 

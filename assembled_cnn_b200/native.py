@@ -7,8 +7,9 @@ by libacnn.so (csrc/model_plan.cu, csrc/model_exec.cu); this module only
   * and wraps the host CRC-32C of include/acnn.h (crc32c) for the TFRecord reader and writer.
 
 `NativeModel` (plan + introspection) needs no GPU; `NativeRuntime` (execution) has no CPU path.
-plan.py / runtime.py remain as the op-by-op executor the parity tests drive in lockstep with the
-oracle's plan interpreter; tests/test_native_plan_cpu.py pins the two plans to the same text.
+The parity tests run NativeRuntime op by op in lockstep with the oracle's plan interpreter, which walks
+plan.py's Python plan of the same configuration (NativeModel.python_mirror); tests/test_native_plan_cpu.py
+pins the two plans to the same text.
 """
 from __future__ import annotations
 
@@ -17,6 +18,7 @@ import os
 from collections import OrderedDict
 
 import numpy as np
+import torch
 
 from . import _lib
 from .plan import ModelConfig, Param, Slot, Tensor
@@ -171,7 +173,7 @@ class NativeOp:
 class NativeModel:
     """acnn_create() + introspection.  Quacks like plan.Plan where model_fns / dp / checkpoint read
     it: .params / .state (name -> Param), .tensors, .meta, .param_elems ..., .forward / .backward /
-    .update (NativeOp lists whose slices Runtime.run() turns into acnn_run_ops ranges)."""
+    .update (NativeOp lists whose slices NativeRuntime.run() turns into acnn_run_ops ranges)."""
 
     def __init__(self, cfg: ModelConfig, batch, height=224, width=224, **kw):
         self.lib = lib()
@@ -276,20 +278,61 @@ class NativeModel:
             pass
 
 
-def _runtime_base():
-    from .runtime import Runtime
-    return Runtime
+def _check_u8_images(images_u8, images, mean):
+    """Arguments of set_images_u8: uint8 NHWC of the input buffer's shape on its device, float32 mean[3]."""
+    if images_u8.dtype != torch.uint8 or tuple(images_u8.shape) != tuple(images.shape) \
+            or images_u8.device != images.device or not images_u8.is_contiguous():
+        raise ValueError("images_u8 must be a contiguous uint8 tensor %s on %s, got %s %s on %s"
+                         % (tuple(images.shape), images.device, images_u8.dtype, tuple(images_u8.shape),
+                            images_u8.device))
+    if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
+        raise ValueError("mean must be a contiguous float32 tensor of 3 values")
 
 
-class NativeRuntime(_runtime_base()):
-    """Executes a NativeModel on one H100 through acnn_bind / acnn_run_ops.  Same surface as
-    runtime.Runtime (params / state / grads / momentum / hp / t[name] / run(ops) / capture ...), so that
-    Model, Trainer, checkpoint and the data-parallel schedule work on either; here every buffer of the
-    step is a view into ONE workspace tensor laid out by the library, and run() is a loop inside
-    libacnn.so over launch records resolved at bind time."""
+def _check_desc_args(method, desc, images, mean, n_valid=None):
+    """Arguments of set_images_resized / set_images_cropped (`method`): a square input buffer, B descriptors
+    of 32 bytes on its device, n_valid (when given) in [0, B], float32 mean[3].  Returns (B, S)."""
+    b, h, w, _ = images.shape
+    if h != w:
+        raise ValueError("%s needs a square input buffer, got %dx%d" % (method, h, w))
+    if desc.dtype != torch.uint8 or desc.numel() != 32 * b or desc.device != images.device \
+            or not desc.is_contiguous():
+        raise ValueError("desc must be a contiguous uint8 tensor of %d descriptors (%d bytes) on %s"
+                         % (b, 32 * b, images.device))
+    if n_valid is not None and not 0 <= int(n_valid) <= b:
+        raise ValueError("n_valid=%d outside [0, %d]" % (int(n_valid), b))
+    if mean.dtype != torch.float32 or mean.numel() != 3 or not mean.is_contiguous():
+        raise ValueError("mean must be a contiguous float32 tensor of 3 values")
+    return b, h
+
+
+def _check_augment_args(desc, aug, work, images, mean):
+    """Arguments of set_images_augmented: those of set_images_cropped, B descriptors of 88 bytes and a work
+    buffer of acnn_autoaugment_work_bytes(B, S) bytes, both uint8 on the input buffer's device.
+    Returns (B, S)."""
+    b, s = _check_desc_args("set_images_cropped", desc, images, mean)
+    if aug.dtype != torch.uint8 or aug.numel() != 88 * b or aug.device != images.device or not aug.is_contiguous():
+        raise ValueError("aug must be a contiguous uint8 tensor of %d AutoAugment descriptors (%d bytes) on %s"
+                         % (b, 88 * b, images.device))
+    need = _lib.load().acnn_autoaugment_work_bytes(b, s)
+    if work.dtype != torch.uint8 or work.numel() < need or work.device != images.device \
+            or not work.is_contiguous():
+        raise ValueError("work must be a contiguous uint8 tensor of at least %d bytes on %s" % (need, images.device))
+    return b, s
+
+
+class NativeRuntime:
+    """Executes a NativeModel on one H100 through acnn_bind / acnn_run_ops: params / state / grads /
+    momentum / hp / t[name] / run(ops) / capture ..., what Model, Trainer, checkpoint and the
+    data-parallel schedule drive.  Every buffer of the step but the variables is a view into ONE
+    workspace tensor laid out by the library, and run() is a loop inside libacnn.so over launch
+    records resolved at bind time.  torch is the device-memory container only, for streams and for
+    CUDA-graph capture; there is no CPU path."""
+
+    REPLICA_SAVE, REPLICA_FIRST, REPLICA_MIDDLE, REPLICA_LAST = 0, 1, 2, 3     # acnn.h ACNN_REPLICA_*
+    REPLICA_LOSS_FLOATS = 4                                                    # acnn_model.h
 
     def __init__(self, model: NativeModel, device="cuda:0", share: "NativeRuntime | None" = None):
-        import torch
         if not torch.cuda.is_available():
             raise _lib.AcnnError("assembled_cnn_b200.NativeRuntime needs a CUDA device (sm_90a); "
                                  "there is no CPU fallback")
@@ -298,16 +341,16 @@ class NativeRuntime(_runtime_base()):
         self.dev = torch.device(device)
         torch.cuda.set_device(self.dev)
         c, s = model.config, model.sizes
-        self.eps = c.bn_epsilon
-        self.bn_momentum = c.bn_momentum
         self.training = bool(c.training)
-        self.fp32 = c.dtype == 1
         self.adt = c.dtype                   # ACNN_BF16 / ACNN_F32 / ACNN_F16
-        self.planes = 3 if self.fp32 else 1
         wdt = torch.float16 if self.adt == 3 else torch.bfloat16
-        self.det = int(self.fp32 if c.deterministic < 0 else bool(c.deterministic))
+        # deterministic: also the split-K of wgrad and of the small SK / SE GEMMs is disabled (one add
+        # per output element).  Every reduction is ordered in both modes (split-K partials are summed
+        # in split order), so two runs are bit-identical either way.
+        self.det = int(c.dtype == 1 if c.deterministic < 0 else bool(c.deterministic))
         f32 = dict(dtype=torch.float32, device=self.dev)
         if share is not None:
+            # same model, another batch shape / mode: the variables are shared, not copied
             if share.plan.param_elems != s.param_elems or share.plan.state_elems != s.state_elems \
                     or share.adt != self.adt:
                 raise ValueError("NativeRuntime(share=...): parameter layouts differ")
@@ -331,6 +374,8 @@ class NativeRuntime(_runtime_base()):
 
         def view(off, nbytes, dtype):
             return ws[off:off + nbytes].view(dtype)
+        # device hyper-parameters: lr, momentum, wd, grad_scale, dropblock keep_prob, global step
+        # (uint32 bits, the Philox counter of the DropBlock masks), 2 spare
         self.hp = view(s.hp_offset, 32, torch.float32)
         self.zero = view(s.zero_offset, max(s.zero_bytes, 4), torch.float32)
         self.work = view(s.work_offset, max(s.work_bytes, 4), torch.float32)
@@ -351,7 +396,66 @@ class NativeRuntime(_runtime_base()):
         self._loss_scale = c.loss_scale
         self._db_seed, self._db_feed = 0x5EED5EED, False
         self.graph = None
-        self._side_stream = None
+
+    @property
+    def stream(self):
+        return torch.cuda.current_stream(self.dev).cuda_stream
+
+    # ---------------------------------------------------------------- views
+    def slot_view(self, slot: Slot):
+        buf = self.zero if slot.buf == "zero" else self.work
+        return buf[slot.offset:slot.offset + slot.size]
+
+    def pview(self, name, buf=None):
+        p = self.plan.params.get(name) or self.plan.state[name]
+        base = buf if buf is not None else (self.params if p.trainable else self.state)
+        return base[p.offset:p.offset + p.size].view(p.store_shape)
+
+    # ---------------------------------------------------------------- weights (TF layout)
+    def set_weights(self, tf_vars):
+        """tf_vars: name -> array-like in the reference's layout (HWIO kernels, [in,out] dense)."""
+        for name, p in list(self.plan.params.items()) + list(self.plan.state.items()):
+            v = torch.as_tensor(tf_vars[name]).to(torch.float32)
+            if tuple(v.shape) != tuple(p.tf_shape):
+                raise ValueError("shape of %s: got %s, expected %s" % (name, tuple(v.shape), p.tf_shape))
+            self.set_tf(name, v)
+
+    def set_tf(self, name, value, buf=None):
+        """Inverse of get_tf for one variable (or its momentum slot with buf=self.momentum)."""
+        p = self.plan.params.get(name) or self.plan.state[name]
+        v = torch.as_tensor(value).to(torch.float32)
+        dst = self.pview(name, buf)
+        if p.kind == "conv_kernel":
+            dst.copy_(v.permute(3, 0, 1, 2))
+        elif p.kind == "dense_kernel":
+            dst.zero_()
+            dst[:v.shape[1], 0, 0, :] = v.t()
+        elif p.kind == "dense_bias":
+            dst.zero_()
+            dst[:v.shape[0]] = v
+        else:
+            dst.copy_(v)
+
+    def get_tf(self, name, buf=None):
+        p = self.plan.params.get(name) or self.plan.state[name]
+        v = self.pview(name, buf)
+        if p.kind == "conv_kernel":
+            return v.permute(1, 2, 3, 0)
+        if p.kind == "dense_kernel":
+            return v[:p.tf_shape[1], 0, 0, :].t()
+        if p.kind == "dense_bias":
+            return v[:p.tf_shape[0]]
+        return v
+
+    def set_hparams(self, lr=None, momentum=None, weight_decay=None, grad_scale=None,
+                    keep_prob=None, step=None):
+        cur = self.hp.cpu()
+        for i, v in enumerate((lr, momentum, weight_decay, grad_scale, keep_prob)):
+            if v is not None:
+                cur[i] = float(v)
+        if step is not None:
+            cur.view(torch.int32)[5] = int(step) & 0x7fffffff
+        self.hp.copy_(cur, non_blocking=True)
 
     # settings the launch records read at enqueue time
     @property
@@ -378,6 +482,7 @@ class NativeRuntime(_runtime_base()):
 
     @property
     def dropblock_feed(self):
+        """True: the DropBlock masks come from the uniforms in the plan's dropblock_u tensors."""
         return self._db_feed
 
     @dropblock_feed.setter
@@ -385,8 +490,10 @@ class NativeRuntime(_runtime_base()):
         self._db_feed = bool(v)
         self._push_dropblock()
 
-    # execution: consecutive ops of one phase become one acnn_run_ops range
-    def run(self, ops, overlap_wgrad=False):
+    # ---------------------------------------------------------------- execution
+    def run(self, ops):
+        """Enqueue ops (any list or slice of the model's NativeOps) in order: consecutive ops of one
+        phase become one acnn_run_ops range."""
         h, st, i, n = self.model.handle, self.stream, 0, len(ops)
         while i < n:
             j = i
@@ -399,7 +506,6 @@ class NativeRuntime(_runtime_base()):
     def set_images_u8(self, images_u8, mean):
         """acnn_set_images_u8: the "images" buffer = (float)images_u8 - mean[c], images_u8 a CUDA uint8
         tensor [input_batch, H, W, 3] on this device, mean a float32 tensor of 3 (host or device)."""
-        from .runtime import _check_u8_images
         _check_u8_images(images_u8, self.t[self.plan.meta["images"]], mean)
         _lib.check(self.lib.acnn_set_images_u8(self.model.handle, images_u8.data_ptr(), mean.data_ptr(),
                                                self.stream), "acnn_set_images_u8")
@@ -408,7 +514,6 @@ class NativeRuntime(_runtime_base()):
         """acnn_set_images_resized: the "images" buffer from decoded uint8 images of any sizes (resize,
         central crop, - mean[c]); desc a CUDA uint8 tensor of input_batch 32-byte acnn_resize_desc on
         this device, validated by the caller; mean a float32 tensor of 3 (host or device)."""
-        from .runtime import _check_desc_args
         _check_desc_args("set_images_resized", desc, self.t[self.plan.meta["images"]], mean, n_valid)
         _lib.check(self.lib.acnn_set_images_resized(self.model.handle, desc.data_ptr(), int(n_valid),
                                                     mean.data_ptr(), self.stream), "acnn_set_images_resized")
@@ -417,7 +522,6 @@ class NativeRuntime(_runtime_base()):
         """acnn_set_images_cropped: every row of the "images" buffer from training crop windows (flip,
         resize to S x S, - mean[c]); desc a CUDA uint8 tensor of input_batch 32-byte acnn_crop_desc on this
         device, validated by the caller; mean a float32 tensor of 3 (host or device)."""
-        from .runtime import _check_desc_args
         _check_desc_args("set_images_cropped", desc, self.t[self.plan.meta["images"]], mean)
         _lib.check(self.lib.acnn_set_images_cropped(self.model.handle, desc.data_ptr(), mean.data_ptr(),
                                                     self.stream), "acnn_set_images_cropped")
@@ -427,7 +531,6 @@ class NativeRuntime(_runtime_base()):
         uint8, aug's two operations, - mean[c]); aug a CUDA uint8 tensor of input_batch 88-byte
         acnn_autoaugment_desc (autoaugment.AUTOAUG_DESC_DTYPE), validated by the caller; work a CUDA uint8
         tensor of acnn_autoaugment_work_bytes(input_batch, S) bytes."""
-        from .runtime import _check_augment_args
         _check_augment_args(desc, aug, work, self.t[self.plan.meta["images"]], mean)
         _lib.check(self.lib.acnn_set_images_augmented(self.model.handle, desc.data_ptr(), aug.data_ptr(),
                                                       work.data_ptr(), mean.data_ptr(), self.stream),
@@ -444,7 +547,30 @@ class NativeRuntime(_runtime_base()):
             _lib.check(self.lib.acnn_loss(h, st), "acnn_loss")
 
     def run_step(self):
+        """zero -> forward -> backward -> SGD, all enqueued on the current stream."""
         _lib.check(self.lib.acnn_step(self.model.handle, self.stream), "acnn_step")
+
+    def capture(self, train=True):
+        """Capture one full step (or forward) into a CUDA graph; inputs are read from the static
+        input buffers (plan.meta['images'] ...), hyper-parameters from the device `hp` vector."""
+        fn = self.run_step if train else self.run_forward
+        s = torch.cuda.Stream(self.dev)
+        s.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(s):
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph, stream=s):
+                fn()
+        torch.cuda.current_stream(self.dev).wait_stream(s)
+        return self.graph
+
+    # ---------------------------------------------------------------- several replicas per device
+    def replica_buffers(self):
+        """The device accumulators of several replicas per device: (acc_grads [param_elems], state_base
+        [state_elems], acc_state [state_elems + REPLICA_LOSS_FLOATS], the tail summing the loss)."""
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        ns = self.plan.state_elems
+        return (torch.zeros(self.plan.param_elems, **f32), torch.zeros(max(ns, 1), **f32),
+                torch.zeros(ns + self.REPLICA_LOSS_FLOATS, **f32))
 
     def replica_accumulate(self, phase, bufs, lo, hi, replicas):
         """acnn_replica_accumulate_model over this handle's grads [lo, hi), state and loss."""

@@ -1,8 +1,8 @@
 """GPU checks of AutoAugment on the device: acnn_crop_resize_autoaugment_u8 bit for bit against the numpy
 oracle (every operation at every argument the tables produce, both signs, at S in {64, 224, 256, 320}, on
 resized random windows and structured images; every sub-policy of every policy with its operations forced on
-and off; images with no operation), graph replay and two streams, the native and Python executors'
-set_images_augmented, and Trainer.train_step_cropped(augment=) against train_step fed the oracle's images."""
+and off; images with no operation), graph replay and two streams, NativeRuntime.set_images_augmented against the
+op-level call, and Trainer.train_step_cropped(augment=) against train_step fed the oracle's images."""
 import numpy as np
 import pytest
 import torch
@@ -192,14 +192,14 @@ def A_work(B, S):
     return _lib.load().acnn_autoaugment_work_bytes(B, S)
 
 
-def test_native_and_python_executors_agree():
+def test_native_runtime_set_images_augmented_equals_op_level():
+    """NativeRuntime.set_images_augmented (acnn_set_images_augmented into the model's "images" buffer) writes
+    what the op-level acnn_crop_resize_autoaugment_u8 writes into a buffer of its own; both refuse short
+    tables and work buffers, the model level also host tables."""
     from assembled_cnn_b200 import autoaugment as A, native
-    from assembled_cnn_b200.plan import ModelConfig, build_plan
-    from assembled_cnn_b200.runtime import Runtime
+    from assembled_cnn_b200.plan import ModelConfig
     B, S = 8, 64
-    cfg = ModelConfig(resnet_size=50)
-    rt_py = Runtime(build_plan(cfg, B, S, S, training=False))
-    rt_nat = native.NativeRuntime(native.NativeModel(cfg, B, S, S, training=False))
+    rt_nat = native.NativeRuntime(native.NativeModel(ModelConfig(resnet_size=50), B, S, S, training=False))
     rng = np.random.default_rng(4)
     windows = [rng.integers(0, 256, (int(rng.integers(1, 300)), int(rng.integers(1, 300)), 3), dtype=np.uint8)
                for _ in range(B)]
@@ -207,21 +207,20 @@ def test_native_and_python_executors_agree():
     buf, desc, aug = _descs(windows, [i % 2 == 0 for i in range(B)], recs)
     mean = torch.tensor(MEAN, device="cuda")
     work = torch.empty(A_work(B, S), dtype=torch.uint8, device="cuda")
-    got = []
-    for rt in (rt_py, rt_nat):
-        rt.t[rt.plan.meta["images"]].zero_()
-        rt.set_images_augmented(desc, aug, work, mean)
-        torch.cuda.synchronize()
-        got.append(rt.t[rt.plan.meta["images"]].clone())
-    assert torch.equal(got[0], got[1]) and got[0].abs().sum() > 0
+    images = rt_nat.t[rt_nat.plan.meta["images"]]
+    images.zero_()
+    rt_nat.set_images_augmented(desc, aug, work, mean)
+    op_level = torch.zeros_like(images)
+    _run(desc, aug, B, B, S, op_level, mean, work)
+    torch.cuda.synchronize()
+    assert torch.equal(images, op_level) and op_level.abs().sum() > 0
     # host tables and a short work buffer are refused
     assert rt_nat.lib.acnn_set_images_augmented(rt_nat.model.handle, desc.data_ptr(), aug.cpu().pin_memory().data_ptr(),
                                                 work.data_ptr(), mean.data_ptr(), rt_nat.stream) == 1
-    for rt in (rt_py, rt_nat):
-        with pytest.raises(ValueError):
-            rt.set_images_augmented(desc, aug[:88], work, mean)
-        with pytest.raises(ValueError):
-            rt.set_images_augmented(desc, aug, work[:100], mean)
+    with pytest.raises(ValueError):
+        rt_nat.set_images_augmented(desc, aug[:88], work, mean)
+    with pytest.raises(ValueError):
+        rt_nat.set_images_augmented(desc, aug, work[:100], mean)
 
 
 @pytest.mark.parametrize("dtype,mixup_type,kd_temp", [("bf16", 1, 0), ("fp32", 0, 0), ("bf16", 0, 2.0)])

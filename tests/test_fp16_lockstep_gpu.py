@@ -88,11 +88,11 @@ def test_fp16_lockstep_dropblock_224_on_the_halo_kernel(lib):
     halo = []
 
     def hook(plan, rt):
-        for op in plan.forward:
+        for op, native_op in zip(plan.forward, rt.plan.forward):
             g = op.a.get("geom")
             if op.kind != "conv" or op.a.get("x_wpad") or g.kh != 3 or g.stride != 1:
                 continue
-            geom = rt.geom(g)
+            geom = rt.plan.conv_info(native_op)[0]
             prev = lib.acnn_set_conv_halo(0)
             try:
                 n_im2col = lib.acnn_conv_stats_parts(geom)

@@ -86,36 +86,41 @@ def test_fp16_weight_copies(lib):
     nearest even (torch's float16 conversion), bit for bit, with the copies of an out-of-range weight inf;
     acnn_s2d_weight_pack in fp16 is the fp32 pack rounded likewise."""
     import bench
+    from assembled_cnn_b200 import _lib
     from assembled_cnn_b200.plan import ModelConfig, build_plan
-    from assembled_cnn_b200.runtime import Runtime
     cfg = ModelConfig(num_classes=1001, **bench.CONFIGS["c3"]["model"])
-    rt = Runtime(build_plan(cfg, 2, 64, 64, dtype="fp16", training=True))
-    g = torch.Generator(device="cuda").manual_seed(3)
-    rt.params.normal_(0.0, 0.3, generator=g)
-    conv = [p for p in rt.plan.params.values() if p.kind in ("conv_kernel", "dense_kernel")
+    plan = build_plan(cfg, 2, 64, 64, dtype="fp16", training=True)
+    # the weights with GEMM operand copies (Cin % 16 == 0, Cout % 32 == 0), one acnn_weight_desc each: the
+    # master at its offset in params and in w_fprop, the dgrad layout at dgrad_off in w_dgrad
+    conv = [p for p in plan.params.values() if p.kind in ("conv_kernel", "dense_kernel")
             and len(p.store_shape) == 4 and p.store_shape[3] % 16 == 0 and p.store_shape[0] % 32 == 0]
+    descs = [_lib.WeightDesc(p.offset, p.offset, p.dgrad_off, p.store_shape[0], p.store_shape[1] * p.store_shape[2],
+                             p.store_shape[3], 0) for p in conv]
+    n_descs = len(descs)
+    table = torch.frombuffer(bytearray(bytes((_lib.WeightDesc * n_descs)(*descs))), dtype=torch.uint8).cuda()
+    g = torch.Generator(device="cuda").manual_seed(3)
+    params = torch.zeros(plan.param_elems, device="cuda").normal_(0.0, 0.3, generator=g)
     o = conv[0].offset
-    rt.params[o] = 1e6                                          # beyond fp16: inf
-    rt.params[o + 1] = 3e-6                                     # an fp16 subnormal
-    assert rt.w_fprop.dtype == torch.float16 and rt.w_dgrad.dtype == torch.float16
-    rt.w_fprop.fill_(float("nan"))
-    rt.w_dgrad.fill_(float("nan"))
-    S._check(lib.acnn_prep_weights_f16(rt.params.data_ptr(), rt.descs.data_ptr(), rt.n_descs, rt.w_fprop.data_ptr(),
-                                       rt.w_dgrad.data_ptr(), S._st()), "prep_weights_f16")
+    params[o] = 1e6                                             # beyond fp16: inf
+    params[o + 1] = 3e-6                                        # an fp16 subnormal
+    w_fprop = torch.full((plan.param_elems,), float("nan"), dtype=torch.float16, device="cuda")
+    w_dgrad = torch.full((max(plan.dgrad_elems, 1),), float("nan"), dtype=torch.float16, device="cuda")
+    S._check(lib.acnn_prep_weights_f16(params.data_ptr(), table.data_ptr(), n_descs, w_fprop.data_ptr(),
+                                       w_dgrad.data_ptr(), S._st()), "prep_weights_f16")
     torch.cuda.synchronize()
     n = 0
     for p in conv:
         co, kh, kw, ci = p.store_shape
-        master = rt.params[p.offset:p.offset + p.size].view(co, kh, kw, ci)
+        master = params[p.offset:p.offset + p.size].view(co, kh, kw, ci)
         want = master.half()
-        got = rt.w_fprop[p.offset:p.offset + p.size].view(co, kh, kw, ci)
+        got = w_fprop[p.offset:p.offset + p.size].view(co, kh, kw, ci)
         assert torch.equal(got.view(torch.int16), want.view(torch.int16)), p.name
         if p.dgrad_off >= 0:
             wd = want.flip(1, 2).permute(3, 1, 2, 0).contiguous()
-            got_d = rt.w_dgrad[p.dgrad_off:p.dgrad_off + p.size].view(ci, kh, kw, co)
+            got_d = w_dgrad[p.dgrad_off:p.dgrad_off + p.size].view(ci, kh, kw, co)
             assert torch.equal(got_d.view(torch.int16), wd.view(torch.int16)), p.name
         n += 1
-    assert n == rt.n_descs > 50 and torch.isinf(rt.w_fprop[o]) and rt.w_fprop[o + 1] != 0
+    assert n == n_descs > 50 and torch.isinf(w_fprop[o]) and w_fprop[o + 1] != 0
     # the stem's space-to-depth pack
     Cout, k, pad, k2, pad2 = 64, 7, 3, 4, 2
     w = torch.randn(Cout, k, k, 3, generator=g, device="cuda")

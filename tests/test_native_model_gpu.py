@@ -1,14 +1,14 @@
 """GPU tests of the model-level C ABI (include/acnn_model.h, csrc/model_plan.cu + model_exec.cu).
 
-The op-by-op parity of the plan against the oracle is proven on the Python executor (test_plan_gpu.py,
-lockstep with oracle/plan_interp.py) and the two plans are the same text (test_native_plan_cpu.py).
-What remains to prove is that the library's launch records call the op level with the same pointers
-and arguments: run the SAME step through both executors on the same weights and inputs in
-deterministic mode -- and, for the bf16 configurations, in the default mode too, where wgrad and the
-small SK / SE GEMMs run split-K with ordered reductions -- and require every buffer of the step -- logits, loss, every gradient, the updated
-weights, momentum and moving statistics -- to be BIT-IDENTICAL.  Plus: the pure C-ABI call sequence
-with host arrays (acnn_set_inputs ... acnn_get_loss) against the oracle, piecewise == acnn_step, and
-CUDA-graph capture of acnn_step, in both modes."""
+The library's executor runs each configuration of CASES op by op in lock-step with the oracle's plan
+interpreter (test_plan_gpu.lockstep: after every op its outputs are compared and then overwritten with the
+interpreter's) in deterministic mode and, for the bf16 configurations of DEFAULT_MODE_CASES, in the default
+mode too, where wgrad and the small SK / SE GEMMs run split-K with ordered reductions.  The whole step
+(acnn_step / acnn_forward + acnn_loss) must then be BIT-IDENTICAL to the same ops run one acnn_run_ops call
+at a time -- every buffer of the step: logits, loss, every gradient, the updated weights, momentum and
+moving statistics.  Plus: the pure C-ABI call sequence with host arrays (acnn_set_inputs ... acnn_get_loss)
+against the oracle, piecewise == acnn_step, CUDA-graph capture of acnn_step in both modes, and the Model /
+Trainer facade eager == CUDA graph."""
 import ctypes as C
 
 import numpy as np
@@ -75,24 +75,22 @@ def _feeds(plan, seed=9):
 
 
 def _pair(flags, B, hw, kw, deterministic=True):
+    """Two NativeRuntimes of one configuration, each on its own NativeModel, with the same weights,
+    hyper-parameters and inputs.  Returns (model of the first, first, second)."""
     from assembled_cnn_b200 import native
-    from assembled_cnn_b200.plan import ModelConfig, build_plan
-    from assembled_cnn_b200.runtime import Runtime
+    from assembled_cnn_b200.plan import ModelConfig
     cfg = ModelConfig(**flags)
-    plan = build_plan(cfg, B, hw, hw, **kw)
-    rt_py = Runtime(plan, deterministic=deterministic)
-    rt_nat = native.NativeRuntime(native.NativeModel(cfg, B, hw, hw, deterministic=deterministic, **kw))
-    assert rt_py.det == rt_nat.det
-    w = _weights(plan)
-    feeds = _feeds(plan)
-    hp = dict(lr=0.05, momentum=0.9, weight_decay=1e-4, keep_prob=0.9, step=3)
-    for rt in (rt_py, rt_nat):
-        rt.set_weights(w)
-        rt.set_hparams(**hp)
+    rts = []
+    for _ in range(2):
+        nm = native.NativeModel(cfg, B, hw, hw, deterministic=deterministic, **kw)
+        rt = native.NativeRuntime(nm)
+        rt.set_weights(_weights(nm))
+        rt.set_hparams(lr=0.05, momentum=0.9, weight_decay=1e-4, keep_prob=0.9, step=3)
         rt.dropblock_feed = True
-        for name, v in feeds.items():
+        for name, v in _feeds(nm).items():
             rt.t[name].copy_(v)
-    return plan, rt_py, rt_nat
+        rts.append(rt)
+    return rts[0].plan, rts[0], rts[1]
 
 
 def _assert_same(a, b, what):
@@ -103,40 +101,89 @@ def _assert_same(a, b, what):
             what, int((d > 0).sum()), d.numel(), float(d.max())))
 
 
+def lockstep_case(case, deterministic, dtype=None, loss_scale=1.0):
+    """test_plan_gpu.lockstep on the configuration CASES[case] (its batch, size and flags; dtype overrides
+    its dtype, loss_scale applies to training).  Returns (failures, worst error per op kind:output)."""
+    import test_plan_gpu as P
+    flags, B, hw, kw = CASES[case]
+    flags, kw = dict(flags), dict(kw)
+    use_resnet_d = flags.pop("use_resnet_d", False)
+    training = kw.pop("training", True)
+    case_dtype = kw.pop("dtype", "bf16")
+    assert kw.pop("with_loss", True), "lockstep runs the loss"
+    args = dict(B=B, HW=hw, training=training, mix=kw.pop("mixup_type", 0),
+                label_smoothing=kw.pop("label_smoothing", 0.0), dtype=dtype or case_dtype,
+                use_dropblock=kw.pop("use_dropblock", False), kd_temp=kw.pop("kd_temp", 0.0),
+                loss_scale=loss_scale if training else 1.0, deterministic=deterministic)
+    assert not kw, kw
+    return P.lockstep(flags, use_resnet_d, **args)
+
+
 @pytest.mark.parametrize("case", sorted(CASES))
-def test_native_step_bit_identical_to_python_executor(case):
+def test_lockstep_against_interpreter(case):
+    failures, _ = lockstep_case(case, deterministic=True)
+    assert not failures, "\n".join(failures[:20])
+
+
+@pytest.mark.parametrize("case", DEFAULT_MODE_CASES)
+def test_lockstep_against_interpreter_default_mode(case):
+    """The bf16 configurations with deterministic=None: wgrad and the SK / SE GEMMs run split-K."""
+    failures, _ = lockstep_case(case, deterministic=None)
+    assert not failures, "\n".join(failures[:20])
+
+
+def step_equals_op_by_op(case, deterministic, dtype=None, same=_assert_same):
+    """Two steps of CASES[case] (dtype overriding its dtype): run_step / run_forward on one runtime, the
+    same ops one rt.run([op]) at a time after zero_step_buffers on another; every tensor, the zero buffer,
+    the moving statistics, weights, gradients and momentum compared with `same` after each step.
+    Returns (plan, the runtime that ran whole steps, the loss after the first step)."""
+    flags, B, hw, kw = CASES[case]
+    if dtype is not None:
+        kw = dict(kw, dtype=dtype)
+    plan, rt_step, rt_ops = _pair(flags, B, hw, kw, deterministic)
+    assert rt_step.det == (1 if deterministic else int(kw.get("dtype") == "fp32"))
+    training = kw.get("training", True)
+    ops = plan.all_ops() if training else plan.forward
+    loss0 = None
+    for step in range(2):
+        if training:
+            rt_step.run_step()
+        else:
+            rt_step.run_forward()
+        rt_ops.zero_step_buffers()
+        for op in ops:
+            rt_ops.run([op])
+        torch.cuda.synchronize()
+        if step == 0:
+            loss0 = rt_step.slot_view(plan.meta["loss"]).clone()
+        for name in plan.tensors:      # every activation, gradient and input buffer of the step
+            same(rt_step.t[name], rt_ops.t[name], "%s step %d tensor %s" % (case, step, name))
+        same(rt_step.zero, rt_ops.zero, "zero buffer (loss, stem dW)")
+        same(rt_step.state, rt_ops.state, "moving statistics")
+        same(rt_step.params, rt_ops.params, "weights")
+        if training:
+            same(rt_step.grads, rt_ops.grads, "gradients")
+            same(rt_step.momentum, rt_ops.momentum, "momentum")
+    return plan, rt_step, loss0
+
+
+@pytest.mark.parametrize("case", sorted(CASES))
+def test_step_bit_identical_to_op_by_op(case):
     _step_bit_identical(case, deterministic=True)
 
 
 @pytest.mark.parametrize("case", DEFAULT_MODE_CASES)
-def test_native_step_bit_identical_to_python_executor_default_mode(case):
+def test_step_bit_identical_to_op_by_op_default_mode(case):
     """The bf16 configurations with deterministic=None: wgrad and the SK / SE GEMMs run split-K."""
     _step_bit_identical(case, deterministic=None)
 
 
 def _step_bit_identical(case, deterministic):
-    flags, B, hw, kw = CASES[case]
-    plan, rt_py, rt_nat = _pair(flags, B, hw, kw, deterministic)
-    training = kw.get("training", True)
-    for step in range(2):
-        for rt in (rt_py, rt_nat):
-            if training:
-                rt.run_step()
-            else:
-                rt.run_forward()
-        torch.cuda.synchronize()
-        for name in plan.tensors:      # every activation, gradient and input buffer of the step
-            _assert_same(rt_py.t[name], rt_nat.t[name], "%s step %d tensor %s" % (case, step, name))
-        _assert_same(rt_py.zero, rt_nat.zero[:rt_py.zero.numel()], "zero buffer (loss, stem dW)")
-        _assert_same(rt_py.state, rt_nat.state, "moving statistics")
-        _assert_same(rt_py.params, rt_nat.params, "weights")
-        if training:
-            _assert_same(rt_py.grads, rt_nat.grads, "gradients")
-            _assert_same(rt_py.momentum, rt_nat.momentum, "momentum")
-    loss = rt_nat.slot_view(plan.meta["loss"])
+    plan, rt, _ = step_equals_op_by_op(case, deterministic)
+    loss = rt.slot_view(plan.meta["loss"])
     assert torch.isfinite(loss).all() and float(loss[0]) > 0
-    if training:
-        assert float(rt_nat.grads.abs().sum()) > 0 and float(loss[1]) > 0
+    if CASES[case][3].get("training", True):
+        assert float(rt.grads.abs().sum()) > 0 and float(loss[1]) > 0
 
 
 def test_c_abi_call_sequence_with_host_arrays_against_oracle():
@@ -247,8 +294,8 @@ def _piecewise_step_graph(deterministic):
 
 
 def test_model_facade_runs_on_the_native_path():
-    """Model / Trainer use the library's plan by default, and the Python executor gives the same
-    training step bit for bit (ACNN_NATIVE_PLAN=0 / native=False keeps it available)."""
+    """Model / Trainer run on the library's executor, and a Trainer that replays its step as a CUDA graph
+    gives the eager Trainer's losses, weights, moving statistics and eval logits bit for bit."""
     from assembled_cnn_b200.hparams import params_from_flags
     from assembled_cnn_b200.model_fns import Model, Trainer
     from assembled_cnn_b200.native import NativeRuntime
@@ -258,13 +305,13 @@ def test_model_facade_runs_on_the_native_path():
     lab = torch.randint(1, 1001, (2 * B,), generator=g).int()
     lam = torch.rand(B, generator=g)
     res = []
-    for native_flag in (True, False):
+    for use_graph in (False, True):
         model = Model(50, num_classes=1001, resnet_version=2, use_sk_block=True, anti_alias_type="sconv",
-                      anti_alias_filter_size=3, seed=42, deterministic=True, native=native_flag)
+                      anti_alias_filter_size=3, seed=42, deterministic=True)
         p = params_from_flags(batch_size=B, mixup_type=1, label_smoothing=0.1, weight_decay=1e-4,
                               base_learning_rate=0.05, learning_rate_decay_type="fixed", **ASSEMBLE)
-        tr = Trainer(model, p, hw, hw, use_cuda_graph=native_flag)
-        assert isinstance(tr.rt, NativeRuntime) == native_flag
+        tr = Trainer(model, p, hw, hw, use_cuda_graph=use_graph)
+        assert isinstance(tr.rt, NativeRuntime) and tr.use_graph == use_graph
         losses = [tr.train_step(x, lab, lam1=lam).clone() for _ in range(2)]
         ev = model(x[:B], training=False).clone()
         torch.cuda.synchronize()

@@ -1,8 +1,8 @@
 """The model-level C ABI (include/acnn_model.h) builds its layer plan in C++ (csrc/model_plan.cu); the
-op-by-op parity tests drive the Python plan (assembled_cnn_b200/plan.py) in lockstep with the oracle's
-interpreter.  These CPU tests pin the two to the SAME plan -- variables (TF names, creation order,
-layouts, offsets), buffers, and every op with every argument -- by comparing their canonical texts,
-so whatever the lockstep tests prove about the Python plan holds for the native one.  No GPU: acnn_create
+oracle's interpreter walks the Python plan (assembled_cnn_b200/plan.py) in lockstep with the library's
+executor in the op-by-op parity tests.  These CPU tests pin the two to the SAME plan -- variables (TF
+names, creation order, layouts, offsets), buffers, and every op with every argument -- by comparing
+their canonical texts, so the interpreter runs, op for op, what the library runs.  No GPU: acnn_create
 is host logic."""
 import ctypes as C
 import difflib
@@ -220,7 +220,7 @@ def test_plain_c_host_builds_the_plan(tmp_path):
 def test_variable_pack_unpack_match_runtime_layouts():
     """acnn_variable_pack / _unpack (TF checkpoint layout <-> flat-buffer layout, host arrays) against
     the layout code of the Python side (oracle.plan_interp set_weights / get_tf share it with
-    runtime.Runtime.set_tf): HWIO -> OHWI kernels, [in,out] -> padded [ld][in] dense, padded bias."""
+    native.NativeRuntime.set_tf): HWIO -> OHWI kernels, [in,out] -> padded [ld][in] dense, padded bias."""
     import numpy as np
     import torch
     from oracle import plan_interp as PI

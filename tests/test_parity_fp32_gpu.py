@@ -381,16 +381,16 @@ def test_bf16_mode_forward_and_bn_reductions_bit_identical_deterministic():
 
 def _bf16_step_bit_identical(deterministic):
     import ctypes as C
-    from assembled_cnn_b200.plan import ModelConfig, build_plan
-    from assembled_cnn_b200.runtime import Runtime
+    from assembled_cnn_b200.native import NativeModel, NativeRuntime
+    from assembled_cnn_b200.plan import ModelConfig
     B, hw = 8, 128
     x, lab, g = _inputs(2 * B, hw, seed=4)
     lam = torch.rand(B, generator=g)
-    plan = build_plan(ModelConfig(**ASSEMBLE), B, hw, hw, training=True, mixup_type=1,
-                      label_smoothing=0.1)
     outs = []
     for run in ("eager", "eager", "graph"):
-        rt = Runtime(plan, deterministic=deterministic)
+        plan = NativeModel(ModelConfig(**ASSEMBLE), B, hw, hw, training=True, mixup_type=1,
+                           label_smoothing=0.1, deterministic=deterministic)
+        rt = NativeRuntime(plan)
         torch.manual_seed(0)
         rt.params.copy_(torch.randn(rt.params.shape, generator=torch.Generator().manual_seed(1)) * 0.05)
         for p in plan.params.values():
@@ -419,7 +419,7 @@ def _bf16_step_bit_identical(deterministic):
     for op in plan.backward:
         if op.kind == "conv_wgrad":
             splits = C.c_int()
-            assert rt.lib.acnn_conv_wgrad_plan(rt.geom(op.geom, op.a.get("x_wpad")), 0, rt.det, None,
+            assert rt.lib.acnn_conv_wgrad_plan(plan.conv_info(op)[0], 0, rt.det, None,
                                                C.byref(splits), None) == 0
             n_split += splits.value > 1
     assert (n_split > 0) == (not deterministic), n_split

@@ -1,7 +1,9 @@
-"""GPU parity, op by op: the CUDA runtime is run in lock-step with the CPU plan interpreter
-(oracle/plan_interp.py, same bf16 rounding points) on small configurations; after every op the
-op's outputs are compared and then overwritten with the oracle's values, so each kernel is checked
-in isolation on identical inputs.
+"""GPU parity, op by op: the library's executor (native.NativeRuntime, one acnn_run_ops call per op)
+is run in lock-step with the CPU plan interpreter (oracle/plan_interp.py, same bf16 rounding points)
+walking the Python plan of the same configuration (NativeModel.python_mirror, the same plan op for op:
+tests/test_native_plan_cpu.py) on small configurations; after every op the op's outputs are compared
+and then overwritten with the oracle's values, so each kernel is checked in isolation on identical
+inputs.
 
 Tolerances (relative to the output's max magnitude): bf16 tensors 2^-7 (one bf16 ulp at the top
 of the range: accumulation-order differences can flip a rounding), fp32 vectors 2e-3 where sums
@@ -113,22 +115,23 @@ def _err(got, ref):
 
 def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbose=False,
              dtype="bf16", use_dropblock=False, kd_temp=0.0, keep_prob=0.9, loss_scale=1.0,
-             emulate_storage=True, plan_hook=None):
+             emulate_storage=True, plan_hook=None, deterministic=None, label_smoothing=0.1):
     """Returns (failures, worst error per 'op.kind:output kind').  emulate_storage is passed to the
     interpreter of the 16-bit modes (a type name there makes it round to the wrong type on purpose);
-    plan_hook(plan, runtime) runs once before the first op."""
+    plan_hook(plan, runtime) runs once before the first op (runtime.plan is the NativeModel)."""
     H, W = (HW, HW) if isinstance(HW, int) else HW
     from oracle import model as M, plan_interp as PI
-    from assembled_cnn_b200.plan import ModelConfig, build_plan
-    from assembled_cnn_b200.runtime import Runtime
+    from assembled_cnn_b200.native import NativeModel, NativeRuntime
+    from assembled_cnn_b200.plan import ModelConfig
 
     cfg = ModelConfig(use_resnet_d=use_resnet_d, **cfg_kw)
     fp32 = dtype == "fp32"
     # tensors by their storage type; fp32 slots, gradients and partial rows
     t_tol = {"bf16": 2e-5, "f32": 2e-5} if fp32 else {"bf16": BF16_TOL, "f16": F16_TOL, "f32": 1e-4}
     f32_tol = 2e-4 if fp32 else F32_TOL
-    plan = build_plan(cfg, B, H, W, training=training, mixup_type=mix, label_smoothing=0.1,
-                      dtype=dtype, use_dropblock=use_dropblock, kd_temp=kd_temp)
+    nm = NativeModel(cfg, B, H, W, training=training, mixup_type=mix, label_smoothing=label_smoothing,
+                     dtype=dtype, use_dropblock=use_dropblock, kd_temp=kd_temp, deterministic=deterministic)
+    plan = nm.python_mirror()
     _, vs = M.build(seed=42, input_hw=64, use_resnet_d=use_resnet_d, **cfg_kw)
     g = torch.Generator().manual_seed(3)
     for n in vs.vars:       # non-trivial BN parameters / statistics
@@ -142,7 +145,7 @@ def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbo
     # fp32, so what remains is fp32 summation order and one storage rounding)
     it = PI.PlanInterpreter(plan, dtype=torch.float32 if dtype == "bf16" else torch.float64,
                             emulate_storage=False if fp32 else emulate_storage)
-    rt = Runtime(plan)
+    rt = NativeRuntime(nm)
     it.set_weights(vs.vars)
     rt.set_weights(vs.vars)
     hp = dict(lr=0.05, momentum=0.9, weight_decay=1e-4, keep_prob=keep_prob)
@@ -178,9 +181,11 @@ def lockstep(cfg_kw, use_resnet_d=False, B=4, HW=64, mix=0, training=True, verbo
 
     worst = {}
     failures = []
-    for idx, op in enumerate(plan.all_ops()):
+    assert len(plan.all_ops()) == len(nm.all_ops())
+    for idx, (op, native_op) in enumerate(zip(plan.all_ops(), nm.all_ops())):
+        assert op.kind == native_op.kind, (idx, op.kind, native_op.kind)
         it.run([op])
-        rt.run([op])
+        rt.run([native_op])
         torch.cuda.synchronize()
         for out in _outputs(op):
             kind = out[0]

@@ -196,7 +196,8 @@ PRODUCTION_SPLIT_MIN = 42
 
 
 def _production_wgrad_geoms():
-    """Distinct conv_wgrad geometries of the C3 plan as the library receives them (Runtime.geom)."""
+    """Distinct conv_wgrad geometries of the C3 plan as the library launches them (model_exec.cu's launch
+    geometry: acnn_op_conv_info reports the plan's, without the W-padded stem form)."""
     from assembled_cnn_b200._lib import ConvGeom
     from assembled_cnn_b200.plan import ModelConfig, build_plan
     cfg = ModelConfig(resnet_size=50, resnet_version=2, use_sk_block=True, anti_alias_type="sconv",
@@ -209,7 +210,7 @@ def _production_wgrad_geoms():
         g, wpad = op.geom, op.a.get("x_wpad")
         if wpad is None:
             cg = ConvGeom(*g.astuple())
-        else:                     # the W-padded space-to-depth stem input (see Runtime.geom)
+        else:                     # the W-padded space-to-depth stem input
             lo, hi = wpad
             row = (g.W + lo + hi) * g.Cin
             cg = ConvGeom(g.B, g.H, g.W, g.Cin * g.kw, g.Cout, g.kh, 1, 1, g.pad_h_lo, g.pad_h_hi,

@@ -1,13 +1,12 @@
 #!/usr/bin/env python
-"""Per-op timing of one eager training step (CUDA events around every plan op), grouped by op kind
-and by conv layer.  Also the entry used under ncu (`--ncu` runs exactly one un-timed step after
-warm-up so `-s/-c` can select it).
+"""Per-op timing of one eager training step on the library's executor (CUDA events around every
+plan op, each run as its own acnn_run_ops range), grouped by op kind and by conv layer.  Also the
+entry used under ncu (`--ncu` runs exactly one un-timed step after warm-up so `-s/-c` can select it).
 
     python tools/profile_step.py [--batch 256] [--ncu]
 """
 import argparse
 import os
-os.environ.setdefault('ACNN_NATIVE_PLAN', '0')   # per-op hooks live in the Python executor (same plan, same launches)
 import sys
 from collections import defaultdict
 
@@ -55,19 +54,24 @@ records = []
 orig_run = rt.run
 
 
-def timed_run(ops, overlap_wgrad=False):
+def timed_run(ops):
     for op in ops:
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
-        getattr(rt, "op_" + op.kind)(op)
+        orig_run([op])
         b.record()
         records.append((op, a, b))
 
 
-rt.run = timed_run
+def timed_forward():
+    rt.zero_step_buffers()
+    timed_run(rt.plan.forward)
+
+
+rt.run, rt.run_forward = timed_run, timed_forward
 tr.train_step(x, y)
 torch.cuda.synchronize()
-rt.run = orig_run
+del rt.run, rt.run_forward
 by_kind = defaultdict(lambda: [0.0, 0])
 rows = []
 for op, a, b in records:
@@ -75,12 +79,13 @@ for op, a, b in records:
     by_kind[op.kind][0] += ms
     by_kind[op.kind][1] += 1
     if op.kind in ("conv", "conv_dgrad", "conv_wgrad"):
-        g = op.geom
-        fl = 2.0 * g.B * g.Ho * g.Wo * g.Cout * g.kh * g.kw * g.Cin
-        nin, nout = g.B * g.H * g.W * g.Cin, g.B * g.Ho * g.Wo * g.Cout
+        g, _, aux = rt.plan.conv_info(op)       # the geometry the library launches (acnn_op_conv_info)
+        Ho, Wo = g.out_hw()
+        fl = 2.0 * g.B * Ho * Wo * g.Cout * g.kh * g.kw * g.Cin
+        nin, nout = g.B * g.H * g.W * g.Cin, g.B * Ho * Wo * g.Cout
         byt = 2.0 * (nin + nout)
         if op.kind == "conv_dgrad":
-            byt += 2.0 * nin * ((op.add_src is not None) + (op.mask_src is not None))
+            byt += 2.0 * nin * aux
         ideal = max(fl / 989e9, byt / 3350e6)   # ms: tensor vs HBM roofline (H100 SXM data sheet)
         rows.append((ms, op.kind, "%dx%d %d->%d k%d s%d" % (g.H, g.W, g.Cin, g.Cout, g.kh, g.stride),
                      fl / ms / 1e9, ideal))

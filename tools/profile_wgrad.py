@@ -28,7 +28,8 @@ SWEEP = (1, 2, 3, 4, 6, 8, 11, 16, 22, 32, 44, 66, 88, 131, 176, 264)
 
 def production_geoms():
     """{geometry key: (ConvGeom, launches per step)} of the c3 plan's conv_wgrad ops, as the library
-    receives them (the W-padded space-to-depth stem input as Runtime.geom passes it)."""
+    launches them: the stem's input is the W-padded space-to-depth image (model_exec.cu's launch
+    geometry; acnn_op_conv_info reports the plan's, without that form)."""
     cfg = ModelConfig(resnet_size=50, resnet_version=2, use_sk_block=True, anti_alias_type="sconv",
                       anti_alias_filter_size=3)
     plan = build_plan(cfg, 256, 224, 224, training=True, mixup_type=1, label_smoothing=0.1)
