@@ -4,7 +4,9 @@ best-checkpoint keeper (utils/hook_utils.py:29-56, utils/checkpoint_utils.py:24-
 File format: one `.npz` per checkpoint (TensorFlow's tensor-bundle format cannot be written without
 TensorFlow).  Keys are the reference's variable names -- `resnet_model/conv2d/kernel`,
 `.../batch_normalization_3/moving_mean`, ... -- with values in the reference's layouts (HWIO conv
-kernels, [in, out] dense kernel), the MomentumOptimizer slots as `<var>/Momentum` and `global_step`,
+kernels, [in, out] dense kernel), the MomentumOptimizer slots as `<var>/Momentum`, `global_step` and,
+for a run with dynamic loss scaling, its state as `loss_scale/current_loss_scale`, `loss_scale/good_steps`
+and `loss_scale/skipped_steps`,
 i.e. exactly what `tf.train.load_checkpoint(path).get_tensor(name)` returns for a TF-1.14 checkpoint
 of the reference.  A released checkpoint converts with four lines run where TensorFlow exists:
 
@@ -22,9 +24,14 @@ import numpy as np
 import torch
 
 
+# the dynamic loss scale's state (TF 2 Keras' LossScaleOptimizer keeps current_loss_scale and good_steps)
+LOSS_SCALE_KEYS = ("loss_scale/current_loss_scale", "loss_scale/good_steps", "loss_scale/skipped_steps")
+
+
 def save_checkpoint(path, model, trainer=None, use_resnet_d=None):
     """Write `<path>.npz` with every variable of the model (trainables + BN moving statistics) and,
-    when a Trainer is given, the momentum slots and global_step.  Returns the file name."""
+    when a Trainer is given, the momentum slots, global_step and, with dynamic loss scaling, its state.
+    Returns the file name."""
     if use_resnet_d is None:
         use_resnet_d = getattr(model, "use_resnet_d", False)
     arrays = {n: v.numpy() for n, v in model.get_weights(use_resnet_d).items()}
@@ -33,6 +40,11 @@ def save_checkpoint(path, model, trainer=None, use_resnet_d=None):
         for n in rt.plan.params:
             arrays[n + "/Momentum"] = rt.get_tf(n, rt.momentum).detach().float().cpu().numpy().copy()
         arrays["global_step"] = np.asarray(trainer.global_step, dtype=np.int64)
+        ls = trainer.loss_scale_state() if getattr(trainer, "dynamic", False) else None
+        if ls is not None:
+            arrays[LOSS_SCALE_KEYS[0]] = np.asarray(ls["scale"], dtype=np.float32)
+            arrays[LOSS_SCALE_KEYS[1]] = np.asarray(ls["good_steps"], dtype=np.int64)
+            arrays[LOSS_SCALE_KEYS[2]] = np.asarray(ls["skipped_steps"], dtype=np.int64)
     fname = path if path.endswith(".npz") else path + ".npz"
     os.makedirs(os.path.dirname(os.path.abspath(fname)), exist_ok=True)
     np.savez(fname, **arrays)
@@ -61,7 +73,9 @@ def latest_checkpoint(directory):
 
 
 def restore(model, ckpt, trainer=None, strict=True):
-    """Full restore (every variable; momentum + global_step into the Trainer if present)."""
+    """Full restore (every variable; momentum + global_step into the Trainer if present, and the dynamic loss
+    scale's state into a Trainer with dynamic loss scaling: without it that run keeps its initial scale; a
+    static Trainer ignores it)."""
     if isinstance(ckpt, str):
         ckpt = load_checkpoint(ckpt)
     cur = model.get_weights()
@@ -78,6 +92,9 @@ def restore(model, ckpt, trainer=None, strict=True):
                 rt.set_tf(n, torch.as_tensor(ckpt[key]), rt.momentum)
         if "global_step" in ckpt:
             trainer.global_step = int(ckpt["global_step"])
+        if getattr(trainer, "dynamic", False) and LOSS_SCALE_KEYS[0] in ckpt:
+            trainer.set_loss_scale_state(float(ckpt[LOSS_SCALE_KEYS[0]]), int(ckpt.get(LOSS_SCALE_KEYS[1], 0)),
+                                         int(ckpt.get(LOSS_SCALE_KEYS[2], 0)))
     return missing
 
 

@@ -4,6 +4,7 @@
 // its records -- no lookups, no allocation, nothing but kernel launches on the given stream.
 #include <string.h>
 
+#include <cmath>
 #include <memory>
 
 #include "common.h"
@@ -23,6 +24,10 @@ struct acnn_model {
   int n_descs = 0;
   // settings read at enqueue time
   double loss_scale = 1.0;
+  // dynamic loss scaling (acnn_set_dynamic_loss_scale): the caller's device state, NULL for the static scale
+  acnn_loss_scale_state* ls = nullptr;
+  int ls_growth = 2000, ls_divisor = 1;
+  acnn_loss_scale_state ls_init{};   // cudaMemcpyAsync source of the state's initialisation
   uint64_t dropblock_seed = 0x5EED5EEDull;
   int dropblock_feed = 0;
   int det = 0, planes = 1, adt = ACNN_BF16;
@@ -409,6 +414,9 @@ acnn_model::Launch resolve(acnn_model* m, const Op& op) {
     const int B = (int)r.I("B"), NC = (int)r.I("NC"), ld = (int)r.I("ld");
     float *loss = r.S("loss"), *dbias = r.G("dbias"), *work = r.S("work");
     return [=](void* st) {
+      if (m->ls)
+        return acnn_softmax_ce_scaled((const float*)logits, (const float*)y, (const float*)yt, T, B, NC, ld, ls,
+                                      &m->ls->scale, loss, dl, dbias, work, adt, st);
       return acnn_softmax_ce((const float*)logits, (const float*)y, (const float*)yt, T, B, NC, ld, ls,
                              (float)m->loss_scale, loss, dl, dbias, work, adt, st);
     };
@@ -531,7 +539,10 @@ acnn_model::Launch resolve(acnn_model* m, const Op& op) {
     float *w = m->params, *g = m->grads, *acc = m->momentum, *l2 = r.S("loss", 1), *scratch = r.S("scratch");
     const int64_t n = p.param_elems;
     const uint8_t* flags = reinterpret_cast<const uint8_t*>(m->ws + m->flags_off);
-    return [=](void* st) { return acnn_sgd_momentum(w, g, acc, n, flags, hp, l2, scratch, st); };
+    return [=](void* st) {
+      if (m->ls) return acnn_sgd_momentum_loss_scaled(w, g, acc, n, flags, hp, m->ls, m->ls_divisor, l2, scratch, st);
+      return acnn_sgd_momentum(w, g, acc, n, flags, hp, l2, scratch, st);
+    };
   }
   set_error("acnn_bind: unknown op kind '%s'", k.c_str());
   return acnn_model::Launch();
@@ -873,6 +884,33 @@ int acnn_set_loss_scale(acnn_model* m, double loss_scale) {
   return ACNN_OK;
 }
 
+int acnn_set_dynamic_loss_scale(acnn_model* m, acnn_loss_scale_state* state_dev, double initial_scale,
+                                int growth_interval, int grad_divisor, void* stream) {
+  ACNN_REQUIRE(m && m->bound && m->grads, "acnn_set_dynamic_loss_scale: not bound for training");
+  if (!state_dev) {
+    m->ls = nullptr;
+    return ACNN_OK;
+  }
+  const float s0 = (float)initial_scale;
+  ACNN_REQUIRE(initial_scale > 0 && std::isfinite(s0) && growth_interval >= 1 && grad_divisor >= 1,
+               "acnn_set_dynamic_loss_scale: bad argument (initial_scale > 0 and finite in fp32, growth_interval >= 1, "
+               "grad_divisor >= 1)");
+  const int rc = require_device("acnn_set_dynamic_loss_scale", "state_dev", state_dev);
+  if (rc != ACNN_OK) return rc;
+  m->ls_init = acnn_loss_scale_state{};
+  m->ls_init.scale = m->ls_init.last_scale = s0;
+  m->ls = state_dev;
+  m->ls_growth = growth_interval;
+  m->ls_divisor = grad_divisor;
+  return memcpy_async(state_dev, &m->ls_init, sizeof(acnn_loss_scale_state), stream, "acnn_set_dynamic_loss_scale");
+}
+
+int acnn_get_loss_scale_state(acnn_model* m, acnn_loss_scale_state* out, void* stream) {
+  ACNN_REQUIRE(m && out, "acnn_get_loss_scale_state: null argument");
+  ACNN_REQUIRE(m->ls, "acnn_get_loss_scale_state: dynamic loss scaling is not enabled");
+  return memcpy_async(out, m->ls, sizeof(acnn_loss_scale_state), stream, "acnn_get_loss_scale_state");
+}
+
 int acnn_set_dropblock(acnn_model* m, uint64_t seed, int feed_uniforms) {
   ACNN_REQUIRE(m, "acnn_set_dropblock: null model");
   m->dropblock_seed = seed;
@@ -998,7 +1036,11 @@ int acnn_backward(acnn_model* m, void* stream) {
 }
 int acnn_sgd_step(acnn_model* m, void* stream) {
   ACNN_REQUIRE(m, "acnn_sgd_step: null model");
-  return run_range(m, m->upd, 0, (int)m->upd.size(), stream);
+  int rc = ACNN_OK;
+  if (m->ls) rc = acnn_grads_nonfinite(m->grads, m->plan.param_elems, &m->ls->nonfinite, stream);
+  if (rc == ACNN_OK) rc = run_range(m, m->upd, 0, (int)m->upd.size(), stream);
+  if (rc == ACNN_OK && m->ls) rc = acnn_loss_scale_update(m->ls, m->ls_growth, stream);
+  return rc;
 }
 int acnn_step(acnn_model* m, void* stream) {
   int rc = acnn_forward(m, stream);

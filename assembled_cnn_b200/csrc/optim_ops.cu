@@ -1,6 +1,8 @@
 // Parameter handling: bf16 / fp16 operand copies of the fp32 master weights (fprop + dgrad layouts), the
 // space-to-depth stem weight transform, and the fused weight-decay + momentum SGD step over the
 // flat parameter buffer.  nets/optimizer_setting.py:23-38, nets/run_loop_classification.py:166-179.
+#include <algorithm>
+
 #include "common.h"
 #include "vec.cuh"
 
@@ -145,13 +147,26 @@ __global__ void s2d_wgrad_unpack_kernel(const float* __restrict__ dw2, float* __
 // than the previous one would read that call's partial sum as its counter and never finish the sum
 constexpr int kSgdMaxBlocks = kMaxSms * 8;
 
+// kScaled: the gradient scale comes from the dynamic loss-scale state, 1 / (grad_divisor * scale) rounded
+// once from double (what the host computes for a static scale), and a step whose gradients are not finite
+// writes neither w nor acc; its L2 sum is still taken
+template <bool kScaled>
 __global__ void __launch_bounds__(256)
 sgd_momentum_kernel(float* __restrict__ w, const float* __restrict__ grad, float* __restrict__ acc,
                     int64_t n, const uint8_t* __restrict__ decay_flag, const float* __restrict__ hp,
-                    float* l2_acc, float* l2_part) {
+                    const acnn_loss_scale_state* __restrict__ ls, int grad_divisor, float* l2_acc,
+                    float* l2_part) {
   pdl_wait();   // multi-wave grid: an early trigger would let the next kernel's CTAs take SM slots from this one
   __shared__ float sh[8];
-  const float lr = hp[0], mom = hp[1], wd = hp[2], gs = hp[3];
+  const float lr = hp[0], mom = hp[1], wd = hp[2];
+  float gs = 0.f;
+  bool skip = false;
+  if constexpr (kScaled) {
+    gs = (float)(1.0 / ((double)grad_divisor * (double)ls->scale));
+    skip = ls->nonfinite != 0u;
+  } else {
+    gs = hp[3];
+  }
   float l2 = 0.f;
   const int64_t nvec = n >> 2;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nvec;
@@ -173,6 +188,7 @@ sgd_momentum_kernel(float* __restrict__ w, const float* __restrict__ grad, float
       aa[k] = fmaf(mom, aa[k], g);
       ww[k] = fmaf(-lr, aa[k], ww[k]);
     }
+    if (skip) continue;
     reinterpret_cast<float4*>(w)[i] = make_float4(ww[0], ww[1], ww[2], ww[3]);
     reinterpret_cast<float4*>(acc)[i] = make_float4(aa[0], aa[1], aa[2], aa[3]);
   }
@@ -210,6 +226,58 @@ sgd_momentum_kernel(float* __restrict__ w, const float* __restrict__ grad, float
       }
     }
   }
+}
+
+// exponent bits all ones: +-inf or NaN (the complement of isfinite)
+__device__ __forceinline__ bool nonfinite(float v) { return (__float_as_uint(v) & 0x7f800000u) == 0x7f800000u; }
+__device__ __forceinline__ bool nonfinite4(float4 v) {
+  return nonfinite(v.x) | nonfinite(v.y) | nonfinite(v.z) | nonfinite(v.w);
+}
+
+// *flag = 1 when any of x[0, n) is not finite; nothing is written otherwise.  An OR of per-element tests:
+// neither the grid nor the order of the CTAs changes the result.  The `head` elements before the first
+// 16-byte boundary and the tail after the last whole float4 are tested one by one.
+__global__ void __launch_bounds__(256)
+grads_nonfinite_kernel(const float* __restrict__ x, int64_t head, int64_t nvec, int64_t tail,
+                       uint32_t* __restrict__ flag) {
+  pdl_wait();
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const float4* v = reinterpret_cast<const float4*>(x + head);
+  bool bad = false;
+  int64_t i = tid;
+  // four independent 16-byte loads in flight per thread and iteration
+  for (; i + 3 * stride < nvec; i += 4 * stride) {
+    const float4 a = __ldcs(v + i), b = __ldcs(v + i + stride), c = __ldcs(v + i + 2 * stride),
+                 d = __ldcs(v + i + 3 * stride);
+    bad |= nonfinite4(a) | nonfinite4(b) | nonfinite4(c) | nonfinite4(d);
+  }
+  for (; i < nvec; i += stride) bad |= nonfinite4(__ldcs(v + i));
+  if (tid < head) bad |= nonfinite(x[tid]);
+  if (tid < tail) bad |= nonfinite(x[head + 4 * nvec + tid]);
+  if (__syncthreads_or(bad) && threadIdx.x == 0) *flag = 1u;
+}
+
+// TF 2 Keras LossScaleOptimizer's update of the dynamic loss scale, after the SGD step of the flagged
+// gradients; clears the flag for the next step.  One thread: the whole state is 32 bytes.
+__global__ void loss_scale_update_kernel(acnn_loss_scale_state* __restrict__ s, int growth_interval) {
+  pdl_wait();
+  const float scale = s->scale;
+  s->last_scale = scale;
+  if (s->nonfinite != 0u) {
+    s->scale = fmaxf(scale * 0.5f, 1.f);
+    s->good_steps = 0;
+    s->skipped_steps += 1;
+  } else {
+    int good = s->good_steps + 1;
+    if (good >= growth_interval) {
+      const float up = scale * 2.f;
+      if (!nonfinite(up)) s->scale = up;
+      good = 0;
+    }
+    s->good_steps = good;
+  }
+  s->nonfinite = 0u;
 }
 
 }  // namespace acnn
@@ -282,10 +350,42 @@ int acnn_sgd_momentum(float* w, const float* grad, float* acc, int64_t n,
                       void* stream) {
   ACNN_REQUIRE(w && grad && acc && decay_flag && hp && n % 256 == 0 && (!l2_acc || scratch),
                "sgd_momentum: bad arguments (n must be a multiple of 256; l2_acc needs scratch)");
-  launch_k(sgd_momentum_kernel, dim3(grid_for(n / 4, 256, acnn::kSgdMaxBlocks)), dim3(256), 0,
-           (cudaStream_t)stream, w, grad, acc, n, decay_flag, hp, l2_acc, scratch);
+  launch_k(sgd_momentum_kernel<false>, dim3(grid_for(n / 4, 256, acnn::kSgdMaxBlocks)), dim3(256), 0,
+           (cudaStream_t)stream, w, grad, acc, n, decay_flag, hp, (const acnn_loss_scale_state*)nullptr, 1,
+           l2_acc, scratch);
   count_launch();
   return check_launch("sgd_momentum");
+}
+
+int acnn_sgd_momentum_loss_scaled(float* w, const float* grad, float* acc, int64_t n, const uint8_t* decay_flag,
+                                  const float* hp, const acnn_loss_scale_state* ls, int grad_divisor,
+                                  float* l2_acc, float* scratch, void* stream) {
+  ACNN_REQUIRE(w && grad && acc && decay_flag && hp && ls && grad_divisor >= 1 && n % 256 == 0 &&
+                   (!l2_acc || scratch),
+               "sgd_momentum_loss_scaled: bad arguments (n must be a multiple of 256; grad_divisor >= 1; l2_acc "
+               "needs scratch)");
+  launch_k(sgd_momentum_kernel<true>, dim3(grid_for(n / 4, 256, acnn::kSgdMaxBlocks)), dim3(256), 0,
+           (cudaStream_t)stream, w, grad, acc, n, decay_flag, hp, ls, grad_divisor, l2_acc, scratch);
+  count_launch();
+  return check_launch("sgd_momentum_loss_scaled");
+}
+
+int acnn_grads_nonfinite(const float* x, int64_t n, uint32_t* flag, void* stream) {
+  ACNN_REQUIRE(x && flag && n > 0 && ((uintptr_t)x & 3) == 0,
+               "grads_nonfinite: bad arguments (n > 0, x 4-byte aligned)");
+  const int64_t head = std::min<int64_t>(n, (int64_t)((16 - ((uintptr_t)x & 15)) & 15) / 4);
+  const int64_t nvec = (n - head) / 4, tail = n - head - 4 * nvec;
+  launch_k(grads_nonfinite_kernel, dim3(grid_for(std::max<int64_t>(nvec, 1), 256, acnn::kMaxSms * 8)), dim3(256), 0,
+           (cudaStream_t)stream, x, head, nvec, tail, flag);
+  count_launch();
+  return check_launch("grads_nonfinite");
+}
+
+int acnn_loss_scale_update(acnn_loss_scale_state* state, int growth_interval, void* stream) {
+  ACNN_REQUIRE(state && growth_interval >= 1, "loss_scale_update: bad arguments (growth_interval >= 1)");
+  launch_k(loss_scale_update_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, state, growth_interval);
+  count_launch();
+  return check_launch("loss_scale_update");
 }
 
 int acnn_fill_zero(void* p, int64_t bytes, void* stream) {

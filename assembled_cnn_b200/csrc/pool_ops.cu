@@ -582,7 +582,7 @@ template <class T>
 __global__ void __launch_bounds__(kPT)
 softmax_ce_kernel(const float* __restrict__ logits, const float* __restrict__ y,
                   const float* __restrict__ yt, float kd_temp, int B, int NC, int ld, float ls,
-                  float grad_scale, float* __restrict__ loss_rows, float* __restrict__ kd_rows,
+                  float grad_scale, const float* __restrict__ grad_scale_dev, float* __restrict__ loss_rows, float* __restrict__ kd_rows,
                   float* __restrict__ g32, T* __restrict__ dlogits) {
   pdl_wait();   // multi-wave grid: an early trigger would let the next kernel's CTAs take SM slots from this one
   __shared__ float sh[kPT / 32];
@@ -625,7 +625,7 @@ softmax_ce_kernel(const float* __restrict__ logits, const float* __restrict__ y,
     lse_t = mx * inv_t + logf(se_t);
     if (threadIdx.x == 0) kd_rows[b] = kd_temp * kd_temp * (lse_t * st - stl) / B;
   }
-  const float gs = grad_scale / B;
+  const float gs = (grad_scale_dev ? *grad_scale_dev : grad_scale) / B;
   for (int c = threadIdx.x; c < ld; c += kPT) {
     float g = 0.f;
     if (c < NC) {
@@ -855,9 +855,9 @@ int acnn_mix_labels(const int32_t* labels, const float* lam1, const float* lam2,
   return check_launch("mix_labels");
 }
 
-int acnn_softmax_ce(const float* logits, const float* y, const float* teacher, float kd_temp, int B,
-                    int NC, int ld, float label_smoothing, float grad_scale, float* loss_acc,
-                    void* dlogits, float* dbias, float* work, int dtype, void* stream) {
+static int softmax_ce(const float* logits, const float* y, const float* teacher, float kd_temp, int B, int NC,
+                      int ld, float label_smoothing, float grad_scale, const float* grad_scale_dev,
+                      float* loss_acc, void* dlogits, float* dbias, float* work, int dtype, void* stream) {
   ACNN_REQUIRE(logits && y && loss_acc && dlogits && work && NC <= ld && B > 0 &&
                    ACNN_DTYPE_OK(dtype) && (!teacher || kd_temp > 0.f), "softmax_ce: bad arguments");
   const int Bp = ((B + 31) / 32) * 32;
@@ -866,7 +866,7 @@ int acnn_softmax_ce(const float* logits, const float* y, const float* teacher, f
   float* g32 = work + 2 * Bp;                  // [B][ld]
   ACNN_BY_DTYPE(dtype, launch_k(softmax_ce_kernel<T>, dim3(B), dim3(kPT), 0, (cudaStream_t)stream,
                                 logits, y, teacher, kd_temp, B, NC, ld, label_smoothing, grad_scale,
-                                loss_rows, kd_rows, g32, (T*)dlogits));
+                                grad_scale_dev, loss_rows, kd_rows, g32, (T*)dlogits));
   count_launch();
   int rc = check_launch("softmax_ce");
   if (rc) return rc;
@@ -875,6 +875,22 @@ int acnn_softmax_ce(const float* logits, const float* y, const float* teacher, f
            (const float*)g32, B, NC, ld, loss_acc, dbias);
   count_launch();
   return check_launch("ce_finalize");
+}
+
+int acnn_softmax_ce(const float* logits, const float* y, const float* teacher, float kd_temp, int B,
+                    int NC, int ld, float label_smoothing, float grad_scale, float* loss_acc,
+                    void* dlogits, float* dbias, float* work, int dtype, void* stream) {
+  return softmax_ce(logits, y, teacher, kd_temp, B, NC, ld, label_smoothing, grad_scale, nullptr, loss_acc, dlogits,
+                    dbias, work, dtype, stream);
+}
+
+int acnn_softmax_ce_scaled(const float* logits, const float* y, const float* teacher, float kd_temp, int B,
+                           int NC, int ld, float label_smoothing, const float* grad_scale_dev,
+                           float* loss_acc, void* dlogits, float* dbias, float* work, int dtype,
+                           void* stream) {
+  ACNN_REQUIRE(grad_scale_dev, "softmax_ce_scaled: null grad_scale_dev");
+  return softmax_ce(logits, y, teacher, kd_temp, B, NC, ld, label_smoothing, 0.f, grad_scale_dev, loss_acc, dlogits,
+                    dbias, work, dtype, stream);
 }
 
 }  // extern "C"

@@ -68,7 +68,8 @@ DEFAULTS = {
     "batch_size": 32,
     "train_epochs": 90,                   # main_classification.py:38
     "dtype": "bf16",                      # reference enum is fp32|fp16; bf16 added (the default here)
-    "loss_scale": None,                   # None: the dtype's default, get_loss_scale (fp16: 128, else 1)
+    "loss_scale": None,                   # None: the dtype's default, get_loss_scale (fp16: 128, else 1);
+                                          # "dynamic": dynamic loss scaling (model_fns.Trainer)
     "data_format": "channels_last",       # NHWC is the only layout of this implementation
     "num_gpus": 1,
 }
@@ -93,6 +94,7 @@ def params_from_flags(**overrides) -> dict:
     unknown = set(overrides) - set(DEFAULTS)
     if unknown:
         raise KeyError("unknown flag(s): %s" % ", ".join(sorted(unknown)))
+    check_loss_scale(overrides.get("loss_scale"))
     p = dict(DEFAULTS)
     p.update(overrides)
     return p
@@ -103,11 +105,22 @@ def params_from_flags(**overrides) -> dict:
 DEFAULT_LOSS_SCALE = {"fp16": 128, "fp32": 1, "bf16": 1}
 
 
+def check_loss_scale(loss_scale):
+    """loss_scale: None, a number, or the string "dynamic" (the spelling later versions of the reference's
+    official/utils/flags/_performance.py accept); any other string raises ValueError."""
+    if isinstance(loss_scale, str) and loss_scale != "dynamic":
+        raise ValueError('loss_scale must be None, a number or "dynamic" (got %r)' % (loss_scale,))
+    return loss_scale
+
+
 def get_loss_scale(loss_scale, dtype):
     """official/utils/flags/_performance.py:39-42 get_loss_scale: an explicit loss_scale wins, otherwise the
-    dtype's default (fp16: 128; bf16 / fp32: 1).  0 counts as 1 (no scaling)."""
+    dtype's default (fp16: 128; bf16 / fp32: 1).  0 counts as 1 (no scaling).  "dynamic" is returned as it
+    is, for every dtype; any other string raises ValueError."""
     if dtype not in DEFAULT_LOSS_SCALE:
         raise ValueError("dtype must be one of: {}".format(tuple(DEFAULT_LOSS_SCALE)))
+    if check_loss_scale(loss_scale) == "dynamic":
+        return "dynamic"
     if loss_scale is None:
         return float(DEFAULT_LOSS_SCALE[dtype])
     return float(loss_scale or 1)

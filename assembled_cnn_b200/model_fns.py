@@ -36,7 +36,7 @@ from . import _lib, dp
 from .hparams import DATASETS, DEFAULTS, get_loss_scale, params_from_flags
 from .plan import BLOCK_SIZES, ModelConfig, build_plan
 from .metrics import EvalMetrics, RecallAtK
-from .native import NativeModel, NativeRuntime
+from .native import NativeModel, NativeRuntime, check_dynamic_loss_scale
 from .staging import StagingRing, pack_u8, read_ahead
 
 DEFAULT_VERSION = 1
@@ -303,6 +303,14 @@ class Trainer:
     the reported loss averaged (acnn_replica_accumulate), then one SGD step with grad_scale 1 / (world * R *
     loss_scale).  The reference's --num_gpus=N is world * replicas_per_device = N.
 
+    params["loss_scale"] = "dynamic" turns on dynamic loss scaling, for every dtype (the rules at
+    acnn_loss_scale_state in include/acnn.h, TF 2 Keras' LossScaleOptimizer): the scale starts at
+    initial_loss_scale, a step whose summed (and all-reduced) gradients are not all finite leaves the weights
+    and momentum as they were and halves the scale (not below 1), and loss_scale_growth_interval finite steps
+    in a row double it.  The decision and the scale live on the device, inside the update graph: no host read.
+    The moving statistics, the reported losses and the global step (so the LR and keep-prob schedules) advance
+    on every step, skipped or not.  loss_scale_state() reads the state.
+
     train_metrics=True accumulates the training summaries' metrics on the device (acnn_classify_rows and
     acnn_train_metrics_accumulate after every micro-step's backward, on the current stream; no host read):
     the top-1 / top-5 hits and the ECE bins since reset_train_metrics(), and the step's rows and confidence
@@ -312,9 +320,11 @@ class Trainer:
     the step's confidence is meaningful."""
 
     def __init__(self, model: Model, params: dict, height=224, width=224, *, use_cuda_graph=True,
-                 lam_seed=7, num_images=None, replicas_per_device=1, train_metrics=False):
+                 lam_seed=7, num_images=None, replicas_per_device=1, train_metrics=False,
+                 initial_loss_scale=2.0 ** 15, loss_scale_growth_interval=2000):
         """num_images: training images per epoch for the LR and keep-prob schedules (default: the
-        dataset's data_config count)."""
+        dataset's data_config count).  initial_loss_scale and loss_scale_growth_interval apply with
+        params["loss_scale"] = "dynamic" only."""
         p = params
         if p.get("cls_loss_type", "softmax") != "softmax":
             raise NotImplementedError("only cls_loss_type='softmax' is on the hot path")
@@ -323,6 +333,11 @@ class Trainer:
         self.replicas = check_replicas_per_device(replicas_per_device)
         self.world = torch.distributed.get_world_size() if torch.distributed.is_initialized() else 1
         self.local_batch = per_device_batch_size(p["batch_size"], self.world * self.replicas)
+        # the reference's get_loss_scale: an explicit loss_scale wins, else 128 for fp16 and 1 otherwise
+        loss_scale = get_loss_scale(p.get("loss_scale"), model.dtype)
+        self.dynamic = loss_scale == "dynamic"
+        if self.dynamic:
+            check_dynamic_loss_scale(initial_loss_scale, loss_scale_growth_interval)
         self.mixup_type = int(p.get("mixup_type", 0))
         self.kd_temp = float(p.get("kd_temp", 0) or 0)
         self.use_dropblock = bool(p.get("use_dropblock", False))
@@ -352,9 +367,12 @@ class Trainer:
             warmup_epochs=p["lr_warmup_epochs"])
         self.global_step = 0
         self.rng = np.random.default_rng(lam_seed)
-        # the reference's get_loss_scale: an explicit loss_scale wins, else 128 for fp16 and 1 otherwise
-        self.loss_scale = get_loss_scale(p.get("loss_scale"), model.dtype)
-        self.rt.loss_scale = self.loss_scale
+        self.loss_scale = loss_scale
+        if self.dynamic:
+            self.rt.enable_dynamic_loss_scale(initial_loss_scale, loss_scale_growth_interval,
+                                              self.world * self.replicas)
+        else:
+            self.rt.loss_scale = self.loss_scale
         self.use_graph = use_cuda_graph
         self._graphs = None
         m = self.rt.plan.meta
@@ -391,6 +409,16 @@ class Trainer:
             self._metrics = train_metrics_buffer(self.rt.dev)
             self._metric_rows = tuple(torch.empty(self.local_batch, dtype=dt, device=self.rt.dev)
                                       for dt in (torch.int32, torch.float32, torch.int32, torch.float32))
+
+    def loss_scale_state(self):
+        """{scale, good_steps, skipped_steps} of dynamic loss scaling, with one device read (for tests and
+        logging; the step never reads it); None with a static scale."""
+        st = self.rt.loss_scale_state()
+        return None if st is None else {k: st[k] for k in ("scale", "good_steps", "skipped_steps")}
+
+    def set_loss_scale_state(self, scale, good_steps=0, skipped_steps=0):
+        """Overwrite the dynamic state (a resumed run), on the current stream."""
+        self.rt.set_loss_scale_state(scale, good_steps, skipped_steps)
 
     @property
     def train_metrics(self):
@@ -443,7 +471,7 @@ class Trainer:
                     fns.append(lambda ops=bwd[a:b]: rt.run(ops))
         graphs = []
         with torch.cuda.stream(s):
-            for fn in fns + [lambda: rt.run(rt.plan.update)]:
+            for fn in fns + [rt.run_update]:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, stream=s):
                     fn()
@@ -595,7 +623,8 @@ class Trainer:
         hp[0] = lr
         hp[1] = self.p["momentum"]
         hp[2] = self.p["weight_decay"]
-        hp[3] = 1.0 / (self.world * self.replicas * self.loss_scale)
+        # dynamic loss scaling takes the gradient scale from its device state
+        hp[3] = 0.0 if self.dynamic else 1.0 / (self.world * self.replicas * self.loss_scale)
         if keep_prob is None:
             keep_prob = self.keep_prob_fn(self.global_step) if self.keep_prob_fn else 1.0
         hp[4] = keep_prob
@@ -627,7 +656,7 @@ class Trainer:
         if self.use_graph:
             self._graphs[-1].replay()
         else:
-            rt.run(rt.plan.update)
+            rt.run_update()
         if self.world > 1:
             self.sync_moving_statistics()
         self.global_step += 1

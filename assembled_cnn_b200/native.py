@@ -86,6 +86,8 @@ PROTOTYPES = {
     "acnn_bind": (_i, [_vp] * 9),
     "acnn_validate": (_i, [_vp]),
     "acnn_set_loss_scale": (_i, [_vp, C.c_double]),
+    "acnn_set_dynamic_loss_scale": (_i, [_vp, _vp, C.c_double, _i, _i, _vp]),
+    "acnn_get_loss_scale_state": (_i, [_vp, _vp, _vp]),
     "acnn_set_dropblock": (_i, [_vp, C.c_uint64, _i]),
     "acnn_set_inputs": (_i, [_vp] * 7),
     "acnn_set_images_u8": (_i, [_vp] * 4),
@@ -278,6 +280,26 @@ class NativeModel:
             pass
 
 
+def check_dynamic_loss_scale(initial_scale, growth_interval):
+    """The initial scale of dynamic loss scaling must be > 0 and finite in fp32, the growth interval an integer
+    >= 1 (ValueError otherwise)."""
+    s = float(initial_scale)
+    with np.errstate(over="ignore"):
+        ok = s > 0 and np.isfinite(np.float32(s))
+    if not ok:
+        raise ValueError("initial loss scale must be > 0 and finite in fp32 (got %r)" % (initial_scale,))
+    g = growth_interval
+    if isinstance(g, bool) or not isinstance(g, (int, np.integer)) or g < 1:
+        raise ValueError("loss scale growth interval must be an integer >= 1 (got %r)" % (g,))
+
+
+def decode_loss_scale_state(words):
+    """struct acnn_loss_scale_state from its 8 int32 words (a CPU tensor or array)."""
+    v = np.asarray(words, dtype=np.int32)
+    f = v.view(np.float32)
+    return {"scale": float(f[0]), "good_steps": int(v[1]), "skipped_steps": int(v[2]), "last_scale": float(f[4])}
+
+
 def _check_u8_images(images_u8, images, mean):
     """Arguments of set_images_u8: uint8 NHWC of the input buffer's shape on its device, float32 mean[3]."""
     if images_u8.dtype != torch.uint8 or tuple(images_u8.shape) != tuple(images.shape) \
@@ -394,6 +416,7 @@ class NativeRuntime:
                                       ptr(self.state), ptr(self.w_fprop), ptr(self.w_dgrad), ptr(ws),
                                       self.stream), "acnn_bind")
         self._loss_scale = c.loss_scale
+        self.loss_scale_state_buf = None     # int32 [8], struct acnn_loss_scale_state, with dynamic scaling
         self._db_seed, self._db_feed = 0x5EED5EED, False
         self.graph = None
 
@@ -464,8 +487,51 @@ class NativeRuntime:
 
     @loss_scale.setter
     def loss_scale(self, v):
+        """A number: the static scale (and dynamic scaling off); "dynamic": enable_dynamic_loss_scale() with
+        its defaults."""
+        if isinstance(v, str):
+            if v != "dynamic":
+                raise ValueError('loss_scale must be a number or "dynamic" (got %r)' % (v,))
+            self.enable_dynamic_loss_scale()
+            return
+        if self.loss_scale_state_buf is not None:
+            _lib.check(self.lib.acnn_set_dynamic_loss_scale(self.model.handle, None, 0.0, 1, 1, self.stream),
+                       "acnn_set_dynamic_loss_scale")
+            self.loss_scale_state_buf = None
         self._loss_scale = float(v)
         _lib.check(self.lib.acnn_set_loss_scale(self.model.handle, float(v)), "acnn_set_loss_scale")
+
+    def enable_dynamic_loss_scale(self, initial_scale=2.0 ** 15, growth_interval=2000, grad_divisor=1):
+        """acnn_set_dynamic_loss_scale: the loss seed, the skip and the gradient scale of every later step come
+        from a device state this runtime owns (`loss_scale_state_buf`, initialised on the current stream).
+        grad_divisor: world * replicas per device, the replicas the gradient buffer sums."""
+        check_dynamic_loss_scale(initial_scale, growth_interval)
+        if self.grads is None:
+            raise ValueError("dynamic loss scaling needs a training runtime")
+        buf = torch.zeros(8, dtype=torch.int32, device=self.dev)
+        _lib.check(self.lib.acnn_set_dynamic_loss_scale(self.model.handle, buf.data_ptr(), float(initial_scale),
+                                                        int(growth_interval), int(grad_divisor), self.stream),
+                   "acnn_set_dynamic_loss_scale")
+        self.loss_scale_state_buf = buf
+        self._loss_scale = "dynamic"
+
+    def loss_scale_state(self):
+        """{scale, good_steps, skipped_steps, last_scale} of the dynamic state: one device read (it waits for
+        the work enqueued so far).  None with a static scale."""
+        if self.loss_scale_state_buf is None:
+            return None
+        return decode_loss_scale_state(self.loss_scale_state_buf.cpu())
+
+    def set_loss_scale_state(self, scale, good_steps=0, skipped_steps=0):
+        """Overwrite the dynamic state (a resumed run), on the current stream."""
+        if self.loss_scale_state_buf is None:
+            raise ValueError("set_loss_scale_state: dynamic loss scaling is not enabled")
+        scale = float(np.float32(scale))
+        check_dynamic_loss_scale(scale, 1)
+        v = np.zeros(8, np.int32)
+        v[[0, 4]] = np.array([scale, scale], np.float32).view(np.int32)
+        v[1], v[2] = int(good_steps), int(skipped_steps)
+        self.loss_scale_state_buf.copy_(torch.from_numpy(v))
 
     def _push_dropblock(self):
         _lib.check(self.lib.acnn_set_dropblock(self.model.handle, self._db_seed & 0xFFFFFFFFFFFFFFFF,
@@ -545,6 +611,10 @@ class NativeRuntime:
         _lib.check(self.lib.acnn_forward(h, st), "acnn_forward")
         if self.model.sizes.n_loss_first < self.model.sizes.n_forward:
             _lib.check(self.lib.acnn_loss(h, st), "acnn_loss")
+
+    def run_update(self):
+        """acnn_sgd_step: the update phase (with dynamic loss scaling also its check and scale update)."""
+        _lib.check(self.lib.acnn_sgd_step(self.model.handle, self.stream), "acnn_sgd_step")
 
     def run_step(self):
         """zero -> forward -> backward -> SGD, all enqueued on the current stream."""

@@ -21,6 +21,7 @@ import torch
 
 from .imagenet_eval import write_record
 from .metrics import TRAIN_METRICS_DTYPE, train_metric_values
+from .native import decode_loss_scale_state
 
 log = logging.getLogger("assembled_cnn_b200")
 
@@ -133,6 +134,8 @@ class TrainSummaries:
     ahead of the device (Trainer's hyper-parameter ring), so a full ring's oldest slot has completed."""
 
     RING = 8
+    # dynamic loss scaling: per slot the state after the step (the scale it used, the steps skipped so far)
+    _ls_host = None
 
     def __init__(self, model_dir, trainer):
         self.writer = SummaryWriter(model_dir)
@@ -142,6 +145,8 @@ class TrainSummaries:
         self._host = [(torch.zeros(3, dtype=torch.float32).pin_memory(),
                        torch.zeros(TRAIN_METRICS_DTYPE.itemsize, dtype=torch.uint8).pin_memory())
                       for _ in range(self.RING)]
+        if trainer.dynamic:
+            self._ls_host = [torch.zeros(8, dtype=torch.int32).pin_memory() for _ in range(self.RING)]
         self._pending = deque()      # (slot, event, step, lr, keep_prob, wall time, steps/s or None)
         self._next = 0
         self._last = None            # (step, host clock) of the previous summary
@@ -154,6 +159,8 @@ class TrainSummaries:
         hloss, hacc = self._host[slot]
         hloss[:loss.numel()].copy_(loss, non_blocking=True)
         hacc.copy_(self.tr.train_metrics, non_blocking=True)
+        if self._ls_host is not None:
+            self._ls_host[slot].copy_(self.tr.rt.loss_scale_state_buf, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.tr.rt.dev))
         now = time.time()
@@ -194,10 +201,15 @@ class TrainSummaries:
             scalars += [(k, m[k]) for k in ("train_accuracy", "train_accuracy_top_5", "train_ece")]
         if rate is not None:
             scalars.append(("global_step/sec", rate))
+        ls = ""
+        if self._ls_host is not None:
+            st = decode_loss_scale_state(self._ls_host[slot].numpy())
+            scalars += [("loss_scale", st["last_scale"]), ("loss_scale/skipped_steps", st["skipped_steps"])]
+            ls = ", loss_scale = %g, skipped_steps = %d" % (st["last_scale"], st["skipped_steps"])
         self.writer.add_scalars(step, scalars, wall)
         log.info("step %d: learning_rate = %.6g, cross_entropy = %.6g, train_accuracy = %.6g, train_ece = %.6g, "
-                 "global_step/sec = %s", step, lr, ce, m.get("train_accuracy", 0), m.get("train_ece", 0),
-                 "-" if rate is None else "%.4g" % rate)
+                 "global_step/sec = %s%s", step, lr, ce, m.get("train_accuracy", 0), m.get("train_ece", 0),
+                 "-" if rate is None else "%.4g" % rate, ls)
 
     def close(self):
         self.drain()

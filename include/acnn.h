@@ -353,6 +353,12 @@ int acnn_mix_labels(const int32_t* labels, const float* lam1, const float* lam2,
 int acnn_softmax_ce(const float* logits, const float* y, const float* teacher, float kd_temp, int B,
                     int NC, int ld, float label_smoothing, float grad_scale, float* loss_acc,
                     void* dlogits, float* dbias, float* work, int dtype, void* stream);
+/* acnn_softmax_ce with grad_scale read from DEVICE memory when the kernel runs (the scale of a dynamic
+ * loss-scale state, acnn_loss_scale_state.scale), so a captured graph follows its changes. */
+int acnn_softmax_ce_scaled(const float* logits, const float* y, const float* teacher, float kd_temp, int B,
+                           int NC, int ld, float label_smoothing, const float* grad_scale_dev,
+                           float* loss_acc, void* dlogits, float* dbias, float* work, int dtype,
+                           void* stream);
 /* Teacher labels of knowledge distillation: softmax(teacher_logits[Bin,NC] / kd_temp) mixed with the
  * images' mixup pairing (utils/data_util.py:128-156, modes as acnn_pack_input; the second half of a
  * type-2 batch mixes the supervised one-hot of `labels`, as the reference does at :154). */
@@ -423,6 +429,39 @@ int acnn_sgd_momentum(float* w, const float* grad, float* acc, int64_t n,
                       void* stream);
 int acnn_sgd_scratch_floats(void);
 int acnn_fill_zero(void* p, int64_t bytes, void* stream);
+
+/* Dynamic loss scaling, decided and applied on the device (the rules of TF 2 Keras' LossScaleOptimizer).
+ * A step's loss seed is scale / B (acnn_softmax_ce_scaled); after the backward (and any gradient sum or
+ * all-reduce) acnn_grads_nonfinite tests the gradient buffer, acnn_sgd_momentum_loss_scaled applies or skips
+ * the update and acnn_loss_scale_update moves the scale:
+ *   finite step:      update with grad_scale 1 / (grad_divisor * scale); good_steps += 1; when good_steps
+ *                     reaches growth_interval, scale *= 2 (kept only if finite) and good_steps = 0
+ *   non-finite step:  w and acc untouched; scale = max(scale / 2, 1); good_steps = 0; skipped_steps += 1
+ * Nothing reaches the host: the sequence replays in a CUDA graph.  32 bytes of DEVICE memory: */
+typedef struct acnn_loss_scale_state {
+  float scale;            /* the loss scale of the next step */
+  int32_t good_steps;     /* finite steps since the scale last changed */
+  int32_t skipped_steps;  /* non-finite steps so far */
+  uint32_t nonfinite;     /* != 0: the gradients of the step in flight are not all finite; 0 between steps */
+  float last_scale;       /* the scale the last updated step ran with */
+  int32_t reserved_[3];
+} acnn_loss_scale_state;
+/* *flag = 1 when any of the fp32 x[0, n) is +-inf or NaN (isfinite per element); nothing is written
+ * otherwise, so the caller clears it (acnn_loss_scale_update does).  One pass in float4 vectors (scalar head
+ * and tail); an OR of per-element tests, independent of the grid and of the order of the CTAs.  x: 4-byte
+ * aligned. */
+int acnn_grads_nonfinite(const float* x, int64_t n, uint32_t* flag, void* stream);
+/* acnn_sgd_momentum with the gradient scale taken from `ls`: grad_scale = (float)(1 / (grad_divisor *
+ * ls->scale)) computed in double and rounded once (grad_divisor: the data-parallel replicas the gradient
+ * sums, world * replicas per device); hp[3] is not read.  ls->nonfinite != 0 leaves w and acc bit for bit as
+ * they were and still adds the L2 sum to l2_acc. */
+int acnn_sgd_momentum_loss_scaled(float* w, const float* grad, float* acc, int64_t n,
+                                  const uint8_t* decay_flag, const float* hp,
+                                  const acnn_loss_scale_state* ls, int grad_divisor, float* l2_acc,
+                                  float* scratch, void* stream);
+/* The scale update of the rules above from state->nonfinite, then state->last_scale = the scale the step
+ * used and state->nonfinite = 0.  One thread. */
+int acnn_loss_scale_update(acnn_loss_scale_state* state, int growth_interval, void* stream);
 
 /* Several data-parallel replicas run one after another on one device (micro-steps r = 0 .. R-1 of one
  * global step, each a full forward + backward from the same moving statistics).  One fused pass per

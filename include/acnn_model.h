@@ -170,6 +170,19 @@ int acnn_validate(acnn_model* m);
 /* Mutable step settings (read at enqueue time, not captured values of a CUDA graph's kernels: the
  * loss scale is a kernel argument, so re-capture after changing it). */
 int acnn_set_loss_scale(acnn_model* m, double loss_scale);
+/* Dynamic loss scaling (the rules at acnn_loss_scale_state in acnn.h) on a bound training handle.  state_dev:
+ * caller-owned DEVICE memory of one acnn_loss_scale_state, initialised here on `stream` to {initial_scale, 0,
+ * 0, 0, initial_scale}; the caller may overwrite it between steps (a resumed run).  growth_interval >= 1;
+ * grad_divisor: the data-parallel replicas the gradient buffer sums (world * replicas per device; 1 for one
+ * model on one device).  From then on the loss op seeds scale / B from the state, and acnn_sgd_step (so
+ * acnn_step) runs acnn_grads_nonfinite over the gradients, the skip-aware SGD and acnn_loss_scale_update:
+ * no host read, capturable.  hp[3] is not read and acnn_set_loss_scale's value is not used.  NULL state_dev
+ * returns the handle to its static scale.  Read at enqueue time: re-capture after a change. */
+int acnn_set_dynamic_loss_scale(acnn_model* m, acnn_loss_scale_state* state_dev, double initial_scale,
+                                int growth_interval, int grad_divisor, void* stream);
+/* Copies the dynamic loss-scale state (32 bytes) to a host or device `out` on `stream`;
+ * ACNN_ERR_INVALID when dynamic scaling is not enabled. */
+int acnn_get_loss_scale_state(acnn_model* m, acnn_loss_scale_state* out, void* stream);
 /* DropBlock randomness: Philox key, and feed != 0 takes the uniforms from the "dropblock_u" tensors. */
 int acnn_set_dropblock(acnn_model* m, uint64_t seed, int feed_uniforms);
 
@@ -212,7 +225,9 @@ int acnn_backward(acnn_model* m, void* stream);  /* all gradients into the flat 
 /* Backward ops [first, last): lets a data-parallel host all-reduce a gradient bucket as soon as
  * acnn_variable_info.grad_ready_op of all its variables has run. */
 int acnn_backward_range(acnn_model* m, int first, int last, void* stream);
-int acnn_sgd_step(acnn_model* m, void* stream);  /* weight decay + momentum + L2 loss, from hp */
+/* weight decay + momentum + L2 loss, from hp; with dynamic loss scaling also the finiteness check before and
+ * the scale update after (acnn_set_dynamic_loss_scale) */
+int acnn_sgd_step(acnn_model* m, void* stream);
 int acnn_step(acnn_model* m, void* stream);      /* forward + loss + backward + sgd_step */
 /* Several data-parallel replicas per device (acnn_replica_accumulate of acnn.h over this handle's grads,
  * state and loss): a global step of R = `replicas` replicas is
