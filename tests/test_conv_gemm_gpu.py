@@ -367,6 +367,13 @@ def test_cta_pair_fprop_dgrad_match_single_cta_and_oracle(lib, case):
     xd = x.bfloat16().cuda()
     wd = w_hwio.permute(3, 0, 1, 2).contiguous().bfloat16().cuda()
     addd, maskd = add.bfloat16().cuda(), mask.bfloat16().cuda()
+    # the data gradient: its GEMM N is Cin, its K channels are Cout; add / mask have the shape of dx
+    dy = _rand_bf16(B, H, W, Cout, seed=25)
+    dadd = _rand_bf16(B, H, W, Cin, seed=26)
+    dmask = _rand_bf16(B, H, W, Cin, seed=27)
+    dmask[dmask.abs() < 0.3] = 0.0                  # the exact zeros of a ReLU output
+    wdg = w_hwio.flip(0, 1).permute(2, 0, 1, 3).contiguous().bfloat16().cuda()
+    dyd, daddd, dmaskd = dy.bfloat16().cuda(), dadd.bfloat16().cuda(), dmask.bfloat16().cuda()
     outs = {}
     for on in (0, 1):
         with _pairs(lib, on):
@@ -374,14 +381,22 @@ def test_cta_pair_fprop_dgrad_match_single_cta_and_oracle(lib, case):
             sp = torch.full((parts, 2, Cout), float("nan"), device="cuda")
             y = torch.full((B, H, W, Cout), float("nan"), dtype=torch.bfloat16, device="cuda")
             y2 = torch.full((B, H, W, Cout), float("nan"), dtype=torch.bfloat16, device="cuda")
+            dx = torch.full((B, H, W, Cin), float("nan"), dtype=torch.bfloat16, device="cuda")
+            dx2 = torch.full((B, H, W, Cin), float("nan"), dtype=torch.bfloat16, device="cuda")
             _lib.check(lib.acnn_conv_fprop(g, xd.data_ptr(), wd.data_ptr(), y.data_ptr(),
                                            sp.data_ptr(), None, None, None, 0, 0, 0, st), "fprop")
             _lib.check(lib.acnn_conv_fprop(g, xd.data_ptr(), wd.data_ptr(), y2.data_ptr(), None,
                                            addd.data_ptr(), maskd.data_ptr(), None, 0, 0, 0, st))
+            _lib.check(lib.acnn_conv_dgrad(g, dyd.data_ptr(), wdg.data_ptr(), dx.data_ptr(), None, None,
+                                           0, 0, st), "dgrad")
+            _lib.check(lib.acnn_conv_dgrad(g, dyd.data_ptr(), wdg.data_ptr(), dx2.data_ptr(),
+                                           daddd.data_ptr(), dmaskd.data_ptr(), 0, 0, st), "dgrad add / mask")
             torch.cuda.synchronize()
-            outs[on] = (y.float().cpu(), y2.float().cpu(), sp.double().sum(0).cpu(), parts)
+            outs[on] = (y.float().cpu(), y2.float().cpu(), sp.double().sum(0).cpu(), parts,
+                        dx.float().cpu(), dx2.float().cpu())
     # identical math, identical k order within a tile: the pair path reproduces the single-CTA path
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
+    assert torch.equal(outs[0][4], outs[1][4]) and torch.equal(outs[0][5], outs[1][5])
     assert _relerr(outs[1][2], outs[0][2]) < 1e-5
     # and a sampled check against the oracle (first and last image)
     for b in (0, B - 1):
@@ -389,6 +404,12 @@ def test_cta_pair_fprop_dgrad_match_single_cta_and_oracle(lib, case):
         assert _relerr(outs[1][0][b:b + 1], ref) < BF16_TOL
         want = (ref + add[b:b + 1]) * (mask[b:b + 1] > 0)
         assert _relerr(outs[1][1][b:b + 1], want) < BF16_TOL
+        xb = x[b:b + 1].clone().requires_grad_(True)
+        (dx_ref,) = torch.autograd.grad(_ref_conv(xb, w_hwio, g), xb, dy[b:b + 1])
+        assert _relerr(outs[1][4][b:b + 1], dx_ref) < BF16_TOL
+        want = (dx_ref + dadd[b:b + 1]) * (dmask[b:b + 1] > 0)
+        assert _relerr(outs[1][5][b:b + 1], want) < BF16_TOL
+        assert bool((outs[1][5][b:b + 1][dmask[b:b + 1] <= 0] == 0).all())
 
 
 @contextlib.contextmanager
