@@ -9,12 +9,15 @@
 //                      both operands are MN-major (the pixel index is the GEMM K dimension).
 //
 // Warp roles (384 threads): warp 0 = TMA producer (warps 1..3 idle), warpgroups 1 and 2 = wgmma
-// consumers + epilogue, 64 accumulator rows each.
+// consumers + epilogue, 64 accumulator rows each.  The bf16 / fp16 fprop and dgrad GEMMs with
+// K <= 512 run conv_gemm_kernel two CTAs per SM instead (160 threads: one consumer warpgroup for all
+// 128 rows, warp 4 = TMA producer), so one CTA's epilogue overlaps the other's MMAs.
 //
 // Reference semantics: nets/model_helper.py:67-78 (conv2d_fixed_padding), tf.gradients backward.
 #include <stdlib.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.h"
 #include "ptx.cuh"
@@ -95,6 +98,11 @@ constexpr int kConsumerThreads = 256;
 constexpr int kConsumerWarps = 8;
 constexpr int kMaxStages = 8;
 constexpr int kSmemBudget = 224 * 1024;   // dynamic smem (227 KiB max per CTA on sm_90)
+// Two co-resident CTAs per SM (WG = 1 below): one consumer warpgroup (warps 0..3, both 64-row halves
+// of the 128-row tile) + one TMA producer warp (warp 4), so one CTA's epilogue runs while the other's
+// MMAs do.  Dynamic smem per CTA: 2 x (dynamic + static barriers + 1 KiB reserved) <= 228 KiB.
+constexpr int kSmemBudget2 = 112 * 1024 + 512;
+__host__ __device__ constexpr int conv_threads(int wg) { return wg == 2 ? kThreads : 160; }
 
 // (a-plane, b-plane) of the t-th cross product of two 3-plane operands, smallest magnitude first:
 // (2,0) (1,1) (0,2) [2^-16]  (1,0) (0,1) [2^-8]  (0,0)
@@ -106,27 +114,33 @@ __host__ __device__ constexpr int plane_term_b(int t) { return t == 2 ? 2 : ((t 
 // fp32 -- the fp32 parity mode (acnn.h ACNN_F32) on the same TMA / im2col / descriptor / epilogue
 // code as the bf16 path.
 static inline int fprop_stage_bytes(int bn, int np) { return np * (kBM * kStageK * 2 + bn * kStageK * 2); }
-static inline int fprop_stages(int bn, int np, bool has_add, bool has_mask, bool out_f32) {
-  const int half_n = bn > 128 ? 128 : bn;
-  const int tile = kBM * half_n * 2;
+// column width of one epilogue step (one staged tile): 128 with two consumer warpgroups; with one
+// (two CTAs per SM) the kSubW = 64-column TMA sub-tile, so that the staging leaves room for stages
+__host__ __device__ constexpr int fprop_epi_cols(int bn, int wg) {
+  return wg == 2 ? (bn > 128 ? 128 : bn) : (bn > 64 ? 64 : bn);
+}
+static inline int fprop_stages(int bn, int np, int wg, bool has_add, bool has_mask, bool out_f32) {
+  const int tile = kBM * fprop_epi_cols(bn, wg) * 2;
   const int fixed = 1024 + (out_f32 ? 0 : tile) + (has_add ? tile : 0) + (has_mask ? tile : 0);
-  int st = (kSmemBudget - fixed) / fprop_stage_bytes(bn, np);
+  int st = ((wg == 2 ? kSmemBudget : kSmemBudget2) - fixed) / fprop_stage_bytes(bn, np);
   if (st > kMaxStages) st = kMaxStages;
   if (st < 2) st = 2;
   return st;
 }
 
-template <int BN, int NP = 1>
+template <int BN, int NP = 1, int WG = 2>
 struct FpropCfg {
   static constexpr int kABytes = kBM * kStageK * 2;       // one plane, 16 KiB
   static constexpr int kBBytes = BN * kStageK * 2;        // one plane
   static constexpr int kStageBytes = NP * (kABytes + kBBytes);
-  static_assert(2 * kStageBytes + 1024 <= kSmemBudget, "two pipeline stages must fit");
-  // the epilogue stages the tile in column halves of <= 128 (one staging buffer each for the
-  // output, add and mask tiles), so a 128 x 256 tile needs no more staging than 128 x 128
-  static constexpr int kHalfN = BN > 128 ? 128 : BN;
+  static_assert(2 * kStageBytes + 1024 <= (WG == 2 ? kSmemBudget : kSmemBudget2),
+                "two pipeline stages must fit");
+  static_assert(WG == 2 || NP == 1, "two CTAs per SM: bf16 / fp16 operands only");
+  // the epilogue stages the tile in column groups of fprop_epi_cols (one staging buffer each for
+  // the output, add and mask tiles), so a 128 x 256 tile needs no more staging than 128 x 128
+  static constexpr int kHalfN = fprop_epi_cols(BN, WG);
   static constexpr int kNHalf = BN / kHalfN;
-  static constexpr int kSubW = kHalfN < 64 ? kHalfN : 64;  // staging sub-tile width (TMA box)
+  static constexpr int kSubW = BN < 64 ? BN : 64;         // staging sub-tile width (TMA box)
   static constexpr int kTileBytes = kBM * kHalfN * 2;      // one staged half tile (bf16)
   // NP == 3 keeps TWO accumulators -- the hi*hi products and the five small cross terms
   // separately (added in the epilogue) -- because the tensor core truncates an addend below the
@@ -137,7 +151,7 @@ struct FpropCfg {
   // correctness mode, the bf16 path does not spill)
   // smem: [stages x (A|B)] [out staging] [add staging] [mask staging]
   static int stages_for(bool has_add, bool has_mask, bool out_f32) {
-    return fprop_stages(BN, NP, has_add, has_mask, out_f32);
+    return fprop_stages(BN, NP, WG, has_add, has_mask, out_f32);
   }
   static int smem_bytes(int stages, bool has_add, bool has_mask, bool out_f32) {
     return 1024 + stages * kStageBytes + (out_f32 ? 0 : kTileBytes) + (has_add ? kTileBytes : 0) +
@@ -162,14 +176,18 @@ __device__ __forceinline__ int staged_offset(int r, int c) {
 // consumers run the epilogue); each consumer warpgroup accumulates 64 rows x BN in registers with
 // wgmma, keeping one k-block of MMAs in flight, and releases a stage as soon as the MMAs that read
 // it have completed.
-template <int BN, int CW, bool IM2COL, int NP, bool CG2, bool F16>
-__global__ void __launch_bounds__(kThreads, 1)
+// WG = consumer warpgroups: 2 = one 384-thread CTA per SM (warp 0 produces, warpgroup g computes rows
+// 64g ..); 1 = two 160-thread CTAs per SM (warps 0..3 compute all 128 rows as two 64-row blocks,
+// warp 4 produces), which lets the SM run one CTA's epilogue under the other's MMAs.
+template <int BN, int CW, bool IM2COL, int NP, bool CG2, bool F16, int WG>
+__global__ void __launch_bounds__(conv_threads(WG), WG == 2 ? 1 : 2)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAdd,
                  const __grid_constant__ CUtensorMap tmMask, const __grid_constant__ CUtensorMap tmA1,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB1,
                  const __grid_constant__ CUtensorMap tmB2, const ConvGemmParams p) {
-  using Cfg = FpropCfg<BN, NP>;
+  using Cfg = FpropCfg<BN, NP, WG>;
+  static_assert(WG == 2 || !CG2, "CTA pairs: two consumer warpgroups");
   constexpr int kChunks = kStageK / CW;        // A chunks (one filter tap each when Cin < 64)
   constexpr int kChunkBytes = kBM * CW * 2;
   constexpr int kKSteps = CW / 16;             // wgmma K = 16 bf16
@@ -178,6 +196,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int kSubW = Cfg::kSubW;
   constexpr int kSubBytes = kBM * kSubW * 2;
   constexpr int kNSub = kHalfN / kSubW;
+  constexpr int kConsThreads = 128 * WG;
+  constexpr int kRB = 2 / WG;                  // 64-row accumulator blocks per consumer warpgroup
+  constexpr int kProducerWarp = WG == 2 ? 0 : 4;
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[kMaxStages];
@@ -222,7 +243,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       // one arrival per consumer warp (CG2: of both CTAs -- the stage receives the peer's multicast)
-      mbar_init(&empty_bar[s], kConsumerWarps * (CG2 ? 2 : 1));
+      mbar_init(&empty_bar[s], 4 * WG * (CG2 ? 2 : 1));
     }
     mbar_init(&aux_bar, 1);
     fence_barrier_init();
@@ -239,7 +260,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // a stage, i.e. Cin < 64 with an odd tap count)
   const int tail_chunks = kChunks == 1 ? 1 : ((p.Ktot - (num_kb - 1) * kStageK + CW - 1) / CW);
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------------------------------------------ TMA producer
     // The whole warp stays converged and every lane tracks the same loop state; one elected lane
     // issues.
@@ -307,28 +328,29 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++stage == static_cast<uint32_t>(kStages)) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp >= 4) {
+  } else if (WG == 2 ? warp >= 4 : warp < 4) {
     // ------------------------------------------------------------------ wgmma consumers
-    const int cg = (warp >> 2) - 1;                    // consumer warpgroup: rows cg*64 ..
-    const int ct = static_cast<int>(threadIdx.x) - 128;   // 0 .. 255
+    const int cg = WG == 2 ? (warp >> 2) - 1 : 0;      // consumer warpgroup: rows cg*64*kRB ..
+    const int ct = static_cast<int>(threadIdx.x) - (WG == 2 ? 128 : 0);   // 0 .. kConsThreads-1
     const bool leader = ct == 0;
     const bool stats = p.ch_part != nullptr;
     const bool has_aux = p.has_add || p.has_mask;
-    const int r0 = cg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r0, r0 + 8
+    // fragment rows rb*64 + r0 and rb*64 + r0 + 8 of accumulator block rb
+    const int r0 = cg * kRB * 64 + (warp & 3) * 16 + (lane >> 2);
     const int cq = (lane & 3) * 2;                              // fragment column offset
-    // descriptors of stage 0 / chunk 0 (K-major, 8-row groups SBO apart); this group's 64 rows
-    // start 64 rows into every A chunk
-    const uint64_t a_desc0 = make_smem_desc(smem_a0 + cg * 64 * CW * 2, 16, 8 * CW * 2,
+    // descriptors of stage 0 / chunk 0 (K-major, 8-row groups SBO apart); this group's first 64
+    // rows start cg*kRB*64 rows into every A chunk
+    const uint64_t a_desc0 = make_smem_desc(smem_a0 + cg * kRB * 64 * CW * 2, 16, 8 * CW * 2,
                                             swizzle_layout_type(CW * 2));
     const uint64_t b_desc0 = make_smem_desc(smem_a0 + NP * Cfg::kABytes, 16, 8 * p.b_sw_bytes,
                                             swizzle_layout_type(p.b_sw_bytes));
-    float acc[BN / 2];
+    float acc[kRB][BN / 2];
     float acc2[NP == 3 ? BN / 2 : 1];
     // batch-norm statistics: thread t owns the 8 columns of 16-byte chunk `st_chunk` (of every
-    // column half) over the rows st_rg, st_rg + kNRg, ... of every tile, read back from the staged
-    // bf16 tile
+    // staged column group) over the rows st_rg, st_rg + kNRg, ... of every tile, read back from the
+    // staged bf16 tile
     constexpr int kNChunk = kHalfN / 8;
-    constexpr int kStatThreads = (BN == 32) ? 128 : kConsumerThreads;
+    constexpr int kStatThreads = (BN == 32) ? 128 : kConsThreads;
     constexpr int kNRg = kStatThreads / kNChunk;       // row groups; kBM / kNRg rows per thread
     const bool st_on = ct < kStatThreads;
     const int st_chunk = ct % kNChunk, st_rg = ct / kNChunk;
@@ -338,9 +360,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc_s[hf][e] = acc_q[hf][e] = 0.f;
     uint32_t aux_n = 0;                                // completed aux-barrier phases
-    // add / mask half tiles are fetched ONE HALF AHEAD: the loads of the next half are issued as
-    // soon as every thread has consumed the current one (they overlap this half's TMA store, the
-    // statistics pass and the next tile's k-loop)
+    // add / mask column groups are fetched ONE GROUP AHEAD: the loads of the next group are issued
+    // as soon as every thread has consumed the current one (they overlap this group's TMA store,
+    // the statistics pass and the next tile's k-loop)
     auto issue_aux = [&](int am0, int anh) {
       mbar_expect_tx(&aux_bar, (p.has_add ? Cfg::kTileBytes : 0) +
                                    (p.has_mask ? Cfg::kTileBytes : 0));
@@ -363,6 +385,49 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         mbar_arrive(&empty_bar[st]);
       }
     };
+    auto fence_acc = [&]() {
+#pragma unroll
+      for (int rb = 0; rb < kRB; ++rb) wgmma_fence_operand(acc[rb]);
+      if (NP == 3) wgmma_fence_operand(acc2);
+    };
+    // the MMAs of one k-block over its first N chunks as one straight-line wgmma group: a
+    // data-dependent branch between the wgmmas of a group makes ptxas serialise them (C7520)
+    auto mma_kblock = [&](auto n_chunks, uint32_t stage_off, uint32_t first_accum) {
+      constexpr int kN = decltype(n_chunks)::value;
+      fence_acc();
+      wgmma_fence();
+      const uint64_t da0 = a_desc0 + (stage_off >> 4);
+      const uint64_t db0 = b_desc0 + (stage_off >> 4);
+#pragma unroll
+      for (int j = 0; j < kN; ++j) {
+#pragma unroll
+        for (int ks = 0; ks < kKSteps; ++ks) {
+          // NP == 3: the six cross products of the (hi, mid, lo) planes that are significant
+          // at fp32 precision, smallest first; t = 5 is hi*hi -> acc, t < 5 -> acc2
+#pragma unroll
+          for (int t = 0; t < (NP == 3 ? 6 : 1); ++t) {
+            const int pa = NP == 3 ? plane_term_a(t) : 0;
+            const int pb = NP == 3 ? plane_term_b(t) : 0;
+            const bool small = NP == 3 && t < 5;
+            const uint64_t db = db0 + ((pb * Cfg::kBBytes + (j * kKSteps + ks) * 32) >> 4);
+            const uint32_t accum = (j | ks | (small ? t : 0)) ? 1u : first_accum;
+#pragma unroll
+            for (int rb = 0; rb < kRB; ++rb) {
+              const uint64_t da =
+                  da0 + ((pa * Cfg::kABytes + j * kChunkBytes + rb * 64 * CW * 2 + ks * 32) >> 4);
+              if constexpr (NP == 3) {
+                if (small) WgmmaOp<BN, F16>::type::template mma<0, 0>(acc2, da, db, accum);
+                else WgmmaOp<BN, F16>::type::template mma<0, 0>(acc[rb], da, db, accum);
+              } else {
+                WgmmaOp<BN, F16>::type::template mma<0, 0>(acc[rb], da, db, accum);
+              }
+            }
+          }
+        }
+      }
+      wgmma_commit();
+      fence_acc();
+    };
 
     uint32_t stage = 0, phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
@@ -373,39 +438,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const bool last = kb == num_kb - 1;
         const int nch = (kChunks > 1 && last) ? tail_chunks : kChunks;
         mbar_wait_a(full0 + stage * 8, phase);
-        wgmma_fence_operand(acc);
-        if (NP == 3) wgmma_fence_operand(acc2);
-        wgmma_fence();
-        const uint64_t da0 = a_desc0 + ((stage * Cfg::kStageBytes) >> 4);
-        const uint64_t db0 = b_desc0 + ((stage * Cfg::kStageBytes) >> 4);
-#pragma unroll
-        for (int j = 0; j < kChunks; ++j) {
-          if (j < nch) {
-#pragma unroll
-            for (int ks = 0; ks < kKSteps; ++ks) {
-              // NP == 3: the six cross products of the (hi, mid, lo) planes that are significant
-              // at fp32 precision, smallest first; t = 5 is hi*hi -> acc, t < 5 -> acc2
-#pragma unroll
-              for (int t = 0; t < (NP == 3 ? 6 : 1); ++t) {
-                const int pa = NP == 3 ? plane_term_a(t) : 0;
-                const int pb = NP == 3 ? plane_term_b(t) : 0;
-                const bool small = NP == 3 && t < 5;
-                const uint64_t da = da0 + ((pa * Cfg::kABytes + j * kChunkBytes + ks * 32) >> 4);
-                const uint64_t db = db0 + ((pb * Cfg::kBBytes + (j * kKSteps + ks) * 32) >> 4);
-                const uint32_t accum = (j | ks | (small ? t : 0)) ? 1u : static_cast<uint32_t>(kb != 0);
-                if constexpr (NP == 3) {
-                  if (small) WgmmaOp<BN, F16>::type::template mma<0, 0>(acc2, da, db, accum);
-                  else WgmmaOp<BN, F16>::type::template mma<0, 0>(acc, da, db, accum);
-                } else {
-                  WgmmaOp<BN, F16>::type::template mma<0, 0>(acc, da, db, accum);
-                }
-              }
-            }
+        const uint32_t stage_off = stage * Cfg::kStageBytes;
+        const uint32_t first_accum = static_cast<uint32_t>(kb != 0);
+        if (nch == kChunks) {
+          mma_kblock(std::integral_constant<int, kChunks>{}, stage_off, first_accum);
+        } else if constexpr (kChunks > 1) {     // the partial last k-block (Cin < 64, odd taps)
+          if (nch == 1) {
+            mma_kblock(std::integral_constant<int, 1>{}, stage_off, first_accum);
+          } else if constexpr (kChunks > 2) {
+            if (nch == 2) mma_kblock(std::integral_constant<int, 2>{}, stage_off, first_accum);
+            else mma_kblock(std::integral_constant<int, 3>{}, stage_off, first_accum);
           }
         }
-        wgmma_commit();
-        wgmma_fence_operand(acc);
-        if (NP == 3) wgmma_fence_operand(acc2);
         wgmma_wait<1>();
         __syncwarp();
         if (prev >= 0 && lane == 0) release(prev);
@@ -413,23 +457,22 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++stage == static_cast<uint32_t>(kStages)) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
-      wgmma_fence_operand(acc);
+      fence_acc();
       if (NP == 3) {
-        wgmma_fence_operand(acc2);
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] += acc2[i];
+        for (int i = 0; i < BN / 2; ++i) acc[0][i] += acc2[i];
       }
       __syncwarp();
       if (lane == 0) release(prev);
 
-      // ---- epilogue, per column half: (+bias) (+add) (x mask) -> bf16 -> swizzled staging ->
+      // ---- epilogue, per column group: (+bias) (+add) (x mask) -> bf16 -> swizzled staging ->
       // TMA store; statistics from the staged (rounded) tile
 #pragma unroll
       for (int hf = 0; hf < kNHalf; ++hf) {
-        const int nh = n0 + hf * kHalfN;               // first output column of this half
+        const int nh = n0 + hf * kHalfN;               // first output column of this group
         // the TMA store that last used the staging buffer must have finished READING it
         if (leader && !p.out_f32) tma_store_wait_read();
-        named_bar_sync(1, kConsumerThreads);
+        named_bar_sync(1, kConsThreads);
         if (has_aux) {
           mbar_wait(&aux_bar, aux_n & 1);
           ++aux_n;
@@ -437,16 +480,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int jj = 0; jj < kHalfN / 8; ++jj) {
           const int j = hf * (kHalfN / 8) + jj;
-          const int c = jj * 8 + cq;                   // column inside the half
+          const int c = jj * 8 + cq;                   // column inside the group
           float b0 = 0.f, b1 = 0.f;
           if (p.bias) {
             b0 = __ldg(p.bias + nh + c);
             b1 = __ldg(p.bias + nh + c + 1);
           }
 #pragma unroll
+          for (int rb = 0; rb < kRB; ++rb)
+#pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int r = r0 + h * 8;
-            float v0 = acc[j * 4 + h * 2] + b0, v1 = acc[j * 4 + h * 2 + 1] + b1;
+            const int r = r0 + rb * 64 + h * 8;
+            float v0 = acc[rb][j * 4 + h * 2] + b0, v1 = acc[rb][j * 4 + h * 2 + 1] + b1;
             const int off = staged_offset<kSubW>(r, c);
             if (p.has_add) x2_add<F16>(v0, v1, *reinterpret_cast<const uint32_t*>(s_add + off));
             // ReLU mask of the destination tensor: 0xffff per bf16 half that is > 0, applied to the
@@ -469,7 +514,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
         if (!p.out_f32) fence_proxy_async();             // generic smem writes -> async proxy
-        named_bar_sync(1, kConsumerThreads);
+        named_bar_sync(1, kConsThreads);
         if (leader) {
           if (!p.out_f32) {
 #pragma unroll
@@ -479,13 +524,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           if (has_aux) {
             // the staging tiles were consumed by everyone before the barrier above: fetch the next
-            // half's (same rows / next column half, else the next M tile of this CTA)
+            // group's (same rows / next columns, else the next M tile of this CTA)
             if (hf + 1 < kNHalf) issue_aux(m0, nh + kHalfN);
             else if (it + 1 < my_tiles) issue_aux((m_first + (it + 1) * m_step) * kTileM + m_rank_off, n0);
           }
         }
         if (stats && st_on) {
-          // column sums of the half tile as stored (bf16-rounded); rows past M were computed
+          // column sums of the group as stored (bf16-rounded); rows past M were computed
           // from zero-filled operands and contribute zero.  Overlaps the TMA store (both read).
           constexpr int kRowBytes = kSubW * 2;
           const int sub = st_chunk / (kSubW / 8), jj = st_chunk % (kSubW / 8);
@@ -510,7 +555,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       float* red_sum = reinterpret_cast<float*>(s_out);
       float* red_sq = red_sum + kNRg * BN;
       static_assert(2 * kNRg * BN * 4 <= Cfg::kTileBytes, "staging buffer too small for stats");
-      named_bar_sync(1, kConsumerThreads);             // the last TMA store has drained
+      named_bar_sync(1, kConsThreads);                 // the last TMA store has drained
       if (st_on) {
 #pragma unroll
         for (int hf = 0; hf < kNHalf; ++hf)
@@ -520,8 +565,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             red_sq[st_rg * BN + hf * kHalfN + st_chunk * 8 + e] = acc_q[hf][e];
           }
       }
-      named_bar_sync(1, kConsumerThreads);
-      for (int col = ct; col < BN; col += kConsumerThreads) {
+      named_bar_sync(1, kConsThreads);
+      for (int col = ct; col < BN; col += kConsThreads) {
         float ss = 0.f, qq = 0.f;
         for (int g2 = 0; g2 < kNRg; ++g2) {
           ss += red_sum[g2 * BN + col];
@@ -1140,16 +1185,27 @@ static int g_conv_mtiles_mode = -1;
 // K >= 512 and enough tiles for every SM; 0 (default) = single CTAs (acnn_set_conv_cta_pairs).  Off
 // by default: c3 step on an H100 SXM at 700 W, 80.3 ms with pairs against 61.3 ms without
 static int g_conv_pairs = 0;
+// Two CTAs per SM only up to this GEMM K (kh*kw*Cin): there the per-tile fixed cost (pipeline fill,
+// epilogue) rivals the MMAs and overlapping it pays; on deeper K the 128 x 64 tiles' extra operand
+// traffic from L2 costs more (c3 step on an H100 SXM at 700 W, fprop + dgrad launches: K <= 512
+// 10.9 -> 9.5 ms; K = 576 .. 1024 unchanged; K >= 1152 6.2 -> 7.7 ms)
+constexpr int kTwoCtaMaxK = 512;
 
-template <int BN, int CW, bool IM2COL, int NP, bool CG2 = false, bool F16 = false>
+// occ != null: report the CTAs of this instantiation that fit one SM at the launch's shared memory
+// (cudaOccupancyMaxActiveBlocksPerMultiprocessor) instead of launching
+template <int BN, int CW, bool IM2COL, int NP, bool CG2, bool F16, int WG>
 static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per_n,
-                            cudaStream_t stream) {
-  using Cfg = FpropCfg<BN, NP>;
+                            cudaStream_t stream, int* occ) {
+  using Cfg = FpropCfg<BN, NP, WG>;
   static bool attr_set = false;
-  auto kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2, F16>;
+  auto kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2, F16, WG>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         kSmemBudget + 2048);
+                                         WG == 2 ? kSmemBudget + 2048 : kSmemBudget2);
+    // two CTAs per SM need the largest shared-memory carveout
+    if (e == cudaSuccess && WG == 1)
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                               cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(conv_gemm): %s", cudaGetErrorString(e));
       return ACNN_ERR_CUDA;
@@ -1161,6 +1217,15 @@ static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per
   q.m_tiles = ceil_div(p.M, (CG2 ? 2 : 1) * kBM);
   q.n_tiles = p.Cout / BN;
   const int smem = Cfg::smem_bytes(q.stages, p.has_add, p.has_mask, p.out_f32);
+  if (occ) {
+    const cudaError_t e =
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, conv_threads(WG), smem);
+    if (e != cudaSuccess) {
+      set_error("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_gemm): %s", cudaGetErrorString(e));
+      return ACNN_ERR_CUDA;
+    }
+    return ACNN_OK;
+  }
   if (CG2) {
     // per_n CTA PAIRS per N tile, launched as clusters of two
     cudaLaunchConfig_t cfg{};
@@ -1178,8 +1243,8 @@ static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per
     (void)cudaLaunchKernelEx(&cfg, kern, tm.a[0], tm.b[0], tm.c, tm.add, tm.mask, tm.a[1], tm.a[2],
                              tm.b[1], tm.b[2], q);
   } else {
-    launch_k(kern, dim3(per_n * q.n_tiles), dim3(kThreads), smem, stream, tm.a[0], tm.b[0], tm.c,
-             tm.add, tm.mask, tm.a[1], tm.a[2], tm.b[1], tm.b[2], q);
+    launch_k(kern, dim3(per_n * q.n_tiles), dim3(conv_threads(WG)), smem, stream, tm.a[0], tm.b[0],
+             tm.c, tm.add, tm.mask, tm.a[1], tm.a[2], tm.b[1], tm.b[2], q);
   }
   count_launch();
   return check_launch("conv_gemm_kernel");
@@ -1191,6 +1256,7 @@ struct ConvTiling {
   int bn;      // N tile
   int per_n;   // CTAs (pair = 1: CTA pairs) per N tile
   int pair;    // 1: clusters of two CTAs sharing the weight stages, one 256 x bn tile per pair
+  int wg;      // consumer warpgroups per CTA: 2 = one CTA per SM, 1 = two CTAs per SM
   int parts;   // rows of the partial statistics buffer (= CTAs per N tile)
 };
 
@@ -1202,53 +1268,68 @@ static ConvTiling conv_tiling(int M, int Cout, int Ktot, int cw, bool has_add, b
   // N tile <= 128: a 64 x 256 fp32 accumulator per consumer warpgroup (128 registers per thread)
   // does not fit next to the epilogue under the 168-register limit of a 384-thread CTA
   t.bn = (Cout % 128 == 0) ? 128 : ((Cout % 64 == 0) ? 64 : 32);
-  // persistent grid: a multiple of n_tiles so that every CTA keeps one N tile (its weights and
-  // its per-channel statistics), at most one CTA per SM
-  const int n_tiles = Cout / t.bn;
   // CTA pairs: full-width (64-channel) chunks, K >= 512 (the k-loop, not the epilogue, paces the
   // tile) and at least one pair tile per SM pair
   t.pair = (g_conv_pairs && t.bn == 128 && np == 1 && !out_f32 && cw == 64 && Ktot >= 512 &&
-            (int64_t)ceil_div(M, 2 * kBM) * n_tiles >= num_sms() / 2) ? 1 : 0;
+            (int64_t)ceil_div(M, 2 * kBM) * (Cout / 128) >= num_sms() / 2) ? 1 : 0;
+  // bf16 / fp16 operands with K <= kTwoCtaMaxK: two co-resident CTAs per SM on 128 x 64 (Cout % 64
+  // != 0: 128 x 32) tiles -- a 128 x 128 fp32 accumulator does not fit one warpgroup under the 168
+  // registers per thread of two 5-warp CTAs (ptxas spills) -- where that gives >= 2 N tiles (<=
+  // kMaxSms CTAs, i.e. partial statistics rows, per N tile).  The fp32 parity mode's three operand
+  // planes and the CTA pairs keep one CTA per SM.
+  const int bn2 = (Cout % 64 == 0 && Cout >= 128) ? 64 : 32;
+  t.wg = (np == 1 && !t.pair && Cout / bn2 >= 2 && Ktot <= kTwoCtaMaxK) ? 1 : 2;
+  if (t.wg == 1) t.bn = bn2;
+  const int n_tiles = Cout / t.bn;
+  // persistent grid: a multiple of n_tiles so that every CTA keeps one N tile (its weights and
+  // its per-channel statistics), at most one CTA per SM (two with wg = 1)
   const int m_tiles = ceil_div(M, (t.pair ? 2 : 1) * kBM);
-  t.per_n = (t.pair ? num_sms() / 2 : num_sms()) / n_tiles;
+  t.per_n = (t.pair ? num_sms() / 2 : (t.wg == 1 ? 2 * num_sms() : num_sms())) / n_tiles;
   if (t.per_n < 1) t.per_n = 1;
   if (t.per_n > m_tiles) t.per_n = m_tiles;
   t.parts = t.pair ? 2 * t.per_n : t.per_n;
   return t;
 }
 
-template <int BN, int NP, bool F16 = false>
+template <int BN, int NP, bool F16, int WG>
 static int dispatch_conv_cw(int cw, bool im2col, const ConvMaps& tm, const ConvGemmParams& p,
-                            int per_n, cudaStream_t s) {
+                            int per_n, cudaStream_t s, int* occ) {
   if (im2col) {
-    if (cw == 64) return launch_conv_gemm<BN, 64, true, NP, false, F16>(tm, p, per_n, s);
-    if (cw == 32) return launch_conv_gemm<BN, 32, true, NP, false, F16>(tm, p, per_n, s);
-    return launch_conv_gemm<BN, 16, true, NP, false, F16>(tm, p, per_n, s);
+    if (cw == 64) return launch_conv_gemm<BN, 64, true, NP, false, F16, WG>(tm, p, per_n, s, occ);
+    if (cw == 32) return launch_conv_gemm<BN, 32, true, NP, false, F16, WG>(tm, p, per_n, s, occ);
+    return launch_conv_gemm<BN, 16, true, NP, false, F16, WG>(tm, p, per_n, s, occ);
   }
-  if (cw == 64) return launch_conv_gemm<BN, 64, false, NP, false, F16>(tm, p, per_n, s);
-  if (cw == 32) return launch_conv_gemm<BN, 32, false, NP, false, F16>(tm, p, per_n, s);
-  return launch_conv_gemm<BN, 16, false, NP, false, F16>(tm, p, per_n, s);
+  if (cw == 64) return launch_conv_gemm<BN, 64, false, NP, false, F16, WG>(tm, p, per_n, s, occ);
+  if (cw == 32) return launch_conv_gemm<BN, 32, false, NP, false, F16, WG>(tm, p, per_n, s, occ);
+  return launch_conv_gemm<BN, 16, false, NP, false, F16, WG>(tm, p, per_n, s, occ);
 }
 
 // f16: fp16 operands and output (ACNN_F16), one plane, the bf16 path's tiles
 template <int BN>
 static int dispatch_conv_gemm(const ConvTiling& t, int np, bool f16, int cw, bool im2col,
-                              const ConvMaps& tm, const ConvGemmParams& p, cudaStream_t s) {
+                              const ConvMaps& tm, const ConvGemmParams& p, cudaStream_t s,
+                              int* occ) {
   if constexpr (BN == 128) {
     if (t.pair) {     // full-width (64-channel) chunks only: bounds the instantiation count
       if (f16) {
-        if (im2col) return launch_conv_gemm<128, 64, true, 1, true, true>(tm, p, t.per_n, s);
-        return launch_conv_gemm<128, 64, false, 1, true, true>(tm, p, t.per_n, s);
+        if (im2col) return launch_conv_gemm<128, 64, true, 1, true, true, 2>(tm, p, t.per_n, s, occ);
+        return launch_conv_gemm<128, 64, false, 1, true, true, 2>(tm, p, t.per_n, s, occ);
       }
-      if (im2col) return launch_conv_gemm<128, 64, true, 1, true>(tm, p, t.per_n, s);
-      return launch_conv_gemm<128, 64, false, 1, true>(tm, p, t.per_n, s);
+      if (im2col) return launch_conv_gemm<128, 64, true, 1, true, false, 2>(tm, p, t.per_n, s, occ);
+      return launch_conv_gemm<128, 64, false, 1, true, false, 2>(tm, p, t.per_n, s, occ);
     }
   }
   if constexpr (BN <= 128) {
-    if (np == 3) return dispatch_conv_cw<BN, 3>(cw, im2col, tm, p, t.per_n, s);
+    if (np == 3) return dispatch_conv_cw<BN, 3, false, 2>(cw, im2col, tm, p, t.per_n, s, occ);
   }
-  if (f16) return dispatch_conv_cw<BN, 1, true>(cw, im2col, tm, p, t.per_n, s);
-  return dispatch_conv_cw<BN, 1>(cw, im2col, tm, p, t.per_n, s);
+  if constexpr (BN <= 64) {
+    if (t.wg == 1) {
+      if (f16) return dispatch_conv_cw<BN, 1, true, 1>(cw, im2col, tm, p, t.per_n, s, occ);
+      return dispatch_conv_cw<BN, 1, false, 1>(cw, im2col, tm, p, t.per_n, s, occ);
+    }
+  }
+  if (f16) return dispatch_conv_cw<BN, 1, true, 2>(cw, im2col, tm, p, t.per_n, s, occ);
+  return dispatch_conv_cw<BN, 1, false, 2>(cw, im2col, tm, p, t.per_n, s, occ);
 }
 
 static int chunk_width(int cin) { return cin % 64 == 0 ? 64 : (cin % 32 == 0 ? 32 : 16); }
@@ -1422,10 +1503,12 @@ static int conv_halo_host(const acnn_conv_geom& g, const void* x, const void* w,
 // bf16 planes (acnn_split3 / acnn_prep_weights with planes = 3), plane p of x at x + p * numel(x),
 // plane p of w at w + p * w_plane_stride elements; y must be fp32 (out_f32), no fused epilogue.
 // precision ACNN_F16: x / w (and y, add, mask unless out_f32) are fp16, on the bf16 path's tiles.
+// occ != null: nothing is launched or read; *occ = resident CTAs per SM of the conv GEMM kernel this
+// problem selects (add_src / mask_src / ch_part only say whether those epilogue parts are present).
 static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w, void* y,
                           float* ch_part, const void* add_src, const void* mask_src,
                           const float* bias, int out_f32, int precision, int64_t w_plane_stride,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, int* occ = nullptr) {
   ACNN_REQUIRE(g.B > 0 && g.H > 0 && g.W > 0 && g.Cin > 0 && g.Cout > 0, "conv: empty geometry");
   ACNN_REQUIRE(g.Cin % 16 == 0, "conv: Cin=%d must be a multiple of 16", g.Cin);
   ACNN_REQUIRE(g.Cout % 32 == 0, "conv: Cout=%d must be a multiple of 32", g.Cout);
@@ -1444,9 +1527,11 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   if (rc) return rc;
   const int np = precision == ACNN_F32 ? 3 : 1;
   const bool f16 = precision == ACNN_F16;
-  if (use_halo(g, np, out_f32 != 0, bias != nullptr, add_src != nullptr, mask_src != nullptr))
+  if (use_halo(g, np, out_f32 != 0, bias != nullptr, add_src != nullptr, mask_src != nullptr)) {
+    ACNN_REQUIRE(!occ, "conv: this geometry runs on the halo kernel");
     return f16 ? conv_halo_host<true>(g, x, w, y, ch_part, add_src, mask_src, stream)
                : conv_halo_host<false>(g, x, w, y, ch_part, add_src, mask_src, stream);
+  }
   const bool plain = is_plain(g);
   const int cw = chunk_width(g.Cin);
   const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -1477,7 +1562,7 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   const int bn = t.bn;
   ConvMaps tm;
   const int64_t x_plane = input_elems(g);
-  for (int pl = 0; pl < np; ++pl) {
+  for (int pl = 0; pl < (occ ? 0 : np); ++pl) {
     const __nv_bfloat16* xp = static_cast<const __nv_bfloat16*>(x) + pl * x_plane;
     const __nv_bfloat16* wp = static_cast<const __nv_bfloat16*>(w) + pl * w_plane_stride;
     if (plain) {
@@ -1496,12 +1581,16 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   }
   tm.c = tm.add = tm.mask = tm.b[0];   // placeholders when unused
   const int subw = bn < 64 ? bn : 64;
-  if (!out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
-  if (add_src && (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
-  if (mask_src && (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
-  if (bn == 128) return dispatch_conv_gemm<128>(t, np, f16, cw, !plain, tm, p, stream);
-  if (bn == 64) return dispatch_conv_gemm<64>(t, np, f16, cw, !plain, tm, p, stream);
-  return dispatch_conv_gemm<32>(t, np, f16, cw, !plain, tm, p, stream);
+  if (!occ && !out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
+  if (!occ && add_src &&
+      (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw, dt)))
+    return rc;
+  if (!occ && mask_src &&
+      (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw, dt)))
+    return rc;
+  if (bn == 128) return dispatch_conv_gemm<128>(t, np, f16, cw, !plain, tm, p, stream, occ);
+  if (bn == 64) return dispatch_conv_gemm<64>(t, np, f16, cw, !plain, tm, p, stream, occ);
+  return dispatch_conv_gemm<32>(t, np, f16, cw, !plain, tm, p, stream, occ);
 }
 
 struct WgradMaps {
@@ -1823,6 +1912,20 @@ int acnn_conv_stats_parts(const acnn_conv_geom* g) {
   if (acnn::use_halo(*g, 1, false, false, false, false)) return acnn::halo_per_n(*g);
   return acnn::conv_tiling(g->B * Ho * Wo, g->Cout, g->kh * g->kw * g->Cin,
                            acnn::chunk_width(g->Cin), false, false, false, 1).parts;
+}
+
+int acnn_conv_ctas_per_sm(const acnn_conv_geom* g, int precision, int has_add, int has_mask,
+                          int* ctas) {
+  if (!g || !ctas) {
+    acnn::set_error("acnn_conv_ctas_per_sm: null argument");
+    return ACNN_ERR_INVALID;
+  }
+  // non-null placeholders: only their presence selects the epilogue (nothing is read)
+  const void* tag = g;
+  *ctas = 0;
+  return acnn::conv_gemm_host(*g, nullptr, nullptr, nullptr, nullptr, has_add ? tag : nullptr,
+                              has_mask ? tag : nullptr, nullptr, precision == ACNN_F32 ? 1 : 0,
+                              precision, precision == ACNN_F32 ? 1 : 0, nullptr, ctas);
 }
 
 int acnn_set_conv_cta_pairs(int on) {

@@ -143,6 +143,12 @@ int acnn_conv_fprop(const acnn_conv_geom* g, const void* x, const void* w, void*
 /* Rows of the partial statistics buffer acnn_conv_fprop(g, ..., ch_part, ...) writes (a pure
  * function of the geometry and the device's SM count; <= 132). */
 int acnn_conv_stats_parts(const acnn_conv_geom* g);
+/* *ctas = how many CTAs of the conv GEMM kernel acnn_conv_fprop(g, ..., precision) launches fit one
+ * SM together (cudaOccupancyMaxActiveBlocksPerMultiprocessor at that launch's shared memory, with the
+ * add / mask epilogue staging when has_add / has_mask); nothing is launched.  The bf16 and fp16
+ * kernels are laid out for 2.  ACNN_ERR_INVALID for geometries on the 3x3 halo kernel. */
+int acnn_conv_ctas_per_sm(const acnn_conv_geom* g, int precision, int has_add, int has_mask,
+                          int* ctas);
 
 /* dx[B,H,W,Cin] = conv_transpose(dy[B,Ho,Wo,Cout]) for a stride-1 conv of geometry g (the backward
  * of tf.layers.conv2d the reference gets from tf.gradients, nets/optimizer_setting.py:30).
