@@ -1,5 +1,6 @@
 """Per-element checks of the 16-bit conv GEMMs (csrc/gemm.cu: fprop, dgrad, wgrad) against float64
-references: tests/test_conv_plan_bf16_gpu.py runs them at the training plans' geometries and
+references: tests/test_conv_plan_bf16_gpu.py and tests/test_conv_plan_fp16_gpu.py run them at the
+training plans' geometries (the fp16 file also at fp16's overflow and subnormal edges) and
 tests/test_conv_checks_cpu.py shows on synthetic data that they reject the errors they are meant to find.
 
 TEST INFRASTRUCTURE ONLY.
@@ -25,12 +26,21 @@ does, not fitted to what it returns:
     element.  It cannot fail on a correct kernel, and it fails on truncation, on a one-ulp bias, on an
     add epilogue rounded twice (through 16 bits before the add) and on an fp32 add done in 16 bits.  How
     many elements are decided depends on the data: with K products of one sign per output element
-    mag = |ref| and acc / |ref| = 2 K u, so at K = 4608 (3x3x512) about four in five are.
-  * ReLU mask.  Wherever mask <= 0 (+0, -0 and negatives) the output is exactly 0.
+    mag = |ref| and acc / |ref| = 2 K u, so at K = 4608 (3x3x512) about four in five bf16 outputs are.
+    fp16's spacing is eight times finer: at that K next to none are (the per-element bound still holds
+    every element), at the fp16 range edges of tests/test_conv_plan_fp16_gpu.py at least a third are.
+  * fp16's range.  The store overflows as round to nearest even does: |fp32 value| >= 65520 is +-inf
+    (the dynamic loss scale's overflow check reads those infs; a saturating store would hide them), and
+    below 2^-14 it keeps fp16's subnormals (spacing 2^-24) instead of flushing them to zero.  An
+    element whose interval lies beyond 65520 must be the inf of its sign; one whose interval crosses
+    65520 may be the inf of that side or finite within the bound.
+  * ReLU mask.  Wherever mask <= 0 (+0, -0 and negatives) the output is exactly 0, also where the
+    value before the mask overflowed (a mask applied as a multiply gives inf x 0 = NaN there).
   * Batch-norm partial statistics.  Every CTA row stores its column sums and sums of squares of the
     stored 16-bit output in fp32.  Summed over the rows they are within n u sum|y| (sums) and 2 n u
     sum y^2 (squares: one more rounding per term) of the float64 sums of the stored output, n = rows of
-    the output (the longest possible fp32 chain; Higham eq. 4.4).
+    the output (the longest possible fp32 chain; Higham eq. 4.4).  A column whose stored output holds
+    an inf sums to that inf (its squares to +inf).
   * Weight gradient.  dw (fp32) += sum over the P output pixels of x (*) dy.  Per element
     |got - ref| <= 2 P u mag_w + u (|dw0| + mag_w) (the P-term sum, then the add into the running dw0).
     At P = 200k - 3.2M that bound is loose: it grows with P where the actual rounding error grows with
@@ -61,28 +71,36 @@ import torch
 
 U32 = 2.0 ** -24
 
-# significant bits, smallest normal exponent (2^emin) of the 16-bit storage formats
-FORMATS = {"bf16": (8, -126), "fp16": (11, -14)}
+# significant bits, smallest normal exponent (2^emin), largest finite value of the 16-bit storage formats
+FORMATS = {"bf16": (8, -126, (2.0 - 2.0 ** -7) * 2.0 ** 127), "fp16": (11, -14, 65504.0)}
+
+# the NaN that the statistics rows are poisoned with before a launch (stats_poison): a stored row
+# never holds this payload, while a sum over an inf and a -inf would be the default NaN
+STATS_POISON_BITS = 0x7FC0DEAD
 
 WGRAD_TILE_TOL = 1e-3
 
 
 def ulp16(x: torch.Tensor, fmt: str = "bf16") -> torch.Tensor:
     """Spacing of the 16-bit format's numbers at |x|, float64 (the subnormal spacing below the
-    smallest normal)."""
-    p, emin = FORMATS[fmt]
-    x = x.double().abs().clamp_min(2.0 ** emin)
+    smallest normal, the spacing of the largest binade at and beyond the largest finite value, inf
+    included)."""
+    p, emin, top = FORMATS[fmt]
+    x = x.double().abs().clamp(2.0 ** emin, top)
     _, e = torch.frexp(x)              # x = m * 2^e, m in [0.5, 1)
     return torch.ldexp(torch.ones_like(x), (e - p).to(torch.int64))
 
 
 def round16(x: torch.Tensor, fmt: str = "bf16") -> torch.Tensor:
     """x (float64) rounded to the nearest 16-bit value, ties to even, computed in float64 (one
-    rounding; torch's float64 -> bf16 conversion goes through fp32 and can round twice).  No overflow
-    handling: the checks' values are far inside both ranges."""
+    rounding; torch's float64 -> bf16 conversion goes through fp32 and can round twice).  Beyond the
+    largest finite value it overflows as round to nearest even does: fp16 |x| >= 65520 (half an ulp
+    above 65504) is +-inf, 65504 < |x| < 65520 is +-65504 (bf16 alike at its own limit)."""
     x = x.double()
     q = ulp16(x, fmt)
-    return torch.round(x / q) * q      # x / q is exact (a power of two); torch.round: half to even
+    r = torch.round(x / q) * q         # x / q is exact (a power of two); torch.round: half to even
+    top = FORMATS[fmt][2]
+    return torch.where(r.abs() > top, torch.copysign(torch.full_like(r, float("inf")), x), r)
 
 
 def acc_bound(mag: torch.Tensor, K: int) -> torch.Tensor:
@@ -99,9 +117,14 @@ def decided(ref: torch.Tensor, acc: torch.Tensor, fmt: str = "bf16") -> torch.Te
     """Elements whose whole interval [ref - acc, ref + acc] rounds to one 16-bit value.  Rounding is
     monotone, so comparing the two ends decides it; the ends are widened by a relative 2^-40 for the
     float64 rounding of ref -+ acc."""
+    lo, hi = _rounded_ends(ref, acc, fmt)
+    return lo == hi
+
+
+def _rounded_ends(ref, acc, fmt):
     ref, acc = ref.double(), acc.double()
     w = acc + ref.abs() * 2.0 ** -40
-    return round16(ref - w, fmt) == round16(ref + w, fmt)
+    return round16(ref - w, fmt), round16(ref + w, fmt)
 
 
 def _first_bad(bad, got, ref):
@@ -112,16 +135,29 @@ def _first_bad(bad, got, ref):
 def check_16bit(got: torch.Tensor, ref: torch.Tensor, acc: torch.Tensor, what: str,
                 fmt: str = "bf16") -> float:
     """The per-element bound and the exact-rounding check of a 16-bit output; returns the decided
-    fraction.  got: the kernel's 16-bit output, ref / acc: float64, same shape."""
+    fraction.  got: the kernel's 16-bit output, ref / acc: float64, same shape.
+
+    Overflow (fp16): an element whose whole interval [ref - acc, ref + acc] rounds to +-inf must be
+    that inf (not the saturated 65504); one whose interval reaches half an ulp beyond the largest
+    finite value on one side only may be that inf or, within the bound, finite; every finite element
+    is under the bound, so an inf anywhere else fails."""
     g = got.double()
     ref, acc = ref.double(), acc.double()
+    lo, hi = _rounded_ends(ref, acc, fmt)
+    over = (lo == hi) & torch.isinf(lo)
+    bad = over & (g != lo)
+    if bool(bad.any()):
+        raise AssertionError("%s: %d of %d elements that overflow are not the inf of their sign; %s" % (
+            what, int(bad.sum()), int(over.sum()), _first_bad(bad, g, ref)))
+    # the straddling elements that stored the inf of the side whose end overflows
+    inf_ok = ~over & torch.isinf(g) & ((torch.isinf(lo) & (g == lo)) | (torch.isinf(hi) & (g == hi)))
     tol = acc + ulp16(ref.abs() + acc, fmt)
-    bad = ~((g - ref).abs() <= tol)
+    bad = ~over & ~inf_ok & ~((g - ref).abs() <= tol)
     if bool(bad.any()):
         raise AssertionError("%s: %d of %d elements outside acc + ulp; %s" % (
             what, int(bad.sum()), bad.numel(), _first_bad(bad, g, ref)))
-    dec = decided(ref, acc, fmt)
-    wrong = dec & (g != round16(ref, fmt))
+    dec = lo == hi
+    wrong = dec & (g != lo)
     if bool(wrong.any()):
         raise AssertionError("%s: %d of %d decided elements are not round-to-nearest-even of the "
                              "reference; %s" % (what, int(wrong.sum()), int(dec.sum()),
@@ -130,7 +166,8 @@ def check_16bit(got: torch.Tensor, ref: torch.Tensor, acc: torch.Tensor, what: s
 
 
 def check_mask(got: torch.Tensor, mask: torch.Tensor, what: str) -> None:
-    """Exactly 0 wherever mask <= 0 (+0, -0 and negatives)."""
+    """Exactly 0 (+0 or -0) wherever mask <= 0 (+0, -0 and negatives), whatever the value before the
+    mask was: a mask applied as a multiply leaves NaN where that value overflowed to inf."""
     off = ~(mask > 0)
     bad = off & (got != 0)
     if bool(bad.any()):
@@ -138,20 +175,39 @@ def check_mask(got: torch.Tensor, mask: torch.Tensor, what: str) -> None:
             what, int(bad.sum()), int(off.sum()), _first_bad(bad, got.double(), torch.zeros_like(got.double()))))
 
 
+def stats_poison(shape, device="cuda") -> torch.Tensor:
+    """fp32 statistics rows filled with the STATS_POISON_BITS NaN, for check_stats."""
+    return torch.full(shape, STATS_POISON_BITS, dtype=torch.int32, device=device).view(torch.float32)
+
+
 def check_stats(rows: torch.Tensor, y: torch.Tensor, what: str) -> None:
-    """rows [parts][2][C] (fp32, poisoned with NaN before the launch): every row stored (finite), and
-    the row sums within n u sum|y| / 2 n u sum y^2 of the float64 column sums of the stored output
-    y [..., C]."""
+    """rows [parts][2][C] (fp32, poisoned with stats_poison before the launch): every row stored (no
+    element keeps the poison payload), and the row sums within n u sum|y| / 2 n u sum y^2 of the
+    float64 column sums of the stored output y [..., C].  A column whose stored output holds an inf
+    (fp16 overflow; one sign per column) must total exactly that inf, its squares +inf."""
     C = rows.shape[-1]
-    if not bool(torch.isfinite(rows).all()):
-        raise AssertionError("%s: %d of %d statistics rows not stored (NaN poison left)" % (
-            what, int((~torch.isfinite(rows)).any(-1).any(-1).sum()), rows.shape[0]))
+    left = (rows.contiguous().view(torch.int32) == STATS_POISON_BITS).flatten(1).any(1)
+    if bool(left.any()):
+        raise AssertionError("%s: %d of %d statistics rows not stored (poison left)" % (
+            what, int(left.sum()), rows.shape[0]))
     yd = y.double().reshape(-1, C)
     n = yd.shape[0]
+    pos, neg = (yd == float("inf")).any(0), (yd == -float("inf")).any(0)
+    if bool((pos & neg).any()):
+        raise AssertionError("%s: columns with both +inf and -inf outputs (the check needs one overflow "
+                             "sign per column)" % what)
+    inf_col = pos | neg
     s, q = rows.double().sum(0)
-    for got, ref, tol, name in ((s, yd.sum(0), n * U32 * yd.abs().sum(0), "column sums"),
-                                (q, (yd * yd).sum(0), 2 * n * U32 * (yd * yd).sum(0), "column sums of squares")):
-        bad = ~((got - ref).abs() <= tol + 1e-30)
+    want = torch.where(pos, float("inf"), -float("inf"))
+    for got, ref, name in ((s, want, "column sums"), (q, torch.full_like(q, float("inf")), "column sums of squares")):
+        bad = inf_col & (got != ref)
+        if bool(bad.any()):
+            raise AssertionError("%s %s: %d of %d columns with an inf output do not total that inf; %s" % (
+                what, name, int(bad.sum()), int(inf_col.sum()), _first_bad(bad, got, ref)))
+    yf = torch.where(inf_col, torch.zeros_like(yd), yd)
+    for got, ref, tol, name in ((s, yf.sum(0), n * U32 * yf.abs().sum(0), "column sums"),
+                                (q, (yf * yf).sum(0), 2 * n * U32 * (yf * yf).sum(0), "column sums of squares")):
+        bad = ~inf_col & ~((got - ref).abs() <= tol + 1e-30)
         if bool(bad.any()):
             raise AssertionError("%s %s: %d of %d channels outside the bound; %s" % (
                 what, name, int(bad.sum()), C, _first_bad(bad, got, ref)))

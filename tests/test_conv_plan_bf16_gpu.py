@@ -14,6 +14,9 @@ smoothing 0.1) at its own geometry against float64, element by element (oracle/c
     overlapped-pixel conv, its wgrad and acnn_s2d_wgrad_unpack) against the raw 7x7 stride-2 conv;
   * acnn_prep_weights: the bf16 and 3-plane operand copies of every weight, bit for bit.
 
+tests/test_conv_plan_fp16_gpu.py reruns the conv, dgrad and wgrad tests on fp16 storage with the fp16
+plans' cases (the `fmt` fixture selects the format of their operands, launches and checks).
+
 The library runs with its default knobs (halo kernel mode 1, the default wgrad split), as training does.
 Inputs are generated on the device as 16-bit values; references are float64 on the device.  The conv
 operands have one sign per output element (non-negative activations, weights of one sign per output
@@ -34,12 +37,16 @@ ACNN_BF16, ACNN_F16 = 0, 3
 NUM_SMS = 132
 
 
-def _plans():
+# storage format -> (acnn precision code, torch dtype)
+FMT = {"bf16": (ACNN_BF16, torch.bfloat16), "fp16": (ACNN_F16, torch.float16)}
+
+
+def _plans(dtype="bf16"):
     import bench
     from assembled_cnn_b200.plan import ModelConfig, build_plan
     for name in ("c3", "c5"):
         cfg = ModelConfig(num_classes=1001, **bench.CONFIGS[name]["model"])
-        yield build_plan(cfg, 256, 224, 224, training=True, mixup_type=1, label_smoothing=0.1, dtype="bf16")
+        yield build_plan(cfg, 256, 224, 224, training=True, mixup_type=1, label_smoothing=0.1, dtype=dtype)
 
 
 CASES = CC.plan_cases(_plans())
@@ -47,23 +54,33 @@ CONV = [c for c in CASES if c.kind == "conv"]
 DGRAD = [c for c in CASES if c.kind == "conv_dgrad"]
 WGRAD = [c for c in CASES if c.kind == "conv_wgrad"]
 
-REPORT = {"decided": {}, "wgrad_tile": {}}
+REPORT = {f: {"decided": {}, "wgrad_tile": {}} for f in FMT}
+
+
+@pytest.fixture
+def fmt():
+    return "bf16"
+
+
+def report(fmt):
+    """Print the minimum decided fraction per kind and the worst wgrad tiles of the tests run on fmt."""
+    dec = REPORT[fmt]["decided"]
+    if dec:
+        k = min(dec, key=dec.get)
+        print("\nminimum decided fraction: %.4f (%s)" % (dec[k], k[1]))
+        for kind in ("conv", "conv_dgrad", "stem", "conv range", "dgrad range"):
+            v = [f for (kd, _), f in dec.items() if kd == kind]
+            if v:
+                print("  %-10s %3d outputs, decided fraction min %.4f" % (kind, len(v), min(v)))
+    for (n, P), e in sorted(REPORT[fmt]["wgrad_tile"].items(), key=lambda kv: (kv[0][1], kv[0][0])):
+        print("worst wgrad tile norm-relative error P=%d %s: split-K %.3e (tolerance %.3e), deterministic %.3e "
+              "(tolerance %.3e)" % (P, n, e[0][0], e[0][1], e[1][0], e[1][1]))
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    dec = REPORT["decided"]
-    if dec:
-        k = min(dec, key=dec.get)
-        print("\nminimum decided fraction: %.4f (%s)" % (dec[k], k[1]))
-        for kind in ("conv", "conv_dgrad", "stem"):
-            v = [f for (kd, _), f in dec.items() if kd == kind]
-            if v:
-                print("  %-10s %3d outputs, decided fraction min %.4f" % (kind, len(v), min(v)))
-    for (n, P), e in sorted(REPORT["wgrad_tile"].items(), key=lambda kv: (kv[0][1], kv[0][0])):
-        print("worst wgrad tile norm-relative error P=%d %s: split-K %.3e (tolerance %.3e), deterministic %.3e "
-              "(tolerance %.3e)" % (P, n, e[0][0], e[0][1], e[1][0], e[1][1]))
+    report("bf16")
 
 
 @pytest.fixture(autouse=True)
@@ -137,15 +154,33 @@ def _x_shape(geom, x_wpad):
     return (B, H, W, Cin)
 
 
-def _x_input(geom, x_wpad, seed, signed):
+def _x_input(geom, x_wpad, seed, signed, dtype=torch.bfloat16):
     """x as the kernel reads it; the stem's space-to-depth buffer has zero W-padding columns (as
     acnn_pack_input writes them)."""
     shape = _x_shape(geom, x_wpad)
-    x = _randn(shape, seed) if signed else _pos(shape, seed)
+    x = _randn(shape, seed, dtype=dtype) if signed else _pos(shape, seed, dtype=dtype)
     if x_wpad is not None:
         x[:, :, :x_wpad[0]] = 0
         x[:, :, x.shape[2] - x_wpad[1]:] = 0
     return x
+
+
+def _fprop_ref(x, w, geom, x_wpad):
+    """float64 NHWC conv of a plan geometry and the same conv of |x|, |w| (ref, mag)."""
+    xp = _pad_x(x, geom, x_wpad)
+    w64 = w.double().permute(0, 3, 1, 2)
+    ref = _nhwc(F.conv2d(xp, w64, stride=geom[7]))
+    mag = _nhwc(F.conv2d(xp.abs(), w64.abs(), stride=geom[7]))
+    return ref, mag
+
+
+def _dgrad_ref(w, dy, fwd):
+    """float64 NHWC data gradient of the forward conv geometry fwd, [B][H][W][Cin]."""
+    B, H, W, Cin = fwd[:4]
+    _, _, _, _, _, _, _, st, phl, phh, pwl, pwh = fwd
+    full = torch.nn.grad.conv2d_input((B, Cin, H + phl + phh, W + pwl + pwh), w.double().permute(0, 3, 1, 2),
+                                      _nchw(dy), stride=st)
+    return _nhwc(full[:, :, phl:phl + H, pwl:pwl + W])
 
 
 def _wgrad_chain(lib, cg, precision, det):
@@ -169,44 +204,41 @@ def _pairs_apply(cg, M, out_f32):
 # ---------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("B", [256, 7])
 @pytest.mark.parametrize("case", CONV, ids=[c.id() for c in CONV])
-def test_conv_plan_geometry(lib, case, B):
+def test_conv_plan_geometry(lib, case, B, fmt):
+    code, tdt = FMT[fmt]
     geom = _with_batch(case.geom, B)
     cg = CC.launch_geom(geom, case.x_wpad)
     Ho, Wo = cg.out_hw()
     Cout, kh, kw, Cin = geom[4], geom[5], geom[6], geom[3]
     K = kh * kw * Cin
     M = B * Ho * Wo
-    x = _x_input(geom, case.x_wpad, 1, signed=False)
+    x = _x_input(geom, case.x_wpad, 1, signed=False, dtype=tdt)
     s = _signs(Cout, 2)
-    w = (_pos((Cout, kh, kw, Cin), 3, 1.0 / math.sqrt(K)).double() * s[:, None, None, None]).bfloat16()
+    w = (_pos((Cout, kh, kw, Cin), 3, 1.0 / math.sqrt(K)).double() * s[:, None, None, None]).to(tdt)
     bias = torch.randn(Cout, device="cuda", generator=_gen(4)) if case.bias else None
-    out_dt = torch.float32 if case.out_f32 else torch.bfloat16
+    out_dt = torch.float32 if case.out_f32 else tdt
 
     def launch(stats):
         y = _nan((B, Ho, Wo, Cout), out_dt)
-        sp = _nan((lib.acnn_conv_stats_parts(cg), 2, Cout), torch.float32) if stats else None
+        sp = CC.stats_poison((lib.acnn_conv_stats_parts(cg), 2, Cout)) if stats else None
         _check(lib.acnn_conv_fprop(cg, x.data_ptr(), w.data_ptr(), y.data_ptr(),
                                    sp.data_ptr() if stats else None, None, None,
                                    bias.data_ptr() if bias is not None else None, int(case.out_f32),
-                                   ACNN_BF16, 0, _st()), "conv_fprop")
+                                   code, 0, _st()), "conv_fprop")
         torch.cuda.synchronize()
         return y, sp
 
     y, sp = launch(case.stats)
-    xp = _pad_x(x, geom, case.x_wpad)
-    w64 = w.double().permute(0, 3, 1, 2)
-    ref = _nhwc(F.conv2d(xp, w64, stride=case.geom[7]))
-    mag = _nhwc(F.conv2d(xp.abs(), w64.abs(), stride=case.geom[7]))
-    del xp
+    ref, mag = _fprop_ref(x, w, geom, case.x_wpad)
     acc = CC.acc_bound(mag, K)
-    what = "%s B=%d" % (case.id(), B)
+    what = "%s B=%d %s" % (case.id(), B, fmt)
     if case.out_f32:
         ref = ref + bias.double()
         tol = acc + CC.U32 * (ref.abs() + acc)
         bad = ~((y.double() - ref).abs() <= tol)
         assert not bool(bad.any()), "%s: %d of %d logits outside acc + u |ref|" % (what, int(bad.sum()), bad.numel())
     else:
-        REPORT["decided"][("conv", what)] = CC.check_16bit(y, ref, acc, what)
+        REPORT[fmt]["decided"][("conv", what)] = CC.check_16bit(y, ref, acc, what, fmt)
     del ref, mag, acc
     if case.stats:
         CC.check_stats(sp, y, what + " statistics")
@@ -229,7 +261,8 @@ def test_conv_plan_geometry(lib, case, B):
 # dgrad
 # ---------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", DGRAD, ids=[c.id() for c in DGRAD])
-def test_dgrad_plan_geometry(lib, case):
+def test_dgrad_plan_geometry(lib, case, fmt):
+    code, tdt = FMT[fmt]
     from assembled_cnn_b200._lib import ConvGeom
     geom = case.geom
     g = ConvGeom(*geom)
@@ -238,59 +271,55 @@ def test_dgrad_plan_geometry(lib, case):
     fwd = case.src or geom                       # the forward conv whose data gradient this is
     gf = ConvGeom(*fwd)
     Hf, Wf = gf.out_hw()
-    dy = _pos((B, Hf, Wf, Cout), 11)
+    dy = _pos((B, Hf, Wf, Cout), 11, dtype=tdt)
     s = _signs(Cin, 12)
     K = kh * kw * Cout
-    w = (_pos((Cout, kh, kw, Cin), 13, 1.0 / math.sqrt(K)).double() * s).bfloat16()
+    w = (_pos((Cout, kh, kw, Cin), 13, 1.0 / math.sqrt(K)).double() * s).to(tdt)
     wd = w.flip(1, 2).permute(3, 1, 2, 0).contiguous()
     if case.src:
         # the plan's composition: zero-insert dy to (B, H, W, Cout), then the stride-1 dgrad on g1
         assert gf.stride == 2 and geom[9] == kh - 1 - geom[8] and geom[11] == kw - 1 - geom[10]
-        dyz = _nan((B, H, W, Cout), torch.bfloat16)
-        _check(lib.acnn_zero_insert2x(dy.data_ptr(), dyz.data_ptr(), B, Hf, Wf, H, W, Cout, ACNN_BF16, _st()),
+        dyz = _nan((B, H, W, Cout), tdt)
+        _check(lib.acnn_zero_insert2x(dy.data_ptr(), dyz.data_ptr(), B, Hf, Wf, H, W, Cout, code, _st()),
                "zero_insert2x")
     else:
         dyz = dy
-    add = (_pos((B, H, W, Cin), 14, 0.5).double() * s).bfloat16() if case.add else None
-    mask = _mask((B, H, W, Cin), 15) if case.mask else None
-    dx = _nan((B, H, W, Cin), torch.bfloat16)
+    add = (_pos((B, H, W, Cin), 14, 0.5).double() * s).to(tdt) if case.add else None
+    mask = _mask((B, H, W, Cin), 15, tdt) if case.mask else None
+    dx = _nan((B, H, W, Cin), tdt)
     _check(lib.acnn_conv_dgrad(g, dyz.data_ptr(), wd.data_ptr(), dx.data_ptr(),
                                add.data_ptr() if add is not None else None,
-                               mask.data_ptr() if mask is not None else None, ACNN_BF16, 0, _st()), "conv_dgrad")
+                               mask.data_ptr() if mask is not None else None, code, 0, _st()), "conv_dgrad")
     torch.cuda.synchronize()
     del dyz, wd
-    _, _, _, _, _, _, _, st, phl, phh, pwl, pwh = fwd
-    shape = (B, Cin, H + phl + phh, W + pwl + pwh)
-
-    def grad_in(w_, dy_):
-        full = torch.nn.grad.conv2d_input(shape, w_.double().permute(0, 3, 1, 2), _nchw(dy_), stride=st)
-        return _nhwc(full[:, :, phl:phl + H, pwl:pwl + W])
-    ref = grad_in(w, dy)
-    mag = grad_in(w.abs(), dy.abs())
+    ref = _dgrad_ref(w, dy, fwd)
+    mag = _dgrad_ref(w.abs(), dy.abs(), fwd)
     acc = CC.acc_bound(mag, K)
     if add is not None:
         acc = CC.add_epilogue_bound(acc, mag, add)
         ref = ref + add.double()
     del mag
+    what = "%s %s" % (case.id(), fmt)
     if mask is not None:
         keep = (mask > 0).double()
         ref, acc = ref * keep, acc * keep
-        CC.check_mask(dx, mask, case.id())
-    REPORT["decided"][("conv_dgrad", case.id())] = CC.check_16bit(dx, ref, acc, case.id())
+        CC.check_mask(dx, mask, what)
+    REPORT[fmt]["decided"][("conv_dgrad", what)] = CC.check_16bit(dx, ref, acc, what, fmt)
 
 
 # ---------------------------------------------------------------------------------------------------
 # wgrad
 # ---------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", WGRAD, ids=[c.id() for c in WGRAD])
-def test_wgrad_plan_geometry(lib, case):
+def test_wgrad_plan_geometry(lib, case, fmt):
+    code, tdt = FMT[fmt]
     geom = case.geom
     cg = CC.launch_geom(geom, case.x_wpad)
     B, _, _, Cin, Cout, kh, kw, stride = geom[:8]
     Ho, Wo = cg.out_hw()
     P = B * Ho * Wo
-    x = _x_input(geom, case.x_wpad, 21, signed=True)
-    dy = _randn((B, Ho, Wo, Cout), 22)
+    x = _x_input(geom, case.x_wpad, 21, signed=True, dtype=tdt)
+    dy = _randn((B, Ho, Wo, Cout), 22, dtype=tdt)
     dw0 = torch.randn((Cout, kh, kw, Cin), device="cuda", generator=_gen(23))
     xp = _pad_x(x, geom, case.x_wpad)
     wshape = (Cout, Cin, kh, kw)
@@ -302,15 +331,15 @@ def test_wgrad_plan_geometry(lib, case):
         dws = []
         for _ in range(2):
             dw = dw0.clone()
-            _check(lib.acnn_conv_wgrad(cg, x.data_ptr(), dy.data_ptr(), dw.data_ptr(), ACNN_BF16, det, _st()),
+            _check(lib.acnn_conv_wgrad(cg, x.data_ptr(), dy.data_ptr(), dw.data_ptr(), code, det, _st()),
                    "conv_wgrad")
             dws.append(dw)
         torch.cuda.synchronize()
-        what = "%s det=%d" % (case.id(), det)
+        what = "%s det=%d %s" % (case.id(), det, fmt)
         assert torch.equal(dws[0], dws[1]), what + ": a repeated launch differs"
-        chain = _wgrad_chain(lib, cg, ACNN_BF16, det)
+        chain = _wgrad_chain(lib, cg, code, det)
         worst.append((CC.check_wgrad(dws[0], ref, mag, dw0, P, what, chain), CC.wgrad_tile_tol(min(P, chain))))
-    REPORT["wgrad_tile"][(case.id(), P)] = worst
+    REPORT[fmt]["wgrad_tile"][(case.id(), P)] = worst
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -323,7 +352,7 @@ def test_stem_space_to_depth_end_to_end(lib, fmt):
     pixels) with its statistics, its wgrad into the packed layout and acnn_s2d_wgrad_unpack -- against the
     raw 7 x 7 stride-2 fixed_padding conv of the 16-bit-rounded images and weights and its weight gradient."""
     from assembled_cnn_b200.plan import PlanBuilder
-    code, tdt = {"bf16": (ACNN_BF16, torch.bfloat16), "fp16": (ACNN_F16, torch.float16)}[fmt]
+    code, tdt = FMT[fmt]
     B, HW, k, Cout = 256, 224, 7, 64
     pad, k2, lo, hi = PlanBuilder.stem_s2d_taps(k)
     H2 = HW // 2
@@ -339,7 +368,7 @@ def test_stem_space_to_depth_end_to_end(lib, fmt):
     w2 = _nan((Cout, k2, k2, 16), tdt)
     _check(lib.acnn_s2d_weight_pack(w.data_ptr(), w2.data_ptr(), Cout, k, pad, k2, lo, code, _st()), "s2d_weight_pack")
     y = _nan((B, H2, H2, Cout), tdt)
-    sp = _nan((lib.acnn_conv_stats_parts(cg), 2, Cout), torch.float32)
+    sp = CC.stats_poison((lib.acnn_conv_stats_parts(cg), 2, Cout))
     _check(lib.acnn_conv_fprop(cg, xs.data_ptr(), w2.data_ptr(), y.data_ptr(), sp.data_ptr(), None, None, None, 0,
                                code, 0, _st()), "stem conv_fprop")
     torch.cuda.synchronize()
@@ -350,7 +379,7 @@ def test_stem_space_to_depth_end_to_end(lib, fmt):
     acc = CC.acc_bound(mag, k2 * k2 * 16)      # the launched K (its zero taps add exactly)
     del mag
     what = "stem %s" % fmt
-    REPORT["decided"][("stem", what)] = CC.check_16bit(y, ref, acc, what, fmt)
+    REPORT["bf16"]["decided"][("stem", what)] = CC.check_16bit(y, ref, acc, what, fmt)
     del ref, acc
     CC.check_stats(sp, y, what + " statistics")
     # weight gradient: into the packed layout (the plan's zeroed slot), then unpacked into dw
@@ -366,7 +395,7 @@ def test_stem_space_to_depth_end_to_end(lib, fmt):
     P = B * H2 * H2
     chain = _wgrad_chain(lib, cg, code, 0)
     e = CC.check_wgrad(dw, ref_w, mag_w, torch.zeros_like(dw), P, what + " wgrad", chain)
-    REPORT["wgrad_tile"][(what, P)] = ((e, CC.wgrad_tile_tol(min(P, chain))), (float("nan"), float("nan")))
+    REPORT["bf16"]["wgrad_tile"][(what, P)] = ((e, CC.wgrad_tile_tol(min(P, chain))), (float("nan"), float("nan")))
 
 
 # ---------------------------------------------------------------------------------------------------

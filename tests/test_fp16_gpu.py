@@ -382,81 +382,3 @@ def test_fp16_retrieval_search_against_restatement(metric):
     for r in torch.nonzero(both).flatten().tolist():
         l = idx[r].tolist()
         assert l.index(5) < l.index(7)
-
-
-def _plan_geoms():
-    """Every distinct (pass, geometry) of the conv GEMMs of the c3 and c5 training plans at B = 256, 224 px
-    (dgrad geometries as the plan launches them: stride 1 over the zero-inserted gradient of a stride-2 conv)."""
-    import bench
-    from assembled_cnn_b200.plan import ModelConfig, build_plan
-    seen = set()
-    for name in ("c3", "c5"):
-        cfg = ModelConfig(num_classes=1001, **bench.CONFIGS[name]["model"])
-        plan = build_plan(cfg, 256, 224, 224, mixup_type=1, label_smoothing=0.1, dtype="fp16")
-        for op in plan.all_ops():
-            if op.kind in ("conv", "conv_dgrad", "conv_wgrad"):
-                seen.add((op.kind, tuple(op.geom.astuple())))
-    return sorted(seen)
-
-
-PLAN_GEOMS = _plan_geoms()
-
-
-@pytest.mark.parametrize("kind,geom", PLAN_GEOMS, ids=["%s-%s" % (k, "x".join(map(str, g))) for k, g in PLAN_GEOMS])
-def test_conv_gemms_fp16_plan_geometries(kind, geom):
-    """Each GEMM pass of the plans at its own B = 256 geometry against float64: norm-relative error within
-    one fp16 rounding (fprop, dgrad) or the fp32 accumulation (wgrad), the per-element bound for fprop;
-    and with CTA pairs (acnn_set_conv_cta_pairs(1), the clusters of two that conv_tiling picks at large M)
-    the fprop / dgrad output is bit-identical to single CTAs."""
-    from assembled_cnn_b200 import _lib
-    from assembled_cnn_b200._lib import ConvGeom
-    lib = _lib.load()
-    g = ConvGeom(*geom)
-    Ho, Wo = g.out_hw()
-    st = torch.cuda.current_stream().cuda_stream
-    K = g.kh * g.kw * g.Cin
-    x = _rand_f16((g.B, g.H, g.W, g.Cin), 11)
-    if kind == "conv_wgrad":
-        dy = _rand_f16((g.B, Ho, Wo, g.Cout), 12, 0.1)
-        dw = torch.zeros(g.Cout, g.kh, g.kw, g.Cin, device="cuda")
-        _lib.check(lib.acnn_conv_wgrad(g, x.data_ptr(), dy.data_ptr(), dw.data_ptr(), ACNN_F16, 0, st), "wgrad")
-        torch.cuda.synchronize()
-        xp = F.pad(_nchw(x), (g.pad_w_lo, g.pad_w_hi, g.pad_h_lo, g.pad_h_hi))
-        ref = torch.nn.grad.conv2d_weight(xp, (g.Cout, g.Cin, g.kh, g.kw), _nchw(dy), stride=g.stride)
-        assert _nrel(dw, ref.permute(0, 2, 3, 1)) < 1e-3
-        return
-    w = _rand_f16((g.Cout, g.kh, g.kw, g.Cin), 13, 1.0 / math.sqrt(K))
-    dy = _rand_f16((g.B, Ho, Wo, g.Cout), 14)
-    wd = w.flip(1, 2).permute(3, 1, 2, 0).contiguous()
-
-    def run():
-        if kind == "conv":
-            y = torch.full((g.B, Ho, Wo, g.Cout), float("nan"), dtype=torch.float16, device="cuda")
-            _lib.check(lib.acnn_conv_fprop(g, x.data_ptr(), w.data_ptr(), y.data_ptr(), None, None, None, None, 0,
-                                           ACNN_F16, 0, st), "fprop")
-        else:
-            # the plan's dgrad: g is the (stride-1) forward geometry whose data gradient it computes
-            y = torch.full((g.B, g.H, g.W, g.Cin), float("nan"), dtype=torch.float16, device="cuda")
-            _lib.check(lib.acnn_conv_dgrad(g, dy.data_ptr(), wd.data_ptr(), y.data_ptr(), None, None, ACNN_F16, 0,
-                                           st), "dgrad")
-        torch.cuda.synchronize()
-        return y
-
-    y = run()
-    if kind == "conv":
-        ref = _fwd64(x, w, g)
-        mag = _fwd64(x.abs(), w.abs(), g)
-        tol = 2 * K * U32 * mag
-        _check(y, ref, tol + _ulp_f16(ref.abs() + tol), "fprop")
-    else:
-        assert g.stride == 1
-        shape = (g.B, g.Cin, g.H + g.pad_h_lo + g.pad_h_hi, g.W + g.pad_w_lo + g.pad_w_hi)
-        full = torch.nn.grad.conv2d_input(shape, w.double().permute(0, 3, 1, 2), _nchw(dy))
-        ref = full[:, :, g.pad_h_lo:g.pad_h_lo + g.H, g.pad_w_lo:g.pad_w_lo + g.W].permute(0, 2, 3, 1)
-    assert _nrel(y, ref) < 2.0 ** -11, _nrel(y, ref)
-    prev = lib.acnn_set_conv_cta_pairs(1)
-    try:
-        y2 = run()
-    finally:
-        lib.acnn_set_conv_cta_pairs(prev)
-    assert torch.equal(y.view(torch.int16), y2.view(torch.int16))
