@@ -97,4 +97,14 @@ int make_map_2d(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, in
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// acnn_sk_fc_fwd / acnn_se_fc_fwd with their GEMMs' split-K chosen as for max(B, split_rows) rows
+// (acnn_set_fc_split_rows): each row gets the bits of the same row in a batch of split_rows.
+int sk_fc_fwd(const float* s, const float* w1, const float* gamma, const float* beta, float* moving_mean,
+              float* moving_var, float momentum, float eps, int training, const float* w2, float* zpre,
+              float* bnstat, float* z, float* att, float* scratch, int B, int f, int d, int deterministic,
+              int split_rows, void* stream);
+int se_fc_fwd(const float* q, const float* w1, const float* w2, float* h, float* e, int B, int C, int r,
+              int deterministic, int split_rows, void* stream);
+int fc_split_rows();   // acnn_set_fc_split_rows
+
 }  // namespace acnn

@@ -166,6 +166,8 @@ acnn_model::Launch resolve(acnn_model* m, const Op& op) {
   const Plan& p = m->plan;
   const std::string& k = op.kind;
   const int adt = m->adt, det = m->det, training = p.cfg.training ? 1 : 0;
+  // the small SK / SE GEMMs of an eval handle may take the split-K of a larger batch (a serving ladder)
+  const int fc_rows = training ? 0 : acnn::fc_split_rows();
   const bool fp32 = p.cfg.fp32;
   const float bn_mom = (float)p.cfg.bn_momentum, eps = (float)p.cfg.bn_epsilon;
   float* hp = reinterpret_cast<float*>(m->ws + m->hp_off);
@@ -302,8 +304,8 @@ acnn_model::Launch resolve(acnn_model* m, const Op& op) {
           *att = r.S("att"), *scratch = r.S("scratch");
     if (k == "sk_fc")
       return [=](void* st) {
-        return acnn_sk_fc_fwd(s, w1, gamma, beta, mm, mv, bn_mom, eps, training, w2, zpre, bw, z, att,
-                              scratch, B, f, d, det, st);
+        return acnn::sk_fc_fwd(s, w1, gamma, beta, mm, mv, bn_mom, eps, training, w2, zpre, bw, z, att,
+                               scratch, B, f, d, det, fc_rows, st);
       };
     float *dA = r.S("dA"), *ds = r.S("ds"), *dw1 = r.G("w1"), *dw2 = r.G("w2"), *dg = r.Gv(bn.gamma),
           *db = r.Gv(bn.beta);
@@ -328,7 +330,7 @@ acnn_model::Launch resolve(acnn_model* m, const Op& op) {
   if (k == "se_fc") {
     float *q = r.S("q"), *w1 = r.P("w1"), *w2 = r.P("w2"), *h = r.S("h"), *e = r.S("e");
     const int B = (int)r.I("B"), C = (int)r.I("C"), rr = (int)r.I("r");
-    return [=](void* st) { return acnn_se_fc_fwd(q, w1, w2, h, e, B, C, rr, det, st); };
+    return [=](void* st) { return acnn::se_fc_fwd(q, w1, w2, h, e, B, C, rr, det, fc_rows, st); };
   }
   if (k == "se_fc_bwd") {
     float *de = r.S("de"), *e = r.S("e"), *h = r.S("h"), *q = r.S("q"), *w1 = r.P("w1"), *w2 = r.P("w2"),

@@ -109,9 +109,10 @@ sgemm_reduce_kernel(const float* __restrict__ part, float* C, int64_t n, int spl
 
 // C (+)= A*B with split-K sized so that ~2 CTAs per SM are in flight; the partials of a split-K
 // product are summed in split order (bit-reproducible).  det: no split-K -- every element of C
-// receives exactly one add.
+// receives exactly one add.  split_rows > M: the split count is the one of a split_rows-row product,
+// so each row of C gets the bits it would get in that larger product.
 static int sgemm(const float* A, const float* B, float* C, int M, int N, int K, int sAm, int sAk,
-                 int sBk, int sBn, bool zero_c, int det, cudaStream_t s) {
+                 int sBk, int sBn, bool zero_c, int det, cudaStream_t s, int split_rows = 0) {
   if (zero_c) {
     cudaError_t e = cudaMemsetAsync(C, 0, (size_t)M * N * sizeof(float), s);
     if (e != cudaSuccess) {
@@ -119,7 +120,7 @@ static int sgemm(const float* A, const float* B, float* C, int M, int N, int K, 
       return ACNN_ERR_CUDA;
     }
   }
-  const int tiles = ceil_div(M, kTM) * ceil_div(N, kTN);
+  const int tiles = ceil_div(M > split_rows ? M : split_rows, kTM) * ceil_div(N, kTN);
   int splits = ceil_div(2 * num_sms_small(), tiles);
   const int max_splits = ceil_div(K, 2 * kTK);
   if (splits > max_splits) splits = max_splits;
@@ -312,9 +313,9 @@ static int job_splits(int M, int N, int K, int share) {
 }
 
 static GJob make_job(const float* A, const float* B, float* P, int M, int N, int K, int sAm, int sAk,
-                     int sBk, int sBn, int share) {
+                     int sBk, int sBn, int share, int split_rows = 0) {
   GJob j{A, B, P, M, N, K, sAm, sAk, sBk, sBn, 0, 0, 0, 0};
-  j.splits = job_splits(M, N, K, share);
+  j.splits = job_splits(M > split_rows ? M : split_rows, N, K, share);
   j.kper = ceil_div(ceil_div(K, j.splits), kTK) * kTK;
   j.splits = ceil_div(K, j.kper);
   j.tn = ceil_div(N, kTN);
@@ -590,6 +591,10 @@ static bool use_fused(int deterministic) {
   return g_sk_fc_fused == 1 || (g_sk_fc_fused == -1 && deterministic);
 }
 
+// acnn_set_fc_split_rows: read by the executor when it binds an eval handle
+static int g_fc_split_rows = 0;
+int fc_split_rows() { return g_fc_split_rows; }
+
 }  // namespace acnn
 
 using namespace acnn;
@@ -618,10 +623,33 @@ int acnn_set_sk_fc_fused(int on) {
   return prev;
 }
 
+int acnn_set_fc_split_rows(int rows) {
+  const int prev = g_fc_split_rows;
+  g_fc_split_rows = rows > 0 ? rows : 0;
+  return prev;
+}
+
 int acnn_sk_fc_fwd(const float* s, const float* w1, const float* gamma, const float* beta,
                    float* moving_mean, float* moving_var, float momentum, float eps, int training,
                    const float* w2, float* zpre, float* bnstat, float* z, float* att,
                    float* scratch, int B, int f, int d, int deterministic, void* stream) {
+  return acnn::sk_fc_fwd(s, w1, gamma, beta, moving_mean, moving_var, momentum, eps, training, w2, zpre,
+                         bnstat, z, att, scratch, B, f, d, deterministic, 0, stream);
+}
+
+int acnn_se_fc_fwd(const float* q, const float* w1, const float* w2, float* h, float* e, int B,
+                   int C, int r, int deterministic, void* stream) {
+  return acnn::se_fc_fwd(q, w1, w2, h, e, B, C, r, deterministic, 0, stream);
+}
+
+}  // extern "C"
+
+namespace acnn {
+
+int sk_fc_fwd(const float* s, const float* w1, const float* gamma, const float* beta, float* moving_mean,
+              float* moving_var, float momentum, float eps, int training, const float* w2, float* zpre,
+              float* bnstat, float* z, float* att, float* scratch, int B, int f, int d, int deterministic,
+              int split_rows, void* stream) {
   ACNN_REQUIRE(s && w1 && gamma && beta && moving_mean && moving_var && w2 && zpre && bnstat && z &&
                    att && scratch, "sk_fc_fwd: null argument");
   cudaStream_t st = (cudaStream_t)stream;
@@ -629,8 +657,8 @@ int acnn_sk_fc_fwd(const float* s, const float* w1, const float* gamma, const fl
     const int G = num_sms_small() < kGridMax ? num_sms_small() : kGridMax;
     float* part = scratch + (size_t)B * (2 * f + d);
     SkFcFwdArgs a{};
-    a.fc1 = make_job(s, w1, part, B, d, f, f, 1, 1, f, G);
-    a.fc2 = make_job(z, w2, part, B, 2 * f, d, d, 1, 1, d, G);
+    a.fc1 = make_job(s, w1, part, B, d, f, f, 1, 1, f, G, split_rows);
+    a.fc2 = make_job(z, w2, part, B, 2 * f, d, d, 1, 1, d, G, split_rows);
     a.gamma = gamma; a.beta = beta; a.moving_mean = moving_mean; a.moving_var = moving_var;
     a.zpre = zpre; a.bnstat = bnstat; a.z = z; a.att = att;
     a.momentum = momentum; a.eps = eps; a.training = training; a.B = B; a.f = f; a.d = d;
@@ -638,17 +666,33 @@ int acnn_sk_fc_fwd(const float* s, const float* w1, const float* gamma, const fl
     return launch_coop(sk_fc_fwd_fused_kernel, a, fused_grid(units), st, "sk_fc_fwd_fused");
   }
   // zpre[B,d] = s[B,f] * W1[d,f]^T
-  int rc = sgemm(s, w1, zpre, B, d, f, f, 1, 1, f, true, deterministic, st);
+  int rc = sgemm(s, w1, zpre, B, d, f, f, 1, 1, f, true, deterministic, st, split_rows);
   if (rc) return rc;
   launch_k(bn_batch_relu_fwd_kernel, dim3(ceil_div(d, kFT / 32)), dim3(kFT), 0, st, zpre, gamma, beta, moving_mean, moving_var, momentum, eps, training, z, bnstat, B, d);
   count_launch();
   if ((rc = check_launch("sk bn_batch_relu_fwd"))) return rc;
   // a[B,2f] = z[B,d] * W2[2f,d]^T
-  if ((rc = sgemm(z, w2, scratch, B, 2 * f, d, d, 1, 1, d, true, deterministic, st))) return rc;
+  if ((rc = sgemm(z, w2, scratch, B, 2 * f, d, d, 1, 1, d, true, deterministic, st, split_rows))) return rc;
   launch_k(sk_gate_fwd_kernel, dim3((int)ceil_div64((int64_t)B * f, 256)), dim3(256), 0, st, scratch, att, B, f);
   count_launch();
   return check_launch("sk_gate_fwd");
 }
+
+int se_fc_fwd(const float* q, const float* w1, const float* w2, float* h, float* e, int B, int C, int r,
+              int deterministic, int split_rows, void* stream) {
+  ACNN_REQUIRE(q && w1 && w2 && h && e, "se_fc_fwd: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  // h = relu(q[B,C] * W1[r,C]^T) ; e = sigmoid(h[B,r] * W2[C,r]^T)
+  int rc = sgemm(q, w1, h, B, r, C, C, 1, 1, C, true, deterministic, st, split_rows);
+  if (rc) return rc;
+  if ((rc = ew(h, nullptr, h, (int64_t)B * r, 1, 0.f, st))) return rc;
+  if ((rc = sgemm(h, w2, e, B, C, r, r, 1, 1, r, true, deterministic, st, split_rows))) return rc;
+  return ew(e, nullptr, e, (int64_t)B * C, 2, 0.f, st);
+}
+
+}  // namespace acnn
+
+extern "C" {
 
 int acnn_sk_fc_bwd(const float* dA, const float* att, const float* z, const float* zpre,
                    const float* bnstat, const float* gamma, const float* s, const float* w1,
@@ -692,18 +736,6 @@ int acnn_sk_fc_bwd(const float* dA, const float* att, const float* z, const floa
   if ((rc = sgemm(dz, s, dw1, d, f, B, 1, d, f, 1, false, deterministic, st))) return rc;
   // ds[B,f] = dzpre[B,d] * W1[d,f]
   return sgemm(dz, w1, ds, B, f, d, d, 1, f, 1, true, deterministic, st);
-}
-
-int acnn_se_fc_fwd(const float* q, const float* w1, const float* w2, float* h, float* e, int B,
-                   int C, int r, int deterministic, void* stream) {
-  ACNN_REQUIRE(q && w1 && w2 && h && e, "se_fc_fwd: null argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  // h = relu(q[B,C] * W1[r,C]^T) ; e = sigmoid(h[B,r] * W2[C,r]^T)
-  int rc = sgemm(q, w1, h, B, r, C, C, 1, 1, C, true, deterministic, st);
-  if (rc) return rc;
-  if ((rc = ew(h, nullptr, h, (int64_t)B * r, 1, 0.f, st))) return rc;
-  if ((rc = sgemm(h, w2, e, B, C, r, r, 1, 1, r, true, deterministic, st))) return rc;
-  return ew(e, nullptr, e, (int64_t)B * C, 2, 0.f, st);
 }
 
 int acnn_se_fc_bwd(const float* de, const float* e, const float* h, const float* q,

@@ -166,10 +166,15 @@ class Model:
 
     # ---------------------------------------------------------------- runtimes / parameters
     def runtime(self, batch, height, width, *, training, use_resnet_d=False, mixup_type=0,
-                label_smoothing=0.0, with_loss=False, use_dropblock=False, kd_temp=0.0) -> NativeRuntime:
+                label_smoothing=0.0, with_loss=False, use_dropblock=False, kd_temp=0.0,
+                fc_split_rows=0) -> NativeRuntime:
+        """The runtime of one batch shape and mode, built on first use over this model's variables.
+        fc_split_rows > batch (eval only): the SK / SE attention GEMMs split K as a batch of that many rows
+        would (acnn_set_fc_split_rows), so each row gets the bits it gets in such a batch."""
+        rows = int(fc_split_rows) if not training and int(fc_split_rows) > batch else 0
         key = (batch, height, width, bool(training), bool(use_resnet_d), mixup_type,
                float(label_smoothing), bool(with_loss or training), bool(use_dropblock and training),
-               float(kd_temp) if training else 0.0)
+               float(kd_temp) if training else 0.0, rows)
         rt = self._runtimes.get(key)
         if rt is None:
             cfg = ModelConfig(use_resnet_d=bool(use_resnet_d), **self.cfg_kwargs)
@@ -178,8 +183,15 @@ class Model:
                         kd_temp=kd_temp)
             prim = self._primary.get(bool(use_resnet_d))
             # the layer plan is built and executed inside libacnn.so (include/acnn_model.h)
-            rt = NativeRuntime(NativeModel(cfg, batch, height, width, deterministic=self.deterministic, **step),
-                               self.device, share=prim)
+            nm = NativeModel(cfg, batch, height, width, deterministic=self.deterministic, **step)
+            if rows:
+                prev = nm.lib.acnn_set_fc_split_rows(rows)       # read by acnn_bind
+                try:
+                    rt = NativeRuntime(nm, self.device, share=prim)
+                finally:
+                    nm.lib.acnn_set_fc_split_rows(prev)
+            else:
+                rt = NativeRuntime(nm, self.device, share=prim)
             if prim is None:
                 self._primary[bool(use_resnet_d)] = rt
                 if self._pending_weights is not None:
@@ -844,10 +856,11 @@ class _EvalPipeline(StagingRing):
     A subclass gives the host sets and slots, stages a batch's labels beside its images (`_fill`) and defines
     `_body`."""
 
-    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, host, slots):
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, host, slots, fc_split_rows=0):
         torch.cuda.set_device(model.device)
         super().__init__(torch.device(model.device), host, slots)
-        self.rt = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d)
+        self.rt = model.runtime(batch, size, size, training=False, use_resnet_d=use_resnet_d,
+                                fc_split_rows=fc_split_rows)
         self.batch, self.use_graph = batch, use_cuda_graph
         self.logits = self.rt.t[self.rt.plan.meta["logits"]][:, :model.num_classes]
         self.graphs = {}
@@ -946,7 +959,8 @@ class _ResizedEvalPipeline(_EvalPipeline):
     (run_batch_encoded), and the batch's labels (`label_dtype`) go to the device slot with them; a subclass's
     `_body` starts with rt.set_images_resized (resize + crop + mean)."""
 
-    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_dtype=torch.int32):
+    def __init__(self, model, batch, size, use_resnet_d, use_cuda_graph, label_dtype=torch.int32,
+                 fc_split_rows=0):
         dev, lab = torch.device(model.device), dict(dtype=label_dtype)
         # pinned image bytes (grown on demand), labels, descriptors
         host = [[None, torch.zeros(batch, **lab).pin_memory(), torch.zeros(32 * batch, dtype=torch.uint8).pin_memory()]
@@ -955,7 +969,7 @@ class _ResizedEvalPipeline(_EvalPipeline):
         # holds the descriptor table's address only, so the image bytes may move
         slots = [[None, torch.zeros(batch, **lab, device=dev), torch.zeros(32 * batch, dtype=torch.uint8, device=dev)]
                  for _ in range(2)]
-        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph, host, slots)
+        super().__init__(model, batch, size, use_resnet_d, use_cuda_graph, host, slots, fc_split_rows)
         self.size = size
 
     def run_batch(self, images, labels):
@@ -1408,8 +1422,8 @@ class _PredictDevice(_ResizedEvalPipeline):
 
     OUT_RING = 3
 
-    def __init__(self, model, batch, size, use_resnet_d, embedding):
-        super().__init__(model, batch, size, use_resnet_d, True)
+    def __init__(self, model, batch, size, use_resnet_d, embedding, fc_split_rows=0):
+        super().__init__(model, batch, size, use_resnet_d, True, fc_split_rows=fc_split_rows)
         nc, m = model.num_classes, self.rt.plan.meta
         self.out = [torch.zeros(batch, dtype=torch.int32, device=self.dev),
                     torch.zeros(batch, nc, dtype=torch.float32, device=self.dev),
@@ -1471,6 +1485,34 @@ class _PredictDevice(_ResizedEvalPipeline):
             self._deliver()
 
 
+def check_batch_sizes(batch_sizes, max_batch):
+    """The rungs of a servable's batch ladder: (max_batch,) for None, else batch_sizes as a tuple of
+    positive, strictly increasing ints whose largest is max_batch (ValueError otherwise)."""
+    if int(max_batch) < 1:
+        raise ValueError("max_batch must be >= 1 (got %r)" % (max_batch,))
+    max_batch = int(max_batch)
+    if batch_sizes is None:
+        return (max_batch,)
+    sizes = tuple(batch_sizes)
+    if not sizes or any(isinstance(b, bool) or not isinstance(b, (int, np.integer)) or b < 1 for b in sizes):
+        raise ValueError("batch_sizes must be positive ints (got %r)" % (batch_sizes,))
+    if any(a >= b for a, b in zip(sizes, sizes[1:])):
+        raise ValueError("batch_sizes must be strictly increasing (got %r)" % (batch_sizes,))
+    if sizes[-1] != max_batch:
+        raise ValueError("the largest of batch_sizes must be max_batch = %d (got %r)" % (max_batch, batch_sizes))
+    return tuple(int(b) for b in sizes)
+
+
+def ladder_chunks(n, batch_sizes):
+    """The (rung, start, stop) chunks of a request of n rows on the rungs batch_sizes (check_batch_sizes):
+    chunks of max(batch_sizes) rows, then the rest on the smallest rung that holds it."""
+    top = batch_sizes[-1]
+    out = [(top, a, a + top) for a in range(0, n - n % top, top)]
+    if n % top:
+        out.append((next(b for b in batch_sizes if b >= n % top), n - n % top, n))
+    return out
+
+
 class Servable:
     """An exported model (export_model / load_servable) or an in-memory `model` serving the PREDICT dict of
     nets/run_loop_classification.py:126-130 for encoded images (predict, the reference's binary_input
@@ -1479,21 +1521,40 @@ class Servable:
     [n, num_classes]} plus 'embedding' float32 [n, d] when the model has an embedding layer or was exported
     with return_embedding (without an embedding layer, the pooled features, as Model.__call__ returns them).
 
-    The device work runs in chunks of max_batch images on the model's device; the first call builds it."""
+    The device work runs in chunks of max_batch images on the model's device; the first call builds it.
+    batch_sizes, e.g. (1, 8, 64, 256), is a ladder of eval runtimes over the model's one copy of the
+    weights, each with its own workspace and CUDA graphs, built on its first use: a request's chunks of
+    max_batch = max(batch_sizes) rows run on the largest rung and its remainder on the smallest rung that
+    holds it (ladder_chunks), so a small request costs a small forward.  Every rung gives each image the
+    bits the largest gives it (the SK / SE attention GEMMs of the smaller rungs split K as max_batch rows
+    would: acnn_set_fc_split_rows).  None: the one rung max_batch."""
 
     def __init__(self, model, *, preprocessing_type="imagenet", image_size=224, use_resnet_d=None,
-                 return_embedding=False, max_batch=256, signature="binary_input", decoder_type="jpeg"):
+                 return_embedding=False, max_batch=256, signature="binary_input", decoder_type="jpeg",
+                 batch_sizes=None):
         from .imagenet_eval import eval_size
         self.size, _ = eval_size(preprocessing_type, image_size)
-        if int(max_batch) < 1:
-            raise ValueError("max_batch must be >= 1 (got %r)" % (max_batch,))
+        self.batch_sizes = check_batch_sizes(batch_sizes, max_batch)
         self.model, self.max_batch = model, int(max_batch)
         self.preprocessing_type, self.image_size = preprocessing_type, int(image_size)
         self.use_resnet_d = bool(getattr(model, "use_resnet_d", False) if use_resnet_d is None else use_resnet_d)
         self.embedding = bool(return_embedding) or model.cfg_kwargs["embedding_size"] > 0
         self.signature, self.decoder_type = signature, decoder_type
         self.outputs = PREDICT_OUTPUTS + (("embedding",) if self.embedding else ())
-        self._pipe = None
+        self._pipes = {}             # rung -> _PredictDevice
+
+    @property
+    def _pipe(self):
+        """The pipeline of the max_batch rung (None before its first use)."""
+        return self._pipes.get(self.max_batch)
+
+    def _rung(self, batch):
+        pipe = self._pipes.get(batch)
+        if pipe is None:
+            pipe = _PredictDevice(self.model, batch, self.size, self.use_resnet_d, self.embedding,
+                                  fc_split_rows=self.max_batch)
+            self._pipes[batch] = pipe
+        return pipe
 
     def _empty(self, n):
         nc = self.model.num_classes
@@ -1503,16 +1564,14 @@ class Servable:
             res["embedding"] = None          # its width is the runtime's: set by the first delivery
         return res
 
-    def _collect(self, n, work):
-        """Runs work(pipeline) and returns the outputs of its n rows, delivered in order."""
+    def _collect(self, n, run):
+        """Runs run(pipeline, start, stop) for every chunk of the n rows on its rung (ladder_chunks) and
+        returns the outputs of the n rows, delivered in order."""
         res, pos = self._empty(n), 0
         if n == 0:
             if self.embedding:
                 res["embedding"] = np.zeros((0, 0), np.float32)
             return res
-        if self._pipe is None:
-            self._pipe = _PredictDevice(self.model, self.max_batch, self.size, self.use_resnet_d, self.embedding)
-        pipe = self._pipe
 
         def sink(arrays):
             nonlocal pos
@@ -1523,14 +1582,20 @@ class Servable:
                 res[name][pos:pos + k] = a
             pos += k
 
-        pipe.sink = sink
+        pipe = None
         try:
-            work(pipe)
+            for rung, a, b in ladder_chunks(n, self.batch_sizes):
+                if pipe is not None and pipe.batch != rung:
+                    pipe.finish()            # the rows of the previous rung are delivered first
+                pipe = self._rung(rung)
+                pipe.sink = sink
+                run(pipe, a, b)
             pipe.finish()
         except BaseException:
-            # a batch may be staged and not run: the next call starts a new pipeline
-            torch.cuda.synchronize(pipe.dev)
-            self._pipe = None
+            # a batch may be staged and not run: the next call starts new pipelines
+            if pipe is not None:
+                torch.cuda.synchronize(pipe.dev)
+            self._pipes.clear()
             raise
         assert pos == n, (pos, n)
         return res
@@ -1546,16 +1611,13 @@ class Servable:
             if not isinstance(b, (bytes, bytearray, memoryview)):
                 raise TypeError("predict: image %d is a %s, not encoded bytes" % (i, type(b).__name__))
         images = [b if isinstance(b, bytes) else bytes(b) for b in images]
-        B = self.max_batch
 
         def geometry(h, w):
             return eval_geometry(h, w, self.preprocessing_type, self.image_size)
 
-        def work(pipe):
-            for a in range(0, len(images), B):
-                chunk = images[a:a + B]
-                pipe.run_batch_encoded(chunk, [0] * len(chunk), geometry)
-        return self._collect(len(images), work)
+        def run(pipe, a, b):
+            pipe.run_batch_encoded(images[a:b], [0] * (b - a), geometry)
+        return self._collect(len(images), run)
 
     def predict_images(self, images):
         """The PREDICT dict of float32 [n, S, S, 3] images already preprocessed (S: the eval size of the
@@ -1565,12 +1627,7 @@ class Servable:
         if x.dim() != 4 or tuple(x.shape[1:]) != (S, S, 3):
             raise ValueError("predict_images: images must be [n, %d, %d, 3] (got %s)" % (S, S, tuple(x.shape)))
         x = x.to(torch.float32)
-        B = self.max_batch
-
-        def work(pipe):
-            for a in range(0, x.shape[0], B):
-                pipe.run_images(x[a:a + B])
-        return self._collect(x.shape[0], work)
+        return self._collect(x.shape[0], lambda pipe, a, b: pipe.run_images(x[a:b]))
 
 
 def _variable_names(cfg_kwargs, use_resnet_d, size):
@@ -1681,12 +1738,13 @@ def read_servable_config(path):
     return cfg
 
 
-def load_servable(path, *, device=None, max_batch=256):
+def load_servable(path, *, device=None, max_batch=256, batch_sizes=None):
     """The Servable of a directory export_model wrote: a new Model of the directory's flags and dtype with
-    its variables (on `device`, default the current CUDA device).  Host work only: the device work starts
-    with the first predict."""
+    its variables (on `device`, default the current CUDA device), on the rungs batch_sizes (Servable).
+    Host work only: the device work starts with the first predict."""
     from .checkpoint import load_checkpoint
     from .imagenet_eval import eval_size
+    check_batch_sizes(batch_sizes, max_batch)
     cfg = read_servable_config(path)
     size, _ = eval_size(cfg["preprocessing_type"], cfg["image_size"])
     model = Model(dtype=cfg["dtype"], device=device or "cuda:%d" % torch.cuda.current_device(), **cfg["model"])
@@ -1699,7 +1757,7 @@ def load_servable(path, *, device=None, max_batch=256):
     model.set_weights({n: torch.as_tensor(weights[n]) for n in names})
     return Servable(model, preprocessing_type=cfg["preprocessing_type"], image_size=cfg["image_size"],
                     use_resnet_d=model.use_resnet_d, return_embedding=cfg["return_embedding"], max_batch=max_batch,
-                    signature=cfg["signature"], decoder_type=cfg["decoder_type"])
+                    signature=cfg["signature"], decoder_type=cfg["decoder_type"], batch_sizes=batch_sizes)
 
 
 def export_recall_at_1(embedding, labels, device=None):

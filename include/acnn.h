@@ -101,6 +101,13 @@ int acnn_set_stream_grid_cap(int blocks);
  * when the call asks for deterministic results, multi-launch otherwise.
  * Same results up to fp32 summation order.  Returns the previous setting. */
 int acnn_set_sk_fc_fused(int on);
+/* The K splits of the SK / SE attention GEMMs in the EVAL model handles bound (acnn_bind) while this is
+ * set: rows > 0 chooses them as for a batch of max(rows, B) rows, so that each image's outputs are
+ * bit for bit those of a handle of `rows` rows (the splits depend on the batch's 64-row tiles, and
+ * a different split count sums a row in a different fp32 order).  Needs no more scratch: a larger
+ * batch never has more splits.  0 (default): the handle's own batch.  Training handles and the
+ * direct entry points acnn_sk_fc_fwd / acnn_se_fc_fwd ignore it.  Returns the previous setting. */
+int acnn_set_fc_split_rows(int rows);
 /* floats of the `scratch` argument of acnn_sk_fc_fwd / acnn_sk_fc_bwd (da [B,2f] + dz [B,d] + the
  * K-split partial tiles of the widest phase, sized for 132 CTAs; callable without a GPU) */
 int64_t acnn_sk_fc_scratch_floats(int B, int f, int d);
