@@ -13,7 +13,11 @@
 //                     is merged into the row's sorted list when it could overflow.  The list lives in
 //                     the (row, split) partial output.  A row is owned by one quad of one warp, so
 //                     the warp maintains its 16 rows without any CTA-wide synchronisation.
-//   knn_merge_kernel: the final k of every row from its per-split sorted lists.
+//   knn_merge_kernel: the final k of every row from its per-split sorted lists, W lists per pass.
+//
+// acnn_knn_topk runs all three on Q and X.  For serving, acnn_knn_prepare_index runs the prep of X
+// once into a caller-owned index, and acnn_knn_search prepares Q only and searches that index in up
+// to one column split per SM (a small query batch is one row block), merged 16 lists per pass.
 //
 // Every selection uses the total order (similarity desc, index asc) and every similarity is the same
 // fp32 value whatever the tile schedule, so the result does not depend on the split count.
@@ -402,7 +406,10 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-// One thread per row: k-way merge of the row's per-split sorted lists.
+// One thread per row: W-way merge of the row's sorted lists.  blockIdx.y = g merges lists
+// [g * W, min((g + 1) * W, splits)) into output list g (out + g * nq * k), so passes of W-way merges
+// reduce any number of lists.
+template <int W>
 __global__ void __launch_bounds__(128)
 knn_merge_kernel(const float* __restrict__ ps, const int* __restrict__ pi, int nq, int k, int splits,
                  int32_t* __restrict__ out_idx, float* __restrict__ out_sim) {
@@ -411,11 +418,16 @@ knn_merge_kernel(const float* __restrict__ ps, const int* __restrict__ pi, int n
   if (row >= nq) return;
   const size_t stride = (size_t)nq * k;
   const size_t base = (size_t)row * k;
-  int head[kMaxSplits];
-  float hs[kMaxSplits];
-  int hi[kMaxSplits];
+  ps += blockIdx.y * W * stride;
+  pi += blockIdx.y * W * stride;
+  out_idx += blockIdx.y * stride;
+  out_sim += blockIdx.y * stride;
+  splits = min(splits - (int)blockIdx.y * W, W);
+  int head[W];
+  float hs[W];
+  int hi[W];
 #pragma unroll
-  for (int s = 0; s < kMaxSplits; ++s) {
+  for (int s = 0; s < W; ++s) {
     head[s] = 0;
     hs[s] = -INFINITY;
     hi[s] = INT_MAX;
@@ -425,20 +437,18 @@ knn_merge_kernel(const float* __restrict__ ps, const int* __restrict__ pi, int n
     }
   }
   for (int o = 0; o < k; ++o) {
+    // the best head, carried in scalars: the arrays are indexed by unrolled constants only, so they
+    // stay in registers
     int best = 0;
-#pragma unroll
-    for (int s = 1; s < kMaxSplits; ++s)
-      if (s < splits && beats(hs[s], hi[s], hs[best], hi[best])) best = s;
-    // (best indexes registers only through the unrolled selects below)
     float bs = hs[0];
     int bi = hi[0];
 #pragma unroll
-    for (int s = 1; s < kMaxSplits; ++s)
-      if (s == best) { bs = hs[s]; bi = hi[s]; }
+    for (int s = 1; s < W; ++s)
+      if (s < splits && beats(hs[s], hi[s], bs, bi)) { best = s; bs = hs[s]; bi = hi[s]; }
     out_sim[base + o] = bs;
     out_idx[base + o] = bi;
 #pragma unroll
-    for (int s = 0; s < kMaxSplits; ++s) {
+    for (int s = 0; s < W; ++s) {
       if (s == best) {
         ++head[s];
         hs[s] = head[s] < k ? ps[s * stride + base + head[s]] : -INFINITY;
@@ -475,10 +485,43 @@ KnnLayout knn_layout(int nq, int nx, int d, int k, int dtype) {
   return l;
 }
 
+// acnn_knn_search: up to one column split per SM, reduced by passes of kMergeFanIn-way merges
+constexpr int kMaxSearchSplits = kMaxSms;
+constexpr int kMergeFanIn = 16;
+
+int search_max_splits(int nx) { return std::min(ceil_div(nx, kCols), kMaxSearchSplits); }
+
+// The prepared index (X' [nx][K'], then |x|^2 [nx]) and the search work (Q' [nq][K'], |q|^2 [nq],
+// the per-split lists, the lists of the first merge pass when there is more than one pass)
+struct SearchLayout {
+  int dp, planes;
+  int64_t kp, xn, index_total;                    // index
+  int64_t qn, ps, pi, ms, mi, total;              // work
+};
+
+SearchLayout search_layout(int nq, int nx, int d, int k, int dtype) {
+  SearchLayout l;
+  l.dp = (d + kStageK - 1) / kStageK * kStageK;
+  l.planes = dtype == ACNN_F32 ? 6 : 1;
+  l.kp = (int64_t)l.planes * l.dp;
+  l.xn = align256((int64_t)nx * l.kp * 2);
+  l.index_total = align256(l.xn + (int64_t)nx * 4);
+  const int64_t lists = (int64_t)search_max_splits(nx);
+  const int64_t mlists = lists > kMergeFanIn ? ceil_div64(lists, kMergeFanIn) : 0;
+  l.qn = align256((int64_t)nq * l.kp * 2);
+  l.ps = align256(l.qn + (int64_t)nq * 4);
+  l.pi = align256(l.ps + lists * nq * k * 4);
+  l.ms = align256(l.pi + lists * nq * k * 4);
+  l.mi = align256(l.ms + mlists * nq * k * 4);
+  l.total = align256(l.mi + mlists * nq * k * 4);
+  return l;
+}
+
 // Column splits: forced by acnn_set_knn_splits, else the count that minimises
-// waves x (tiles per split + 1 tile of pipeline fill and list writes) with one CTA per SM
-int knn_splits(int q_blocks, int col_tiles) {
-  const int cap = std::min(col_tiles, kMaxSplits);
+// waves x (tiles per split + 1 tile of pipeline fill and list writes) with one CTA per SM;
+// at most max_splits (kMaxSplits for acnn_knn_topk)
+int knn_splits(int q_blocks, int col_tiles, int max_splits = kMaxSplits) {
+  const int cap = std::min(col_tiles, max_splits);
   int s = g_knn_splits;
   if (s <= 0) {
     int64_t best = INT64_MAX;
@@ -503,6 +546,84 @@ int knn_check(int nq, int nx, int d, int k, int metric, int dtype) {
   }
   ACNN_REQUIRE(k <= nx, "knn_topk: k=%d exceeds the %d index rows", k, nx);
   return ACNN_OK;
+}
+
+
+// knn_prep_kernel over nq query rows and nx index rows (either may be 0)
+int knn_prep(const float* q, const float* x, int nq, int nx, int d, int dp, int planes, int metric, bool f16,
+             void* qp, void* xp, float* qn, float* xn, cudaStream_t st) {
+  const int cosine = metric == 0 ? 1 : 0;
+  if (f16) {
+    launch_k(knn_prep_kernel<__half>, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, dp, planes,
+             cosine, static_cast<__half*>(qp), static_cast<__half*>(xp), qn, xn);
+  } else {
+    launch_k(knn_prep_kernel<bf16>, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, dp, planes,
+             cosine, static_cast<bf16*>(qp), static_cast<bf16*>(xp), qn, xn);
+  }
+  return check_launch("knn_prep_kernel");
+}
+
+// knn_topk_kernel over prepared operands (Q' [nq][kp], X' [nx][kp] and their squared norms) in up to
+// max_splits column splits, then the merges of the per-split lists (ps / pi, [splits][nq][k]) into
+// out: one pass of kMaxSplits-way merges when max_splits <= kMaxSplits, else passes of
+// kMergeFanIn-way merges through ms / mi ([ceil(splits / kMergeFanIn)][nq][k]) and back.
+// `launches` counts the launches before this one (the prep).
+int knn_run(const void* qp, const void* xp, const float* qn, const float* xn, int nq, int nx, int kp, int k,
+            int metric, bool f16, int max_splits, float* ps, int* pi, float* ms, int* mi, int32_t* out_idx,
+            float* out_sim, cudaStream_t st, int launches) {
+  int rc;
+  auto* topk = f16 ? knn_topk_kernel<true> : knn_topk_kernel<false>;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[f16]) {
+    cudaError_t e = cudaFuncSetAttribute(topk, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    if (e != cudaSuccess) {
+      set_error("cudaFuncSetAttribute(knn_topk): %s", cudaGetErrorString(e));
+      return ACNN_ERR_CUDA;
+    }
+    attr_set[f16] = true;
+  }
+  CUtensorMap tmQ, tmX;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  if ((rc = make_map_2d(&tmQ, qp, nq, kp, kp, kRows, kStageK, dt))) return rc;
+  if ((rc = make_map_2d(&tmX, xp, nx, kp, kp, kCols, kStageK, dt))) return rc;
+
+  KnnParams p;
+  p.nq = nq;
+  p.nx = nx;
+  p.kp = kp;
+  p.k = k;
+  p.euclid = metric == 1;
+  p.col_tiles = ceil_div(nx, kCols);
+  const int q_blocks = ceil_div(nq, kRows);
+  const int splits_req = knn_splits(q_blocks, p.col_tiles, max_splits);
+  p.tiles_per_split = ceil_div(p.col_tiles, splits_req);
+  const int splits = ceil_div(p.col_tiles, p.tiles_per_split);   // no empty split
+  p.qn = qn;
+  p.xn = xn;
+  p.part_sim = ps;
+  p.part_idx = pi;
+  launch_k(topk, dim3(q_blocks, splits), dim3(kThreads), kSmemBytes, st, tmQ, tmX, p);
+  if ((rc = check_launch("knn_topk_kernel"))) return rc;
+
+  const int fan_in = max_splits <= kMaxSplits ? kMaxSplits : kMergeFanIn;
+  auto* merge = fan_in == kMaxSplits ? knn_merge_kernel<kMaxSplits> : knn_merge_kernel<kMergeFanIn>;
+  const float* ls = ps;
+  const int* li = pi;
+  int lists = splits;
+  launches += 2;
+  for (bool to_m = true; lists > fan_in; to_m = !to_m, ++launches) {
+    const int groups = ceil_div(lists, fan_in);
+    float* os = to_m ? ms : ps;
+    int* oi = to_m ? mi : pi;
+    launch_k(merge, dim3(ceil_div(nq, 128), groups), dim3(128), 0, st, ls, li, nq, k, lists, oi, os);
+    if ((rc = check_launch("knn_merge_kernel"))) return rc;
+    ls = os;
+    li = oi;
+    lists = groups;
+  }
+  launch_k(merge, dim3(ceil_div(nq, 128)), dim3(128), 0, st, ls, li, nq, k, lists, out_idx, out_sim);
+  count_launch(launches);
+  return check_launch("knn_merge_kernel");
 }
 
 }  // namespace
@@ -534,58 +655,66 @@ int acnn_knn_topk(const float* q, const float* x, int nq, int nx, int d, int k, 
   if ((rc = load_driver_fns())) return rc;
   // fp16 mode (ACNN_F16): fp16 operands, wgmma .f16.f16, fp32 accumulation; the rest is shared
   const bool f16 = dtype == ACNN_F16;
-  auto* topk = f16 ? knn_topk_kernel<true> : knn_topk_kernel<false>;
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[f16]) {
-    cudaError_t e = cudaFuncSetAttribute(topk, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) {
-      set_error("cudaFuncSetAttribute(knn_topk): %s", cudaGetErrorString(e));
-      return ACNN_ERR_CUDA;
-    }
-    attr_set[f16] = true;
-  }
   uint8_t* w = static_cast<uint8_t*>(work);
   float* qn = reinterpret_cast<float*>(w + l.qn);
   float* xn = reinterpret_cast<float*>(w + l.xn);
-  CUtensorMap tmQ, tmX;
-  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  if ((rc = make_map_2d(&tmQ, w + l.q, nq, l.kp, l.kp, kRows, kStageK, dt))) return rc;
-  if ((rc = make_map_2d(&tmX, w + l.x, nx, l.kp, l.kp, kCols, kStageK, dt))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if ((rc = knn_prep(q, x, nq, nx, d, l.dp, l.planes, metric, f16, w + l.q, w + l.x, qn, xn, st))) return rc;
+  float* ps = reinterpret_cast<float*>(w + l.ps);
+  int* pi = reinterpret_cast<int*>(w + l.pi);
+  return knn_run(w + l.q, w + l.x, qn, xn, nq, nx, (int)l.kp, k, metric, f16, kMaxSplits, ps, pi, ps, pi,
+                 out_idx, out_sim, st, 1);
+}
 
-  if (f16) {
-    launch_k(knn_prep_kernel<__half>, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, l.dp,
-             l.planes, metric == 0 ? 1 : 0, reinterpret_cast<__half*>(w + l.q),
-             reinterpret_cast<__half*>(w + l.x), qn, xn);
-  } else {
-    launch_k(knn_prep_kernel<bf16>, dim3(ceil_div(nq + nx, 8)), dim3(256), 0, st, q, x, nq, nx, d, l.dp,
-             l.planes, metric == 0 ? 1 : 0, reinterpret_cast<bf16*>(w + l.q), reinterpret_cast<bf16*>(w + l.x),
-             qn, xn);
-  }
-  if ((rc = check_launch("knn_prep_kernel"))) return rc;
+int64_t acnn_knn_index_bytes(int nx, int d, int dtype) {
+  if (acnn::knn_check(1, nx, d, 1, 0, dtype) != ACNN_OK) return -1;
+  return acnn::search_layout(1, nx, d, 1, dtype).index_total;
+}
 
-  KnnParams p;
-  p.nq = nq;
-  p.nx = nx;
-  p.kp = (int)l.kp;
-  p.k = k;
-  p.euclid = metric == 1;
-  p.col_tiles = ceil_div(nx, kCols);
-  const int q_blocks = ceil_div(nq, kRows);
-  const int splits_req = knn_splits(q_blocks, p.col_tiles);
-  p.tiles_per_split = ceil_div(p.col_tiles, splits_req);
-  const int splits = ceil_div(p.col_tiles, p.tiles_per_split);   // no empty split
-  p.qn = qn;
-  p.xn = xn;
-  p.part_sim = reinterpret_cast<float*>(w + l.ps);
-  p.part_idx = reinterpret_cast<int*>(w + l.pi);
-  launch_k(topk, dim3(q_blocks, splits), dim3(kThreads), kSmemBytes, st, tmQ, tmX, p);
-  if ((rc = check_launch("knn_topk_kernel"))) return rc;
+int acnn_knn_prepare_index(const float* x, int nx, int d, int metric, int dtype, void* index,
+                           int64_t index_bytes, void* stream) {
+  using namespace acnn;
+  int rc = knn_check(1, nx, d, 1, metric, dtype);
+  if (rc) return rc;
+  ACNN_REQUIRE(x && index, "knn_prepare_index: null pointer");
+  const SearchLayout l = search_layout(1, nx, d, 1, dtype);
+  ACNN_REQUIRE(index_bytes >= l.index_total, "knn_prepare_index: index of %lld bytes, %lld needed",
+               (long long)index_bytes, (long long)l.index_total);
+  ACNN_REQUIRE(reinterpret_cast<uintptr_t>(index) % 256 == 0,
+               "knn_prepare_index: index must be 256-byte aligned");
+  uint8_t* ix = static_cast<uint8_t*>(index);
+  count_launch(1);
+  return knn_prep(nullptr, x, 0, nx, d, l.dp, l.planes, metric, dtype == ACNN_F16, nullptr, ix,
+                  nullptr, reinterpret_cast<float*>(ix + l.xn), static_cast<cudaStream_t>(stream));
+}
 
-  launch_k(knn_merge_kernel, dim3(ceil_div(nq, 128)), dim3(128), 0, st, p.part_sim, p.part_idx, nq,
-           k, splits, out_idx, out_sim);
-  count_launch(3);
-  return check_launch("knn_merge_kernel");
+int64_t acnn_knn_search_work_bytes(int nq, int nx, int d, int k, int dtype) {
+  if (acnn::knn_check(nq, nx, d, k, 0, dtype) != ACNN_OK) return -1;
+  return acnn::search_layout(nq, nx, d, k, dtype).total;
+}
+
+int acnn_knn_search(const float* q, int nq, const void* index, int nx, int d, int k, int metric, int dtype,
+                    int32_t* out_idx, float* out_sim, void* work, int64_t work_bytes, void* stream) {
+  using namespace acnn;
+  int rc = knn_check(nq, nx, d, k, metric, dtype);
+  if (rc) return rc;
+  ACNN_REQUIRE(q && index && out_idx && out_sim && work, "knn_search: null pointer");
+  const SearchLayout l = search_layout(nq, nx, d, k, dtype);
+  ACNN_REQUIRE(work_bytes >= l.total, "knn_search: work of %lld bytes, %lld needed",
+               (long long)work_bytes, (long long)l.total);
+  ACNN_REQUIRE(reinterpret_cast<uintptr_t>(work) % 256 == 0 && reinterpret_cast<uintptr_t>(index) % 256 == 0,
+               "knn_search: work and index must be 256-byte aligned");
+  if ((rc = load_driver_fns())) return rc;
+  const bool f16 = dtype == ACNN_F16;
+  uint8_t* w = static_cast<uint8_t*>(work);
+  const uint8_t* ix = static_cast<const uint8_t*>(index);
+  float* qn = reinterpret_cast<float*>(w + l.qn);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if ((rc = knn_prep(q, nullptr, nq, 0, d, l.dp, l.planes, metric, f16, w, nullptr, qn, nullptr, st))) return rc;
+  return knn_run(w, ix, qn, reinterpret_cast<const float*>(ix + l.xn), nq, nx, (int)l.kp, k, metric, f16,
+                 std::min(search_max_splits(nx), num_sms()), reinterpret_cast<float*>(w + l.ps),
+                 reinterpret_cast<int*>(w + l.pi), reinterpret_cast<float*>(w + l.ms),
+                 reinterpret_cast<int*>(w + l.mi), out_idx, out_sim, st, 1);
 }
 
 }  // extern "C"

@@ -103,6 +103,73 @@ def knn_topk(query, index, k, similarity="cosine", dtype="bf16"):
     return idx, sim
 
 
+class KnnIndex:
+    """A gallery prepared once on the device for repeated searches (acnn_knn_prepare_index): `embedding`
+    [nx, d] (a CUDA tensor) is l2-normalised ('cosine') and rounded to the operands of `dtype`, as
+    knn_topk does on every call.  search(query, k) returns knn_topk(query, embedding, k, similarity, dtype)
+    bit for bit (acnn_knn_search).  Non-finite gallery rows raise ValueError, as recall_of_index does:
+    their similarities cannot be ranked."""
+
+    def __init__(self, embedding, similarity="cosine", dtype="bf16"):
+        from . import _lib
+        self.lib = lib = _lib.load()
+        if similarity not in SIMILARITIES:
+            raise NotImplementedError("eval_similarity must be one of %s" % sorted(SIMILARITIES))
+        if dtype not in DTYPES:
+            raise ValueError("dtype must be one of %s" % sorted(DTYPES))
+        x = embedding.detach().to(torch.float32).contiguous()
+        if x.dim() != 2 or x.shape[0] < 1 or x.shape[1] < 1:
+            raise ValueError("the gallery must be a non-empty [nx, d] tensor (got %s)" % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise _lib.AcnnError("KnnIndex runs on the GPU: the gallery must be a CUDA tensor")
+        if not bool(torch.isfinite(x).all()):
+            raise ValueError("KnnIndex: the gallery contains NaN or infinite values")
+        self.similarity, self.dtype, self.device = similarity, dtype, x.device
+        self.metric, self.dt = SIMILARITIES[similarity], DTYPES[dtype]
+        self.nx, self.d = x.shape
+        nbytes = lib.acnn_knn_index_bytes(self.nx, self.d, self.dt)
+        self.index = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+        _lib.check(lib.acnn_knn_prepare_index(x.data_ptr(), self.nx, self.d, self.metric, self.dt,
+                                              self.index.data_ptr(), nbytes,
+                                              torch.cuda.current_stream(x.device).cuda_stream),
+                   "acnn_knn_prepare_index")
+
+    def work_bytes(self, nq, k):
+        """Bytes of search's work buffer for nq query rows (-1 for invalid sizes)."""
+        return self.lib.acnn_knn_search_work_bytes(int(nq), self.nx, self.d, int(k), self.dt)
+
+    def search(self, query, k, out=None, work=None):
+        """(indices int32 [nq, k], similarities fp32 [nq, k]) of the CUDA tensor `query` [nq, d], enqueued on
+        the current stream.  `out` (two such contiguous tensors with at least nq rows) and `work` (uint8,
+        at least work_bytes(nq, k), 256-byte aligned) are allocated unless given."""
+        from . import _lib
+        q = query.detach().to(torch.float32).contiguous()
+        if q.dim() != 2 or q.shape[1] != self.d:
+            raise ValueError("query must be [nq, %d] (got %s)" % (self.d, tuple(q.shape)))
+        if not (q.is_cuda and q.device == self.device):
+            raise _lib.AcnnError("KnnIndex.search: the query must be a CUDA tensor on %s" % self.device)
+        nq = q.shape[0]
+        nbytes = self.work_bytes(nq, k)
+        if nbytes < 0:       # the library's argument check names the problem
+            _lib.check(self.lib.acnn_knn_search(None, nq, None, self.nx, self.d, k, self.metric, self.dt, None,
+                                                None, None, 0, None), "acnn_knn_search")
+        if work is None:
+            work = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+        if out is None:
+            out = (torch.empty(nq, k, dtype=torch.int32, device=q.device),
+                   torch.empty(nq, k, dtype=torch.float32, device=q.device))
+        idx, sim = out
+        for t, dt in ((idx, torch.int32), (sim, torch.float32)):
+            if t.dtype != dt or t.shape[0] < nq or t.shape[1:] != (k,) or not t.is_contiguous():
+                raise ValueError("out must be contiguous (int32, float32) [>= %d, %d] tensors" % (nq, k))
+        _lib.check(self.lib.acnn_knn_search(q.data_ptr(), nq, self.index.data_ptr(), self.nx, self.d, k,
+                                            self.metric, self.dt, idx.data_ptr(), sim.data_ptr(),
+                                            work.data_ptr(), work.numel(),
+                                            torch.cuda.current_stream(q.device).cuda_stream),
+                   "acnn_knn_search")
+        return idx[:nq], sim[:nq]
+
+
 def recall_from_sorted_idx(sorted_idx, query_labels, labels, k_list=(1, 5)):
     """get_recall (metric/recall_metric.py:217-228) as tensor ops on the device of `sorted_idx`:
     query q's list drops the entries equal to q's position among the queries, and a hit is q's label

@@ -27,7 +27,7 @@ from __future__ import annotations
 
 import os
 import math
-from collections import deque, namedtuple
+from collections import OrderedDict, deque, namedtuple
 
 import numpy as np
 import torch
@@ -1439,12 +1439,55 @@ class _PredictDevice(_ResizedEvalPipeline):
         self.copies = 0
         self.pending = deque()       # (event, pinned set, rows) of the enqueued copies not yet delivered
         self.sink = None
+        # gallery search (Servable.search): the index and k of the current call, one set of buffers sized
+        # for the largest k seen (work, device outputs, pinned host ring), and the graphs of each k apart
+        # (self.graphs is the current k's set) for the SEARCH_KS most recently used k
+        self.knn, self.k, self.k_cap = None, 0, 0
+        self.search_bufs = None
+        self.graph_sets = OrderedDict({0: self.graphs})
+
+    SEARCH_KS = 4
+
+    def use_search(self, knn, k):
+        """Run the gallery search of k neighbours (a metrics.KnnIndex; None, 0: none) after each forward.  A
+        call without a search leaves the search's buffers and graphs in place for the next one."""
+        if knn is not None and knn is not self.knn:      # a new gallery: the old one's buffers and graphs go
+            self._drop_search()
+            self.knn, self.k_cap = knn, 0
+        if k > self.k_cap:                               # larger buffers: the graphs holding the old ones go
+            self._drop_search()
+            work = torch.empty(knn.work_bytes(self.batch, k), dtype=torch.uint8, device=self.dev)
+            dev_out = (torch.zeros(self.batch * k, dtype=torch.int32, device=self.dev),
+                       torch.zeros(self.batch * k, dtype=torch.float32, device=self.dev))
+            host = [[torch.zeros(t.shape, dtype=t.dtype).pin_memory() for t in dev_out] for _ in range(self.OUT_RING)]
+            self.search_bufs, self.k_cap = (work, dev_out, host), k
+        self.k = k
+        if k not in self.graph_sets:
+            if len(self.graph_sets) > self.SEARCH_KS:    # the least recently used k's graphs go
+                del self.graph_sets[next(kk for kk in self.graph_sets if kk)]
+            self.graph_sets[k] = {}
+            self.warm = False            # its first batch runs eagerly, before any capture
+        self.graph_sets.move_to_end(k)
+        self.graphs = self.graph_sets[k]
+
+    def _drop_search(self):
+        self.graph_sets = OrderedDict({0: self.graph_sets[0]})
+        self.search_bufs = None
+
+    def _search_out(self):
+        """The device outputs (int32, fp32 [batch, k]) and pinned host ring of the current k."""
+        _, dev_out, host = self.search_bufs
+        n = self.batch * self.k
+        return ([t[:n].view(self.batch, self.k) for t in dev_out],
+                [[t[:n].view(self.batch, self.k) for t in h] for h in host])
 
     def _outputs(self, n_valid):
         from .metrics import predict_rows
         predict_rows(self.logits, n_valid, self.out[:3])
         if self.feat is not None:
             self.out[3].copy_(self.feat)
+        if self.k:
+            self.knn.search(self.out[3][:n_valid], self.k, out=self._search_out()[0], work=self.search_bufs[0])
 
     def _body(self, slot, n_valid):
         _, _, desc = self.slots[slot]
@@ -1467,9 +1510,12 @@ class _PredictDevice(_ResizedEvalPipeline):
     def _copy_out(self, n):
         while len(self.pending) >= self.OUT_RING:
             self._deliver()
-        host = self.host_out[self.copies % self.OUT_RING]
+        host, dev = self.host_out[self.copies % self.OUT_RING], self.out
+        if self.k:
+            dev_out, ring = self._search_out()
+            host, dev = host + ring[self.copies % self.OUT_RING], dev + dev_out
         self.copies += 1
-        for h, d in zip(host, self.out):
+        for h, d in zip(host, dev):
             h[:n].copy_(d[:n], non_blocking=True)
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.dev))
@@ -1527,7 +1573,12 @@ class Servable:
     max_batch = max(batch_sizes) rows run on the largest rung and its remainder on the smallest rung that
     holds it (ladder_chunks), so a small request costs a small forward.  Every rung gives each image the
     bits the largest gives it (the SK / SE attention GEMMs of the smaller rungs split K as max_batch rows
-    would: acnn_set_fc_split_rows).  None: the one rung max_batch."""
+    would: acnn_set_fc_split_rows).  None: the one rung max_batch.
+
+    Image search: set_gallery(embedding, labels) gives a servable with an embedding output a gallery, and
+    search / search_images return the PREDICT dict plus each image's k nearest gallery rows.  The search
+    runs on the device in the same CUDA graph as the forward of each chunk (metrics.KnnIndex, prepared
+    once in the model's dtype), and only the valid rows' neighbours are copied back."""
 
     def __init__(self, model, *, preprocessing_type="imagenet", image_size=224, use_resnet_d=None,
                  return_embedding=False, max_batch=256, signature="binary_input", decoder_type="jpeg",
@@ -1542,6 +1593,92 @@ class Servable:
         self.signature, self.decoder_type = signature, decoder_type
         self.outputs = PREDICT_OUTPUTS + (("embedding",) if self.embedding else ())
         self._pipes = {}             # rung -> _PredictDevice
+        self._width = None
+        self._gallery = None         # (fp32 [nx, d] tensor, similarity) until the first search prepares it
+        self._index = None           # metrics.KnnIndex
+        self.gallery_labels = None
+
+    @property
+    def embedding_width(self):
+        """The width of the embedding output, from the host plan (no GPU work)."""
+        if self._width is None:
+            cfg = ModelConfig(use_resnet_d=self.use_resnet_d, **self.model.cfg_kwargs)
+            plan = build_plan(cfg, 1, self.size, self.size, training=False)
+            t = plan.tensors[plan.meta["embedding"] if "embedding" in plan.meta else plan.meta["pooled"]]
+            self._width = int(np.prod(t.shape[1:]))
+        return self._width
+
+    @property
+    def gallery_rows(self):
+        """The rows of the gallery (0 without one)."""
+        return 0 if self._gallery is None and self._index is None else \
+            (self._index.nx if self._index is not None else int(self._gallery[0].shape[0]))
+
+    def set_gallery(self, embedding, labels=None, similarity="cosine"):
+        """Replaces the gallery that search ranks: `embedding` [nx, d] (numpy or torch; d = the embedding's
+        width), optional int `labels` [nx] returned as neighbor_labels, similarity 'cosine' or 'euclidean'
+        (metrics.knn_topk).  A servable without an embedding output, a width that is not the embedding's,
+        labels of another length and non-finite rows raise here; the gallery is prepared on the device (in
+        the model's dtype) by the first search."""
+        from .metrics import SIMILARITIES
+        if not self.embedding:
+            raise ValueError("set_gallery: the servable has no embedding output; export with return_embedding=True")
+        if similarity not in SIMILARITIES:
+            raise NotImplementedError("similarity must be one of %s" % sorted(SIMILARITIES))
+        emb = torch.as_tensor(embedding).detach().to(torch.float32)
+        if emb.dim() != 2 or emb.shape[0] < 1 or emb.shape[1] != self.embedding_width:
+            raise ValueError("set_gallery: the gallery must be [nx >= 1, %d] like the embedding (got %s)"
+                             % (self.embedding_width, tuple(emb.shape)))
+        if labels is not None:
+            labels = np.asarray(torch.as_tensor(labels).cpu(), np.int64).reshape(-1)
+            if len(labels) != emb.shape[0]:
+                raise ValueError("set_gallery: %d labels for %d gallery rows" % (len(labels), emb.shape[0]))
+        if not bool(torch.isfinite(emb).all()):
+            raise ValueError("set_gallery: the gallery contains NaN or infinite values")
+        self._gallery, self._index, self.gallery_labels = (emb, similarity), None, labels
+
+    def _check_k(self, k):
+        from .metrics import KNN_MAX_K
+        if self._gallery is None and self._index is None:
+            raise ValueError("search: no gallery; call set_gallery first")
+        top = min(KNN_MAX_K, self.gallery_rows)
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= top:
+            raise ValueError("search: k must be an int in [1, %d] (got %r)" % (top, k))
+        return int(k)
+
+    def _knn_index(self):
+        from .metrics import KnnIndex
+        if self._index is None:
+            emb, similarity = self._gallery
+            with torch.cuda.device(self.model.device):
+                self._index = KnnIndex(emb.to(self.model.device), similarity, self.model.dtype)
+            self._gallery = None
+        return self._index
+
+    def _neighbors(self, res, k):
+        idx = res.pop("neighbors_i32", None)
+        res["neighbors"] = np.zeros((0, k), np.int64) if idx is None else idx.astype(np.int64)
+        if res["neighbor_similarities"] is None:
+            res["neighbor_similarities"] = np.zeros((0, k), np.float32)
+        if self.gallery_labels is not None:
+            nb = res["neighbors"]
+            ok = nb < len(self.gallery_labels)      # the padding of a query with fewer than k finite similarities
+            res["neighbor_labels"] = np.where(ok, self.gallery_labels[np.where(ok, nb, 0)], -1)
+        return res
+
+    def search(self, images, k):
+        """predict(images) plus each image's k nearest gallery rows, nearest first (ties: lower row first):
+        'neighbors' int64 [n, k], 'neighbor_similarities' float32 [n, k] and, with gallery labels,
+        'neighbor_labels' int64 [n, k] -- equal to metrics.knn_topk(embedding, gallery, k) in the model's
+        dtype.  A query with fewer than k finite similarities gets neighbours 2147483647 (label -1) at
+        similarity -inf.  k outside [1, min(128, gallery rows)] and a missing gallery raise first."""
+        k = self._check_k(k)
+        return self._neighbors(self._predict(images, k), k)
+
+    def search_images(self, images, k):
+        """search for float32 [n, S, S, 3] images already preprocessed (predict_images)."""
+        k = self._check_k(k)
+        return self._neighbors(self._predict_images(images, k), k)
 
     @property
     def _pipe(self):
@@ -1556,18 +1693,20 @@ class Servable:
             self._pipes[batch] = pipe
         return pipe
 
-    def _empty(self, n):
+    def _empty(self, n, names):
         nc = self.model.num_classes
         res = {"classes": np.zeros(n, np.int64), "probabilities": np.zeros((n, nc), np.float32),
                "probabilities_sigmoid": np.zeros((n, nc), np.float32)}
-        if self.embedding:
-            res["embedding"] = None          # its width is the runtime's: set by the first delivery
+        for name in names[3:]:
+            res[name] = None                 # its width is the runtime's: set by the first delivery
         return res
 
-    def _collect(self, n, run):
+    def _collect(self, n, run, k=0):
         """Runs run(pipeline, start, stop) for every chunk of the n rows on its rung (ladder_chunks) and
-        returns the outputs of the n rows, delivered in order."""
-        res, pos = self._empty(n), 0
+        returns the outputs of the n rows, delivered in order; with k, the gallery search's too."""
+        names = self.outputs + (("neighbors_i32", "neighbor_similarities") if k else ())
+        knn = self._knn_index() if k and n else None
+        res, pos = self._empty(n, names), 0
         if n == 0:
             if self.embedding:
                 res["embedding"] = np.zeros((0, 0), np.float32)
@@ -1575,12 +1714,12 @@ class Servable:
 
         def sink(arrays):
             nonlocal pos
-            k = len(arrays[0])
-            for name, a in zip(self.outputs, arrays):
+            rows = len(arrays[0])
+            for name, a in zip(names, arrays):
                 if res[name] is None:
                     res[name] = np.zeros((n,) + a.shape[1:], a.dtype)
-                res[name][pos:pos + k] = a
-            pos += k
+                res[name][pos:pos + rows] = a
+            pos += rows
 
         pipe = None
         try:
@@ -1589,6 +1728,7 @@ class Servable:
                     pipe.finish()            # the rows of the previous rung are delivered first
                 pipe = self._rung(rung)
                 pipe.sink = sink
+                pipe.use_search(knn, k)
                 run(pipe, a, b)
             pipe.finish()
         except BaseException:
@@ -1605,6 +1745,9 @@ class Servable:
         where the device decoder handles it, by PIL otherwise, and given the eval preprocessing of the
         servable's preprocessing_type (imagenet_eval.eval_geometry); a chunk's decode runs on the copy stream
         while the previous chunk computes."""
+        return self._predict(images, 0)
+
+    def _predict(self, images, k):
         from .imagenet_eval import eval_geometry
         images = list(images)
         for i, b in enumerate(images):
@@ -1617,17 +1760,20 @@ class Servable:
 
         def run(pipe, a, b):
             pipe.run_batch_encoded(images[a:b], [0] * (b - a), geometry)
-        return self._collect(len(images), run)
+        return self._collect(len(images), run, k)
 
     def predict_images(self, images):
         """The PREDICT dict of float32 [n, S, S, 3] images already preprocessed (S: the eval size of the
         servable's preprocessing_type), numpy or torch."""
+        return self._predict_images(images, 0)
+
+    def _predict_images(self, images, k):
         x = torch.as_tensor(images)
         S = self.size
         if x.dim() != 4 or tuple(x.shape[1:]) != (S, S, 3):
             raise ValueError("predict_images: images must be [n, %d, %d, 3] (got %s)" % (S, S, tuple(x.shape)))
         x = x.to(torch.float32)
-        return self._collect(x.shape[0], lambda pipe, a, b: pipe.run_images(x[a:b]))
+        return self._collect(x.shape[0], lambda pipe, a, b: pipe.run_images(x[a:b]), k)
 
 
 def _variable_names(cfg_kwargs, use_resnet_d, size):
@@ -1741,7 +1887,8 @@ def read_servable_config(path):
 def load_servable(path, *, device=None, max_batch=256, batch_sizes=None):
     """The Servable of a directory export_model wrote: a new Model of the directory's flags and dtype with
     its variables (on `device`, default the current CUDA device), on the rungs batch_sizes (Servable).
-    Host work only: the device work starts with the first predict."""
+    Host work only: the device work starts with the first predict.  The directory's gallery.npz
+    (export_gallery), when present, becomes the servable's cosine gallery (Servable.set_gallery)."""
     from .checkpoint import load_checkpoint
     from .imagenet_eval import eval_size
     check_batch_sizes(batch_sizes, max_batch)
@@ -1755,9 +1902,61 @@ def load_servable(path, *, device=None, max_batch=256, batch_sizes=None):
     if missing:
         raise ValueError("%s: variables.npz lacks %d variable(s), e.g. %s" % (path, len(missing), missing[:3]))
     model.set_weights({n: torch.as_tensor(weights[n]) for n in names})
-    return Servable(model, preprocessing_type=cfg["preprocessing_type"], image_size=cfg["image_size"],
-                    use_resnet_d=model.use_resnet_d, return_embedding=cfg["return_embedding"], max_batch=max_batch,
-                    signature=cfg["signature"], decoder_type=cfg["decoder_type"], batch_sizes=batch_sizes)
+    sv = Servable(model, preprocessing_type=cfg["preprocessing_type"], image_size=cfg["image_size"],
+                  use_resnet_d=model.use_resnet_d, return_embedding=cfg["return_embedding"], max_batch=max_batch,
+                  signature=cfg["signature"], decoder_type=cfg["decoder_type"], batch_sizes=batch_sizes)
+    gallery = os.path.join(path, GALLERY_FILE)
+    if os.path.isfile(gallery):
+        with np.load(gallery) as g:
+            sv.set_gallery(g["embedding"], g["label"])
+    return sv
+
+
+GALLERY_FILE = "gallery.npz"
+
+
+def export_gallery(binary_dir, data_dir, *, val_regex="validation-*", batch_size=256, num_workers=None):
+    """The image-search gallery of the exported binary_input servable at binary_dir: every record of the
+    validation shards data_dir/val_regex (read as export_test reads them) embedded by the servable's own
+    model, preprocessing and image size (the retrieval evaluation's loop, in batches of batch_size).  Writes
+    binary_dir/gallery.npz, which load_servable loads, and returns its path: 'embedding' float32 [N, d],
+    'label' int64 [N] (-1 for a record without one), 'shard' int32 [N] (the record's shard, an index into
+    'shard_names', the sorted shard file names) and 'record' int64 [N] (its position in that shard), so that
+    a neighbour maps back to its record.  A servable without an embedding output, an existing gallery.npz,
+    an empty glob and a corrupt record raise before any GPU work.  The file is written under a hidden name
+    and renamed when complete."""
+    from . import imagenet_eval as ie
+    target = os.path.join(binary_dir, GALLERY_FILE)
+    if os.path.lexists(target) or os.path.lexists(_partial(target)):
+        raise FileExistsError("export_gallery: %s already exists" % target)
+    sv = load_servable(binary_dir, max_batch=batch_size)
+    if not sv.embedding:
+        raise ValueError("export_gallery: the servable has no embedding output; export with return_embedding=True")
+    files = ie.validation_files(data_dir, val_regex)
+    records, shard, record = [], [], []
+    for i, path in enumerate(files):
+        for j, (label, offset, length) in enumerate(ie.read_records(path, missing_label=-1)):
+            records.append((path, offset, length, label))
+            shard.append(i)
+            record.append(j)
+    if not records:
+        raise ValueError("export_gallery: the shards under %s hold no record" % data_dir)
+    index, labels = _retrieval_index(sv.model, records, sv.size, sv.max_batch, sv.preprocessing_type,
+                                     sv.image_size, True, sv.use_resnet_d, True, num_workers)
+    tmp = _partial(target)
+    try:
+        with open(tmp, "wb") as f:
+            np.savez(f, embedding=index.cpu().numpy(), label=labels.cpu().numpy(),
+                     shard=np.asarray(shard, np.int32), record=np.asarray(record, np.int64),
+                     shard_names=np.asarray([os.path.basename(p) for p in files]))
+            f.flush()
+            os.fsync(f.fileno())
+        os.rename(tmp, target)
+    except BaseException:
+        if os.path.lexists(tmp):
+            os.remove(tmp)
+        raise
+    return target
 
 
 def export_recall_at_1(embedding, labels, device=None):

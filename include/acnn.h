@@ -530,6 +530,27 @@ int64_t acnn_knn_work_bytes(int nq, int nx, int d, int k, int dtype);
  * [1, min(8, ceil(nx / 128))]; 0 (default) = the cost model that fills the SMs.  Returns the previous
  * setting. */
 int acnn_set_knn_splits(int n);
+/* Search of a prepared index, for serving: the prep of X is run once (acnn_knn_prepare_index) and
+ * each query batch prepares only its own rows (acnn_knn_search).
+ * acnn_knn_prepare_index: X[nx][d] (fp32) -> `index`, caller-owned, 256-byte aligned, of
+ * acnn_knn_index_bytes(nx, d, dtype) bytes: X' [nx][K'] then, at the next 256-byte boundary, |x|^2 fp32
+ * [nx], the formats of acnn_knn_topk's work sections (metric as there: 0 cosine, 1 euclidean).
+ * acnn_knn_search: for every row of Q[nq][d] (fp32) the k best rows of a prepared index, which must
+ * have been prepared with the same nx, d, metric and dtype.  Results, padding and argument rules are
+ * acnn_knn_topk's, and equal to acnn_knn_topk(Q, X) bit for bit.  The index is read only, so one index
+ * may serve concurrent searches with separate work buffers.  The column splits come from acnn_knn_topk's
+ * cost model (acnn_set_knn_splits applies too) with up to one split per SM: at most min(SMs, 132,
+ * ceil(nx / 128)).  work: acnn_knn_search_work_bytes(...) bytes, caller-owned, 256-byte aligned:
+ *   Q' [nq][K'], |q|^2 fp32 [nq], partial lists: similarity fp32 [S][nq][k], index int32 [S][nq][k]
+ *   (S = min(132, ceil(nx / 128))), then, when S > 16, the lists of the first 16-way merge pass
+ *   (similarity fp32 [ceil(S / 16)][nq][k], index int32 [ceil(S / 16)][nq][k]).
+ * Both byte counts are host only (callable without a GPU); -1 for invalid sizes. */
+int64_t acnn_knn_index_bytes(int nx, int d, int dtype);
+int acnn_knn_prepare_index(const float* x, int nx, int d, int metric, int dtype, void* index,
+                           int64_t index_bytes, void* stream);
+int64_t acnn_knn_search_work_bytes(int nq, int nx, int d, int k, int dtype);
+int acnn_knn_search(const float* q, int nq, const void* index, int nx, int d, int k, int metric, int dtype,
+                    int32_t* out_idx, float* out_sim, void* work, int64_t work_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Robustness evaluation (mce/eval_robustness.py: ImageNet-C corruption error)
