@@ -119,13 +119,17 @@ static inline int fprop_stage_bytes(int bn, int np) { return np * (kBM * kStageK
 __host__ __device__ constexpr int fprop_epi_cols(int bn, int wg) {
   return wg == 2 ? (bn > 128 ? 128 : bn) : (bn > 64 ? 64 : bn);
 }
-static inline int fprop_stages(int bn, int np, int wg, bool has_add, bool has_mask, bool out_f32) {
+// dynamic shared memory of one conv_gemm_kernel launch, and its pipeline depth in *stages:
+// [stages x (A|B)] [out staging] [add staging] [mask staging]
+static inline int fprop_smem(int bn, int np, int wg, bool has_add, bool has_mask, bool out_f32,
+                             int* stages) {
   const int tile = kBM * fprop_epi_cols(bn, wg) * 2;
   const int fixed = 1024 + (out_f32 ? 0 : tile) + (has_add ? tile : 0) + (has_mask ? tile : 0);
   int st = ((wg == 2 ? kSmemBudget : kSmemBudget2) - fixed) / fprop_stage_bytes(bn, np);
   if (st > kMaxStages) st = kMaxStages;
   if (st < 2) st = 2;
-  return st;
+  *stages = st;
+  return fixed + st * fprop_stage_bytes(bn, np);
 }
 
 template <int BN, int NP = 1, int WG = 2>
@@ -149,14 +153,7 @@ struct FpropCfg {
   // (NP == 3 at BN = 128: acc + acc2 are 128 fp32 registers per thread under the 168-register cap of
   // a 384-thread CTA, so the epilogue spills a few hundred bytes; the fp32 parity mode is a
   // correctness mode, the bf16 path does not spill)
-  // smem: [stages x (A|B)] [out staging] [add staging] [mask staging]
-  static int stages_for(bool has_add, bool has_mask, bool out_f32) {
-    return fprop_stages(BN, NP, WG, has_add, has_mask, out_f32);
-  }
-  static int smem_bytes(int stages, bool has_add, bool has_mask, bool out_f32) {
-    return 1024 + stages * kStageBytes + (out_f32 ? 0 : kTileBytes) + (has_add ? kTileBytes : 0) +
-           (has_mask ? kTileBytes : 0);
-  }
+  // smem layout: fprop_smem
 };
 
 // byte offset of the bf16 pair (row r, column c, c even) of a staged half tile: sub-tiles of kSubW
@@ -1181,6 +1178,9 @@ static int g_conv_out_bufs = 1;
 static int g_conv_split_epi = 1;
 static int g_conv_split_mt2 = 1;
 static int g_conv_mtiles_mode = -1;
+// epilogue organisation of an earlier kernel generation: the sm_90 halo kernel has one (the
+// consumer warpgroups drain their registers); acnn_set_conv_halo_split keeps and returns the value
+static int g_conv_halo_split = 1;
 // CTA pairs (clusters of two sharing the weight stages by TMA multicast): 1 = the N = 128 tiles with
 // K >= 512 and enough tiles for every SM; 0 (default) = single CTAs (acnn_set_conv_cta_pairs).  Off
 // by default: c3 step on an H100 SXM at 700 W, 80.3 ms with pairs against 61.3 ms without
@@ -1190,147 +1190,10 @@ static int g_conv_pairs = 0;
 // traffic from L2 costs more (c3 step on an H100 SXM at 700 W, fprop + dgrad launches: K <= 512
 // 10.9 -> 9.5 ms; K = 576 .. 1024 unchanged; K >= 1152 6.2 -> 7.7 ms)
 constexpr int kTwoCtaMaxK = 512;
-
-// occ != null: report the CTAs of this instantiation that fit one SM at the launch's shared memory
-// (cudaOccupancyMaxActiveBlocksPerMultiprocessor) instead of launching
-template <int BN, int CW, bool IM2COL, int NP, bool CG2, bool F16, int WG>
-static int launch_conv_gemm(const ConvMaps& tm, const ConvGemmParams& p, int per_n,
-                            cudaStream_t stream, int* occ) {
-  using Cfg = FpropCfg<BN, NP, WG>;
-  static bool attr_set = false;
-  auto kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2, F16, WG>;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         WG == 2 ? kSmemBudget + 2048 : kSmemBudget2);
-    // two CTAs per SM need the largest shared-memory carveout
-    if (e == cudaSuccess && WG == 1)
-      e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                               cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) {
-      set_error("cudaFuncSetAttribute(conv_gemm): %s", cudaGetErrorString(e));
-      return ACNN_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  ConvGemmParams q = p;
-  q.stages = Cfg::stages_for(p.has_add, p.has_mask, p.out_f32);
-  q.m_tiles = ceil_div(p.M, (CG2 ? 2 : 1) * kBM);
-  q.n_tiles = p.Cout / BN;
-  const int smem = Cfg::smem_bytes(q.stages, p.has_add, p.has_mask, p.out_f32);
-  if (occ) {
-    const cudaError_t e =
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, conv_threads(WG), smem);
-    if (e != cudaSuccess) {
-      set_error("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_gemm): %s", cudaGetErrorString(e));
-      return ACNN_ERR_CUDA;
-    }
-    return ACNN_OK;
-  }
-  if (CG2) {
-    // per_n CTA PAIRS per N tile, launched as clusters of two
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * per_n * q.n_tiles);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2;
-    at[0].val.clusterDim.y = 1;
-    at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    (void)cudaLaunchKernelEx(&cfg, kern, tm.a[0], tm.b[0], tm.c, tm.add, tm.mask, tm.a[1], tm.a[2],
-                             tm.b[1], tm.b[2], q);
-  } else {
-    launch_k(kern, dim3(per_n * q.n_tiles), dim3(conv_threads(WG)), smem, stream, tm.a[0], tm.b[0],
-             tm.c, tm.add, tm.mask, tm.a[1], tm.a[2], tm.b[1], tm.b[2], q);
-  }
-  count_launch();
-  return check_launch("conv_gemm_kernel");
-}
-
-// Tile shape and persistent grid of one conv GEMM: a pure function of the problem, shared by the
-// launcher and by acnn_conv_stats_parts() (the number of partial statistics rows = per_n).
-struct ConvTiling {
-  int bn;      // N tile
-  int per_n;   // CTAs (pair = 1: CTA pairs) per N tile
-  int pair;    // 1: clusters of two CTAs sharing the weight stages, one 256 x bn tile per pair
-  int wg;      // consumer warpgroups per CTA: 2 = one CTA per SM, 1 = two CTAs per SM
-  int parts;   // rows of the partial statistics buffer (= CTAs per N tile)
-};
-
-static ConvTiling conv_tiling(int M, int Cout, int Ktot, int cw, bool has_add, bool has_mask,
-                              bool out_f32, int np) {
-  (void)has_add;
-  (void)has_mask;
-  ConvTiling t;
-  // N tile <= 128: a 64 x 256 fp32 accumulator per consumer warpgroup (128 registers per thread)
-  // does not fit next to the epilogue under the 168-register limit of a 384-thread CTA
-  t.bn = (Cout % 128 == 0) ? 128 : ((Cout % 64 == 0) ? 64 : 32);
-  // CTA pairs: full-width (64-channel) chunks, K >= 512 (the k-loop, not the epilogue, paces the
-  // tile) and at least one pair tile per SM pair
-  t.pair = (g_conv_pairs && t.bn == 128 && np == 1 && !out_f32 && cw == 64 && Ktot >= 512 &&
-            (int64_t)ceil_div(M, 2 * kBM) * (Cout / 128) >= num_sms() / 2) ? 1 : 0;
-  // bf16 / fp16 operands with K <= kTwoCtaMaxK: two co-resident CTAs per SM on 128 x 64 (Cout % 64
-  // != 0: 128 x 32) tiles -- a 128 x 128 fp32 accumulator does not fit one warpgroup under the 168
-  // registers per thread of two 5-warp CTAs (ptxas spills) -- where that gives >= 2 N tiles (<=
-  // kMaxSms CTAs, i.e. partial statistics rows, per N tile).  The fp32 parity mode's three operand
-  // planes and the CTA pairs keep one CTA per SM.
-  const int bn2 = (Cout % 64 == 0 && Cout >= 128) ? 64 : 32;
-  t.wg = (np == 1 && !t.pair && Cout / bn2 >= 2 && Ktot <= kTwoCtaMaxK) ? 1 : 2;
-  if (t.wg == 1) t.bn = bn2;
-  const int n_tiles = Cout / t.bn;
-  // persistent grid: a multiple of n_tiles so that every CTA keeps one N tile (its weights and
-  // its per-channel statistics), at most one CTA per SM (two with wg = 1)
-  const int m_tiles = ceil_div(M, (t.pair ? 2 : 1) * kBM);
-  t.per_n = (t.pair ? num_sms() / 2 : (t.wg == 1 ? 2 * num_sms() : num_sms())) / n_tiles;
-  if (t.per_n < 1) t.per_n = 1;
-  if (t.per_n > m_tiles) t.per_n = m_tiles;
-  t.parts = t.pair ? 2 * t.per_n : t.per_n;
-  return t;
-}
-
-template <int BN, int NP, bool F16, int WG>
-static int dispatch_conv_cw(int cw, bool im2col, const ConvMaps& tm, const ConvGemmParams& p,
-                            int per_n, cudaStream_t s, int* occ) {
-  if (im2col) {
-    if (cw == 64) return launch_conv_gemm<BN, 64, true, NP, false, F16, WG>(tm, p, per_n, s, occ);
-    if (cw == 32) return launch_conv_gemm<BN, 32, true, NP, false, F16, WG>(tm, p, per_n, s, occ);
-    return launch_conv_gemm<BN, 16, true, NP, false, F16, WG>(tm, p, per_n, s, occ);
-  }
-  if (cw == 64) return launch_conv_gemm<BN, 64, false, NP, false, F16, WG>(tm, p, per_n, s, occ);
-  if (cw == 32) return launch_conv_gemm<BN, 32, false, NP, false, F16, WG>(tm, p, per_n, s, occ);
-  return launch_conv_gemm<BN, 16, false, NP, false, F16, WG>(tm, p, per_n, s, occ);
-}
-
-// f16: fp16 operands and output (ACNN_F16), one plane, the bf16 path's tiles
-template <int BN>
-static int dispatch_conv_gemm(const ConvTiling& t, int np, bool f16, int cw, bool im2col,
-                              const ConvMaps& tm, const ConvGemmParams& p, cudaStream_t s,
-                              int* occ) {
-  if constexpr (BN == 128) {
-    if (t.pair) {     // full-width (64-channel) chunks only: bounds the instantiation count
-      if (f16) {
-        if (im2col) return launch_conv_gemm<128, 64, true, 1, true, true, 2>(tm, p, t.per_n, s, occ);
-        return launch_conv_gemm<128, 64, false, 1, true, true, 2>(tm, p, t.per_n, s, occ);
-      }
-      if (im2col) return launch_conv_gemm<128, 64, true, 1, true, false, 2>(tm, p, t.per_n, s, occ);
-      return launch_conv_gemm<128, 64, false, 1, true, false, 2>(tm, p, t.per_n, s, occ);
-    }
-  }
-  if constexpr (BN <= 128) {
-    if (np == 3) return dispatch_conv_cw<BN, 3, false, 2>(cw, im2col, tm, p, t.per_n, s, occ);
-  }
-  if constexpr (BN <= 64) {
-    if (t.wg == 1) {
-      if (f16) return dispatch_conv_cw<BN, 1, true, 1>(cw, im2col, tm, p, t.per_n, s, occ);
-      return dispatch_conv_cw<BN, 1, false, 1>(cw, im2col, tm, p, t.per_n, s, occ);
-    }
-  }
-  if (f16) return dispatch_conv_cw<BN, 1, true, 2>(cw, im2col, tm, p, t.per_n, s, occ);
-  return dispatch_conv_cw<BN, 1, false, 2>(cw, im2col, tm, p, t.per_n, s, occ);
-}
+// halo (im2col-free 3x3) kernel: 0: off; 1 (default): where the weight slab stays in shared memory
+// and the images are large (the mode 1 rule of conv_choice; c3 step on an H100 SXM at 700 W: 59.8 ms
+// against 61.3 ms with 0); 2: wherever the kernel applies (acnn_set_conv_halo)
+static int g_conv_halo = 1;
 
 static int chunk_width(int cin) { return cin % 64 == 0 ? 64 : (cin % 32 == 0 ? 32 : 16); }
 
@@ -1347,21 +1210,10 @@ static int64_t input_elems(const acnn_conv_geom& g) {
   return (int64_t)g.B * img;
 }
 
-// ---- halo (im2col-free 3x3) kernel: eligibility, tiling, launch --------------------------------
-// 0: off; 1 (default): where the weight slab stays in shared memory and the images are large (the
-// use_halo rule below; c3 step on an H100 SXM at 700 W: 59.8 ms against 61.3 ms with 0); 2: wherever
-// the kernel applies (acnn_set_conv_halo)
-static int g_conv_halo = 1;
-
-static int halo_bn(int Cout) { return Cout % 128 == 0 ? 128 : (Cout % 64 == 0 ? 64 : 32); }
-
 // Shared-memory plan of the halo kernel for one problem (a pure function of the shape).
 struct HaloPlan {
   int a_stages, b_slots, stationary, smem;
 };
-// epilogue organisation of an earlier kernel generation: the sm_90 halo kernel has one (the
-// consumer warpgroups drain their registers); acnn_set_conv_halo_split keeps and returns the value
-static int g_conv_halo_split = 1;
 
 static HaloPlan halo_plan(int bn, int cw, int Cin, bool has_add, bool has_mask) {
   HaloPlan h;
@@ -1387,30 +1239,148 @@ static HaloPlan halo_plan(int bn, int cw, int Cin, bool has_add, bool has_mask) 
   return h;
 }
 
-static bool use_halo(const acnn_conv_geom& g, int np, bool out_f32, bool has_bias, bool has_add,
-                     bool has_mask) {
-  if (g_conv_halo <= 0) return false;
-  const bool applies = g.kh == 3 && g.kw == 3 && g.stride == 1 && g.pad_h_lo == 1 &&
-                       g.pad_h_hi == 1 && g.pad_w_lo == 1 && g.pad_w_hi == 1 &&
-                       g.x_pix_stride <= 0 && g.x_row_pitch <= 0 && g.x_img_pitch <= 0 && np == 1 &&
-                       !out_f32 && !has_bias && (g.Cin % 64 == 0 || g.Cin == 32) &&
-                       g.Cout % 32 == 0;
-  if (!applies) return false;
-  if (g_conv_halo >= 2) return true;
-  // mode 1: the weight slab of an N tile stays in shared memory (otherwise the weight stream
-  // replaces the im2col re-reads as the ingest bound) and the images have >= 56 rows (16 x 8 patches
-  // waste <= 12.5 % of a 56 x 56 image, 27 % of 28 x 28)
-  const HaloPlan h = halo_plan(halo_bn(g.Cout), g.Cin % 64 == 0 ? 64 : 32, g.Cin, has_add, has_mask);
-  return h.stationary && g.H >= 56;
+// What one fprop / dgrad launch runs: its kernel, tile and persistent grid.  A pure host function of
+// the geometry, the precision, the fused epilogue parts present, the tuning knobs and the SM count;
+// conv_gemm_host launches it, acnn_conv_stats_parts() reports its statistics rows and
+// acnn_conv_ctas_per_sm() its occupancy.
+struct ConvChoice {
+  bool halo;     // conv_halo_kernel (im2col-free 3x3) instead of conv_gemm_kernel
+  int bn;        // N tile
+  int cw;        // channels per A chunk (one filter tap each when Cin < 64)
+  bool im2col;   // A tiles by im2col TMA (else 2-D tiles: dense 1x1, stride 1)
+  int np;        // operand planes: 1 = bf16 / fp16, 3 = the fp32 parity mode
+  bool f16;      // fp16 operands and output (ACNN_F16), one plane, the bf16 path's tiles
+  int wg;        // consumer warpgroups per CTA: 2 = one CTA per SM, 1 = two CTAs per SM
+  int pair;      // 1: clusters of two CTAs sharing the weight stages, one 256 x bn tile per pair
+  int per_n;     // CTAs (pair = 1: CTA pairs) per N tile
+  int parts;     // rows of the partial statistics buffer (= CTAs per N tile)
+  int stages;    // conv_gemm_kernel: smem pipeline depth
+  int smem;      // dynamic shared memory per CTA
+  HaloPlan hp;   // conv_halo_kernel: its shared-memory plan
+};
+
+static ConvChoice conv_choice(const acnn_conv_geom& g, int precision, bool has_add, bool has_mask,
+                              bool out_f32, bool has_bias) {
+  ConvChoice c{};
+  c.np = precision == ACNN_F32 ? 3 : 1;
+  c.f16 = precision == ACNN_F16;
+  c.cw = chunk_width(g.Cin);
+  c.im2col = !is_plain(g);
+  // N tile <= 128: a 64 x 256 fp32 accumulator per consumer warpgroup (128 registers per thread)
+  // does not fit next to the epilogue under the 168-register limit of a 384-thread CTA
+  c.bn = (g.Cout % 128 == 0) ? 128 : ((g.Cout % 64 == 0) ? 64 : 32);
+  c.wg = 2;
+  const bool halo_applies = g_conv_halo > 0 && g.kh == 3 && g.kw == 3 && g.stride == 1 &&
+                            g.pad_h_lo == 1 && g.pad_h_hi == 1 && g.pad_w_lo == 1 &&
+                            g.pad_w_hi == 1 && g.x_pix_stride <= 0 && g.x_row_pitch <= 0 &&
+                            g.x_img_pitch <= 0 && c.np == 1 && !out_f32 && !has_bias &&
+                            (g.Cin % 64 == 0 || g.Cin == 32) && g.Cout % 32 == 0;
+  if (halo_applies) {
+    c.hp = halo_plan(c.bn, c.cw, g.Cin, has_add, has_mask);
+    // mode 1: the weight slab of an N tile stays in shared memory (otherwise the weight stream
+    // replaces the im2col re-reads as the ingest bound) and the images have >= 56 rows (16 x 8
+    // patches waste <= 12.5 % of a 56 x 56 image, 27 % of 28 x 28)
+    c.halo = g_conv_halo >= 2 || (c.hp.stationary && g.H >= 56);
+  }
+  int m_tiles;
+  if (c.halo) {
+    c.smem = c.hp.smem;
+    m_tiles = g.B * ceil_div(g.H, kPatchH) * ceil_div(g.W, kPatchW);
+    c.per_n = num_sms() / (g.Cout / c.bn);
+  } else {
+    int Ho, Wo;
+    out_hw(g, &Ho, &Wo);
+    const int M = g.B * Ho * Wo, Ktot = g.kh * g.kw * g.Cin;
+    // CTA pairs: full-width (64-channel) chunks, K >= 512 (the k-loop, not the epilogue, paces the
+    // tile) and at least one pair tile per SM pair
+    c.pair = (g_conv_pairs && c.bn == 128 && c.np == 1 && !out_f32 && c.cw == 64 && Ktot >= 512 &&
+              (int64_t)ceil_div(M, 2 * kBM) * (g.Cout / 128) >= num_sms() / 2) ? 1 : 0;
+    // bf16 / fp16 operands with K <= kTwoCtaMaxK: two co-resident CTAs per SM on 128 x 64 (Cout % 64
+    // != 0: 128 x 32) tiles -- a 128 x 128 fp32 accumulator does not fit one warpgroup under the 168
+    // registers per thread of two 5-warp CTAs (ptxas spills) -- where that gives >= 2 N tiles (<=
+    // kMaxSms CTAs, i.e. partial statistics rows, per N tile).  The fp32 parity mode's three operand
+    // planes and the CTA pairs keep one CTA per SM.
+    const int bn2 = (g.Cout % 64 == 0 && g.Cout >= 128) ? 64 : 32;
+    c.wg = (c.np == 1 && !c.pair && g.Cout / bn2 >= 2 && Ktot <= kTwoCtaMaxK) ? 1 : 2;
+    if (c.wg == 1) c.bn = bn2;
+    // persistent grid: a multiple of the N tiles so that every CTA keeps one N tile (its weights
+    // and its per-channel statistics), at most one CTA per SM (two with wg = 1)
+    m_tiles = ceil_div(M, (c.pair ? 2 : 1) * kBM);
+    c.per_n = (c.pair ? num_sms() / 2 : (c.wg == 1 ? 2 * num_sms() : num_sms())) / (g.Cout / c.bn);
+    c.smem = fprop_smem(c.bn, c.np, c.wg, has_add, has_mask, out_f32, &c.stages);
+  }
+  if (c.per_n < 1) c.per_n = 1;
+  if (c.per_n > m_tiles) c.per_n = m_tiles;
+  c.parts = c.pair ? 2 * c.per_n : c.per_n;
+  return c;
 }
 
-// CTAs per N tile of the halo kernel's persistent grid (= partial statistics rows)
-static int halo_per_n(const acnn_conv_geom& g) {
-  const int n_tiles = g.Cout / halo_bn(g.Cout);
-  const int m_tiles = g.B * ceil_div(g.H, kPatchH) * ceil_div(g.W, kPatchW);
-  int per_n = num_sms() / n_tiles;
-  if (per_n < 1) per_n = 1;
-  return per_n > m_tiles ? m_tiles : per_n;
+// the type of every conv_gemm_kernel instantiation
+typedef void (*ConvGemmFn)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap,
+                           CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvGemmParams);
+
+// one instantiation, its shared-memory attributes set on first use (nullptr if that fails)
+template <int BN, int CW, bool IM2COL, int NP, bool CG2, bool F16, int WG>
+static ConvGemmFn conv_gemm_instance() {
+  static bool attr_set = false;
+  const ConvGemmFn kern = conv_gemm_kernel<BN, CW, IM2COL, NP, CG2, F16, WG>;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         WG == 2 ? kSmemBudget + 2048 : kSmemBudget2);
+    // two CTAs per SM need the largest shared-memory carveout
+    if (e == cudaSuccess && WG == 1)
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                               cudaSharedmemCarveoutMaxShared);
+    if (e != cudaSuccess) {
+      set_error("cudaFuncSetAttribute(conv_gemm): %s", cudaGetErrorString(e));
+      return nullptr;
+    }
+    attr_set = true;
+  }
+  return kern;
+}
+
+template <int BN, int NP, bool F16, int WG>
+static ConvGemmFn conv_gemm_instance_cw(const ConvChoice& c) {
+  if (c.im2col) {
+    if (c.cw == 64) return conv_gemm_instance<BN, 64, true, NP, false, F16, WG>();
+    if (c.cw == 32) return conv_gemm_instance<BN, 32, true, NP, false, F16, WG>();
+    return conv_gemm_instance<BN, 16, true, NP, false, F16, WG>();
+  }
+  if (c.cw == 64) return conv_gemm_instance<BN, 64, false, NP, false, F16, WG>();
+  if (c.cw == 32) return conv_gemm_instance<BN, 32, false, NP, false, F16, WG>();
+  return conv_gemm_instance<BN, 16, false, NP, false, F16, WG>();
+}
+
+template <int BN>
+static ConvGemmFn conv_gemm_instance_bn(const ConvChoice& c) {
+  if constexpr (BN == 128) {
+    if (c.pair) {     // full-width (64-channel) chunks only: bounds the instantiation count
+      if (c.f16) {
+        if (c.im2col) return conv_gemm_instance<128, 64, true, 1, true, true, 2>();
+        return conv_gemm_instance<128, 64, false, 1, true, true, 2>();
+      }
+      if (c.im2col) return conv_gemm_instance<128, 64, true, 1, true, false, 2>();
+      return conv_gemm_instance<128, 64, false, 1, true, false, 2>();
+    }
+  }
+  if (c.np == 3) return conv_gemm_instance_cw<BN, 3, false, 2>(c);
+  if constexpr (BN <= 64) {
+    if (c.wg == 1) {
+      if (c.f16) return conv_gemm_instance_cw<BN, 1, true, 1>(c);
+      return conv_gemm_instance_cw<BN, 1, false, 1>(c);
+    }
+  }
+  if (c.f16) return conv_gemm_instance_cw<BN, 1, true, 2>(c);
+  return conv_gemm_instance_cw<BN, 1, false, 2>(c);
+}
+
+// The conv_gemm_kernel instantiation of a choice: the kernel conv_gemm_host launches and whose
+// occupancy acnn_conv_ctas_per_sm() reports.  nullptr (error recorded) if its attributes cannot be set.
+static ConvGemmFn conv_gemm_kernel_for(const ConvChoice& c) {
+  if (c.bn == 128) return conv_gemm_instance_bn<128>(c);
+  if (c.bn == 64) return conv_gemm_instance_bn<64>(c);
+  return conv_gemm_instance_bn<32>(c);
 }
 
 static int make_map_4d(CUtensorMap* m, const void* base, int C, int W, int H, int B, int box_c,
@@ -1432,9 +1402,9 @@ static int make_map_4d(CUtensorMap* m, const void* base, int C, int W, int H, in
 }
 
 template <int BN, int CW, bool F16>
-static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* w, void* y,
-                            float* ch_part, const void* add_src, const void* mask_src,
-                            cudaStream_t stream) {
+static int launch_conv_halo(const acnn_conv_geom& g, const ConvChoice& c, const void* x,
+                            const void* w, void* y, float* ch_part, const void* add_src,
+                            const void* mask_src, cudaStream_t stream) {
   using Cfg = HaloCfg<BN, CW>;
   static bool attr_set = false;
   auto kern = conv_halo_kernel<BN, CW, F16>;
@@ -1457,12 +1427,10 @@ static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* 
   p.ch_part = ch_part;
   p.has_add = add_src != nullptr;
   p.has_mask = mask_src != nullptr;
-  const HaloPlan hp = halo_plan(BN, CW, g.Cin, p.has_add != 0, p.has_mask != 0);
-  p.a_stages = hp.a_stages;
-  p.b_slots = hp.b_slots;
-  p.stationary = hp.stationary;
+  p.a_stages = c.hp.a_stages;
+  p.b_slots = c.hp.b_slots;
+  p.stationary = c.hp.stationary;
   ACNN_REQUIRE(p.b_slots >= 2, "conv (halo): shared memory does not fit");
-  const int smem = hp.smem;
   CUtensorMap tmA, tmB, tmC, tmAdd, tmMask;
   int rc = make_map_4d(&tmA, x, g.Cin, g.W, g.H, g.B, CW, kHaloW, kHaloH, dt);
   if (rc) return rc;
@@ -1475,66 +1443,83 @@ static int launch_conv_halo(const acnn_conv_geom& g, const void* x, const void* 
   if (mask_src && (rc = make_map_4d(&tmMask, mask_src, g.Cout, g.W, g.H, g.B, Cfg::kSubW, kPatchW,
                                     kPatchH, dt)))
     return rc;
-  launch_k(kern, dim3(halo_per_n(g) * p.n_tiles), dim3(kThreads), smem, stream, tmA, tmB, tmC,
-           tmAdd, tmMask, p);
+  launch_k(kern, dim3(c.per_n * p.n_tiles), dim3(kThreads), c.smem, stream, tmA, tmB, tmC, tmAdd,
+           tmMask, p);
   count_launch();
   return check_launch("conv_halo_kernel");
 }
 
 template <bool F16>
-static int conv_halo_host(const acnn_conv_geom& g, const void* x, const void* w, void* y,
-                          float* ch_part, const void* add_src, const void* mask_src,
+static int conv_halo_host(const acnn_conv_geom& g, const ConvChoice& c, const void* x, const void* w,
+                          void* y, float* ch_part, const void* add_src, const void* mask_src,
                           cudaStream_t stream) {
-  const int bn = halo_bn(g.Cout);
-  const bool c64 = g.Cin % 64 == 0;
-  if (bn == 128) {
-    return c64 ? launch_conv_halo<128, 64, F16>(g, x, w, y, ch_part, add_src, mask_src, stream)
-               : launch_conv_halo<128, 32, F16>(g, x, w, y, ch_part, add_src, mask_src, stream);
+  const bool c64 = c.cw == 64;
+  if (c.bn == 128) {
+    return c64 ? launch_conv_halo<128, 64, F16>(g, c, x, w, y, ch_part, add_src, mask_src, stream)
+               : launch_conv_halo<128, 32, F16>(g, c, x, w, y, ch_part, add_src, mask_src, stream);
   }
-  if (bn == 64) {
-    return c64 ? launch_conv_halo<64, 64, F16>(g, x, w, y, ch_part, add_src, mask_src, stream)
-               : launch_conv_halo<64, 32, F16>(g, x, w, y, ch_part, add_src, mask_src, stream);
+  if (c.bn == 64) {
+    return c64 ? launch_conv_halo<64, 64, F16>(g, c, x, w, y, ch_part, add_src, mask_src, stream)
+               : launch_conv_halo<64, 32, F16>(g, c, x, w, y, ch_part, add_src, mask_src, stream);
   }
-  return c64 ? launch_conv_halo<32, 64, F16>(g, x, w, y, ch_part, add_src, mask_src, stream)
-             : launch_conv_halo<32, 32, F16>(g, x, w, y, ch_part, add_src, mask_src, stream);
+  return c64 ? launch_conv_halo<32, 64, F16>(g, c, x, w, y, ch_part, add_src, mask_src, stream)
+             : launch_conv_halo<32, 32, F16>(g, c, x, w, y, ch_part, add_src, mask_src, stream);
 }
 
-// precision 0: x / w are bf16.  precision 1 (fp32 parity mode): x and w each are THREE consecutive
-// bf16 planes (acnn_split3 / acnn_prep_weights with planes = 3), plane p of x at x + p * numel(x),
-// plane p of w at w + p * w_plane_stride elements; y must be fp32 (out_f32), no fused epilogue.
-// precision ACNN_F16: x / w (and y, add, mask unless out_f32) are fp16, on the bf16 path's tiles.
-// occ != null: nothing is launched or read; *occ = resident CTAs per SM of the conv GEMM kernel this
-// problem selects (add_src / mask_src / ch_part only say whether those epilogue parts are present).
-static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w, void* y,
-                          float* ch_part, const void* add_src, const void* mask_src,
-                          const float* bias, int out_f32, int precision, int64_t w_plane_stride,
-                          cudaStream_t stream, int* occ = nullptr) {
+// The argument checks of one fprop / dgrad launch with these epilogue parts.
+static int conv_check(const acnn_conv_geom& g, bool has_stats, bool has_add, bool has_mask,
+                      int out_f32, int precision, int64_t w_plane_stride) {
   ACNN_REQUIRE(g.B > 0 && g.H > 0 && g.W > 0 && g.Cin > 0 && g.Cout > 0, "conv: empty geometry");
   ACNN_REQUIRE(g.Cin % 16 == 0, "conv: Cin=%d must be a multiple of 16", g.Cin);
   ACNN_REQUIRE(g.Cout % 32 == 0, "conv: Cout=%d must be a multiple of 32", g.Cout);
   ACNN_REQUIRE(g.stride >= 1 && g.kh >= 1 && g.kw >= 1, "conv: bad kernel/stride");
-  ACNN_REQUIRE(!(ch_part && out_f32), "conv: statistics only with bf16 output");
+  ACNN_REQUIRE(!(has_stats && out_f32), "conv: statistics only with bf16 output");
   ACNN_REQUIRE(precision == ACNN_BF16 || precision == ACNN_F32 || precision == ACNN_F16,
                "conv: precision must be 0 (bf16), 1 (fp32) or 3 (fp16)");
-  ACNN_REQUIRE(precision != ACNN_F32 || (out_f32 && !add_src && !mask_src && !ch_part && w_plane_stride > 0),
+  ACNN_REQUIRE(precision != ACNN_F32 || (out_f32 && !has_add && !has_mask && !has_stats &&
+                                         w_plane_stride > 0),
                "conv: the fp32 (3-plane) mode needs fp32 output, a weight plane stride and no "
                "fused add / mask / statistics epilogue");
   int Ho, Wo;
   ACNN_REQUIRE(out_hw(g, &Ho, &Wo), "conv: empty output");
   ACNN_REQUIRE(g.pad_h_lo <= 128 && g.pad_w_lo <= 128 && g.kh <= 128 && g.kw <= 128,
                "conv: padding / filter exceed the TMA im2col corner range");
-  int rc = load_driver_fns();
+  // the weight tile's swizzle span: 128 bytes, or the whole 32- or 64-byte row of a smaller K
+  const int Ktot = g.kh * g.kw * g.Cin;
+  ACNN_REQUIRE(Ktot >= 64 || Ktot == 32 || Ktot == 16, "conv: unsupported K=%d", Ktot);
+  return ACNN_OK;
+}
+
+// precision 0: x / w are bf16.  precision 1 (fp32 parity mode): x and w each are THREE consecutive
+// bf16 planes (acnn_split3 / acnn_prep_weights with planes = 3), plane p of x at x + p * numel(x),
+// plane p of w at w + p * w_plane_stride elements; y must be fp32 (out_f32), no fused epilogue.
+// precision ACNN_F16: x / w (and y, add, mask unless out_f32) are fp16, on the bf16 path's tiles.
+static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w, void* y,
+                          float* ch_part, const void* add_src, const void* mask_src,
+                          const float* bias, int out_f32, int precision, int64_t w_plane_stride,
+                          cudaStream_t stream) {
+  int rc = conv_check(g, ch_part != nullptr, add_src != nullptr, mask_src != nullptr, out_f32,
+                      precision, w_plane_stride);
   if (rc) return rc;
-  const int np = precision == ACNN_F32 ? 3 : 1;
-  const bool f16 = precision == ACNN_F16;
-  if (use_halo(g, np, out_f32 != 0, bias != nullptr, add_src != nullptr, mask_src != nullptr)) {
-    ACNN_REQUIRE(!occ, "conv: this geometry runs on the halo kernel");
-    return f16 ? conv_halo_host<true>(g, x, w, y, ch_part, add_src, mask_src, stream)
-               : conv_halo_host<false>(g, x, w, y, ch_part, add_src, mask_src, stream);
+  const ConvChoice c = conv_choice(g, precision, add_src != nullptr, mask_src != nullptr,
+                                   out_f32 != 0, bias != nullptr);
+  // ch_part holds the rows acnn_conv_stats_parts() counts, those of the launch without add / mask /
+  // bias: a fused part that moves the launch to another kernel or grid would leave rows unwritten
+  // or write past the buffer
+  if (ch_part) {
+    const int parts = acnn_conv_stats_parts(&g);
+    ACNN_REQUIRE(c.parts == parts,
+                 "conv: with its add / mask / bias epilogue this launch writes %d partial "
+                 "statistics rows, acnn_conv_stats_parts() counts %d", c.parts, parts);
   }
-  const bool plain = is_plain(g);
-  const int cw = chunk_width(g.Cin);
-  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  if ((rc = load_driver_fns())) return rc;
+  if (c.halo) {
+    return c.f16 ? conv_halo_host<true>(g, c, x, w, y, ch_part, add_src, mask_src, stream)
+                 : conv_halo_host<false>(g, c, x, w, y, ch_part, add_src, mask_src, stream);
+  }
+  int Ho, Wo;
+  out_hw(g, &Ho, &Wo);
+  const CUtensorMapDataType dt = c.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   ConvGemmParams p;
   p.M = g.B * Ho * Wo;
   p.Cout = g.Cout;
@@ -1547,50 +1532,66 @@ static int conv_gemm_host(const acnn_conv_geom& g, const void* x, const void* w,
   p.pad_h_lo = g.pad_h_lo;
   p.pad_w_lo = g.pad_w_lo;
   p.b_sw_bytes = p.Ktot >= 64 ? 128 : p.Ktot * 2;
+  p.stages = c.stages;
+  p.m_tiles = ceil_div(p.M, (c.pair ? 2 : 1) * kBM);
+  p.n_tiles = g.Cout / c.bn;
   p.y = y;
   p.ch_part = ch_part;
   p.bias = bias;
   p.has_add = add_src != nullptr;
   p.has_mask = mask_src != nullptr;
   p.out_f32 = out_f32;
-  p.stages = p.m_tiles = p.n_tiles = 0;
-  ACNN_REQUIRE(p.b_sw_bytes == 128 || p.b_sw_bytes == 64 || p.b_sw_bytes == 32,
-               "conv: unsupported K=%d", p.Ktot);
 
-  const ConvTiling t =
-      conv_tiling(p.M, g.Cout, p.Ktot, cw, p.has_add, p.has_mask, out_f32 != 0, np);
-  const int bn = t.bn;
   ConvMaps tm;
   const int64_t x_plane = input_elems(g);
-  for (int pl = 0; pl < (occ ? 0 : np); ++pl) {
+  for (int pl = 0; pl < c.np; ++pl) {
     const __nv_bfloat16* xp = static_cast<const __nv_bfloat16*>(x) + pl * x_plane;
     const __nv_bfloat16* wp = static_cast<const __nv_bfloat16*>(w) + pl * w_plane_stride;
-    if (plain) {
-      rc = make_map_2d(&tm.a[pl], xp, p.M, g.Cin, g.Cin, kBM, cw, dt);
+    if (c.im2col) {
+      rc = make_map_im2col(&tm.a[pl], xp, g, c.cw, kBM, dt);
     } else {
-      rc = make_map_im2col(&tm.a[pl], xp, g, cw, kBM, dt);
+      rc = make_map_2d(&tm.a[pl], xp, p.M, g.Cin, g.Cin, kBM, c.cw, dt);
     }
     if (rc) return rc;
-    rc = make_map_2d(&tm.b[pl], wp, g.Cout, p.Ktot, p.Ktot, t.pair ? bn / 2 : bn,
+    rc = make_map_2d(&tm.b[pl], wp, g.Cout, p.Ktot, p.Ktot, c.pair ? c.bn / 2 : c.bn,
                      p.Ktot >= 64 ? 64 : p.Ktot, dt);
     if (rc) return rc;
   }
-  for (int pl = np; pl < 3; ++pl) {   // placeholders
+  for (int pl = c.np; pl < 3; ++pl) {   // placeholders
     tm.a[pl] = tm.a[0];
     tm.b[pl] = tm.b[0];
   }
   tm.c = tm.add = tm.mask = tm.b[0];   // placeholders when unused
-  const int subw = bn < 64 ? bn : 64;
-  if (!occ && !out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
-  if (!occ && add_src &&
-      (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw, dt)))
+  const int subw = c.bn < 64 ? c.bn : 64;
+  if (!out_f32 && (rc = make_map_2d(&tm.c, y, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
+  if (add_src && (rc = make_map_2d(&tm.add, add_src, p.M, g.Cout, g.Cout, kBM, subw, dt))) return rc;
+  if (mask_src && (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw, dt)))
     return rc;
-  if (!occ && mask_src &&
-      (rc = make_map_2d(&tm.mask, mask_src, p.M, g.Cout, g.Cout, kBM, subw, dt)))
-    return rc;
-  if (bn == 128) return dispatch_conv_gemm<128>(t, np, f16, cw, !plain, tm, p, stream, occ);
-  if (bn == 64) return dispatch_conv_gemm<64>(t, np, f16, cw, !plain, tm, p, stream, occ);
-  return dispatch_conv_gemm<32>(t, np, f16, cw, !plain, tm, p, stream, occ);
+
+  const ConvGemmFn kern = conv_gemm_kernel_for(c);
+  if (!kern) return ACNN_ERR_CUDA;
+  if (c.pair) {
+    // per_n CTA PAIRS per N tile, launched as clusters of two
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(2 * c.per_n * p.n_tiles);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = c.smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = 2;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    (void)cudaLaunchKernelEx(&cfg, kern, tm.a[0], tm.b[0], tm.c, tm.add, tm.mask, tm.a[1], tm.a[2],
+                             tm.b[1], tm.b[2], p);
+  } else {
+    launch_k(kern, dim3(c.per_n * p.n_tiles), dim3(conv_threads(c.wg)), c.smem, stream, tm.a[0],
+             tm.b[0], tm.c, tm.add, tm.mask, tm.a[1], tm.a[2], tm.b[1], tm.b[2], p);
+  }
+  count_launch();
+  return check_launch("conv_gemm_kernel");
 }
 
 struct WgradMaps {
@@ -1614,10 +1615,6 @@ static int g_wgrad_splits = 0;
 
 // 0: choose per problem; 64 / 128: force the pixels per stage where the shape allows it
 static int g_wgrad_pix = 0;
-static bool wgrad_wants_pix128(int) {
-  // 128-pixel stages wherever they fit (N tile <= 128): twice the MMAs per barrier round trip
-  return true;
-}
 
 // Tiling and split-K layout of one wgrad launch: a pure host function of the geometry, the
 // precision, `deterministic`, the tuning knobs and the SM count, shared by the launcher and
@@ -1646,11 +1643,10 @@ static int wgrad_plan(const acnn_conv_geom& g, int precision, int deterministic,
   w->bn = bn;
   w->n_tiles = g.Cout / bn;
   w->m_tiles = ceil_div(g.kh * g.kw * g.Cin, 128);
-  // 128-pixel stages: only the bf16 path, N tile <= 128 (smem), enough pixels to split
+  // 128-pixel stages (twice the MMAs per barrier round trip) wherever they fit, unless 64 are
+  // forced: only the bf16 path, N tile <= 128 (smem), enough pixels to split
   w->pix = kWgPix;
-  if (np == 1 && bn <= 128 && w->P >= 4096 &&
-      (g_wgrad_pix == 128 || (g_wgrad_pix == 0 && wgrad_wants_pix128(bn))))
-    w->pix = 128;
+  if (np == 1 && bn <= 128 && w->P >= 4096 && g_wgrad_pix != 64) w->pix = 128;
   w->stages_total = ceil_div(w->P, w->pix);
   // split the pixel (K) range over CTAs; the partial tiles are summed in split order, so the result
   // does not depend on which split finishes first.  deterministic: no split -- one add per dw
@@ -1908,10 +1904,9 @@ int acnn_conv_wgrad_plan(const acnn_conv_geom* g, int precision, int determinist
 int acnn_conv_stats_parts(const acnn_conv_geom* g) {
   if (!g) return 0;
   int Ho, Wo;
-  if (!acnn::out_hw(*g, &Ho, &Wo) || g->Cout % 32 != 0) return 0;
-  if (acnn::use_halo(*g, 1, false, false, false, false)) return acnn::halo_per_n(*g);
-  return acnn::conv_tiling(g->B * Ho * Wo, g->Cout, g->kh * g->kw * g->Cin,
-                           acnn::chunk_width(g->Cin), false, false, false, 1).parts;
+  if (!acnn::out_hw(*g, &Ho, &Wo) || g->Cout <= 0 || g->Cout % 32 != 0) return 0;
+  // the launch with statistics and no add / mask / bias (precision 0 and 3 choose alike)
+  return acnn::conv_choice(*g, ACNN_BF16, false, false, false, false).parts;
 }
 
 int acnn_conv_ctas_per_sm(const acnn_conv_geom* g, int precision, int has_add, int has_mask,
@@ -1920,12 +1915,24 @@ int acnn_conv_ctas_per_sm(const acnn_conv_geom* g, int precision, int has_add, i
     acnn::set_error("acnn_conv_ctas_per_sm: null argument");
     return ACNN_ERR_INVALID;
   }
-  // non-null placeholders: only their presence selects the epilogue (nothing is read)
-  const void* tag = g;
   *ctas = 0;
-  return acnn::conv_gemm_host(*g, nullptr, nullptr, nullptr, nullptr, has_add ? tag : nullptr,
-                              has_mask ? tag : nullptr, nullptr, precision == ACNN_F32 ? 1 : 0,
-                              precision, precision == ACNN_F32 ? 1 : 0, nullptr, ctas);
+  const int out_f32 = precision == ACNN_F32 ? 1 : 0;   // the fp32 mode stores fp32
+  const int rc = acnn::conv_check(*g, false, has_add != 0, has_mask != 0, out_f32, precision,
+                                  out_f32);
+  if (rc) return rc;
+  const acnn::ConvChoice c =
+      acnn::conv_choice(*g, precision, has_add != 0, has_mask != 0, out_f32 != 0, false);
+  ACNN_REQUIRE(!c.halo, "conv: this geometry runs on the halo kernel");
+  const acnn::ConvGemmFn kern = acnn::conv_gemm_kernel_for(c);
+  if (!kern) return ACNN_ERR_CUDA;
+  const cudaError_t e =
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas, kern, acnn::conv_threads(c.wg), c.smem);
+  if (e != cudaSuccess) {
+    acnn::set_error("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_gemm): %s",
+                    cudaGetErrorString(e));
+    return ACNN_ERR_CUDA;
+  }
+  return ACNN_OK;
 }
 
 int acnn_set_conv_cta_pairs(int on) {

@@ -134,7 +134,9 @@ typedef struct acnn_conv_geom {
  *                                     row of the persistent grid STORES its partial column sums and
  *                                     sums of squares of the bf16-rounded output (no atomics, nothing
  *                                     to zero); parts = acnn_conv_stats_parts(g); acnn_bn_finalize
- *                                     adds the rows in a fixed order (bit-reproducible)
+ *                                     adds the rows in a fixed order (bit-reproducible).  A call
+ *                                     whose add / mask / bias makes the launch write another row
+ *                                     count fails with ACNN_ERR_INVALID (see acnn_conv_stats_parts)
  * out_f32 != 0 stores y as fp32 (logits), else bf16.  Requires Cin % 16 == 0, Cout % 32 == 0.
  * precision ACNN_F16 (3): x, w, add_src, mask_src and a 16-bit y are fp16 instead of bf16 (the
  * statistics are of the fp16-rounded output); everything else as precision 0.
@@ -147,8 +149,13 @@ int acnn_conv_fprop(const acnn_conv_geom* g, const void* x, const void* w, void*
                     float* ch_part, const void* add_src, const void* mask_src,
                     const float* bias, int out_f32, int precision, int64_t w_plane_stride,
                     void* stream);
-/* Rows of the partial statistics buffer acnn_conv_fprop(g, ..., ch_part, ...) writes (a pure
- * function of the geometry and the device's SM count; <= 132). */
+/* Rows of the partial statistics buffer acnn_conv_fprop(g, ..., ch_part, ...) writes without a fused
+ * add / mask / bias (a pure function of the geometry, the conv knobs and the device's SM count;
+ * <= 132; 0 for an empty output or a Cout that is not a positive multiple of 32).  A fused add, mask or
+ * bias can move the launch to another kernel and grid (the 3x3 halo kernel runs no bias, and by
+ * default only where the add / mask staging leaves its weight slab room): acnn_conv_fprop refuses
+ * ch_part with ACNN_ERR_INVALID where that changes the row count, e.g. B = 1, 56 x 56, 64 -> 128
+ * 3x3 with an add (25 rows against 28). */
 int acnn_conv_stats_parts(const acnn_conv_geom* g);
 /* *ctas = how many CTAs of the conv GEMM kernel acnn_conv_fprop(g, ..., precision) launches fit one
  * SM together (cudaOccupancyMaxActiveBlocksPerMultiprocessor at that launch's shared memory, with the

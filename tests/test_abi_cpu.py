@@ -115,6 +115,23 @@ def test_sk_fc_scratch_formula_matches_library():
             assert lib.acnn_sk_fc_scratch_floats(B, f, d) == sk_fc_scratch_floats(B, f, d), (B, f)
 
 
+def test_conv_fprop_refuses_statistics_rows_it_would_not_write():
+    """ch_part holds acnn_conv_stats_parts(g) rows: those of the launch without add / mask / bias.
+    On a B = 1, 56 x 56, 64 -> 128 3x3 conv that launch runs on the halo kernel (28 patch rows);
+    an add tile leaves the weight slab no room there, so the launch moves to the GEMM kernel's 25
+    rows.  fprop with both is refused before any CUDA work (the pointers are never read)."""
+    from assembled_cnn_b200 import _lib
+    lib = _lib.load()
+    g = _lib.ConvGeom(1, 56, 56, 64, 128, 3, 3, 1, 1, 1, 1, 1)
+    assert lib.acnn_conv_stats_parts(g) == 28
+    p = 1 << 20
+    assert lib.acnn_conv_fprop(g, p, p, p, p, p, None, None, 0, 0, 0, None) == 1   # ACNN_ERR_INVALID
+    msg = lib.acnn_last_error().decode()
+    assert "25" in msg and "28" in msg, msg
+    # no output channels: no statistics rows
+    assert lib.acnn_conv_stats_parts(_lib.ConvGeom(1, 8, 8, 64, 0, 1, 1, 1, 0, 0, 0, 0)) == 0
+
+
 def test_conv_wgrad_plan_properties():
     """acnn_conv_wgrad_plan (host only: the SM count is the H100's 132 without a device) against
     the rules include/acnn.h states, over a grid of geometries and both precisions: one split when

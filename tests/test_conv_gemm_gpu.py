@@ -9,6 +9,7 @@ import contextlib
 import pytest
 import torch
 
+from oracle import conv_check as CC
 from oracle import tf_ops
 
 pytestmark = pytest.mark.gpu
@@ -182,6 +183,31 @@ def test_fprop_epilogue_add_mask_bias(lib):
                                    None, None, biasd.data_ptr(), 1, 0, 0, st))
     torch.cuda.synchronize()
     assert _relerr(yf.cpu(), ref + bias) < F32_TOL
+
+
+def test_fprop_add_and_statistics_write_stats_parts_rows(lib):
+    """A fused add with statistics on a 56 x 56, 64 -> 128 3x3 conv: the add tile moves the launch
+    from the halo kernel to the GEMM kernel.  At B = 256 both grids have the rows
+    acnn_conv_stats_parts() counts, so the call is accepted: every row is stored, the rows sum to the
+    statistics of the stored y + add, and the statistics leave y unchanged."""
+    from assembled_cnn_b200 import _lib
+    B, H, W, Cin, Cout = 256, 56, 56, 64, 128
+    g = _geom(B, H, W, Cin, Cout, 3, 1)
+    gen = torch.Generator(device="cuda").manual_seed(41)
+    xd = torch.randn(B, H, W, Cin, generator=gen, device="cuda").bfloat16()
+    wd = (torch.randn(Cout, 3, 3, Cin, generator=gen, device="cuda") * (9 * Cin) ** -0.5).bfloat16()
+    addd = torch.randn(B, H, W, Cout, generator=gen, device="cuda").bfloat16()
+    st = torch.cuda.current_stream().cuda_stream
+    sp = CC.stats_poison((lib.acnn_conv_stats_parts(g), 2, Cout))
+    y = torch.full((B, H, W, Cout), float("nan"), dtype=torch.bfloat16, device="cuda")
+    y2 = torch.full_like(y, float("nan"))
+    _lib.check(lib.acnn_conv_fprop(g, xd.data_ptr(), wd.data_ptr(), y.data_ptr(), sp.data_ptr(),
+                                   addd.data_ptr(), None, None, 0, 0, 0, st), "fprop add + statistics")
+    _lib.check(lib.acnn_conv_fprop(g, xd.data_ptr(), wd.data_ptr(), y2.data_ptr(), None,
+                                   addd.data_ptr(), None, None, 0, 0, 0, st), "fprop add")
+    torch.cuda.synchronize()
+    CC.check_stats(sp, y, "fprop add + statistics")
+    assert torch.equal(y.view(torch.int16), y2.view(torch.int16))
 
 
 DGRAD_CASES = [c for c in CASES if c[6] == 1]

@@ -193,7 +193,7 @@ def _wgrad_chain(lib, cg, precision, det):
 
 
 def _pairs_apply(cg, M, out_f32):
-    """conv_tiling (csrc/gemm.cu) pairs CTAs here under acnn_set_conv_cta_pairs(1)."""
+    """conv_choice (csrc/gemm.cu) pairs CTAs here under acnn_set_conv_cta_pairs(1)."""
     K = cg.kh * cg.kw * cg.Cin
     return (cg.Cout % 128 == 0 and cg.Cin % 64 == 0 and K >= 512 and not out_f32
             and -(-M // 256) * (cg.Cout // 128) >= NUM_SMS // 2)

@@ -93,7 +93,7 @@ def _halo_slab_fits(Cin, Cout, n_aux):
 
 def _family(case, n_aux):
     """The conv GEMM kernel csrc/gemm.cu picks for the case with n_aux staged add / mask tiles under its
-    default knobs (use_halo mode 1, conv_tiling), and whether acnn_set_conv_cta_pairs(1) pairs its CTAs."""
+    default knobs (conv_choice: halo mode 1, tiling), and whether acnn_set_conv_cta_pairs(1) pairs its CTAs."""
     B, H, W, Cin, Cout, kh, kw, stride, phl, phh, pwl, pwh = _gemm_geom(case)
     K = kh * kw * Cin
     M = B * ((H + phl + phh - kh) // stride + 1) * ((W + pwl + pwh - kw) // stride + 1)
